@@ -28,8 +28,13 @@ memory (one launch; plain NCCL all-reduce if peer mapping is unavailable).  `val
 minibatch updates/s.  The weak-scaling figure (4096 rows per rank) is kept under detail.weak
 (`config` is identical in both arms, so everything run-specific lives in `detail`).
 
-`--impl reference` times the reference algorithm's CPU path (the oracle port: /root/reference
-does not exist on the GPU box) with the best host thread count of a sweep.
+`--impl reference` times the reference algorithm's CPU path (the oracle port, so that no copy of
+the reference is needed) with the best host thread count of a sweep.
+
+`--dump-outputs DIR` writes, after the timed steps, what the timed path handed back in its last
+step -- the loss and every parameter of the trained networks -- as DIR/<config>_<name>.npy
+(float32).  Inputs are seeded, so two builds run with the same arguments can be compared
+output for output.
 """
 import argparse
 import json
@@ -62,10 +67,9 @@ CONFIGS = {
                      "B=16384 (global), prioritized replay cap=2^18, actor/critics [256,256] relu"),
 }
 ACTS = ["relu", "relu"]
-# kept for the profiling scripts under profiles/
-S, A, B, CAP = CONFIGS[2]["S"], CONFIGS[2]["A"], CONFIGS[2]["B"], CONFIGS[2]["cap"]
-SIZES = CONFIGS[2]["sizes"]
-METRIC, WORKLOAD = CONFIGS[2]["metric"], CONFIGS[2]["workload"]
+# NVIDIA H100 SXM data sheet, dense: the denominators of the roofline fractions (not measured)
+H100_PEAK_TFLOPS = {"bf16": 989.0, "tf32": 495.0}
+DUMP_LIMIT_BYTES = 64 << 20
 
 
 def _sigma(dims):
@@ -116,7 +120,7 @@ def synth_stream(n, seed, cfg=None):
 
 
 class ClockSampler(threading.Thread):
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
 
     def __init__(self, gpu_index):
         super().__init__(daemon=True)
@@ -309,9 +313,8 @@ def run_reference(args):
         "e2e": {"value": v, "unit": "updates/s", "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0},
         "gpu_launches": 0,
         "detail": {"note": "reference algorithm restated on CPU (oracle/replay_oracle.py + "
-                           "oracle/td_oracle.py): /root/reference is not on the GPU box; a CPU arm "
-                           "has no ranks: the global minibatch is processed by one process on the "
-                           "host cores whatever --gpus says"},
+                           "oracle/td_oracle.py); a CPU arm has no ranks: the global minibatch is "
+                           "processed by one process on the host cores whatever --gpus says"},
     }
     print(json.dumps(line), flush=True)
 
@@ -601,6 +604,7 @@ def run_dqn(env, args, clocks):
     e1.record()
     env.barrier()
     dev_ms = env.max_over_ranks(e0.elapsed_time(e1))
+    outputs = timed_outputs(trainer, g_timed._rb200_last_loss)
 
     # ---- weak scaling (secondary): 4096 rows per rank, rank-specific draws ----
     weak = None
@@ -641,6 +645,7 @@ def run_dqn(env, args, clocks):
     flops = td_kernel_flops(cfg, Bl)
     res = {
         "value": K / (dev_ms * 1e-3), "ms_per_step": dev_ms / K, "config": conf, "detail": detail,
+        "outputs": outputs,
         "e2e": {"value": K / (e2e_ms * 1e-3), "unit": "updates/s",
                 "h2d_bytes_per_step": h2d_online, "d2h_bytes_per_step": d2h_online,
                 "ms_per_step": e2e_ms / K,
@@ -653,12 +658,11 @@ def run_dqn(env, args, clocks):
         # sample, (weight images unless Adam wrote them), TD step, weight gradients, Adam+Polyak
         "gpu_launches": (4 if (not on_tc or os.environ.get("RB200_ADAM_PACK", "1") == "1") else 5) * K,
         "roofline_kernel": {
-            "kernel": ("dqn_td_tc_kernel (fused TD target + loss + dZ chain on tcgen05/TMEM)"
+            "kernel": ("dqn_td_tc_kernel (fused TD target + loss + dZ chain on wgmma)"
                        if on_tc else "dqn_td_rows_kernel (fused TD target + loss + dZ chain, mma.sync)"),
             "flops": flops, "kernel_ms": kern_ms,
-            "pipe_used": ("tcgen05.mma kind::tf32, 3xTF32 as 2 MMAs per k step (N=64 + N=32)"
-                          if on_tc else "mma.sync m16n8k8 tf32, 3xTF32"),
-            "ncu_file": "profiles/r02_ncu_dqn_td_tc.csv" if on_tc else None},
+            "pipe_used": ("wgmma kind tf32, 3xTF32 as 2 MMAs per k step (N=64 + N=32)"
+                          if on_tc else "mma.sync m16n8k8 tf32, 3xTF32")},
     }
     if check:
         res["dp_check"] = check
@@ -676,8 +680,7 @@ def run_generic(env, args, cfg):
     from reagent_b200.replay_memory import PrioritizedReplayBuffer
 
     dev, world, pg = env.dev, env.world, env.pg
-    K = max(3, min(args.steps, {"qrdqn": 20, "sac": 50, "td3": 50}[cfg["algo"]]))
-    W = 3
+    K, W = args.steps, max(args.warmup, 3)
     Bg = cfg["B"]
     lo, hi = env.shard(Bg)
     Bl = hi - lo
@@ -740,10 +743,11 @@ def run_generic(env, args, cfg):
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     e0.record()
     for i in range(K):
-        trainer.train_batch(sample(qs[W + i]), W + i, process_group=pg)
+        out = trainer.train_batch(sample(qs[W + i]), W + i, process_group=pg)
     e1.record()
     env.barrier()
     dev_ms = env.max_over_ranks(e0.elapsed_time(e1))
+    outputs = timed_outputs(trainer, loss_of(out))
     kern_ms = None
     if getattr(trainer, "_kernel_events", None):
         durs = [a.elapsed_time(b) for a, b in trainer._kernel_events]
@@ -757,7 +761,7 @@ def run_generic(env, args, cfg):
         detail["collective"] = env.collective
     res = {
         "value": K / (dev_ms * 1e-3), "ms_per_step": dev_ms / K, "steps": K, "warmup": W,
-        "config": conf, "detail": detail,
+        "config": conf, "detail": detail, "outputs": outputs,
         "e2e": {"value": K / (e2e_ms * 1e-3), "unit": "updates/s", "h2d_bytes_per_step": Bl * 8,
                 "d2h_bytes_per_step": 4, "ms_per_step": e2e_ms / K,
                 "api": "rb.sample_%s_batch(...) (host RNG -> pinned -> H2D -> sample kernel) + "
@@ -770,47 +774,65 @@ def run_generic(env, args, cfg):
             "kernel": "ac_critic_rows_kernel (fused %s TD target: actor(s') + target critics + "
                       "min + losses + critic dZ chains, mma.sync 3xTF32)" % cfg["algo"].upper(),
             "flops": td_kernel_flops(cfg, Bl), "kernel_ms": kern_ms,
-            "pipe_used": "mma.sync m16n8k8 tf32, 3xTF32", "ncu_file": None}
+            "pipe_used": "mma.sync m16n8k8 tf32, 3xTF32"}
     elif cfg["algo"] == "qrdqn":
         res["roofline_kernel"] = {
-            "kernel": "whole QR-DQN update (tc_linear_fwd_kernel on tcgen05: head forward x3 and the "
+            "kernel": "whole QR-DQN update (tc_linear_fwd_kernel on wgmma: head forward x3 and the "
                       "split-K head backward; qr_head_kernel, wgrad_kernel, adam_soft_kernel)",
             "flops": update_flops(cfg, Bl), "kernel_ms": dev_ms / K,
-            "pipe_used": "tcgen05 kind::tf32 (head forward + head dX) + mma.sync tf32 (trunk, wgrad)",
-            "ncu_file": None}
+            "pipe_used": "wgmma kind tf32 (head forward + head dX) + mma.sync tf32 (trunk, wgrad)"}
     if check:
         res["dp_check"] = check
     return res
 
 
-def roofline_of(rk, peaks):
+def roofline_of(rk):
     if not rk or not rk.get("flops"):
         return None
-    peak_tf = float(peaks.get("bf16_tflops", 1700.0))
-    src = ("measured (MEASURED_PEAKS.json bf16_tflops, burst: the kernel is timed alone between "
-           "events)" if peaks else "fallback 1.7 PF/s")
+    peak_tf = H100_PEAK_TFLOPS["bf16"]
     ach = rk["flops"] / (rk["kernel_ms"] * 1e-3) / 1e12
-    traffic, tsrc = None, None
-    if rk.get("ncu_file"):
-        try:  # dram bytes of one ncu --set full launch of this kernel, read from the profile
-            import csv
-
-            with open(os.path.join(ROOT, rk["ncu_file"])) as f:
-                rows = {r[0]: r for r in csv.reader(f) if r}
-            rd = float(rows["dram__bytes_read.sum"][2]) * {"Mbyte": 1e6, "Kbyte": 1e3, "byte": 1, "Gbyte": 1e9}[rows["dram__bytes_read.sum"][1]]
-            wr = float(rows["dram__bytes_write.sum"][2]) * {"Mbyte": 1e6, "Kbyte": 1e3, "byte": 1, "Gbyte": 1e9}[rows["dram__bytes_write.sum"][1]]
-            traffic = rd + wr
-            tsrc = f"dram__bytes_read.sum + dram__bytes_write.sum of one ncu --set full launch ({rk['ncu_file']}), bytes"
-        except Exception:
-            traffic = None
     return {"kernel": rk["kernel"], "bound": "tensor", "achieved": ach, "peak": peak_tf,
-            "unit": "TFLOP/s", "frac": ach / peak_tf, "traffic": traffic, "traffic_source": tsrc,
-            "peak_source": src, "algorithmic_flops_per_launch": rk["flops"],
+            "unit": "TFLOP/s", "frac": ach / peak_tf,
+            "peak_source": "NVIDIA H100 SXM data sheet, dense BF16 (not measured)",
+            "algorithmic_flops_per_launch": rk["flops"],
             "kernel_ms": rk["kernel_ms"], "pipe_used": rk["pipe_used"],
             "executed_over_algorithmic_flops": 3.0,
-            "frac_of_3xtf32_ceiling": ach / (peak_tf / 6.0),
-            "note": "fp32-parity (1e-5) forces 3xTF32: 3 tensor-core flops per algorithmic flop, "
-                    "and TF32 dense peak is half the bf16 peak this fraction is quoted against"}
+            "frac_of_3xtf32_ceiling": ach / (H100_PEAK_TFLOPS["tf32"] / 3.0),
+            "note": "fp32-parity (1e-5) forces 3xTF32: 3 tensor-core flops per algorithmic flop; "
+                    "the ceiling is the data-sheet dense TF32 rate over 3"}
+
+
+def timed_outputs(trainer, loss):
+    """What a caller of the timed path holds after its last step: the loss and the updated
+    parameters (online and target networks), as float32 host arrays."""
+    import numpy as np
+
+    out = {"loss": loss.detach().float().reshape(-1).cpu().numpy()}
+    for name, p in trainer.named_parameters():
+        out["param." + name] = p.detach().float().cpu().numpy()
+    return {k: np.ascontiguousarray(v, dtype=np.float32) for k, v in out.items()}
+
+
+def dump_outputs(directory, results):
+    """results: [(config, outputs)].  Writes DIR/c<config>_<name>.npy, at most DUMP_LIMIT_BYTES
+    in all: an array that would overflow the budget is replaced by a fixed, seeded sample of its
+    elements (the flat indices are stored next to it as <name>.sample_index.npy)."""
+    import numpy as np
+
+    os.makedirs(directory, exist_ok=True)
+    used = 0
+    for c, outputs in results:
+        for name, arr in outputs.items():
+            arr = np.asarray(arr, dtype=np.float32)
+            path = os.path.join(directory, f"c{c}_{name}")
+            if used + arr.nbytes > DUMP_LIMIT_BYTES:
+                n = max(0, min(arr.size, (DUMP_LIMIT_BYTES - used) // 12))
+                idx = np.sort(np.random.RandomState(0).choice(arr.size, n, replace=False))
+                np.save(path + ".sample_index.npy", idx.astype(np.int64))
+                arr = arr.reshape(-1)[idx]
+                used += idx.nbytes
+            np.save(path + ".npy", arr)
+            used += arr.nbytes
 
 
 def run_ours(args):
@@ -837,18 +859,11 @@ def run_ours(args):
             cpu[c] = {"value": v, "unit": "updates/s", "cores": cores, "kind": "port", "sample": sample}
     if env.rank != 0:
         return
-    peaks = {}
-    try:
-        with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
-            peaks = json.load(f)
-    except Exception:
-        pass
-
     def finish(r, c):
         out = {"metric": CONFIGS[c]["metric"], "value": r["value"], "unit": "updates/s",
                "ms_per_step": r["ms_per_step"], "config": r["config"], "e2e": r["e2e"],
                "gpu_launches": r["gpu_launches"], "detail": r["detail"]}
-        rl = roofline_of(r.get("roofline_kernel"), peaks)
+        rl = roofline_of(r.get("roofline_kernel"))
         if rl:
             out["roofline"] = rl
         if c in cpu:
@@ -872,6 +887,9 @@ def run_ours(args):
         line["configs"] = [dict(finish(r, r["_cfg"]), steps=r["steps"], warmup=r["warmup"],
                                 n_gpus=1, note="global batch of this config on ONE GPU")
                            for r in extra]
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, [(args.config, res["outputs"])] +
+                     [(r["_cfg"], r["outputs"]) for r in extra])
     print(json.dumps(line), flush=True)
 
 
@@ -885,6 +903,8 @@ def main():
     ap.add_argument("--only", action="store_true", help="config 2: skip the configs 3-5 array")
     ap.add_argument("--cpu-steps", type=int, default=60)
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the timed path's last-step outputs as DIR/<config>_<name>.npy")
     args = ap.parse_args()
     if args.impl == "reference":
         run_reference(args)

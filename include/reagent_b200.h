@@ -1,4 +1,4 @@
-/* reagent_b200 -- C ABI of the B200-native off-policy training hot path.
+/* reagent_b200 -- C ABI of the H100-native off-policy training hot path.
  *
  * The reference (facebookresearch/ReAgent) has no FFI for this path: it is plain
  * Python over torch (SURVEY.md section 8b).  This header is the boundary one level
@@ -172,8 +172,8 @@ int rb200_num_row_tiles(int batch, int max_dim_in, int max_dim_hidden);
 int rb200_dqn_td_step(const rb200_mlp_t* q_net, const rb200_mlp_t* q_target,
                       const rb200_dqn_args_t* args, const rb200_net_ws_t* ws, void* stream);
 
-/* The same step on the 5th-generation tensor cores (tcgen05.mma kind::tf32 with 3xTF32 error
- * compensation, accumulators in Tensor Memory, weights streamed by bulk async copies):
+/* The same step on the Hopper tensor cores (warpgroup MMAs, wgmma kind tf32 with 3xTF32 error
+ * compensation, accumulators in registers, weights streamed by bulk async copies):
  * rb200_dqn_tc.cu.  Same arguments, semantics and reference lines as rb200_dqn_td_step plus a
  * caller-owned scratch buffer for the packed hi/lo weight images (re-packed on every call,
  * because the weights change on every update).
@@ -311,14 +311,14 @@ typedef struct rb200_qrdqn_args {
 
 int rb200_linear_forward(const float* W, const float* b, int32_t act, int32_t K, int32_t N,
                          const float* in, int32_t batch, float* out, void* stream);
-/* tcgen05.mma (kind::tf32, 3xTF32) + TMEM implementation of rb200_linear_forward, taken
+/* wgmma (kind tf32, 3xTF32) implementation of rb200_linear_forward, taken
  * automatically for batch >= 128 and N >= 128 */
 int rb200_linear_forward_tc(const float* W, const float* b, int32_t act, int32_t K, int32_t N,
                             const float* in, int32_t batch, float* out, void* stream);
 int rb200_linear_backward_dx(const float* W, int32_t K, int32_t N, const float* dz,
                              const float* h_prev, int32_t act_prev, int32_t batch, float* out,
                              void* stream);
-/* tcgen05 implementation of rb200_linear_backward_dx for a wide layer (the contraction runs
+/* wgmma implementation of rb200_linear_backward_dx for a wide layer (the contraction runs
  * over the N out-features: split-K slices of the tensor-core GEMM, added in a fixed order).
  * _scratch_bytes returns 0 when the shape is not taken by this path (N < 1024, batch < 256 or
  * K / N not multiples of 4): call rb200_linear_backward_dx then.  Replaces the same autograd
@@ -388,13 +388,13 @@ int rb200_ac_actor_step(const rb200_mlp_t* actor, const rb200_mlp_t* q1, const r
 /* Weight gradients: dW_l = dZ_l^T . A_{l-1}, db_l = sum_b dZ_l, split over    */
 /* the batch; partial s lands at gpart + s*n_params (arena layout).            */
 /* Default: mma.sync 3xTF32 tiles (rb200_optim.cu).  RB200_WGRAD_TC=1 selects the  */
-/* tcgen05 kernel (rb200_wgrad_tc.cu: operands transposed into K-major planes while */
-/* staging, accumulator in Tensor Memory); same results to 1e-5, same speed today.  */
+/* wgmma kernel (rb200_wgrad_tc.cu: operands transposed into K-major planes while   */
+/* staging, accumulators in registers); same results to 1e-5.                        */
 /* Replaces autograd's Linear backward (torch) reached from                    */
 /* loss.backward() in the Lightning loop (reagent_lightning_module.py:108-133).*/
 /* ------------------------------------------------------------------------- */
 int rb200_wgrad_splits(int batch);
-/* slabs for this network (tcgen05 kernel: enough (tile, slab) jobs to fill the SMs twice) */
+/* slabs for this network (wgmma kernel: enough (tile, slab) jobs to fill the SMs twice) */
 int rb200_wgrad_splits_for(const rb200_mlp_t* net, int32_t batch);
 int rb200_mlp_wgrad(const rb200_mlp_t* net, const float* net_input, int32_t batch,
                     const rb200_net_ws_t* ws, float* gpart, int32_t splits, void* stream);

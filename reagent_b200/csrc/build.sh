@@ -1,12 +1,11 @@
 #!/bin/bash
-# Build libreagent_b200.so in-tree for sm_100a.  Usage: build.sh [extra nvcc flags]
+# Build libreagent_b200.so in-tree for sm_90a (H100).  Usage: build.sh [extra nvcc flags]
 set -euo pipefail
 cd "$(dirname "$0")"
 NVCC=${NVCC:-/usr/local/cuda/bin/nvcc}
 OUT=../libreagent_b200.so
 SRCS=$(ls rb200_*.cu)
-FLAGS="-gencode arch=compute_100a,code=sm_100a -O3 -lineinfo -std=c++17 -Xcompiler -fPIC -Xcompiler -O2 --use_fast_math=false"
-FLAGS="-gencode arch=compute_100a,code=sm_100a -O3 -lineinfo -std=c++17 -Xcompiler -fPIC"
+FLAGS="-gencode arch=compute_90a,code=sm_90a -O3 -lineinfo -std=c++17 -Xcompiler -fPIC"
 mkdir -p build
 objs=""
 pids=""

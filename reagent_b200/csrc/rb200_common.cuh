@@ -1,4 +1,4 @@
-// reagent_b200 -- common device/host helpers (sm_100a only).
+// reagent_b200 -- common device/host helpers (sm_90a only).
 //
 // Data layout conventions used by every kernel in this library
 //   * all batch tensors are dense row-major fp32, one transition per row;
@@ -17,6 +17,7 @@
 namespace rb200 {
 
 constexpr int kThreads = 256;          // every row-tile kernel uses 8 warps
+constexpr int kNumSMs = 132;           // H100 SXM: grid sizes that fill the GPU a whole number of times
 constexpr int kMaxLayers = RB200_MAX_LAYERS;
 
 // Device-side view of one MLP (passed by value as a kernel parameter).

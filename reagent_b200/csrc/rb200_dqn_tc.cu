@@ -1,72 +1,51 @@
-// reagent_b200 -- K2 on the 5th-generation tensor cores: the fused DQN TD-target / loss /
-// backward step (same contract as rb200_dqn.cu) with every matrix product issued as
-// tcgen05.mma (kind::tf32, 3xTF32 error compensation) and the accumulators in Tensor Memory.
+// reagent_b200 -- K2 on the Hopper tensor cores: the fused DQN TD-target / loss / backward step
+// (same contract as rb200_dqn.cu) with every matrix product issued as warpgroup MMAs (wgmma,
+// kind tf32, 3xTF32 error compensation) and the accumulators in registers.
 //
 // Formulation.  A CTA owns 32 batch rows and computes every layer TRANSPOSED:
 //     D_l^T [features x 32 rows]  =  W_l [features x K]  .  H_{l-1}^T [K x 32 rows]
-// so the WEIGHTS are the UMMA A operand (M = 128 output features per tile, always a full
+// so the WEIGHTS are the wgmma A operand (M = 64 output features per warpgroup, always a full
 // tensor-core tile however small the batch tile is) and the ACTIVATIONS are the B operand
-// (N = 32).  4096 rows therefore spread over 128 SMs instead of the 32 an M = 128-row tile
-// would use, and the accumulator of a layer is only 32 TMEM columns per 128 features.
+// (N = 32).  4096 rows therefore spread over 128 SMs instead of the 32 an M = 64-row tile
+// would use, and the accumulator of a 64-feature slice is only 32 registers per thread.
 //
 //   weights      pre-tiled once per update (by the Adam kernel, or dqn_tc_pack_kernel) into one
 //                fp32 image per (128-feature tile, 32-k chunk) -- [k/4][row][4 floats].  The TD
 //                kernel streams the images through a shared-memory ring with 1-D bulk copies
-//                (cp.async.bulk -> mbarrier complete_tx, producer warp; a stage = two chunk
-//                images); FOUR LOADER WARPS (one per TMEM lane quadrant; a thread owns one weight
-//                row) read "my row" with conflict-free 16-byte loads, split it into TF32 hi / lo
-//                in registers and store both into a ring of TENSOR MEMORY columns (tcgen05.st):
-//                the weights are the A operand of the MMAs FROM TENSOR MEMORY.  Measured on B200
-//                (profiles/r02_summary.md): with A in tensor memory an MMA costs exactly its
-//                math (N/2 cycles at M = 128, K = 8), with A in shared memory 39-48 cycles
-//                whatever N <= 64; every weight byte crosses shared memory once in and once out
-//                as raw fp32.  The step is bound by the latency of this producer -> loader ->
-//                MMA chain and of the layer hand-overs, not by any pipe (see DESIGN.md 3.1).
-//   activations  live in shared memory as hi/lo planes in the same canonical layout (rows =
-//                batch rows); the epilogue of layer l (tcgen05.ld -> bias -> activation -> split)
+//                (cp.async.bulk -> mbarrier complete_tx, one producer warp; a stage = two chunk
+//                images).  The two MMA warpgroups read their A fragments straight from the
+//                ring (conflict-free 4-byte loads), split them into TF32 hi / lo in registers
+//                and issue the MMAs with A FROM REGISTERS: every weight byte crosses shared
+//                memory once in and once out as raw fp32.
+//   activations  live in shared memory as hi/lo planes in the canonical K-major layout (rows =
+//                batch rows); the epilogue of layer l (registers -> bias -> activation -> split)
 //                writes them straight into the B operand of layer l+1 and, for the online
 //                pass on `state`, to the global buffers the weight-gradient kernel reads.
 //   backward     dZ_{l-1}^T = W_l^T . dZ_l^T uses pre-transposed weight images; the epilogue
 //                multiplies by act'(h_{l-1}) and stores dZ_{l-1}.
 //
-// Every thread of warps 0-7 owns one output feature (TMEM lane) in the epilogues, which makes
-// the bias a per-thread scalar and the operand stores bank-conflict free; warp 8 streams the
-// weights, warp 9 issues the MMAs (warp-uniform loops, one elected lane issues), warps 10-13
-// move the weights from shared to tensor memory.  Synchronisation is mbarrier-only inside the
-// step loop:
-//     full[s]   bulk copy landed in smem stage s     sfree[s]  the loaders have read stage s
-//     afull[t]  TMEM stage t holds a split chunk     adone[t]  its MMAs retired (tcgen05.commit)
-//     dready    a layer's accumulator is complete    opready   next B operand is in smem
+// Warps 0-7 (two warpgroups; warpgroup g owns features [64 g, 64 g + 64) of every 128-feature
+// tile) issue the MMAs and run the epilogues and the loss; warp 8 streams the weights.  Ring
+// synchronisation is mbarrier-only:
+//     full[s]   bulk copy landed in smem stage s     sfree[s]  the eight MMA warps have read it
+// and the hand-over of an activation operand between layers is a named barrier of warps 0-7.
 //
 // Reference semantics: reagent/training/dqn_trainer.py:157-239, dqn_trainer_base.py:33-77,
 // 216-241 (see rb200_dqn.cu for the line-by-line map; the loss code is the same).
-#include <stdlib.h>
 #include <string.h>
 
 #include "rb200_dqn_tc_layout.cuh"
-#include "rb200_umma.cuh"
+#include "rb200_wgmma.cuh"
 
 namespace rb200 {
 
 constexpr int kQR = 32;                                   // batch rows per CTA
-// A ring stage (shared memory and tensor memory alike) holds kQSub consecutive 32-k chunk images
-// of one feature tile (they are contiguous in the image: the k-quad sequence simply continues).
-// Every mbarrier wait costs 100-150 cycles even when it passes at once, and each agent of the
-// weight stream is a sequential loop with two waits per stage, so the stage is the unit that
-// amortises them: 64 k per stage halves the synchronisation cost per MMA.
-#ifndef RB200_QSUB
-#define RB200_QSUB 2
-#endif
-constexpr int kQSub = RB200_QSUB;
-#ifndef RB200_QSTAGES
-#define RB200_QSTAGES (6 / RB200_QSUB)
-#endif
-constexpr int kQStages = RB200_QSTAGES;                   // shared-memory ring depth (raw fp32 stages)
+// A ring stage holds kQSub consecutive 32-k chunk images of one feature tile (they are
+// contiguous in the image: the k-quad sequence simply continues).  Each mbarrier hand-over has
+// a fixed cost, so the stage is the unit that amortises it.
+constexpr int kQSub = 2;
+constexpr int kQStages = 3;                               // shared-memory ring depth
 constexpr int kQStageBytes = kQSub * (kQKC / 4) * kQFullLbo;  // kQSub chunk images
-constexpr int kAMaxStages = 7;                            // tensor-memory ring depth (split chunks), upper bound:
-                                                          // the plan uses every column the accumulators leave free
-constexpr int kASubCols = 2 * kQKC;                       // hi columns then lo columns of a chunk
-constexpr int kAStageCols = kQSub * kASubCols;
 // B operand (activations): per k quad 64 rows of 16 B -- rows 0-31 hold the hi parts of the 32
 // batch rows, rows 32-63 their lo parts -- plus 16 B of padding.  One N = 64 MMA against W_hi
 // then yields W_hi.X_hi in accumulator columns 0-31 and W_hi.X_lo in columns 32-63; a second
@@ -74,33 +53,12 @@ constexpr int kAStageCols = kQSub * kASubCols;
 // epilogue adds the two column groups.
 constexpr int kQLboB = 64 * 16 + 16;
 constexpr int kQLoOff = 32 * 4;                           // floats from a hi element to its lo
-constexpr int kQEpiThreads = 256;
-#ifndef RB200_QGROUPS
-#define RB200_QGROUPS 1
-#endif
-// Loader warps: kQLoaderGroups groups of four (one warp per TMEM lane quadrant).  Chunk i of the
-// weight stream belongs to group i % kQLoaderGroups, so consecutive chunks are converted by
-// different warps concurrently: one warp needs ~350 cycles per chunk (wait, 8 loads, ~100 ALU
-// instructions, two tensor-memory stores and their completion), the MMAs of a chunk 192.
-constexpr int kQLoaderGroups = RB200_QGROUPS;
-constexpr int kQLoaderWarps = 4 * kQLoaderGroups;
-// registers per thread: the register file is 16 K per SM sub-partition and the warps of a CTA
-// are dealt round-robin to the four sub-partitions
-constexpr int kQRegs = kQLoaderGroups >= 3 ? 80 : (kQLoaderGroups == 2 ? 96 : 128);
-constexpr int kQThreads = kQEpiThreads + 64 + 32 * kQLoaderWarps;  // + producer + MMA + loaders
-constexpr int kQMaxTiles = 4;                             // accumulators: 4 feature tiles x 64 columns
-constexpr int kQAccCols = kQMaxTiles * 64;
-constexpr int kQTmemCols = 512;                           // accumulators + the weight ring
-static_assert(kQAccCols + 2 * kAStageCols <= kQTmemCols, "tensor memory budget");
-static_assert(((10 + kQLoaderWarps + 3) / 4) * 32 * kQRegs <= 16384, "register file budget per sub-partition");
-static_assert(kQKC == 32, "loader warps move 32-k chunks");
-static_assert(kQStages % kQLoaderGroups == 0, "a shared-memory ring stage belongs to one loader group");
+constexpr int kQEpiThreads = 256;                         // the two MMA / epilogue warpgroups
+constexpr int kQThreads = kQEpiThreads + 32;              // + the producer warp
+constexpr int kQMaxTiles = 4;                             // widest layer: 4 x 128 features
 constexpr int kQMaxSteps = 4 * kMaxLayers;
-constexpr int kQMaxSmem = 232448;
-#ifndef RB200_TC_TIMELINE
-#define RB200_TC_TIMELINE 0  // 1: build the clock64 timeline / MMA-skipping hooks (profiling only)
-#endif
-constexpr bool kTimeline = RB200_TC_TIMELINE != 0;                         // 227 KB opt-in limit of sm_100
+constexpr int kQMaxSmem = 232448;                         // 227 KB opt-in limit of sm_90
+static_assert(kQKC == 32, "a chunk is four K = 8 MMA steps");
 
 enum { kStepHidden = 0, kStepLast = 1, kStepBwd = 2 };
 
@@ -117,11 +75,7 @@ struct QDev {
   int nsteps, last_fwd_step;
   int buf_off[3];  // operand buffers (bytes from the smem base); [2] holds dZ of the last layer
   int q_off, ldq, lin_off, bar_off;
-  int acc_cols, a_stages;  // tensor memory: accumulator columns, then a_stages weight stages
   int need_zero;    // some layer width is not a multiple of 8: clear the operand buffers first
-  int dbg_mode;     // profiling only (bits): 1 skip the N=32 MMAs, 2 skip the N=64 MMAs, 4 no ring reads,
-                    // 8 no bulk-copy traffic, 16 no tensor-memory stores, 32 no epilogue stores
-  long long* dbg;  // optional timeline of block 0: [step][8] clock64 stamps (profiling builds)
   QStep steps[kQMaxSteps];
 };
 
@@ -190,75 +144,7 @@ __global__ void __launch_bounds__(256) dqn_tc_pack_kernel(const PackDev p) {
 __device__ __noinline__ float act_fwd_slow(float x, int act) { return act_fwd(x, act); }
 __device__ __noinline__ float act_bwd_slow(float y, int act) { return act_bwd_from_out(y, act); }
 
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&v)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];\n"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]),
-        "=r"(v[7]), "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]),
-        "=r"(v[14]), "=r"(v[15])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;\n" ::: "memory");
-}
-
-// two 16-column groups in flight, one wait
-__device__ __forceinline__ void tmem_ld16x2(uint32_t t0, uint32_t t1, uint32_t (&v)[16],
-                                            uint32_t (&w)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];\n"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]),
-        "=r"(v[7]), "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]),
-        "=r"(v[14]), "=r"(v[15])
-      : "r"(t0));
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];\n"
-      : "=r"(w[0]), "=r"(w[1]), "=r"(w[2]), "=r"(w[3]), "=r"(w[4]), "=r"(w[5]), "=r"(w[6]),
-        "=r"(w[7]), "=r"(w[8]), "=r"(w[9]), "=r"(w[10]), "=r"(w[11]), "=r"(w[12]), "=r"(w[13]),
-        "=r"(w[14]), "=r"(w[15])
-      : "r"(t1));
-  asm volatile("tcgen05.wait::ld.sync.aligned;\n" ::: "memory");
-}
-
-// 32 consecutive TMEM columns of this thread's lane <- 32 registers
-__device__ __forceinline__ void tmem_st32(uint32_t taddr, const float (&v)[32]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,"
-      "%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32};\n" ::"r"(taddr),
-      "f"(v[0]), "f"(v[1]), "f"(v[2]), "f"(v[3]), "f"(v[4]), "f"(v[5]), "f"(v[6]), "f"(v[7]),
-      "f"(v[8]), "f"(v[9]), "f"(v[10]), "f"(v[11]), "f"(v[12]), "f"(v[13]), "f"(v[14]), "f"(v[15]),
-      "f"(v[16]), "f"(v[17]), "f"(v[18]), "f"(v[19]), "f"(v[20]), "f"(v[21]), "f"(v[22]), "f"(v[23]),
-      "f"(v[24]), "f"(v[25]), "f"(v[26]), "f"(v[27]), "f"(v[28]), "f"(v[29]), "f"(v[30]), "f"(v[31])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st16(uint32_t taddr, const float (&v)[32]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-      "{%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16};\n" ::"r"(taddr),
-      "f"(v[0]), "f"(v[1]), "f"(v[2]), "f"(v[3]), "f"(v[4]), "f"(v[5]), "f"(v[6]), "f"(v[7]),
-      "f"(v[8]), "f"(v[9]), "f"(v[10]), "f"(v[11]), "f"(v[12]), "f"(v[13]), "f"(v[14]), "f"(v[15])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_wait_st() {
-  asm volatile("tcgen05.wait::st.sync.aligned;\n" ::: "memory");
-}
-// D[tmem] (+)= A[tmem: 128 lanes x 8 tf32 columns] . B[smem descriptor]
-__device__ __forceinline__ void umma_tf32_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t db,
-                                             uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], [%1], %2, %3, p;\n\t"
-      "}\n" ::"r"(tmem_d), "r"(tmem_a), "l"(db), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-
-// Register cap: threads x registers must fit the 64 K register file (kQRegs; the kernel needs
-// 76-107 depending on the cap, no spills).
-__global__ void __maxnreg__(kQRegs)
+__global__ void __launch_bounds__(kQThreads, 1)
 dqn_td_tc_kernel(const Mlp q, const Mlp qt, const QDev p) {
   extern __shared__ __align__(128) unsigned char smem_raw[];
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
@@ -267,8 +153,6 @@ dqn_td_tc_kernel(const Mlp q, const Mlp qt, const QDev p) {
   const int row0 = blockIdx.x * kQR;
   const int L = q.n_layers;
   const int A = q.dims[L];
-  auto gtime = []() { unsigned long long t; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t)); return (long long)t; };
-  if (kTimeline && p.dbg && tid == 0) p.dbg[kQMaxSteps * 8 + blockIdx.x * 4 + 0] = gtime();
 
   // operand padding (k up to the next multiple of 8) must be finite.  With every layer width a
   // multiple of 8 there is no padding: all operand quads, all 64 B-operand rows (rows past the
@@ -277,11 +161,10 @@ dqn_td_tc_kernel(const Mlp q, const Mlp qt, const QDev p) {
   if (p.need_zero) {
     unsigned nbytes;
     asm("mov.u32 %0, %%dynamic_smem_size;" : "=r"(nbytes));
-    // (the weight ring is fully overwritten by the bulk copies; rows a partial tile over-reads
-    // only feed accumulator lanes nobody looks at)
+    // (the weight ring is fully overwritten by the bulk copies; fragment rows past a partial
+    // tile are read as zeros)
     for (unsigned i = (unsigned)p.buf_off[0] + tid * 16u; i + 15u < nbytes; i += kQThreads * 16u)
       *reinterpret_cast<float4*>(smem_raw + i) = make_float4(0.f, 0.f, 0.f, 0.f);
-    fence_proxy_async_smem();
   }
   __syncthreads();
 
@@ -292,38 +175,20 @@ dqn_td_tc_kernel(const Mlp q, const Mlp qt, const QDev p) {
   float* scal_s = mask_s + kQR * A;                               // [kQR][4] reward, not_terminal, discount src
   uint64_t* full = reinterpret_cast<uint64_t*>(smem_raw + p.bar_off);
   uint64_t* sfree = full + kQStages;
-  uint64_t* afull = sfree + kQStages;
-  uint64_t* adone = afull + kAMaxStages;
-  uint64_t* dready = adone + kAMaxStages;  // one per accumulator tile (see the epilogue)
-  uint64_t* opready = dready + kQMaxTiles;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(opready + 1);
   const int ldq = p.ldq;
 
   if (tid == 0) {
-    // a chunk is handled by the four warps of ONE loader group
-    for (int s = 0; s < kQStages; ++s) { mbar_init(full + s, 1); mbar_init(sfree + s, 4); }
-    for (int t = 0; t < kAMaxStages; ++t) { mbar_init(afull + t, 4); mbar_init(adone + t, 1); }
-    for (int t = 0; t < kQMaxTiles; ++t) mbar_init(dready + t, 1);
-    mbar_init(opready, kQEpiThreads / 32);  // one arrival per epilogue warp
+    for (int s = 0; s < kQStages; ++s) { mbar_init(full + s, 1); mbar_init(sfree + s, kQEpiThreads / 32); }
     asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory");
   }
-  if (warp == 0) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;\n" ::"r"(
-                     smem_u32(tmem_slot)), "n"(kQTmemCols));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;\n" ::);
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = *tmem_slot;
-  if (kTimeline && p.dbg && tid == 0) p.dbg[kQMaxSteps * 8 + blockIdx.x * 4 + 1] = gtime();
 
   // warp-uniform role index (the shuffle lets the compiler keep the role loops in uniform registers)
   const int role = __shfl_sync(0xffffffffu, warp, 0);
   if (role == kQEpiThreads / 32) {
     // =====================  weight producer warp (bulk copies)  =====================
     // Free-running over the static chunk list; the `sfree` barriers of the ring are the only
-    // back-pressure, so up to kQStages chunks are in flight ahead of the loader warps.
+    // back-pressure, so up to kQStages stages are in flight ahead of the MMA warps.
     const bool leader = elect_one();
     int stage = 0;
     uint32_t par = 1;  // parity of the PREVIOUS use of `stage` (first lap: passes immediately)
@@ -341,168 +206,21 @@ dqn_td_tc_kernel(const Mlp q, const Mlp qt, const QDev p) {
         for (int c = 0; c < kch; c += kQSub) {
           const int nsub = kch - c < kQSub ? kch - c : kQSub;
           const uint32_t bytes = (uint32_t)(nsub - 1) * full_bytes + ((c + nsub == kch) ? last_bytes : full_bytes);
-          const uint32_t cbytes = (kTimeline && (p.dbg_mode & 8)) ? 16u : bytes;  // profiling: no copy traffic
           mbar_wait(sfree + stage, par);
           if (leader) {
-            mbar_expect_tx(full + stage, cbytes);
-            bulk_g2s(ring + stage * kQStageBytes, src, cbytes, full + stage);
+            mbar_expect_tx(full + stage, bytes);
+            bulk_g2s(ring + stage * kQStageBytes, src, bytes, full + stage);
           }
           src += bytes;
           if (++stage == kQStages) { stage = 0; par ^= 1u; }
         }
       }
     }
-  } else if (role == kQEpiThreads / 32 + 1) {
-    // =====================  MMA issuer warp  =====================
-    // A operand: the split weights in tensor memory (128 lanes = features, 8 columns per
-    // k step; hi columns then lo columns of the chunk).  B operand: the activations in
-    // shared memory (descriptor).
-    const bool leader = elect_one();
-    const uint32_t idesc64 = umma_idesc_tf32(128, 64), idesc32 = umma_idesc_tf32(128, 32);
-    const uint64_t desc_hi = (uint64_t)((128u >> 4) | (1u << 14)) << 32;  // SBO = 128 B, version 1
-    int ts = 0;
-    uint32_t tpar = 0;
-    for (int s = 0; s < p.nsteps; ++s) {
-      const QStep st = p.steps[s];
-      const int mt = ceil_div(st.N, 128), kch = ceil_div(st.K, kQKC);
-      mbar_wait(opready, (uint32_t)s & 1u);
-      tc_fence_after();
-      long long wafull = 0, tfence = 0, tissue = 0, tcommit = 0;
-      if (kTimeline && p.dbg && blockIdx.x == 0 && leader) p.dbg[s * 8 + 0] = clock64();
-      const uint32_t b0 = ((smem_u32(smem_raw + p.buf_off[st.in_buf]) >> 4) & 0x3fffu) |
-                          ((uint32_t)(kQLboB >> 4) << 16);
-      for (int t = 0; t < mt; ++t) {
-        const uint32_t d = tmem + (uint32_t)(t * 64);
-        uint32_t bdesc = b0;  // advances by two k quads per MMA k step
-        for (int c = 0; c < kch; c += kQSub) {
-          const int nsub = kch - c < kQSub ? kch - c : kQSub;
-          const long long w0 = (kTimeline && p.dbg) ? clock64() : 0;
-          mbar_wait(afull + ts, tpar);
-          const long long w1 = (kTimeline && p.dbg) ? clock64() : 0;
-          if (kTimeline && p.dbg) wafull += w1 - w0;
-          tc_fence_after();
-          const long long w2 = (kTimeline && p.dbg) ? clock64() : 0;
-          if (kTimeline && p.dbg) tfence += w2 - w1;
-          if (leader) {
-            uint32_t bd = bdesc;
-            for (int j = 0; j < nsub; ++j) {
-              const int kl = st.K - kQKC * (c + j);
-              const int ksteps = round_up8(kl < kQKC ? kl : kQKC) / 8;
-              uint32_t a_hi = tmem + (uint32_t)(p.acc_cols + ts * kAStageCols + j * kASubCols);
-              for (int ks = 0; ks < ksteps; ++ks) {
-                if (!kTimeline || !(p.dbg_mode & 2))
-                  umma_tf32_ts(d, a_hi, desc_hi | bd, idesc64, (c + j > 0 || ks > 0) ? 1u : 0u);
-                if (!kTimeline || !(p.dbg_mode & 1))
-                  umma_tf32_ts(d, a_hi + kQKC, desc_hi | bd, idesc32, 1u);
-                a_hi += 8;
-                bd += (2u * kQLboB) >> 4;
-              }
-            }
-            const long long w3 = (kTimeline && p.dbg) ? clock64() : 0;
-            umma_commit(adone + ts);  // this TMEM stage may be refilled once the MMAs retired
-            if (kTimeline && p.dbg) { const long long w4 = clock64(); tissue += w3 - w2; tcommit += w4 - w3; }
-          }
-          bdesc += (uint32_t)nsub * (uint32_t)(kQKC / 4) * (kQLboB >> 4);
-          if (++ts == p.a_stages) { ts = 0; tpar ^= 1u; }
-        }
-        // one accumulator tile complete: its epilogue runs while the next tile's MMAs issue
-        if (leader) umma_commit(dready + t);
-      }
-      if (kTimeline && p.dbg && blockIdx.x == 0 && leader) {
-        p.dbg[s * 8 + 1] = clock64();
-        p.dbg[s * 8 + 2] = wafull;
-        long long* fine = p.dbg + kQMaxSteps * 8 + 4 * 4096 + s * 8;
-        fine[0] = tfence; fine[1] = tissue; fine[2] = tcommit;
-      }
-      __syncwarp();
-    }
-  } else if (role >= kQEpiThreads / 32 + 2) {
-    // =====================  loader warps: shared memory -> TF32 split -> tensor memory  ======
-    // warp (10 + j) may touch TMEM lanes [32*((10+j)%4), +32): the four loader warps cover the
-    // four lane quadrants; lane i of a warp owns weight row 32*quadrant + i of the tile.
-    const int quadrant = warp & 3;
-    const int group = (warp - (kQEpiThreads / 32 + 2)) >> 2;
-    int turn = 0;  // group whose chunk comes next; every warp walks the whole chunk sequence
-    const int r = quadrant * 32 + lane;
-    int ss = 0, ts = 0;
-    uint32_t spar = 0, tpar = 1;  // TMEM stages start free (parity of the previous use)
-    for (int s = 0; s < p.nsteps; ++s) {
-      const QStep st = p.steps[s];
-      const int mt = ceil_div(st.N, 128), kch = ceil_div(st.K, kQKC);
-      long long lwfull = 0, lwdone = 0, lsplit = 0, lstore = 0;
-      for (int t = 0; t < mt; ++t) {
-        const int rows = st.N - 128 * t;
-        const int rows8 = round_up8(rows < 128 ? rows : 128);
-        const uint32_t lbo = (uint32_t)(rows8 * 16 + 16);
-        for (int c = 0; c < kch; c += kQSub) {
-          const int nsub = kch - c < kQSub ? kch - c : kQSub;
-          const bool mine = turn == group;
-          if (++turn == kQLoaderGroups) turn = 0;
-          if (!mine) {
-            if (++ss == kQStages) { ss = 0; spar ^= 1u; }
-            if (++ts == p.a_stages) { ts = 0; tpar ^= 1u; }
-            continue;
-          }
-          const long long l0 = (kTimeline && p.dbg) ? clock64() : 0;
-          mbar_wait(full + ss, spar);
-          const long long l0b = (kTimeline && p.dbg) ? clock64() : 0;
-          if (kTimeline && p.dbg) lwfull += l0b - l0;
-          const uint32_t ta = tmem + ((uint32_t)(quadrant * 32) << 16) +
-                              (uint32_t)(p.acc_cols + ts * kAStageCols);
-#pragma unroll 1
-          for (int j = 0; j < nsub; ++j) {
-            const int kl = st.K - kQKC * (c + j);
-            const int nq = round_up8(kl < kQKC ? kl : kQKC) / 4;
-            float hi[32], lo[32];
-            const unsigned char* src = ring + ss * kQStageBytes + (uint32_t)j * (kQKC / 4) * lbo + r * 16;
-#pragma unroll
-            for (int qd = 0; qd < kQKC / 4; ++qd) {
-              float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-              if (kTimeline && (p.dbg_mode & 4)) v = make_float4(1.f, 2.f, 3.f, 4.f);  // profiling: no ring reads
-              else if (qd < nq && r < rows8) v = *reinterpret_cast<const float4*>(src + qd * lbo);
-              float4 h, l;
-              split4(v, h, l);
-              hi[4 * qd + 0] = h.x; hi[4 * qd + 1] = h.y; hi[4 * qd + 2] = h.z; hi[4 * qd + 3] = h.w;
-              lo[4 * qd + 0] = l.x; lo[4 * qd + 1] = l.y; lo[4 * qd + 2] = l.z; lo[4 * qd + 3] = l.w;
-            }
-            if (j == nsub - 1) {
-              // the stage's values are in registers: the shared-memory stage can be refilled
-              __syncwarp();
-              if (lane == 0) mbar_arrive(sfree + ss);
-            }
-            if (j == 0) {
-              const long long l1 = (kTimeline && p.dbg) ? clock64() : 0;
-              if (kTimeline && p.dbg) lsplit += l1 - l0b;
-              mbar_wait(adone + ts, tpar);  // the MMAs that read this TMEM stage have retired
-              if (kTimeline && p.dbg) lwdone += clock64() - l1;
-              tc_fence_after();
-            }
-            if (!kTimeline || !(p.dbg_mode & 16)) {  // (profiling: no tensor-memory stores)
-              tmem_st32(ta + j * kASubCols, hi);
-              tmem_st32(ta + j * kASubCols + kQKC, lo);
-            }
-          }
-          const long long l2 = (kTimeline && p.dbg) ? clock64() : 0;
-          tmem_wait_st();
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(afull + ts);
-          if (kTimeline && p.dbg) lstore += clock64() - l2;
-          if (++ss == kQStages) { ss = 0; spar ^= 1u; }
-          if (++ts == p.a_stages) { ts = 0; tpar ^= 1u; }
-        }
-      }
-      if (kTimeline && p.dbg && blockIdx.x == 0 && quadrant == 0 && group == 0 && lane == 0) {
-        p.dbg[s * 8 + 6] = lwfull;
-        p.dbg[s * 8 + 7] = lwdone;
-        long long* fine = p.dbg + kQMaxSteps * 8 + 4 * 4096 + s * 8;
-        fine[3] = lsplit; fine[4] = lstore;
-      }
-    }
   } else {
-    // =====================  operand producers / epilogue warps  =====================
-    const int quad = warp & 3, grp = warp >> 2;
-    uint32_t dphase = 0;       // bit t: parity of the next phase of dready[t]
+    // =====================  MMA / epilogue warpgroups  =====================
+    const int wg = warp >> 2, w4 = warp & 3, g = lane >> 2, tq = lane & 3;
+    int ss = 0;
+    uint32_t spar = 0;  // ring position (every MMA warp walks the whole chunk sequence)
 
     // The input tile of a pass: global -> registers (x_fetch, issued early so that the load
     // latency hides behind the previous layer) -> hi/lo split -> B operand (x_store).
@@ -573,101 +291,163 @@ dqn_td_tc_kernel(const Mlp q, const Mlp qt, const QDev p) {
         scal_s[tid * 4 + 2] = (in && a.discount_mode == RB200_DISCOUNT_POW) ? a.discount_src[row] : 0.f;
       }
     };
-    auto epilogue = [&](const QStep& st) {
+    // One step (layer): per 128-feature tile, warpgroup wg accumulates features
+    // [128 t + 64 wg, +64) x 64 columns (32 batch rows hi, then lo) over the weight stream, then
+    // its epilogue writes them out.  The thread holds features n and n + 8 (n = 128 t + 64 wg +
+    // 16 w4 + g) of batch rows 8 i + 2 tq + e (i < 4, e < 2), in acc[4 i + 2 h + e] (+ the lo
+    // column group acc[4 (i + 4) + 2 h + e]).
+    auto step_tiles = [&](const QStep& st) {
       const Mlp& net = st.net ? qt : q;
       const int l = st.layer, N = st.N;
-      const int mt = ceil_div(N, 128);
+      const int mt = ceil_div(N, 128), kch = ceil_div(st.K, kQKC);
       float* obase = reinterpret_cast<float*>(smem_raw + p.buf_off[st.out_buf]);
+      const uint32_t bbase = smem_u32(smem_raw + p.buf_off[st.in_buf]);
       for (int t = 0; t < mt; ++t) {
-        // One barrier per tile: the MMA warp runs ahead through the tiles of a step without
-        // waiting for the epilogues, so a shared barrier could complete two phases before a
-        // slow thread looks at it (and parity waits cannot tell "two ahead" from "not yet").
-        // Per tile there is at most one completion per step, and steps are serialised by
-        // `opready`.
-        mbar_wait(dready + t, (dphase >> t) & 1u);
-        dphase ^= 1u << t;
-        tc_fence_after();
-        const int h16 = grp * 16;
-        const int n = t * 128 + quad * 32 + lane;
-        const bool valid = n < N;
-        uint32_t v[16], w[16];
-        const uint32_t taddr = tmem + ((uint32_t)(quad * 32) << 16) + (uint32_t)(t * 64 + h16);
-        tmem_ld16x2(taddr, taddr + 32, v, w);
-        float x[16];
+        const int rows = N - 128 * t;
+        const int rows8 = round_up8(rows < 128 ? rows : 128);
+        const uint32_t lbo = (uint32_t)(rows8 * 16 + 16);
+        const bool live = 64 * wg < rows;  // warpgroup-uniform: this half of the tile has features
+        const int m0 = 64 * wg + 16 * w4 + g;
+        const bool ok0 = live && m0 < rows8, ok1 = live && m0 + 8 < rows8;
+        float acc[32];
 #pragma unroll
-        for (int j = 0; j < 16; ++j) x[j] = __uint_as_float(v[j]) + __uint_as_float(w[j]);
-        float* ob = obase + (n >> 2) * (kQLboB / 4) + h16 * 4 + (n & 3);
-        bool to_operand, to_global;
-        float* gdst = nullptr;
-        if (st.kind == kStepBwd) {
-          // act'(h_{l-1}) from the forward operand still resident in shared memory (h = hi + lo
-          // exactly); dZ_{l-1} then replaces it in place as the next B operand
-          const int hact = q.act[l - 1];
-          // st.save: the shared-memory copy of h_{l-1} was overwritten by a later forward layer
-          // (networks with >= 3 hidden layers ping-pong over the same two buffers); read the
-          // copy saved for the weight-gradient kernel instead
-          float hv[16];
-          if (st.save) {
-            const float* hs = p.ws.hidden[l - 1];
+        for (int i = 0; i < 32; ++i) acc[i] = 0.f;
+        for (int c = 0; c < kch; c += kQSub) {
+          const int nsub = kch - c < kQSub ? kch - c : kQSub;
+          mbar_wait(full + ss, spar);
+          // A fragments of the stage: raw fp32 from the ring -> TF32 hi / lo in registers
+          uint32_t ah[kQSub * 4][4], al[kQSub * 4][4];
+          int ksteps[kQSub];
 #pragma unroll
-            for (int j = 0; j < 16; ++j) {
-              const int row = row0 + h16 + j;
-              hv[j] = (valid && row < B) ? hs[(size_t)row * N + n] : 0.f;
+          for (int j = 0; j < kQSub; ++j) {
+            const int kl = st.K - kQKC * (c + j);
+            ksteps[j] = j < nsub ? round_up8(kl < kQKC ? kl : kQKC) / 8 : 0;
+            const unsigned char* src = ring + ss * kQStageBytes + (uint32_t)j * (kQKC / 4) * lbo + tq * 4;
+#pragma unroll
+            for (int ks = 0; ks < 4; ++ks) {
+              float v[4] = {0.f, 0.f, 0.f, 0.f};
+              if (ks < ksteps[j]) {
+                const unsigned char* s0 = src + (uint32_t)(2 * ks) * lbo;  // k = 8 ks + tq
+                const unsigned char* s1 = s0 + lbo;                        // k = 8 ks + 4 + tq
+                if (ok0) { v[0] = *reinterpret_cast<const float*>(s0 + m0 * 16); v[2] = *reinterpret_cast<const float*>(s1 + m0 * 16); }
+                if (ok1) { v[1] = *reinterpret_cast<const float*>(s0 + (m0 + 8) * 16); v[3] = *reinterpret_cast<const float*>(s1 + (m0 + 8) * 16); }
+              }
+#pragma unroll
+              for (int e = 0; e < 4; ++e) {
+                float h, lo_;
+                split1(v[e], h, lo_);
+                ah[4 * j + ks][e] = __float_as_uint(h);
+                al[4 * j + ks][e] = __float_as_uint(lo_);
+              }
             }
+          }
+          // the stage's values are in registers: the ring stage can be refilled
+          __syncwarp();
+          if (lane == 0) mbar_arrive(sfree + ss);
+          if (++ss == kQStages) { ss = 0; spar ^= 1u; }
+          // (a warpgroup without features in this tile multiplies zeros: issuing unconditionally
+          // keeps the MMAs out of divergent code, which the compiler would serialise)
+          wgmma_fence();
+#pragma unroll
+          for (int j = 0; j < kQSub; ++j) {
+#pragma unroll
+            for (int ks = 0; ks < 4; ++ks) {
+              if (ks < ksteps[j]) {
+                const uint32_t kq = (uint32_t)(2 * (4 * (c + j) + ks));  // first k quad of this K = 8 step
+                const uint64_t bd = wgmma_desc(bbase + kq * kQLboB, kQLboB, 128);
+                wgmma_rs_n64(acc, ah[4 * j + ks], bd, 1u);  // W_hi . [X_hi | X_lo]
+                wgmma_rs_n32(acc, al[4 * j + ks], bd, 1u);  // W_lo . X_hi
+              }
+            }
+          }
+          wgmma_commit();
+          wgmma_wait<0>();
+        }
+        if (!live) continue;
+
+        // ---- epilogue of this tile ----
+#pragma unroll
+        for (int hh = 0; hh < 2; ++hh) {
+          const int n = 128 * t + m0 + 8 * hh;
+          const bool valid = n < N;
+          float x[8];
+#pragma unroll
+          for (int i = 0; i < 4; ++i)
+#pragma unroll
+            for (int e = 0; e < 2; ++e) x[2 * i + e] = acc[4 * i + 2 * hh + e] + acc[4 * (i + 4) + 2 * hh + e];
+          auto rowof = [&](int k) { return 8 * (k >> 1) + 2 * tq + (k & 1); };
+          float* ob = obase + (n >> 2) * (kQLboB / 4) + (n & 3);  // + 4 r for batch row r
+          bool to_operand, to_global;
+          float* gdst = nullptr;
+          if (st.kind == kStepBwd) {
+            // act'(h_{l-1}) from the forward operand still resident in shared memory (h = hi + lo
+            // exactly); dZ_{l-1} then replaces it in place as the next B operand
+            const int hact = q.act[l - 1];
+            // st.save: the shared-memory copy of h_{l-1} was overwritten by a later forward layer
+            // (networks with >= 3 hidden layers ping-pong over the same two buffers); read the
+            // copy saved for the weight-gradient kernel instead
+            float hv[8];
+            if (st.save) {
+              const float* hs = p.ws.hidden[l - 1];
+#pragma unroll
+              for (int k = 0; k < 8; ++k) {
+                const int row = row0 + rowof(k);
+                hv[k] = (valid && row < B) ? hs[(size_t)row * N + n] : 0.f;
+              }
+            } else {
+#pragma unroll
+              for (int k = 0; k < 8; ++k) hv[k] = valid ? ob[rowof(k) * 4] + ob[rowof(k) * 4 + kQLoOff] : 0.f;
+            }
+            if (hact == RB200_ACT_RELU) {
+#pragma unroll
+              for (int k = 0; k < 8; ++k) x[k] = hv[k] > 0.f ? x[k] : 0.f;
+            } else if (hact != RB200_ACT_LINEAR) {
+#pragma unroll
+              for (int k = 0; k < 8; ++k) x[k] = valid ? x[k] * act_bwd_slow(hv[k], hact) : 0.f;
+            }
+            to_operand = l - 1 >= 1;
+            to_global = true;
+            gdst = p.ws.dz[l - 1];
           } else {
+            const float bias = valid ? __ldg(net.params + net.b_off[l] + n) : 0.f;
+            const int act = net.act[l];
+            if (act == RB200_ACT_RELU) {
 #pragma unroll
-            for (int j = 0; j < 16; ++j) hv[j] = valid ? ob[j * 4] + ob[j * 4 + kQLoOff] : 0.f;
+              for (int k = 0; k < 8; ++k) x[k] = fmaxf(x[k] + bias, 0.f);
+            } else if (act == RB200_ACT_LINEAR) {
+#pragma unroll
+              for (int k = 0; k < 8; ++k) x[k] += bias;
+            } else {
+#pragma unroll
+              for (int k = 0; k < 8; ++k) x[k] = act_fwd_slow(x[k] + bias, act);
+            }
+            to_operand = st.kind != kStepLast;
+            to_global = st.save != 0 && st.kind != kStepLast;
+            gdst = to_global ? p.ws.hidden[l] : nullptr;
           }
-          if (hact == RB200_ACT_RELU) {
+          if (!valid) continue;
+          if (st.kind == kStepLast) {
+            float* qd = qarr + st.qdst * kQR * ldq + n;
 #pragma unroll
-            for (int j = 0; j < 16; ++j) x[j] = hv[j] > 0.f ? x[j] : 0.f;
-          } else if (hact != RB200_ACT_LINEAR) {
-#pragma unroll
-            for (int j = 0; j < 16; ++j) x[j] = valid ? x[j] * act_bwd_slow(hv[j], hact) : 0.f;
+            for (int k = 0; k < 8; ++k) qd[rowof(k) * ldq] = x[k];
+            continue;
           }
-          to_operand = l - 1 >= 1;
-          to_global = true;
-          gdst = p.ws.dz[l - 1];
-        } else {
-          const float bias = valid ? __ldg(net.params + net.b_off[l] + n) : 0.f;
-          const int act = net.act[l];
-          if (act == RB200_ACT_RELU) {
+          if (to_operand) {
 #pragma unroll
-            for (int j = 0; j < 16; ++j) x[j] = fmaxf(x[j] + bias, 0.f);
-          } else if (act == RB200_ACT_LINEAR) {
-#pragma unroll
-            for (int j = 0; j < 16; ++j) x[j] += bias;
-          } else {
-#pragma unroll
-            for (int j = 0; j < 16; ++j) x[j] = act_fwd_slow(x[j] + bias, act);
+            for (int k = 0; k < 8; ++k) {
+              float h, lo_;
+              split1(row0 + rowof(k) < B ? x[k] : 0.f, h, lo_);
+              ob[rowof(k) * 4] = h;
+              ob[rowof(k) * 4 + kQLoOff] = lo_;
+            }
           }
-          to_operand = st.kind != kStepLast;
-          to_global = st.save != 0 && st.kind != kStepLast;
-          gdst = to_global ? p.ws.hidden[l] : nullptr;
-        }
-        if (!valid) continue;
-        if (kTimeline && (p.dbg_mode & 32)) { to_operand = false; to_global = false; }  // profiling: no epilogue stores
-        if (st.kind == kStepLast) {
-          float* qd = qarr + (st.qdst * kQR + h16) * ldq + n;
+          if (to_global) {
 #pragma unroll
-          for (int j = 0; j < 16; ++j) qd[j * ldq] = x[j];
-          continue;
-        }
-        const int nrow = B - (row0 + h16);  // rows of this half that exist
-        if (to_operand) {
-#pragma unroll
-          for (int j = 0; j < 16; ++j) {
-            float h, lo_;
-            split1(j < nrow ? x[j] : 0.f, h, lo_);
-            ob[j * 4] = h;
-            ob[j * 4 + kQLoOff] = lo_;
+            for (int k = 0; k < 8; ++k) {
+              const int row = row0 + rowof(k);
+              if (row < B) gdst[(size_t)row * N + n] = x[k];
+            }
           }
-        }
-        if (to_global) {
-          float* gd = gdst + (size_t)(row0 + h16) * N + n;
-#pragma unroll
-          for (int j = 0; j < 16; ++j)
-            if (j < nrow) gd[(size_t)j * N] = x[j];
         }
       }
     };
@@ -749,38 +529,34 @@ dqn_td_tc_kernel(const Mlp q, const Mlp qt, const QDev p) {
       if (lane == 0) scal_s[kQR * 4 + warp] = ws;  // per-warp loss sums, combined by thread 0 at the end
     };
 
+
     auto x_src = [&](int lx) { return lx == 1 ? a.state : a.next_state; };
-    if (p.steps[0].load_x) { x_fetch(x_src(p.steps[0].load_x)); x_store(x_src(p.steps[0].load_x)); }
-    // hand-over: every thread makes its operand stores visible to the async proxy, the warp
-    // converges, ONE lane arrives (8 arrivals per hand-over instead of 256 serialised ones)
-    auto operand_ready = [&]() {
+    // hand-over between the MMA warpgroups: every thread makes its operand stores visible to
+    // the async proxy (the wgmma operand reads), then warps 0-7 meet at a named barrier
+    auto handover = [&]() {
       fence_proxy_async_smem();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(opready);
+      asm volatile("bar.sync 1, %0;\n" ::"n"(kQEpiThreads) : "memory");
     };
-    operand_ready();
+    if (p.steps[0].load_x) { x_fetch(x_src(p.steps[0].load_x)); x_store(x_src(p.steps[0].load_x)); }
     load_loss_inputs();
+    handover();
     for (int s = 0; s < p.nsteps; ++s) {
       const QStep st = p.steps[s];
       const int lx = (s + 1 < p.nsteps) ? p.steps[s + 1].load_x : 0;
       if (lx) x_fetch(x_src(lx));  // in flight during this step's MMAs and epilogue
-      if (kTimeline && p.dbg && blockIdx.x == 0 && tid == 0) p.dbg[s * 8 + 3] = clock64();
-      epilogue(st);
-      tc_fence_before();
-      if (kTimeline && p.dbg && blockIdx.x == 0 && tid == 0) p.dbg[s * 8 + 4] = clock64();
+      step_tiles(st);
+      handover();  // this step's operand complete, and every MMA that read its input retired
       if (s == p.last_fwd_step) {
-        asm volatile("bar.sync 1, %0;\n" ::"n"(kQEpiThreads) : "memory");
         loss_stage();
+        handover();
       }
-      if (s + 1 < p.nsteps) {
-        if (lx) x_store(x_src(lx));
-        operand_ready();
-        if (kTimeline && p.dbg && blockIdx.x == 0 && tid == 0) p.dbg[s * 8 + 5] = clock64();
+      if (lx) {
+        x_store(x_src(lx));
+        handover();
       }
     }
 
     // publish the loss (off the critical path of the step loop): last tile reduces
-    asm volatile("bar.sync 1, %0;\n" ::"n"(kQEpiThreads) : "memory");
     if (tid == 0) {
       float loss_partial = 0.f;
       for (int w = 0; w < kQEpiThreads / 32; ++w) loss_partial += scal_s[kQR * 4 + w];
@@ -795,14 +571,6 @@ dqn_td_tc_kernel(const Mlp q, const Mlp qt, const QDev p) {
         *a.tile_counter = 0u;
       }
     }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (kTimeline && p.dbg && tid == 0) p.dbg[kQMaxSteps * 8 + blockIdx.x * 4 + 2] = gtime();
-  if (warp == 0) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;\n" ::"r"(tmem),
-                 "n"(kQTmemCols));
   }
 }
 
@@ -902,18 +670,6 @@ static QPlan make_plan(const rb200_mlp_t* qn, const rb200_mlp_t* qtn, int double
     }
   }
   pl.dev.nsteps = ns;
-  {
-    // tensor memory: accumulators for the widest layer, every other column is weight ring
-    int tiles = 1;
-    for (int l = 1; l <= L; ++l) tiles = tiles > ceil_div(qn->dims[l], 128) ? tiles : ceil_div(qn->dims[l], 128);
-    pl.dev.acc_cols = 64 * tiles;
-    int st = (kQTmemCols - pl.dev.acc_cols) / kAStageCols;
-    st = st < kAMaxStages ? st : kAMaxStages;
-    // a ring stage must belong to ONE loader group (tests/test_tc_protocol_model.py): depth is a
-    // multiple of the group count
-    pl.dev.a_stages = st / kQLoaderGroups * kQLoaderGroups;
-    if (pl.dev.a_stages < 2) return pl;
-  }
   pl.dev.need_zero = 0;
   for (int l = 0; l <= L; ++l)
     if (qn->dims[l] % 8 != 0) pl.dev.need_zero = 1;
@@ -934,7 +690,7 @@ static QPlan make_plan(const rb200_mlp_t* qn, const rb200_mlp_t* qtn, int double
   o += ((size_t)2 * kQR * qn->dims[L] + 4 * kQR + 8) * sizeof(float);
   o = (o + 15) & ~(size_t)15;
   pl.dev.bar_off = (int)o;
-  o += (2 * kQStages + 2 * kAMaxStages + kQMaxTiles + 1) * sizeof(uint64_t) + 16;
+  o += 2 * kQStages * sizeof(uint64_t);
   pl.smem_bytes = (o + 15) & ~(size_t)15;
   pl.ok = pl.smem_bytes <= (size_t)kQMaxSmem;
   return pl;
@@ -943,10 +699,6 @@ static QPlan make_plan(const rb200_mlp_t* qn, const rb200_mlp_t* qtn, int double
 }  // namespace rb200
 
 using namespace rb200;
-
-static long long* g_tc_dbg = nullptr;
-// profiling hook (not part of the reference-facing API): device buffer of kQMaxSteps*8 int64
-extern "C" void rb200_debug_set_tc_timeline(void* dev_buf) { g_tc_dbg = static_cast<long long*>(dev_buf); }
 
 extern "C" int64_t rb200_dqn_tc_workspace_bytes(const rb200_mlp_t* q_net, int32_t double_q,
                                                 int32_t do_backward) {
@@ -966,7 +718,7 @@ extern "C" int rb200_dqn_tc_pack(const rb200_mlp_t* q_net, const rb200_mlp_t* q_
     if (q_net->dims[l] != q_target->dims[l]) { set_last_error("q_network / target dims mismatch at %d", l); return RB200_E_INVALID; }
   if ((reinterpret_cast<uintptr_t>(pack_ws) & 127) != 0) { set_last_error("pack workspace must be 128-byte aligned"); return RB200_E_INVALID; }
   QPlan pl = make_plan(q_net, q_target, double_q, do_backward);
-  if (!pl.ok) { set_last_error("rb200_dqn_tc_pack: shapes do not fit the tcgen05 path"); return RB200_E_SMEM; }
+  if (!pl.ok) { set_last_error("rb200_dqn_tc_pack: shapes do not fit the wgmma path"); return RB200_E_SMEM; }
   if (pack_ws_bytes < pl.pack_bytes) { set_last_error("pack workspace too small: %lld < %lld", (long long)pack_ws_bytes, (long long)pl.pack_bytes); return RB200_E_INVALID; }
   pl.pack.pack = static_cast<unsigned char*>(pack_ws);
   dqn_tc_pack_kernel<<<pl.pack_chunks * kPackParts, 256, 0, (cudaStream_t)stream>>>(pl.pack);
@@ -999,13 +751,11 @@ extern "C" int rb200_dqn_td_step_tc(const rb200_mlp_t* q_net, const rb200_mlp_t*
   }
   if ((reinterpret_cast<uintptr_t>(pack_ws) & 127) != 0) { set_last_error("pack workspace must be 128-byte aligned"); return RB200_E_INVALID; }
   QPlan pl = make_plan(q_net, q_target, args->double_q, args->do_backward);
-  if (!pl.ok) { set_last_error("rb200_dqn_td_step_tc: shapes do not fit the tcgen05 path"); return RB200_E_SMEM; }
+  if (!pl.ok) { set_last_error("rb200_dqn_td_step_tc: shapes do not fit the wgmma path"); return RB200_E_SMEM; }
   if (pack_ws_bytes < pl.pack_bytes) { set_last_error("pack workspace too small: %lld < %lld", (long long)pack_ws_bytes, (long long)pl.pack_bytes); return RB200_E_INVALID; }
   pl.dev.a = *args;
   pl.dev.ws = *ws;
   pl.dev.pack = static_cast<const unsigned char*>(pack_ws);
-  pl.dev.dbg = g_tc_dbg;
-  { const char* e = getenv("RB200_TC_DBG_MODE"); pl.dev.dbg_mode = e ? atoi(e) : 0; }
   cudaStream_t st = (cudaStream_t)stream;
   static SmemOptIn optin = {};  // per device; raised outside graph capture by the first eager call
   {

@@ -1,13 +1,14 @@
-// reagent_b200 -- layout of the packed weight images of the tcgen05 TD kernel
+// reagent_b200 -- layout of the packed weight images of the wgmma TD kernel
 // (rb200_dqn_tc.cu), shared with the Adam kernel, which can write the images of the updated
 // parameters itself (rb200_optim.cu) instead of a separate packing launch.
 //
 // Image of an operand A[N rows x K] (N = output features, K = contraction): for every
 // (128-row tile t, kQKC-wide k chunk c) one block of fp32 values laid out [k/4][row][4 floats]
 // with the k-quad stride (LBO) padded by 16 B, so that (a) one 1-D bulk copy moves a whole
-// chunk and (b) the loader warps of the TD kernel read "my row, quad q" as a conflict-free
-// 16-byte shared-memory load.  The TF32 hi/lo split happens in the TD kernel on the way into
-// Tensor Memory (the A operand of the MMAs), so the image holds every parameter ONCE.
+// chunk and (b) the TD kernel reads its wgmma A fragments (rows g / g+8, k t / t+4 of a
+// warp's 16 x 8 slice) as conflict-free 4-byte shared-memory loads.  The TF32 hi/lo split
+// happens in the TD kernel on the way into registers (the A operand of the MMAs), so the image
+// holds every parameter ONCE.
 // Rows / k past the matrix are zero (the buffer is zero-initialised once and those positions
 // are never written).
 #pragma once

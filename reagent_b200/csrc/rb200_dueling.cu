@@ -143,7 +143,7 @@ extern "C" int rb200_dueling_fold(const float* W_adv, const float* b_adv, const 
                                                                       scratch, 0);
   const long long work = (long long)R * 2 * H + R;
   int blocks = (int)((work + 255) / 256);
-  if (blocks > 148 * 8) blocks = 148 * 8;
+  if (blocks > kNumSMs * 8) blocks = kNumSMs * 8;
   dueling_fold_apply_kernel<<<blocks, 256, 0, st>>>(W_adv, b_adv, w_val, b_val, R, num_atoms, H,
                                                     scratch, W_q, b_q);
   return check_cuda(cudaGetLastError(), "dueling fold kernels launch");
@@ -167,7 +167,7 @@ extern "C" int rb200_dueling_unfold(float* grad, int64_t slab_stride, int32_t sp
       grad, slab_stride, num_actions, num_atoms, H, off_W_q, off_b_q, off_w_val, off_b_val);
   const long long work = (long long)R * 2 * H + R;
   int blocks = (int)((work + 255) / 256);
-  if (blocks > 148 * 2) blocks = 148 * 2;
+  if (blocks > kNumSMs * 2) blocks = kNumSMs * 2;
   dueling_unfold_apply_kernel<<<dim3(blocks, splits), 256, 0, st>>>(
       grad, slab_stride, R, num_atoms, H, off_W_q, off_b_q, off_W_adv, off_b_adv, scratch, sstride);
   return check_cuda(cudaGetLastError(), "dueling unfold kernels launch");

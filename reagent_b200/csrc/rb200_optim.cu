@@ -203,7 +203,7 @@ struct AdamDev {
   TcPackView pv;
 };
 
-// images of one updated weight (and of its updated target) for the tcgen05 TD kernel
+// images of one updated weight (and of its updated target) for the wgmma TD kernel
 __device__ __forceinline__ void adam_pack_weight(const TcPackView& pv, long long i, float p,
                                                  bool has_target, float tgt) {
   for (int l = 0; l < pv.n_layers; ++l) {
@@ -353,7 +353,7 @@ using namespace rb200;
 
 extern "C" int rb200_wgrad_splits(int batch) {
   // enough batch splits that even a single 64x64 tile layer fills a good part of the
-  // 148 SMs; rows per split stay a multiple of the 32-row staging step.
+  // SMs; rows per split stay a multiple of the 32-row staging step.
   const char* e = getenv("RB200_WGRAD_ROWS");  // tuning knob (rows per split), default 256
   int rows = e ? atoi(e) : 256;
   if (rows < 32) rows = 32;
@@ -366,24 +366,23 @@ extern "C" int rb200_wgrad_splits(int batch) {
 int rb200_wgrad_tc_launch(const rb200_mlp_t* net, const float* net_input, int32_t batch,
                           const rb200_net_ws_t* ws, float* gpart, int32_t splits, void* stream);
 
-// The tcgen05 weight-gradient kernel (rb200_wgrad_tc.cu) is opt-in (RB200_WGRAD_TC=1): measured
-// inside the captured DQN update it ties with this file's mma.sync kernel (76.2 vs 75.5 us per
-// update at BASELINE config 2, round 2) -- both are bound by their prologue / epilogue at 128-row
-// slabs, not by the tensor pipe -- so the default stays the kernel with the longer track record.
+// The wgmma weight-gradient kernel (rb200_wgrad_tc.cu) is opt-in (RB200_WGRAD_TC=1); the default
+// stays this file's mma.sync kernel: at 128-row slabs both are bound by their prologue /
+// epilogue rather than by the tensor pipe.
 static bool wgrad_use_tc() {
-  const char* d = getenv("RB200_DISABLE_TCGEN05");
+  const char* d = getenv("RB200_DISABLE_WGMMA");
   const char* w = getenv("RB200_WGRAD_TC");
   return !(d && d[0] && d[0] != '0') && (w && w[0] == '1');
 }
 
-// Batch slabs for a network: enough (layer tile, slab) jobs to fill the 148 SMs about twice,
-// slabs of at least 128 rows (the tcgen05 kernel stages 32-row chunks; fewer, longer slabs
+// Batch slabs for a network: enough (layer tile, slab) jobs to fill the SMs about twice,
+// slabs of at least 128 rows (the wgmma kernel stages 32-row chunks; fewer, longer slabs
 // keep the partials the Adam kernel has to read small for wide heads).
 extern "C" int rb200_wgrad_splits_for(const rb200_mlp_t* net, int32_t batch) {
   if (!net || !wgrad_use_tc()) return rb200_wgrad_splits(batch);
   int jobs = 0;
   for (int l = 0; l < net->n_layers; ++l) jobs += ceil_div(net->dims[l + 1], 128) * ceil_div(net->dims[l], 256);
-  int s = ceil_div(296, jobs < 1 ? 1 : jobs);
+  int s = ceil_div(2 * kNumSMs, jobs < 1 ? 1 : jobs);
   const int smax = batch / 128 < 1 ? 1 : batch / 128;
   if (s > smax) s = smax;
   if (s > 64) s = 64;
@@ -429,7 +428,7 @@ extern "C" int rb200_grad_reduce(const float* gpart, int32_t splits, int64_t n, 
                                  void* stream) {
   if (!gpart || !g || n <= 0 || splits <= 0) { set_last_error("rb200_grad_reduce: bad argument"); return RB200_E_INVALID; }
   int blocks = (int)((n + 255) / 256);
-  if (blocks > 148 * 8) blocks = 148 * 8;
+  if (blocks > kNumSMs * 8) blocks = kNumSMs * 8;
   grad_reduce_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(gpart, splits, (long long)n, g);
   return check_cuda(cudaGetLastError(), "grad_reduce_kernel launch");
 }
@@ -473,10 +472,10 @@ extern "C" int rb200_adam_soft_update(const rb200_adam_args_t* a, void* stream) 
   return check_cuda(cudaGetLastError(), "adam_soft_kernel launch");
 }
 
-// grid of rb200_adam_soft_update for an arena of n floats (all blocks co-resident on 148 SMs)
+// grid of rb200_adam_soft_update for an arena of n floats (all blocks co-resident on the SMs)
 extern "C" int rb200_adam_blocks(int64_t n) {
   int blocks = (int)((n + 255) / 256);
-  if (blocks > 148 * 4) blocks = 148 * 4;
+  if (blocks > kNumSMs * 4) blocks = kNumSMs * 4;
   return blocks < 1 ? 1 : blocks;
 }
 
@@ -485,7 +484,7 @@ extern "C" int rb200_soft_update(float* target, const float* source, int64_t n, 
   if (!target || !source || n <= 0) { set_last_error("rb200_soft_update: bad argument"); return RB200_E_INVALID; }
   if (target == source) return RB200_OK;  // aliased: soft_update.py:64-67 skips
   int blocks = (int)((n + 255) / 256);
-  if (blocks > 148 * 4) blocks = 148 * 4;
+  if (blocks > kNumSMs * 4) blocks = kNumSMs * 4;
   soft_update_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(target, source, (long long)n, tau, one_minus_tau);
   return check_cuda(cudaGetLastError(), "soft_update_kernel launch");
 }

@@ -40,7 +40,7 @@ extern "C" int rb200_preprocess(const float* input, const void* presence, int32_
   if (rows == 0) return RB200_OK;
   const long long total = rows * (long long)f_out;
   long long blocks = (total + 255) / 256;
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > kNumSMs * 16) blocks = kNumSMs * 16;
   preprocess_kernel<<<(int)blocks, 256, 0, (cudaStream_t)stream>>>(
       input, (const uint8_t*)presence, presence_is_float, rows, f_in, f_out, cols, quantiles, out);
   return check_cuda(cudaGetLastError(), "preprocess_kernel launch");

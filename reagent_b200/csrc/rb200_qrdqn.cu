@@ -308,8 +308,8 @@ extern "C" int rb200_linear_forward(const float* W, const float* b, int32_t act,
                                     int32_t N, const float* in, int32_t batch, float* out,
                                     void* stream) {
   if (!W || !in || !out || K <= 0 || N <= 0 || batch <= 0) { set_last_error("rb200_linear_forward: bad argument"); return RB200_E_INVALID; }
-  // GEMM-shaped problems (>= one full 128x128 tile) go to the tcgen05 / TMEM kernel
-  static const bool no_tc = getenv("RB200_DISABLE_TCGEN05") != nullptr;  // debugging aid
+  // GEMM-shaped problems (>= one full 128x128 tile) go to the wgmma kernel
+  static const bool no_tc = getenv("RB200_DISABLE_WGMMA") != nullptr;  // debugging aid
   if (!no_tc && batch >= 128 && N >= 128) return rb200_linear_forward_tc(W, b, act, K, N, in, batch, out, stream);
   LinFwdDev p{in, K, W, b, N, act, out, batch, 0, kColBlock + 4};
   RowsCfg cfg = pick_rows_cfg(batch, K, 4, 1, 0, p.ld_o, 0);

@@ -21,7 +21,7 @@
 namespace rb200 {
 
 constexpr int kSPB = 32;  // samples per CTA
-constexpr int kTopLevels = 10;  // 8 KB: small enough to share an SM with the tcgen05 TD kernel
+constexpr int kTopLevels = 10;  // 8 KB: small enough to share an SM with the wgmma TD kernel
 
 struct SampleDev {
   rb200_sample_args_t a;

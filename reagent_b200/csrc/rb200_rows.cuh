@@ -7,7 +7,7 @@
 
 namespace rb200 {
 
-constexpr int kSmemLimit = 227 * 1024;  // B200 opt-in maximum per CTA
+constexpr int kSmemLimit = 227 * 1024;  // H100 opt-in maximum per CTA
 
 struct RowsCfg {
   int nt;      // threads per CTA (256 or 512)
@@ -36,7 +36,7 @@ inline RowsCfg pick_rows_cfg(int batch, int din, int hmax, int n_in, int n_h, in
     const int nt = cand[c][0], tm = cand[c][1], kc = cand[c][2];
     const int R = (nt / 64) * tm;
     if (fnt) { if (nt != fnt || kc != fkc) continue; }
-    else if (R == 32 && batch <= 16 * 148) continue;  // small batch: prefer 16-row tiles
+    else if (R == 32 && batch <= 16 * kNumSMs) continue;  // small batch: prefer 16-row tiles
     const size_t stage = (size_t)(kc == 32 ? wstage_floats<32>() : wstage_floats<16>());
     const size_t floats = 2 * stage + (size_t)R * ((size_t)n_in * ld_in + (size_t)n_h * ld_h +
                                                    (size_t)extra_per_row) + (size_t)extra;

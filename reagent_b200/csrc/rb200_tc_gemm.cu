@@ -1,5 +1,5 @@
-// reagent_b200 -- Blackwell-native wide Linear forward: tcgen05.mma (kind::tf32) with the
-// accumulator in Tensor Memory, 3xTF32 error compensation.
+// reagent_b200 -- wide Linear forward on the Hopper tensor cores: wgmma (kind tf32) with the
+// accumulators in registers, 3xTF32 error compensation.
 //
 //   out[B, N] = act(in[B, K] . W[N, K]^T + b)          (nn.Linear forward, wide N)
 //
@@ -7,26 +7,27 @@
 // 190-217 / reagent/training/qrdqn_trainer.py:125-149): at config 3 it is a
 // 4096 x 6400 x 128 GEMM, the only genuinely GEMM-shaped op of the path.
 //
-// One CTA = one 128 (rows) x 128 (cols) output tile; accumulator D in TMEM (128 lanes x
-// 128 fp32 columns).  K is walked in 32-element chunks through ONE shared-memory stage; the
-// next chunk's global loads are held in registers while the tensor core consumes the stage, and
-// two CTAs share an SM so that one CTA's loads overlap the other's MMAs / epilogue.
-// Per chunk all 256 threads load 16 B pieces of in / W with LDG.128, split every
-// value into hi = rna_tf32(x) and lo = x - hi and store both planes in the canonical K-major
-// no-swizzle UMMA layout  [k/4][row][4 floats]  (core matrix = 8 rows x 16 B contiguous;
-// SBO = 128 B between 8-row groups, LBO = rows*16 B + 16 B pad between the two 16-byte
-// k-slices of one K=8 MMA).  One elected thread then issues, per K=8 step, the three MMAs
+// One CTA = one 128 (rows) x 128 (cols) output tile = two warpgroups, each owning 64 rows
+// (wgmma m64n128k8, 64 fp32 accumulators per thread).  K is walked in 32-element chunks through
+// ONE shared-memory stage; the next chunk's global loads are held in registers while the
+// tensor cores consume the stage, and two CTAs share an SM so that one CTA's loads overlap the
+// other's MMAs / epilogue.  Per chunk all 256 threads load 16 B pieces of in / W with LDG.128,
+// split every value into hi = rna_tf32(x) and lo = x - hi and store both planes in the
+// canonical K-major no-swizzle layout  [k/4][row][4 floats]  (core matrix = 8 rows x 16 B
+// contiguous; SBO = 128 B between 8-row groups, LBO = rows*16 B + 16 B pad between the two
+// 16-byte k-slices of one K=8 MMA).  Each warpgroup then issues, per K=8 step, the three MMAs
 //   D += A_lo.B_hi ;  D += A_hi.B_lo ;  D += A_hi.B_hi
-// and commits the stage to an mbarrier, which the producers wait on before overwriting it.
-// Epilogue: tcgen05.ld (32x32b.x32) -> bias + activation -> global.
-#include "rb200_umma.cuh"
+// and waits for them before the stage is overwritten.
+// Epilogue: registers -> smem tile -> bias + activation -> coalesced global stores.
+#include "rb200_wgmma.cuh"
 
 namespace rb200 {
 
-constexpr int kTcM = 128;     // rows per CTA (UMMA M)
-constexpr int kTcN = 128;     // cols per CTA (UMMA N)
+constexpr int kTcM = 128;     // rows per CTA (two m64 warpgroups)
+constexpr int kTcN = 128;     // cols per CTA (wgmma N)
 constexpr int kTcKC = 32;     // k elements per stage
 constexpr int kTcThreads = 256;
+constexpr int kTcCtasPerSm = 2;
 constexpr int kTcQuadStride = kTcM * 4 + 4;            // floats between k quads: 2048 B + 16 B pad
 constexpr int kTcPlane = (kTcKC / 4) * kTcQuadStride;  // floats per operand plane per stage
 constexpr int kTcStageFloats = 4 * kTcPlane;           // A_hi, A_lo, B_hi, B_lo
@@ -43,17 +44,16 @@ struct TcDev {
   int chunks_per_split;
 };
 
-__global__ void __launch_bounds__(kTcThreads, 3) tc_linear_fwd_kernel(const TcDev p) {
-  // Three CTAs per SM (68 KB smem, 128 TMEM columns each): while one CTA's MMAs or epilogue
-  // run, the others load -- the overlap a deeper ring would give, without the shared memory.
+__global__ void __launch_bounds__(kTcThreads, kTcCtasPerSm) tc_linear_fwd_kernel(const TcDev p) {
+  // Two CTAs per SM (66 KB smem, 64 accumulator registers per thread each): while one CTA's
+  // MMAs or epilogue run, the other loads -- the overlap a deeper ring would give.
   extern __shared__ __align__(128) float smem[];
   float* a_hi = smem;
   float* a_lo = a_hi + kTcPlane;
   float* b_hi = a_lo + kTcPlane;
   float* b_lo = b_hi + kTcPlane;
-  uint64_t* bar = reinterpret_cast<uint64_t*>(smem + kTcBufFloats);  // stage consumed by the MMAs
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bar + 1);
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int wg = warp >> 2;  // warpgroup: rows [64 wg, 64 wg + 64) of the tile
   const int row0 = blockIdx.x * kTcM, col0 = blockIdx.y * kTcN;
   const int K = p.K;
   int c_begin = 0, nchunks = ceil_div(K, kTcKC);
@@ -65,21 +65,6 @@ __global__ void __launch_bounds__(kTcThreads, 3) tc_linear_fwd_kernel(const TcDe
   float* const outp = raw ? p.out + (size_t)blockIdx.z * p.batch * p.N : p.out;
   const bool vin = ((K & 3) == 0) && ((reinterpret_cast<uintptr_t>(p.in) & 15) == 0);
   const bool vw = ((K & 3) == 0) && ((reinterpret_cast<uintptr_t>(p.W) & 15) == 0);
-
-  if (tid == 0) {
-    mbar_init(bar, 1);
-    asm volatile("fence.mbarrier_init.release.cluster;\n" ::);
-  }
-  if (warp == 0) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;\n" ::"r"(
-                     smem_u32(tmem_slot)), "n"(kTcN));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;\n" ::);
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;\n" ::);
-  __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;\n" ::);
-  const uint32_t tmem_d = *tmem_slot;
-  const uint32_t idesc = umma_idesc_tf32(kTcM, kTcN);
 
   // thread -> pieces (row = idx / 8, quad = idx % 8), idx = tid + it*256: a warp reads 4 rows x
   // 128 contiguous bytes of global memory and stores them to the [k quad][row][4] layout whose
@@ -120,10 +105,17 @@ __global__ void __launch_bounds__(kTcThreads, 3) tc_linear_fwd_kernel(const TcDe
     }
   };
 
+  float acc[kTcN / 2];
+#pragma unroll
+  for (int i = 0; i < kTcN / 2; ++i) acc[i] = 0.f;
+  constexpr uint32_t LBO = kTcQuadStride * 4;  // bytes between the two 16 B k-slices of an MMA
+  constexpr uint32_t SBO = 128;                // bytes between 8-row groups
+  const uint32_t a_row_off = (uint32_t)wg * 64 * 16;
+
   load_regs(c_begin);
   for (int c = c_begin; c < nchunks; ++c) {
-    // the MMAs of the previous chunk must have consumed the stage
-    if (c > c_begin) mbar_wait(bar, (c - c_begin - 1) & 1);
+    // the MMAs of the previous chunk (both warpgroups) have completed: the stage is free
+    if (c > c_begin) __syncthreads();
 #pragma unroll
     for (int it = 0; it < kTcIters; ++it) {
       const int idx = tid + it * kTcThreads;
@@ -137,59 +129,39 @@ __global__ void __launch_bounds__(kTcThreads, 3) tc_linear_fwd_kernel(const TcDe
       *reinterpret_cast<float4*>(b_hi + off) = h;
       *reinterpret_cast<float4*>(b_lo + off) = l;
     }
-    // make the generic-proxy stores visible to the tensor core (async proxy)
-    asm volatile("fence.proxy.async.shared::cta;\n" ::);
+    // make the generic-proxy stores visible to the tensor cores (async proxy)
+    fence_proxy_async_smem();
     __syncthreads();
-    if (tid == 0) {
-      asm volatile("tcgen05.fence::after_thread_sync;\n" ::);
-      constexpr uint32_t LBO = kTcQuadStride * 4;  // bytes between the two 16 B k-slices of an MMA
-      constexpr uint32_t SBO = 128;        // bytes between 8-row groups
+    wgmma_fence();
 #pragma unroll
-      for (int s4 = 0; s4 < kTcKC / 8; ++s4) {
-        const uint32_t koff = (uint32_t)(2 * s4) * LBO;  // k quad 2*s4
-        const uint64_t dah = umma_desc(smem_u32(a_hi) + koff, LBO, SBO);
-        const uint64_t dal = umma_desc(smem_u32(a_lo) + koff, LBO, SBO);
-        const uint64_t dbh = umma_desc(smem_u32(b_hi) + koff, LBO, SBO);
-        const uint64_t dbl = umma_desc(smem_u32(b_lo) + koff, LBO, SBO);
-        umma_tf32(tmem_d, dal, dbh, idesc, (c > c_begin || s4 > 0) ? 1u : 0u);
-        umma_tf32(tmem_d, dah, dbl, idesc, 1u);
-        umma_tf32(tmem_d, dah, dbh, idesc, 1u);
-      }
-      umma_commit(bar);
+    for (int s4 = 0; s4 < kTcKC / 8; ++s4) {
+      const uint32_t koff = (uint32_t)(2 * s4) * LBO;  // k quad 2*s4
+      const uint64_t dah = wgmma_desc(smem_u32(a_hi) + koff + a_row_off, LBO, SBO);
+      const uint64_t dal = wgmma_desc(smem_u32(a_lo) + koff + a_row_off, LBO, SBO);
+      const uint64_t dbh = wgmma_desc(smem_u32(b_hi) + koff, LBO, SBO);
+      const uint64_t dbl = wgmma_desc(smem_u32(b_lo) + koff, LBO, SBO);
+      wgmma_ss_n128(acc, dal, dbh, 1u);
+      wgmma_ss_n128(acc, dah, dbl, 1u);
+      wgmma_ss_n128(acc, dah, dbh, 1u);
     }
-    // global loads of the next chunk fly while the tensor core works on this one
+    wgmma_commit();
+    // global loads of the next chunk fly while the tensor cores work on this one
     if (c + 1 < nchunks) load_regs(c + 1);
+    wgmma_wait<0>();
   }
-  mbar_wait(bar, (nchunks - c_begin - 1) & 1);
-  asm volatile("tcgen05.fence::after_thread_sync;\n" ::);
+  __syncthreads();  // every warpgroup is done with the operand stage: it becomes the output tile
 
-  // ---- epilogue: TMEM -> registers -> bias + activation -> smem tile -> coalesced global ----
-  // warp w may touch TMEM lanes [32*(w%4), 32*(w%4)+32); warps 0-3 take columns [0,64),
-  // warps 4-7 columns [64,128).  The staging ring is free (all MMAs completed).
+  // ---- epilogue: registers -> smem tile -> bias + activation -> coalesced global ----
   {
     constexpr int LDO = kTcLdo;    // padded row stride of the output tile in smem
     float* otile = smem;           // 128 x 132 floats, reuses the operand stage
-    const int quad = warp & 3;
-    const int r = quad * 32 + lane;
-    for (int cb = (warp >> 2) * 64; cb < (warp >> 2) * 64 + 64; cb += 32) {
-      uint32_t v[32];
-      const uint32_t taddr = tmem_d + ((uint32_t)(quad * 32) << 16) + (uint32_t)cb;
-      asm volatile(
-          "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-          "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
-          "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];\n"
-          : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]),
-            "=r"(v[7]), "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]),
-            "=r"(v[14]), "=r"(v[15]), "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]),
-            "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]), "=r"(v[25]),
-            "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-          : "r"(taddr));
-      asm volatile("tcgen05.wait::ld.sync.aligned;\n" ::);
+    const int r = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+    const int cq = 2 * (lane & 3);
 #pragma unroll
-      for (int j = 0; j < 32; j += 4)
-        *reinterpret_cast<float4*>(otile + r * LDO + cb + j) =
-            make_float4(__uint_as_float(v[j]), __uint_as_float(v[j + 1]), __uint_as_float(v[j + 2]),
-                        __uint_as_float(v[j + 3]));
+    for (int j = 0; j < kTcN / 8; ++j) {
+      *reinterpret_cast<float2*>(otile + r * LDO + 8 * j + cq) = make_float2(acc[4 * j], acc[4 * j + 1]);
+      *reinterpret_cast<float2*>(otile + (r + 8) * LDO + 8 * j + cq) =
+          make_float2(acc[4 * j + 2], acc[4 * j + 3]);
     }
     __syncthreads();
     // each warp writes whole 512-byte row segments; bias + activation applied on the way out
@@ -212,11 +184,6 @@ __global__ void __launch_bounds__(kTcThreads, 3) tc_linear_fwd_kernel(const TcDe
           if (col + j < p.N) dst[j] = ov[j];
       }
     }
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;\n" ::);
-  __syncthreads();
-  if (warp == 0) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;\n" ::"r"(tmem_d), "n"(kTcN));
   }
 }
 
@@ -258,12 +225,12 @@ __global__ void __launch_bounds__(256) tc_dx_reduce_kernel(const float* __restri
 }
 
 struct DxPlan { int splits, chunks_per_split; size_t wt_floats, partial_floats; };
-// the tcgen05 path pays off for a wide layer (N = out features is the contraction here)
+// the tensor-core path pays off for a wide layer (N = out features is the contraction here)
 static bool dx_plan(int K, int N, int batch, DxPlan* pl) {
   if (N < 1024 || batch < 256 || (K & 3) != 0 || (N & 3) != 0) return false;
   const int tiles = ceil_div(batch, kTcM) * ceil_div(K, kTcN);
   const int nchunks = ceil_div(N, kTcKC);
-  int splits = (3 * 148) / tiles;  // three CTAs per SM
+  int splits = (kTcCtasPerSm * kNumSMs) / tiles;
   splits = splits < 1 ? 1 : (splits > nchunks ? nchunks : splits);
   pl->chunks_per_split = ceil_div(nchunks, splits);
   pl->splits = ceil_div(nchunks, pl->chunks_per_split);
@@ -277,7 +244,7 @@ static bool dx_plan(int K, int N, int batch, DxPlan* pl) {
 using namespace rb200;
 
 // Scratch bytes rb200_linear_backward_dx_tc needs for this shape; 0 = shape not taken by the
-// tcgen05 path (use rb200_linear_backward_dx).
+// tensor-core path (use rb200_linear_backward_dx).
 extern "C" int64_t rb200_linear_backward_dx_tc_scratch_bytes(int32_t K, int32_t N, int32_t batch) {
   DxPlan pl;
   if (K <= 0 || N <= 0 || batch <= 0 || !dx_plan(K, N, batch, &pl)) return 0;
@@ -285,7 +252,7 @@ extern "C" int64_t rb200_linear_backward_dx_tc_scratch_bytes(int32_t K, int32_t 
 }
 
 // Same contract as rb200_linear_backward_dx (W is the nn.Linear weight [N out x K in], dz [B, N],
-// out [B, K] = (dz . W) * act'(h_prev)) on tcgen05: W is transposed into the scratch, the
+// out [B, K] = (dz . W) * act'(h_prev)) on wgmma: W is transposed into the scratch, the
 // contraction over N runs as split-K slices of tc_linear_fwd_kernel, a last pass adds the
 // slices in order and applies act'.
 extern "C" int rb200_linear_backward_dx_tc(const float* W, int32_t K, int32_t N, const float* dz,

@@ -25,9 +25,8 @@ __host__ __device__ constexpr int wstage_floats() {
 // Tensor-core inner product: mma.sync.m16n8k8 TF32 with 3xTF32 error compensation.
 //   x = hi + lo (hi = rna_tf32(x), lo = rna_tf32(x - hi));  a*b ~= a_lo*b_hi + a_hi*b_lo + a_hi*b_hi
 // fp32 accumulation in the MMA; the dropped a_lo*b_lo term is ~2^-22 relative, which keeps the
-// 1e-5 parity bar of the north star (plain TF32 would be ~1e-3).  Measured on this B200 pool
-// (profiles/micro/pipes.cu): FFMA 56 TFLOP/s, mma.sync TF32 277 TFLOP/s -> 92 TFLOP/s
-// algorithmic for 3xTF32 with ~10x fewer issue slots than the FFMA loop.
+// 1e-5 parity bar of the north star (plain TF32 would be ~1e-3), with far fewer issue slots
+// than an FFMA loop.
 // Fragment <-> shared-memory mapping (g = lane/4, t = lane%4), all LDS.32 conflict-free:
 //   A (16x8, row-major tile of the activations, stride == 4 mod 32): a0 (g,t) a1 (g+8,t)
 //                                                                   a2 (g,t+4) a3 (g+8,t+4)

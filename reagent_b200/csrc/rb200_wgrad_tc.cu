@@ -1,9 +1,9 @@
-// reagent_b200 -- weight gradients on the 5th-generation tensor cores.
+// reagent_b200 -- weight gradients on the Hopper tensor cores.
 //
 //   dW_l[n, k] = sum_b dZ_l[b, n] * A_{l-1}[b, k],   db_l[n] = sum_b dZ_l[b, n]
 // (autograd's Linear backward reached from loss.backward() in the reference's Lightning loop,
-// reagent/training/reagent_lightning_module.py:108-133) as tcgen05.mma kind::tf32 with 3xTF32
-// error compensation and the accumulator in Tensor Memory.
+// reagent/training/reagent_lightning_module.py:108-133) as wgmma kind tf32 with 3xTF32 error
+// compensation and the accumulators in registers.
 //
 // The contraction runs over the BATCH, and both factors are stored batch-row-major in HBM
 // ([B, N] and [B, K]), i.e. transposed with respect to the K-major operand layout the MMA
@@ -13,22 +13,21 @@
 // canonical K-major no-swizzle layout
 //     [batch row / 4][feature][4 batch rows]   (row-quad stride = LBO, 8 features = SBO = 128 B)
 // with bank-conflict-free 4-byte stores (the padded row-quad stride spreads a warp's 32 stores
-// over the 32 banks); every 8-row k step issues  D += A_hi.B_hi + A_lo.B_hi + A_hi.B_lo  with M = 128 output
-// features of dZ_l and N <= 256 input features of A_{l-1}.
+// over the 32 banks); every 8-row k step issues  D += A_hi.B_hi + A_lo.B_hi + A_hi.B_lo  with
+// M = 64 output features of dZ_l per warpgroup (two warpgroups: 128) and N <= 256 input
+// features of A_{l-1}.
 //
 // One CTA = (layer, 128-feature tile of dZ_l, 256-feature tile of A_{l-1}, batch slab); the
 // slabs are summed later by the Adam kernel in slab order (deterministic), exactly like the
 // mma.sync kernel this one replaces for shapes that fit (rb200_optim.cu keeps that kernel for
 // the rest).  Two smem stages; the loads of chunk c+1 are in flight while chunk c's MMAs run.
-#include <stdlib.h>
-
-#include "rb200_umma.cuh"
+#include "rb200_wgmma.cuh"
 
 namespace rb200 {
 
 constexpr int kWtRows = 32;                       // batch rows per stage = 4 MMA k steps
-constexpr int kWtM = 128;                         // dZ features per tile (UMMA M)
-constexpr int kWtN = 256;                         // input features per tile (UMMA N, TMEM columns)
+constexpr int kWtM = 128;                         // dZ features per tile (two m64 warpgroups)
+constexpr int kWtN = 256;                         // input features per tile (wgmma N <= 256)
 constexpr int kWtQuadA = kWtM * 16 + 16;          // bytes per 4-row group of the dZ operand
 constexpr int kWtQuadB = kWtN * 16 + 16;          // ... of the activation operand
 constexpr int kWtPlaneA = (kWtRows / 4) * kWtQuadA;
@@ -45,7 +44,6 @@ struct WtLayer {
   int tiles_m, tiles_k, job_start;
 };
 struct WtParams {
-  int dbg;  // profiling only: 1 skip the loads, 2 skip the split, 4 skip the MMAs, 8 skip the epilogue stores
   int n_layers;
   WtLayer L[kMaxLayers];
   int B, rows_per_split;
@@ -53,9 +51,26 @@ struct WtParams {
   long long P;
 };
 
+// the three MMAs of one k step at wgmma N = NT (the staged columns rounded up; columns past the
+// matrix only reach accumulator columns that are not stored)
+template <int NT>
+__device__ __forceinline__ void wt_kstep(float* acc, uint64_t dah, uint64_t dal, uint64_t dbh,
+                                         uint64_t dbl) {
+  if constexpr (NT == 32) {
+    wgmma_ss_n32(acc, dah, dbh, 1u); wgmma_ss_n32(acc, dal, dbh, 1u); wgmma_ss_n32(acc, dah, dbl, 1u);
+  } else if constexpr (NT == 64) {
+    wgmma_ss_n64(acc, dah, dbh, 1u); wgmma_ss_n64(acc, dal, dbh, 1u); wgmma_ss_n64(acc, dah, dbl, 1u);
+  } else if constexpr (NT == 128) {
+    wgmma_ss_n128(acc, dah, dbh, 1u); wgmma_ss_n128(acc, dal, dbh, 1u); wgmma_ss_n128(acc, dah, dbl, 1u);
+  } else {
+    wgmma_ss_n256(acc, dah, dbh, 1u); wgmma_ss_n256(acc, dal, dbh, 1u); wgmma_ss_n256(acc, dah, dbl, 1u);
+  }
+}
+
 __global__ void __launch_bounds__(kWtThreads, 1) wgrad_tc_kernel(const WtParams p) {
   extern __shared__ __align__(128) unsigned char smem[];
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int wg = warp >> 2;  // warpgroup: dZ features [64 wg, 64 wg + 64) of the tile
   int li = 0;
   while (li + 1 < p.n_layers && (int)blockIdx.x >= p.L[li + 1].job_start) ++li;
   const WtLayer& Ly = p.L[li];
@@ -65,35 +80,15 @@ __global__ void __launch_bounds__(kWtThreads, 1) wgrad_tc_kernel(const WtParams 
   const int N = Ly.N, K = Ly.K;
   const int nrows_m = min(kWtM, N - n0);             // valid dZ features of this tile
   const int ncols = min(kWtN, K - k0);               // valid input features of this tile
-  const int n_mma = (ncols + 15) & ~15;              // UMMA N (multiple of 16 for M = 128)
+  const int n_mma = ncols <= 32 ? 32 : (ncols <= 64 ? 64 : (ncols <= 128 ? 128 : 256));
   const int split = blockIdx.y;
   const int b_begin = split * p.rows_per_split;
   const int b_end = min(p.B, b_begin + p.rows_per_split);
   const int nchunks = ceil_div(max(b_end - b_begin, 0), kWtRows);
 
-  uint64_t* mma_done = reinterpret_cast<uint64_t*>(smem + 2 * kWtStage);  // [2] stage reusable
-  uint64_t* acc_done = mma_done + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_done + 1);
-
   // No zero-fill of the stages: every staged feature row is rewritten per chunk (zeros past the
   // slab end); features past the matrix are never written, and whatever they hold only reaches
   // accumulator rows / columns that are not stored (D[m][n] depends on A row m and B row n only).
-  if (tid == 0) {
-    mbar_init(mma_done, 1);
-    mbar_init(mma_done + 1, 1);
-    mbar_init(acc_done, 1);
-    asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory");
-  }
-  if (warp == 0) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;\n" ::"r"(
-                     smem_u32(tmem_slot)), "n"(kWtN));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;\n" ::);
-  }
-  fence_proxy_async_smem();
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = *tmem_slot;
 
   // A chunk (32 batch rows) is moved in "units" of 16 rows x 8 features: lane = (row, 4-feature
   // piece) loads one float4 (16 rows x 32 B: whole sectors), splits it into TF32 hi / lo and
@@ -112,7 +107,7 @@ __global__ void __launch_bounds__(kWtThreads, 1) wgrad_tc_kernel(const WtParams 
     for (int u = 0; u < kMaxUnits; ++u) {
       const int unit = warp + u * (kWtThreads / 32);
       float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-      if (unit < utotal && !(p.dbg & 1)) {
+      if (unit < utotal) {
         const bool isb = unit >= ua;
         const int j = isb ? unit - ua : unit;
         const int h = j & 1, fp = j >> 1;
@@ -167,79 +162,72 @@ __global__ void __launch_bounds__(kWtThreads, 1) wgrad_tc_kernel(const WtParams 
     }
   };
 
-  const uint32_t idesc = umma_idesc_tf32(kWtM, n_mma);
-  uint32_t done_par[2] = {0u, 0u};
+  float acc[kWtN / 2];
+#pragma unroll
+  for (int i = 0; i < kWtN / 2; ++i) acc[i] = 0.f;
+  auto chunk_mma = [&](int st) {
+    const uint32_t sb = smem_u32(smem + st * kWtStage);
+    const uint32_t a_hi = sb + (uint32_t)wg * 64 * 16, a_lo = a_hi + kWtPlaneA;
+    const uint32_t b_hi = sb + 2 * kWtPlaneA, b_lo = b_hi + kWtPlaneB;
+    wgmma_fence();
+#pragma unroll
+    for (int ks = 0; ks < kWtRows / 8; ++ks) {
+      // K-major no-swizzle: leading offset = next 4-row group, stride offset = 8 features
+      const uint32_t oa = ks * 2 * kWtQuadA, ob = ks * 2 * kWtQuadB;
+      const uint64_t dah = wgmma_desc(a_hi + oa, kWtQuadA, 128), dal = wgmma_desc(a_lo + oa, kWtQuadA, 128);
+      const uint64_t dbh = wgmma_desc(b_hi + ob, kWtQuadB, 128), dbl = wgmma_desc(b_lo + ob, kWtQuadB, 128);
+      switch (n_mma) {
+        case 32: wt_kstep<32>(acc, dah, dal, dbh, dbl); break;
+        case 64: wt_kstep<64>(acc, dah, dal, dbh, dbl); break;
+        case 128: wt_kstep<128>(acc, dah, dal, dbh, dbl); break;
+        default: wt_kstep<256>(acc, dah, dal, dbh, dbl); break;
+      }
+    }
+    wgmma_commit();
+  };
+
   if (nchunks > 0) chunk_fetch(0);
   for (int c = 0; c < nchunks; ++c) {
     const int st = c & 1;
-    if (c >= 2) {  // the MMAs of chunk c-2 read this stage
-      mbar_wait(mma_done + st, done_par[st]);
-      done_par[st] ^= 1u;
-    }
-    if (!(p.dbg & 2)) chunk_store(st);
+    // the MMAs of chunk c-2 read this stage: every warpgroup waited for them (wait_group 1 at
+    // the end of chunk c-1) before the barrier of chunk c-1
+    chunk_store(st);
     if (c + 1 < nchunks) chunk_fetch(c + 1);  // in flight during the barrier and the MMAs
     fence_proxy_async_smem();
     __syncthreads();
     chunk_bias(st);
-    if (tid == 0) {
-      tc_fence_after();
-      const uint32_t sb = smem_u32(smem + st * kWtStage);
-      const uint32_t a_hi = sb, a_lo = sb + kWtPlaneA, b_hi = sb + 2 * kWtPlaneA, b_lo = b_hi + kWtPlaneB;
-#pragma unroll
-      for (int ks = 0; ks < ((p.dbg & 4) ? 0 : kWtRows / 8); ++ks) {
-        // K-major no-swizzle: leading offset = next 4-row group, stride offset = 8 features
-        const uint32_t oa = ks * 2 * kWtQuadA, ob = ks * 2 * kWtQuadB;
-        const uint64_t dah = umma_desc(a_hi + oa, kWtQuadA, 128), dal = umma_desc(a_lo + oa, kWtQuadA, 128);
-        const uint64_t dbh = umma_desc(b_hi + ob, kWtQuadB, 128), dbl = umma_desc(b_lo + ob, kWtQuadB, 128);
-        umma_tf32(tmem, dah, dbh, idesc, (c > 0 || ks > 0) ? 1u : 0u);
-        umma_tf32(tmem, dal, dbh, idesc, 1u);
-        umma_tf32(tmem, dah, dbl, idesc, 1u);
-      }
-      umma_commit(mma_done + st);
-      if (c == nchunks - 1) umma_commit(acc_done);
-    }
+    // (a warpgroup whose dZ features lie past the matrix multiplies stale rows that are never
+    // stored: issuing unconditionally keeps the MMAs out of divergent code)
+    chunk_mma(st);
+    wgmma_wait<1>();  // chunk c-1's group retired: its stage is free for chunk c+1
+    __syncthreads();
   }
+  wgmma_wait<0>();
+  __syncthreads();  // all MMAs retired: the operand stages become the output tile
 
-  // ---- epilogue: accumulator -> shared memory (the operand stages are dead) -> this slab's
-  // gradient partial with coalesced 16-byte stores (a thread owns a TMEM lane = a row of dW;
-  // writing it straight out would be 4-byte pieces 1 KB apart) ----
+  // ---- epilogue: accumulators -> shared memory (the operand stages are dead) -> this slab's
+  // gradient partial with coalesced 16-byte stores ----
   float* gp = p.gpart + (size_t)split * p.P;
-  constexpr int kLdT = kWtN + 4;  // floats per staged row: 16-byte aligned, conflict-free
+  constexpr int kLdT = kWtN + 4;  // floats per staged row: 16-byte aligned
   float* tile = reinterpret_cast<float*>(smem);
-  if (nchunks > 0) {
-    mbar_wait(acc_done, 0);
-    tc_fence_after();
-  }
-  if (warp < 4) {
-    const int nl = warp * 32 + lane;
-    for (int c0 = 0; c0 < n_mma; c0 += 16) {
-      uint32_t v[16];
-      if (nchunks > 0) {
-        asm volatile(
-            "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-            "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];\n"
-            : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]),
-              "=r"(v[7]), "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]),
-              "=r"(v[14]), "=r"(v[15])
-            : "r"(tmem + ((uint32_t)(warp * 32) << 16) + (uint32_t)c0));
-        asm volatile("tcgen05.wait::ld.sync.aligned;\n" ::: "memory");
-      } else {
+  {
+    const int r = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+    const int cq = 2 * (lane & 3);
 #pragma unroll
-        for (int j = 0; j < 16; ++j) v[j] = 0u;
+    for (int j = 0; j < kWtN / 8; ++j) {
+      if (8 * j < n_mma) {
+        *reinterpret_cast<float2*>(tile + (size_t)r * kLdT + 8 * j + cq) = make_float2(acc[4 * j], acc[4 * j + 1]);
+        *reinterpret_cast<float2*>(tile + (size_t)(r + 8) * kLdT + 8 * j + cq) =
+            make_float2(acc[4 * j + 2], acc[4 * j + 3]);
       }
-      float4* d = reinterpret_cast<float4*>(tile + (size_t)nl * kLdT + c0);
-#pragma unroll
-      for (int j = 0; j < 4; ++j)
-        d[j] = make_float4(__uint_as_float(v[4 * j]), __uint_as_float(v[4 * j + 1]),
-                           __uint_as_float(v[4 * j + 2]), __uint_as_float(v[4 * j + 3]));
     }
-    if (tk == 0 && n0 + nl < N) gp[Ly.b_off + n0 + nl] = bsum;
   }
+  if (tid < kWtM && tk == 0 && n0 + tid < N) gp[Ly.b_off + n0 + tid] = bsum;
   __syncthreads();
   {
     const bool v4 = ((K & 3) == 0) && ((k0 & 3) == 0) && ((Ly.w_off & 3) == 0) &&
                     ((reinterpret_cast<uintptr_t>(gp) & 15) == 0);
-    for (int r = warp; r < ((p.dbg & 8) ? 0 : nrows_m); r += kWtThreads / 32) {
+    for (int r = warp; r < nrows_m; r += kWtThreads / 32) {
       float* dst = gp + Ly.w_off + (size_t)(n0 + r) * K + k0;
       const float* src = tile + (size_t)r * kLdT;
       if (v4) {
@@ -250,23 +238,16 @@ __global__ void __launch_bounds__(kWtThreads, 1) wgrad_tc_kernel(const WtParams 
       }
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;\n" ::"r"(tmem), "n"(kWtN));
-  }
 }
 
 }  // namespace rb200
 
 using namespace rb200;
 
-// Launch the tcgen05 weight-gradient kernel.  Returns RB200_E_SMEM when the shapes do not fit
-// (the caller then uses the mma.sync kernel); every layer of the in-scope networks does.
+// Launch the wgmma weight-gradient kernel.
 int rb200_wgrad_tc_launch(const rb200_mlp_t* net, const float* net_input, int32_t batch,
                           const rb200_net_ws_t* ws, float* gpart, int32_t splits, void* stream) {
   WtParams p = {};
-  { const char* e = getenv("RB200_WT_DBG"); p.dbg = e ? atoi(e) : 0; }
   p.n_layers = net->n_layers;
   p.B = batch;
   p.rows_per_split = ceil_div(ceil_div(batch, splits), kWtRows) * kWtRows;

@@ -27,5 +27,5 @@ class ModelBase(nn.Module):
 def require_cuda(t: torch.Tensor, what: str):
     if not t.is_cuda:
         raise _lib.Rb200Error(
-            f"{what}: reagent_b200 runs on CUDA (sm_100a) only; got a {t.device} tensor. "
+            f"{what}: reagent_b200 runs on CUDA (sm_90a) only; got a {t.device} tensor. "
             "There is no CPU fallback -- move the model and batch to the GPU.")

@@ -1,7 +1,7 @@
 """Optimizer config surface of the reference (reagent/optimizer/union.py:52-64,
 optimizer.py:47-85, uninferrable_optimizers.py:23-33): `Optimizer__Union.default()` is
 Adam; `make_optimizer_scheduler(params)` returns {"optimizer": ...}.  Only Adam has a fused
-sm_100a kernel (SURVEY.md 8a O2); other members of the reference's union raise."""
+sm_90a kernel (SURVEY.md 8a O2); other members of the reference's union raise."""
 from dataclasses import dataclass, field
 from typing import List, Tuple
 
@@ -34,7 +34,7 @@ class Optimizer__Union:
         (name, value), = kwargs.items()
         if name not in classes:
             raise NotImplementedError(
-                f"optimizer {name!r} has no fused sm_100a kernel; supported: {sorted(classes)}")
+                f"optimizer {name!r} has no fused sm_90a kernel; supported: {sorted(classes)}")
         if isinstance(value, dict):
             value = classes[name](**value)
         self.selected_field = name

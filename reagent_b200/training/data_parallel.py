@@ -40,7 +40,7 @@ class P2PExchange:
     NCCL call and no separate gradient-reduce launch: the Adam kernel of every rank pushes its
     gradient slice to the peers, waits for theirs and sums them in rank order."""
 
-    MAX_BLOCKS = 148 * 4
+    MAX_BLOCKS = 132 * 4  # rb200_adam_blocks(): four blocks per SM of an H100
 
     def __init__(self, group=None, pool_bytes: int = 512 << 20):
         import ctypes as C

@@ -116,8 +116,8 @@ class DQNTrainer(DQNTrainerBaseLightning):
     _tc_prepacked = False  # set by a caller that already ran rb200_dqn_tc_pack (fused_step.py)
 
     def _tc_pack(self, qd, a, device):
-        """Scratch for the tcgen05 path of K2 (packed hi/lo weight images), or None when the
-        network does not fit it (or RB200_DISABLE_TCGEN05 is set): then the mma.sync row-tile
+        """Scratch for the wgmma path of K2 (packed weight images), or None when the
+        network does not fit it (or RB200_DISABLE_WGMMA is set): then the mma.sync row-tile
         kernel runs.  Both are this library's CUDA kernels; there is no other fallback."""
         return self._tc_pack_for((int(a.double_q), int(a.do_backward)), qd, device)
 
@@ -126,7 +126,7 @@ class DQNTrainer(DQNTrainerBaseLightning):
         pack = cache.get(key, False)
         if pack is False or (pack is not None and pack.device != device):
             nbytes = 0
-            if not os.environ.get("RB200_DISABLE_TCGEN05"):
+            if not os.environ.get("RB200_DISABLE_WGMMA"):
                 nbytes = int(_lib.lib().rb200_dqn_tc_workspace_bytes(qd, key[0], key[1]))
             pack = torch.zeros(nbytes, dtype=torch.uint8, device=device) if nbytes > 0 else None
             cache[key] = pack
@@ -165,7 +165,7 @@ class DQNTrainer(DQNTrainerBaseLightning):
         return None if pack is None else (pack, 1)
 
     def tc_prepack(self) -> bool:
-        """Build the weight images of the tcgen05 K2 on the CURRENT stream, for the next
+        """Build the weight images of the wgmma K2 on the CURRENT stream, for the next
         training `_td_step` (which then skips the packing).  The images depend only on the
         parameters, so a caller may run this on a side stream next to the replay sampling
         (fused_step.py).  Returns False when K2 runs on the row-tile kernel instead."""

@@ -127,7 +127,7 @@ class FusedDqnStep:
 
     # -- one update on the current stream ---------------------------------------
     def _one_update(self, rnd_dev):
-        # the tcgen05 K2 wants hi/lo weight images: they only depend on the parameters, so they
+        # the wgmma K2 wants packed weight images: they only depend on the parameters, so they
         # are built on a side stream while the replay-sample kernel runs (fork/join is
         # captured into the graph like any other dependency)
         main = torch.cuda.current_stream()
@@ -322,7 +322,7 @@ def capture_device_only(trainer, rb, batch_size, steps, queries_dev, process_gro
                 with torch.cuda.stream(side):
                     nxt = sample(k + 1)
                 keep.append(nxt)
-            trainer.train_batch(batch, process_group=process_group)
+            loss = trainer.train_batch(batch, process_group=process_group)
             if k + 1 < steps:
                 if nxt is None:
                     nxt = sample(k + 1)
@@ -331,4 +331,5 @@ def capture_device_only(trainer, rb, batch_size, steps, queries_dev, process_gro
                     main.wait_stream(side)
                 batch = nxt
     g._rb200_keep = keep
+    g._rb200_last_loss = loss  # graph-owned: the loss of the last update after every replay
     return g

@@ -44,7 +44,7 @@ def wgrad(arena: ParamArena, ws: NetWorkspace, net_input, batch: int):
 def head_backward_dx(arena: ParamArena, ws: NetWorkspace, batch: int, cache: dict):
     """dZ of the layer below a wide head: dz[L-2] = (dz[L-1] . W_head) * act'(h[L-2])
     (torch.nn.functional.linear's backward w.r.t. its input).  Wide heads (QR-DQN: A*N atoms,
-    C51: A*51) take the tcgen05 split-K path, which needs a scratch buffer kept in `cache`."""
+    C51: A*51) take the wgmma split-K path, which needs a scratch buffer kept in `cache`."""
     lib, st = _lib.lib(), _lib.cur_stream()
     L = len(arena.acts)
     K, N = arena.dims[L - 1], arena.dims[L]

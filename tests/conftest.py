@@ -9,7 +9,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device")
     # The CPU oracle is torch fp32 on the host.  On the many-core GPU boxes torch's default (one
     # thread per core) is pathological for these small GEMMs -- bench.py's sweep measured 0.3
     # updates/s at 128 threads against ~60 at 16 -- and gets worse when the host is shared, so

@@ -1,4 +1,4 @@
-// Host-only consistency check of the tcgen05 weight-image layout (rb200_dqn_tc_layout.cuh):
+// Host-only consistency check of the wgmma weight-image layout (rb200_dqn_tc_layout.cuh):
 // the element -> offset map used by the Adam kernel (image_elem) must be a bijection onto the
 // positions the pack kernel writes (chunk_geo + its in-chunk formula), chunks must not collide,
 // and everything must stay inside image_bytes().  Compiled with nvcc, run on the CPU.

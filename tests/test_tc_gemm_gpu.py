@@ -1,4 +1,4 @@
-"""tcgen05 / TMEM wide Linear forward (rb200_linear_forward -> tc_linear_fwd_kernel) vs an
+"""wgmma wide Linear forward (rb200_linear_forward -> tc_linear_fwd_kernel) vs an
 fp64 torch reference: full tiles, ragged rows / columns / K, scalar-load path, activations."""
 import pytest
 import torch
@@ -49,7 +49,7 @@ def test_linear_forward(B, K, N, act):
     (256, 260, 1024, None),      # three column tiles, no activation below
 ])
 def test_linear_backward_dx_tc(B, K, N, act):
-    """rb200_linear_backward_dx_tc (split-K tcgen05) vs fp64 torch and vs the mma.sync kernel it
+    """rb200_linear_backward_dx_tc (split-K wgmma) vs fp64 torch and vs the mma.sync kernel it
     replaces for wide heads: out = (dz . W) * act'(h_prev)."""
     from reagent_b200 import _lib
 

@@ -1,4 +1,4 @@
-"""The packed weight-image layout of the tcgen05 TD kernel is written by two different kernels
+"""The packed weight-image layout of the wgmma TD kernel is written by two different kernels
 (dqn_tc_pack_kernel and the Adam kernel) and read by a third; this host-only program checks
 that their index maps agree (tests/csrc/tc_layout_check.cu, compiled with nvcc, run on the CPU)."""
 import os
