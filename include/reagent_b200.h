@@ -194,6 +194,24 @@ int rb200_dqn_td_step_tc(const rb200_mlp_t* q_net, const rb200_mlp_t* q_target,
                          int64_t pack_ws_bytes, int32_t weights_packed, void* stream);
 
 /* ------------------------------------------------------------------------- */
+/* Batch-constrained Q-learning filter (rb200_bcq.cu).  Replaces                 */
+/* get_valid_actions_from_imitator (reagent/training/imitator_training.py:12-25) */
+/* as used by DQNTrainer (dqn_trainer.py:206-220, 282-297) and the penalty of    */
+/* BatchConstrainedDQN.forward (reagent/models/bcq.py:26-35):                    */
+/*   r = softmax(logits) / max(softmax(logits)),  keep = r >= drop_threshold     */
+/* per row of imitator_logits [batch, num_actions], 1 <= num_actions <= 1024.    */
+/* Exactly one output mode:                                                       */
+/*   trainer: mask_out [B,A] = mask_in * keep   (mask_in [B,A] or NULL = ones;    */
+/*            q_in must be NULL)                                                  */
+/*   model:   q_out [B,A] = q_in + (-1e10) * (1 - keep)  (mask_in must be NULL;   */
+/*            q_out may equal q_in)                                               */
+/* Row-local, deterministic, no atomics, no allocation (graph-capturable).        */
+/* ------------------------------------------------------------------------- */
+int rb200_bcq_filter(const float* imitator_logits, int32_t batch, int32_t num_actions,
+                     float drop_threshold, const float* mask_in, float* mask_out,
+                     const float* q_in, float* q_out, void* stream);
+
+/* ------------------------------------------------------------------------- */
 /* CPE heads of the DQN step: DQNTrainerBaseLightning._calculate_cpes           */
 /* (reagent/training/dqn_trainer_base.py:332-452), masked_softmax                 */
 /* (reagent/core/torch_utils.py:62-73).  The reward network and the CPE q-network  */

@@ -287,6 +287,7 @@ def _declare(lib):
     lib.rb200_adam_soft_update.argtypes = [C.POINTER(AdamArgsT), _vp]
     lib.rb200_soft_update.argtypes = [_vp, _vp, C.c_int64, C.c_float, C.c_float, _vp]
     lib.rb200_cpe_heads.argtypes = [C.POINTER(CpeArgsT), _vp]
+    lib.rb200_bcq_filter.argtypes = [_vp, C.c_int32, C.c_int32, C.c_float, _vp, _vp, _vp, _vp, _vp]
     lib.rb200_pdqn_head.argtypes = [C.POINTER(PdqnArgsT), _vp]
     lib.rb200_c51_head.argtypes = [C.POINTER(C51ArgsT), _vp]
     lib.rb200_replay_add_device.argtypes = [C.POINTER(AddArgsT), _vp]

@@ -1,6 +1,7 @@
 from .arena import ParamArena, ScalarArena, arena_of  # noqa: F401
 from .actor import FullyConnectedActor, GaussianFullyConnectedActor  # noqa: F401
 from .base import ModelBase  # noqa: F401
+from .bcq import BatchConstrainedDQN  # noqa: F401
 from .categorical_dqn import CategoricalDQN  # noqa: F401
 from .critic import FullyConnectedCritic  # noqa: F401
 from .dqn import FullyConnectedDQN  # noqa: F401

@@ -4,6 +4,10 @@
   rb200_dqn_td_step   (K2+K2') TD target, loss, dZ chain        dqn_trainer.py:157-239
   rb200_mlp_wgrad     weight gradients (split-K partials)        autograd Linear backward
   rb200_adam_soft_update (K3)  Adam + Polyak                     optimizer.py:64-85, soft_update.py:47-71
+
+With `bcq=BCQConfig(...)` two launches run before K2: the imitator's fused forward on next_state
+(rb200_mlp_forward) and rb200_bcq_filter, whose filtered next-action mask K2 reads in place of
+the batch's (dqn_trainer.py:206-220).
 """
 from dataclasses import dataclass
 from typing import List, Optional
@@ -68,12 +72,36 @@ class DQNTrainer(DQNTrainerBaseLightning):
         self.q_network_optimizer = optimizer
         self._initialize_cpe(reward_network, q_network_cpe, q_network_cpe_target,
                              optimizer=optimizer)
+        # Batch constrained q-learning (dqn_trainer.py:112-117): the imitator is a frozen
+        # behaviour-policy network; it is in no optimizer and no soft update
         self.bcq = bcq is not None
         if self.bcq:
-            raise NotImplementedError("batch-constrained q-learning is out of scope of the fused path")
+            self._check_bcq_imitator(imitator)
+            self.bcq_drop_threshold = bcq.drop_threshold
+            self.bcq_imitator = imitator
         self._ws = None
         self.all_action_scores = None
+        self.bcq_next_actions_mask = None  # [B,A] mask the last TD step handed to K2 (BCQ)
         self._kernel_events = None  # bench hook: list collecting (start, end) events of K2
+
+    def _check_bcq_imitator(self, imitator) -> None:
+        from ..models.fully_connected_network import FullyConnectedNetwork
+
+        if imitator is None:
+            raise ValueError("bcq needs an imitator: the behaviour-policy network whose "
+                             "softmax decides which next actions stay possible")
+        if not isinstance(imitator, FullyConnectedNetwork):
+            raise NotImplementedError(
+                "the BCQ imitator must be a reagent_b200.models.FullyConnectedNetwork (its "
+                "forward runs on the fused MLP kernel); got " + type(imitator).__name__)
+        if imitator.layers[-1] != self.num_actions:
+            raise ValueError(f"the BCQ imitator has {imitator.layers[-1]} outputs, but there are "
+                             f"{self.num_actions} actions")
+        if not self.maxq_learning:
+            raise ValueError(
+                "bcq needs maxq_learning=True: the imitator filters the max over possible next "
+                "actions, and the reference DQNTrainer fails on every batch of BCQ with SARSA "
+                "(possible_actions_mask is unbound in train_step_gen)")
 
     # ------------------------------------------------------------------
     def configure_optimizers(self):
@@ -110,8 +138,42 @@ class DQNTrainer(DQNTrainerBaseLightning):
                 "loss": torch.zeros(1, device=device),
                 "counter": torch.zeros(1, dtype=torch.int32, device=device),
             }
+            if self.bcq:
+                ws["bcq_logits"] = torch.empty(B, self.num_actions, device=device)
+                ws["bcq_mask"] = torch.empty(B, self.num_actions, device=device)
             self._ws = ws
         return ws
+
+    def _bcq_filter(self, x: torch.Tensor, mask_in, logits, mask_out) -> torch.Tensor:
+        """mask_out = mask_in * (r >= drop_threshold), r = softmax(imitator(x)) / its row max
+        (imitator_training.py:12-25): the imitator's fused forward, then rb200_bcq_filter.
+        `x` is a contiguous fp32 [B,S] device tensor, `mask_in` a device pointer or None (ones)."""
+        im = self.bcq_imitator
+        if im.arena.flat.device != mask_out.device:
+            raise _lib.Rb200Error(f"DQNTrainer: the BCQ imitator lives on {im.arena.flat.device}, "
+                                  f"the batch on {mask_out.device} (call trainer.to(device))")
+        lib, st = _lib.lib(), _lib.cur_stream()
+        B = x.shape[0]
+        rc = lib.rb200_mlp_forward(im.arena.desc(), x.data_ptr(), x.shape[1], None, 0, B,
+                                   logits.data_ptr(), None, st)
+        _lib.check(rc, "rb200_mlp_forward(imitator)")
+        rc = lib.rb200_bcq_filter(logits.data_ptr(), B, self.num_actions,
+                                  float(self.bcq_drop_threshold), mask_in, mask_out.data_ptr(),
+                                  None, None, st)
+        _lib.check(rc, "rb200_bcq_filter")
+        return mask_out
+
+    def _cpe_next_mask(self, batch: rlt.DiscreteDqnInput) -> Optional[torch.Tensor]:
+        """The next-action mask the CPE head sees.  The reference filters with
+        `possible_next_actions_mask = batch.possible_next_actions_mask.float(); mask *= keep`
+        (dqn_trainer.py:206-216): that writes the batch tensor itself exactly when it already is
+        float32, and _calculate_cpes then reads the filtered mask.  This trainer never writes
+        the batch (the replay buffer hands every batch the same cached mask tensor), so it passes
+        the filtered mask explicitly in that case and leaves the batch mask otherwise."""
+        m = batch.possible_next_actions_mask
+        if self.bcq and self.maxq_learning and m is not None and m.dtype == torch.float32:
+            return self.bcq_next_actions_mask
+        return None
 
     _tc_prepacked = False  # set by a caller that already ran rb200_dqn_tc_pack (fused_step.py)
 
@@ -204,11 +266,16 @@ class DQNTrainer(DQNTrainerBaseLightning):
         a.batch = B
         a.state = P(state)
         a.next_state = P(batch.next_state.float_features)
+        next_state = keep[-1]  # the fp32 contiguous tensor handed to K2 (the imitator reads it too)
         a.action = P(batch.action)
         a.next_action = P(batch.next_action)
         a.reward = P(batch.reward.reshape(-1))
         a.not_terminal = P(batch.not_terminal.reshape(-1))
         a.possible_next_actions_mask = P(batch.possible_next_actions_mask)
+        if self.bcq and self.maxq_learning:  # the SARSA branch ignores BCQ (dqn_trainer.py:221-227)
+            self.bcq_next_actions_mask = self._bcq_filter(
+                next_state, a.possible_next_actions_mask, ws["bcq_logits"], ws["bcq_mask"])
+            a.possible_next_actions_mask = ws["bcq_mask"].data_ptr()
         a.discount_src = None
         a.discount_mode = _lib.DISCOUNT_CONST
         if self.use_seq_num_diff_as_time_diff:
@@ -273,7 +340,7 @@ class DQNTrainer(DQNTrainerBaseLightning):
         if self.calc_cpe_in_training:
             # evaluated here, after the q-network's optimizer step, like the reference's
             # generator (dqn_trainer.py:266-279)
-            cpe = self._calculate_cpes(training_batch)
+            cpe = self._calculate_cpes(training_batch, self._cpe_next_mask(training_batch))
             yield self.fused_loss(cpe[0])
             yield self.fused_loss(cpe[1])
         if self.has_real_reporter or self.logger:
@@ -298,7 +365,7 @@ class DQNTrainer(DQNTrainerBaseLightning):
         if packed:
             self._tc_images_state = self._tc_state()
         if self.calc_cpe_in_training:
-            cpe = self._calculate_cpes(training_batch)
+            cpe = self._calculate_cpes(training_batch, self._cpe_next_mask(training_batch))
             dp_fused_step(opts[1], self.reward_network.arena, process_group)
             dp_fused_step(opts[2], self.q_network_cpe.arena, process_group,
                           target=self.q_network_cpe_target.arena, tau=self.tau)
@@ -323,6 +390,10 @@ class DQNTrainer(DQNTrainerBaseLightning):
         rewards = self.boost_rewards(training_batch.reward, training_batch.action)
         mask = (training_batch.possible_actions_mask if self.maxq_learning
                 else training_batch.action)
+        if self.bcq and self.maxq_learning:  # dqn_trainer.py:287-291, without writing the batch
+            state, mask = _f32c(training_batch.state.float_features), _f32c(mask)
+            mask = self._bcq_filter(state, _lib.ptr(mask, state.device),
+                                    torch.empty_like(scores), torch.empty_like(scores))
         model_action_idxs = self.get_max_q_values(scores, mask.float())[1]
         extras = training_batch.extras
         self.reporter.log(

@@ -133,11 +133,14 @@ class DQNTrainerBaseLightning(DQNTrainerMixin, RLTrainerMixin, ReAgentLightningM
             self._cpe_ws = ws
         return ws
 
-    def _calculate_cpes(self, training_batch: rlt.DiscreteDqnInput):
+    def _calculate_cpes(self, training_batch: rlt.DiscreteDqnInput,
+                        next_actions_mask: Optional[torch.Tensor] = None):
         """_calculate_cpes (:332-452) on the device: returns the [2] loss tensor (reward loss,
         CPE q-value loss) and leaves the gradient partials of both networks in their arenas.
         Runs AFTER the q-network step of the same batch, as in the reference's generator
-        (all_next_action_scores is evaluated after `yield td_loss`, dqn_trainer.py:266-268)."""
+        (all_next_action_scores is evaluated after `yield td_loss`, dqn_trainer.py:266-268).
+        `next_actions_mask` replaces the batch's next-action mask of the model propensities
+        (DQNTrainer with BCQ passes its filtered mask)."""
         from .workspace import wgrad
 
         lib, st = _lib.lib(), _lib.cur_stream()
@@ -172,6 +175,8 @@ class DQNTrainerBaseLightning(DQNTrainerMixin, RLTrainerMixin, ReAgentLightningM
         a.next_scores = ws["next_scores"].data_ptr()
         mask = (training_batch.possible_next_actions_mask if self.maxq_learning
                 else training_batch.next_action)
+        if next_actions_mask is not None:
+            mask = next_actions_mask
         a.mask = P(mask)
         a.temperature = float(self.rl_temperature)
         a.action = P(training_batch.action)
