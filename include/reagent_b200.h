@@ -295,6 +295,25 @@ typedef struct rb200_c51_args {
 } rb200_c51_args_t;
 int rb200_c51_head(const rb200_c51_args_t* args, void* stream);
 
+/* Loss head of BehavioralCloningTrainer (rb200_heads.cu),                          */
+/* reagent/training/behavioral_cloning_trainer.py:38-66, one warp per row:           */
+/*   z = logits + (-1e10) * (1 - mask)   (FullyConnectedDQN.forward, models/dqn.py)  */
+/*   y = first arg max of the label row  (each row's own logged action)              */
+/*   loss = mean_b -log_softmax(z)[y],   dz = (softmax(z) - onehot(y)) / B            */
+/* 1 <= num_actions <= 1024.  dz NULL: loss only.  Deterministic (fixed-order mean),  */
+/* no allocation (graph-capturable).                                                  */
+typedef struct rb200_bc_xent_args {
+  int32_t batch, num_actions;
+  const float* logits;             /* [B,A] bc_net scores, unmasked */
+  const float* labels;             /* [B,A] one-hot logged action */
+  const float* mask;               /* [B,A] possible_actions_mask (1 = possible) */
+  float* dz;                       /* [B,A] d loss / d logits, or NULL */
+  float* loss_partials;            /* [ceil(B/8)] */
+  float* loss;                     /* [1] */
+  uint32_t* tile_counter;          /* [1] zero-initialised, self-resetting */
+} rb200_bc_xent_args_t;
+int rb200_bc_xent_head(const rb200_bc_xent_args_t* args, void* stream);
+
 /* ------------------------------------------------------------------------- */
 /* QR-DQN (reagent/training/qrdqn_trainer.py:108-194).  The [hidden -> A*N] head  */
 /* is too wide for a row tile, so it runs as 2-D tiled launches:                   */

@@ -175,6 +175,15 @@ class C51ArgsT(C.Structure):
                 ("tile_counter", _vp)]
 
 
+BC_ROWS_PER_BLOCK = 8  # rb200_bc_xent_head: loss_partials holds ceil(batch / 8) floats
+
+
+class BcXentArgsT(C.Structure):
+    _fields_ = [("batch", C.c_int32), ("num_actions", C.c_int32), ("logits", _vp),
+                ("labels", _vp), ("mask", _vp), ("dz", _vp), ("loss_partials", _vp),
+                ("loss", _vp), ("tile_counter", _vp)]
+
+
 class CpeArgsT(C.Structure):
     _fields_ = [("batch", C.c_int32), ("num_actions", C.c_int32), ("num_metrics", C.c_int32),
                 ("next_scores", _vp), ("mask", _vp), ("temperature", C.c_float), ("action", _vp),
@@ -290,6 +299,7 @@ def _declare(lib):
     lib.rb200_bcq_filter.argtypes = [_vp, C.c_int32, C.c_int32, C.c_float, _vp, _vp, _vp, _vp, _vp]
     lib.rb200_pdqn_head.argtypes = [C.POINTER(PdqnArgsT), _vp]
     lib.rb200_c51_head.argtypes = [C.POINTER(C51ArgsT), _vp]
+    lib.rb200_bc_xent_head.argtypes = [C.POINTER(BcXentArgsT), _vp]
     lib.rb200_replay_add_device.argtypes = [C.POINTER(AddArgsT), _vp]
     lib.rb200_sumtree_set_device.argtypes = [_vp, C.c_int32, _vp, _vp, C.c_int32, _vp, _vp, _vp]
     lib.rb200_per_draw_indices.argtypes = [C.POINTER(PerDrawArgsT), _vp]

@@ -179,3 +179,24 @@ class ParametricDqnInput(BaseInput):
             extras=batch.get("extras"),
             weight=batch.get("weight"),
         )
+
+
+@dataclass
+class BehavioralCloningModelInput(TensorDataClass):
+    """core/types.py:998-1015: states, the logged action as a one-hot row per state, and the
+    actions that were possible (1) or not (0)."""
+    state: FeatureData
+    action: torch.Tensor
+    possible_actions_mask: Optional[torch.Tensor] = None
+
+    @classmethod
+    def from_dict(cls, batch):
+        return cls(
+            state=FeatureData(float_features=batch["state"]),
+            action=batch["action"],
+            possible_actions_mask=batch.get("possible_actions_mask", None),
+        )
+
+    def batch_size(self):
+        assert self.state.float_features.ndim == 2
+        return self.state.float_features.size()[0]

@@ -18,12 +18,6 @@ namespace rb200 {
 
 constexpr int kBcqRowsPerBlock = 8;  // one warp per row
 
-__device__ __forceinline__ float warp_max(float v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
-  return v;
-}
-
 __global__ void __launch_bounds__(32 * kBcqRowsPerBlock)
 bcq_filter_kernel(const float* __restrict__ logits, int batch, int A, float thr,
                   const float* __restrict__ mask_in, float* __restrict__ mask_out,
@@ -33,12 +27,8 @@ bcq_filter_kernel(const float* __restrict__ logits, int batch, int A, float thr,
   if (row >= batch) return;  // whole warps leave together: no block-level barrier below
   const size_t base = (size_t)row * A;
   const float* x = logits + base;
-  float mx = -INFINITY;
-  for (int c = lane; c < A; c += 32) mx = fmaxf(mx, x[c]);
-  mx = warp_max(mx);
-  float sum = 0.f;
-  for (int c = lane; c < A; c += 32) sum = __fadd_rn(sum, expf(__fsub_rn(x[c], mx)));
-  sum = warp_sum(sum);  // xor butterfly: every lane ends with the same bits
+  float mx, sum;
+  warp_row_max_sumexp([x](int c) { return x[c]; }, A, mx, sum);
   float pmax = 0.f;
   for (int c = lane; c < A; c += 32) pmax = fmaxf(pmax, __fdiv_rn(expf(__fsub_rn(x[c], mx)), sum));
   pmax = warp_max(pmax);

@@ -94,6 +94,29 @@ __device__ __forceinline__ float warp_sum(float v) {
   return v;
 }
 
+__device__ __forceinline__ float warp_max(float v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
+  return v;
+}
+
+// First two passes of a softmax over one row held by one warp (lanes take c = lane, lane + 32,
+// ...), in torch's order: mx = max_c x(c), sum = sum_c exp(x(c) - mx).  `x` is a callable
+// returning element c.  Xor butterflies: every lane ends with the same bits.  The rounded
+// intrinsics keep the subtraction out of expf's FMA; c51_log_softmax lets the compiler fuse it
+// and keeps its own loop so that its results stay as they are.
+template <typename Row>
+__device__ __forceinline__ void warp_row_max_sumexp(const Row& x, int n, float& mx, float& sum) {
+  const int lane = threadIdx.x & 31;
+  float m = -INFINITY;
+  for (int c = lane; c < n; c += 32) m = fmaxf(m, x(c));
+  m = warp_max(m);
+  float s = 0.f;
+  for (int c = lane; c < n; c += 32) s = __fadd_rn(s, expf(__fsub_rn(x(c), m)));
+  mx = m;
+  sum = warp_sum(s);
+}
+
 // Dynamic shared-memory opt-in of a kernel, remembered PER DEVICE (the attribute is per device
 // and per function): a high-water mark indexed by the current device id, so the first launch on
 // a second GPU of the same process opts in as well.  Racing threads at worst set the attribute

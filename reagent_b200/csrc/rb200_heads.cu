@@ -10,6 +10,10 @@
 //       log-softmax over the atoms (reagent/models/categorical_dqn.py:33-35), expected values,
 //       masked arg max, target distribution, categorical projection onto the support (with the
 //       reference's l == u corner-case adjustment), cross-entropy loss and d loss / d logits.
+//   rb200_bc_xent_head  BehavioralCloningTrainer.train_step_gen / validation_step,
+//       reagent/training/behavioral_cloning_trainer.py:38-66: masked logits
+//       (reagent/models/dqn.py:55-63), mean cross entropy against each row's logged action and
+//       d loss / d logits.
 #include "rb200_common.cuh"
 
 namespace rb200 {
@@ -242,9 +246,101 @@ __global__ void __launch_bounds__(256) c51_head_kernel(const C51Dev d) {
   }
 }
 
+// ---------------------------------------------------------------------------
+// Behavioral cloning: one warp per row, lanes striding over the actions
+// ---------------------------------------------------------------------------
+constexpr int kBcRowsPerBlock = 8;
+
+__global__ void __launch_bounds__(32 * kBcRowsPerBlock) bc_xent_head_kernel(const rb200_bc_xent_args_t a) {
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int row = blockIdx.x * kBcRowsPerBlock + warp;
+  const int A = a.num_actions;
+  float le = 0.f;
+  if (row < a.batch) {  // whole warps: the block-level reduction below needs every thread
+    const size_t base = (size_t)row * A;
+    const float* x = a.logits + base;
+    const float* m = a.mask + base;
+    const float* lab = a.labels + base;
+    // z = scores + (-1e10) * (1 - mask), each operation rounded as torch does it
+    const auto z = [x, m](int c) { return __fadd_rn(x[c], __fmul_rn(-1e10f, __fsub_rn(1.f, m[c]))); };
+    // label = first maximal entry of the one-hot row (torch.argmax over dim 1)
+    float lv = -INFINITY;
+    int li = A;
+    for (int c = lane; c < A; c += 32) {
+      const float v = lab[c];
+      if (v > lv) { lv = v; li = c; }
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+      const float ov = __shfl_xor_sync(0xffffffffu, lv, o);
+      const int oi = __shfl_xor_sync(0xffffffffu, li, o);
+      if (ov > lv || (ov == lv && oi < li)) { lv = ov; li = oi; }
+    }
+    if (li >= A) li = 0;  // a row of NaN labels: torch.argmax would also give an arbitrary index
+    // log_softmax: (z - max) - log(sum exp(z - max)); row loss -log_softmax[label]
+    float mx, sum;
+    warp_row_max_sumexp(z, A, mx, sum);
+    const float lsum = logf(sum);
+    le = lane == 0 ? -__fsub_rn(__fsub_rn(z(li), mx), lsum) : 0.f;
+    if (a.dz) {  // (softmax - onehot) / B
+      const float invB = 1.f / (float)a.batch;
+      for (int c = lane; c < A; c += 32) {
+        const float p = expf(__fsub_rn(__fsub_rn(z(c), mx), lsum));
+        a.dz[base + c] = __fmul_rn(__fsub_rn(p, c == li ? 1.f : 0.f), invB);
+      }
+    }
+  }
+  // deterministic mean: per-block partial of the rows in warp order, then the last block to
+  // finish adds the partials in block order (pdqn_head_kernel's pattern)
+  __shared__ float s_l[kBcRowsPerBlock];
+  __shared__ bool s_last;
+  if (lane == 0) s_l[warp] = le;
+  __syncthreads();
+  if (tid == 0) {
+    float t = 0.f;
+    for (int w = 0; w < kBcRowsPerBlock; ++w) t += s_l[w];
+    a.loss_partials[blockIdx.x] = t;
+    __threadfence();
+    const unsigned fin = atomicAdd(a.tile_counter, 1u);
+    s_last = fin == gridDim.x - 1;
+  }
+  __syncthreads();
+  if (s_last) {
+    __threadfence();
+    float tot = 0.f;
+    for (unsigned i = tid; i < gridDim.x; i += blockDim.x) tot += ((volatile float*)a.loss_partials)[i];
+    tot = warp_sum(tot);
+    __syncthreads();
+    if (lane == 0) s_l[warp] = tot;
+    __syncthreads();
+    if (tid == 0) {
+      float t2 = 0.f;
+      for (int w = 0; w < kBcRowsPerBlock; ++w) t2 += s_l[w];
+      *a.loss = t2 / (float)a.batch;
+      *a.tile_counter = 0u;
+    }
+  }
+}
+
 }  // namespace rb200
 
 using namespace rb200;
+
+extern "C" int rb200_bc_xent_head(const rb200_bc_xent_args_t* a, void* stream) {
+  if (!a) { set_last_error("rb200_bc_xent_head: args is null"); return RB200_E_INVALID; }
+  if (a->batch <= 0 || a->num_actions < 1 || a->num_actions > 1024) {
+    set_last_error("rb200_bc_xent_head: need batch > 0 and 1 <= num_actions <= 1024 (got %d, %d)",
+                   a->batch, a->num_actions);
+    return RB200_E_INVALID;
+  }
+  if (!a->logits || !a->labels || !a->mask || !a->loss_partials || !a->loss || !a->tile_counter) {
+    set_last_error("rb200_bc_xent_head: required pointer is null");
+    return RB200_E_INVALID;
+  }
+  bc_xent_head_kernel<<<ceil_div(a->batch, kBcRowsPerBlock), 32 * kBcRowsPerBlock, 0,
+                        (cudaStream_t)stream>>>(*a);
+  return check_cuda(cudaGetLastError(), "bc_xent_head_kernel launch");
+}
 
 extern "C" int rb200_pdqn_head(const rb200_pdqn_args_t* a, void* stream) {
   if (!a || a->batch <= 0 || a->max_num_action < 0) { set_last_error("rb200_pdqn_head: bad argument"); return RB200_E_INVALID; }
