@@ -194,6 +194,7 @@ __global__ void grad_reduce_kernel(const float* __restrict__ gpart, int splits, 
 // (non-amsgrad, non-capturable):
 //   g   = sum_s grad[s] * grad_scale (+ wd * p)
 //   m   = lerp(m, g, 1-b1);  v = v*b2 + (1-b2)*g*g
+//   (the weight decay term and the lerp are fused multiply-adds, like ATen's)
 //   bc1 = 1 - b1^t, bc2 = 1 - b2^t (double), step_size = lr/bc1
 //   p  -= step_size * m / (sqrt(v)/sqrt(bc2) + eps)
 // then target = tau*p + (1-tau)*target  (SoftUpdate.step on the updated source).
@@ -239,6 +240,8 @@ __global__ void __launch_bounds__(256) adam_soft_kernel(const AdamDev d) {
   const float bc2_sqrt = s_bc2_sqrt;
   const float eps = (float)a.eps;
   const float w1 = (float)(1.0 - a.beta1);
+  const bool w1_small = fabsf(w1) < 0.5f;
+  const float w1m1 = w1 - 1.f;
   const float b2 = (float)a.beta2;
   const float w2 = (float)(1.0 - a.beta2);
   const float wd = (float)a.weight_decay;
@@ -310,9 +313,15 @@ __global__ void __launch_bounds__(256) adam_soft_kernel(const AdamDev d) {
     if (wd != 0.f) g = fmaf(wd, p, g);
     float m = a.exp_avg[i];
     float v = a.exp_avg_sq[i];
-    // rounding mirrors ATen's CPU kernels: lerp = fma(w, g-m, m); addcmul / addcdiv
-    // evaluate value*t1 first, each product/quotient rounded separately.
-    m = fmaf(w1, __fsub_rn(g, m), m);
+    // rounding mirrors ATen's CPU kernels:
+    //   lerp:    fma(w, g-m, m) for |w| < 0.5, else fma(w-1, g-m, g)  (at::lerp's two branches)
+    //   addcmul: self + (value*t1)*t2 with every product and the sum rounded separately.  ATen's
+    //            AVX2 / AVX-512 builds contract the last multiply-add into an fma; the two differ
+    //            by at most 1 ulp of exp_avg_sq per step, and this form is kept so that training
+    //            runs reproduce the library's earlier results exactly.
+    //   addcdiv: self + (value*t1)/t2, each product / quotient rounded separately
+    const float gm = __fsub_rn(g, m);
+    m = w1_small ? fmaf(w1, gm, m) : fmaf(w1m1, gm, g);
     v = __fadd_rn(__fmul_rn(v, b2), __fmul_rn(__fmul_rn(w2, g), g));
     const float denom = __fadd_rn(__fdiv_rn(__fsqrt_rn(v), bc2_sqrt), eps);
     p = __fadd_rn(p, __fdiv_rn(__fmul_rn(-step_size, m), denom));

@@ -15,6 +15,12 @@ from .. import _lib
 from ..models.arena import ParamArena, ScalarArena, arena_of
 
 
+_TORCH_FLAGS = dict(amsgrad=False, maximize=False, foreach=None, capturable=False,
+                    differentiable=False, fused=None, decoupled_weight_decay=False)
+# group flags of torch.optim.Adam that change the update rule; the kernel has none of them
+_UNSUPPORTED_FLAGS = ("amsgrad", "maximize", "decoupled_weight_decay")
+
+
 class FusedAdam(torch.optim.Optimizer):
     def __init__(self, params, lr=1e-3, betas=(0.9, 0.999), eps=1e-8, weight_decay=0.0,
                  amsgrad=False, maximize=False, **unused):
@@ -29,7 +35,9 @@ class FusedAdam(torch.optim.Optimizer):
         if not 0.0 <= betas[0] < 1.0 or not 0.0 <= betas[1] < 1.0:
             raise ValueError(f"Invalid beta parameters: {betas}")
         params = list(params)
-        defaults = dict(lr=lr, betas=betas, eps=eps, weight_decay=weight_decay)
+        # torch.optim.Adam's group keys, with the values this kernel implements, so that
+        # checkpoints move between the two optimizers in either direction
+        defaults = dict(lr=lr, betas=betas, eps=eps, weight_decay=weight_decay, **_TORCH_FLAGS)
         super().__init__(params, defaults)
         if len(self.param_groups) != 1:
             raise NotImplementedError("FusedAdam takes one parameter group (one network)")
@@ -170,6 +178,12 @@ class FusedAdam(torch.optim.Optimizer):
         return sd
 
     def load_state_dict(self, state_dict):
+        for group in state_dict.get("param_groups", []):
+            for k in _UNSUPPORTED_FLAGS:
+                if group.get(k, False):
+                    raise NotImplementedError(
+                        f"state dict has {k}=True, which has no fused kernel (reference default "
+                        "is False)")
         self._ensure_state()
         ps = self.param_groups[0]["params"]
         base = self.arena.flat.data_ptr()
