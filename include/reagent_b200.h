@@ -166,6 +166,7 @@ typedef struct rb200_dqn_args {
   float* loss_partials;          /* [>= ceil(B/16)]                */
   float* loss;                   /* [1] mean loss (written by the last tile)   */
   uint32_t* tile_counter;        /* [1] zero-initialised scratch, self-resetting */
+  const float* sample_weight;    /* [B] or NULL: loss = mean(w * loss_row), dZ row scaled by w */
 } rb200_dqn_args_t;
 
 int rb200_num_row_tiles(int batch, int max_dim_in, int max_dim_hidden);
@@ -594,8 +595,18 @@ int rb200_valid_index_build(const uint8_t* valid, int64_t capacity, int32_t* cou
 /*       DEVICE copy of CPython's MT19937 state (624 words + position, as                 */
 /*       random.getstate()[1] lays them out), the tree descents, and the sequential       */
 /*       non-stratified retries of invalid hits with the shared attempt budget.           */
+/*   rb200_per_weights        importance weights of drawn indices for prioritized replay:  */
+/*       w_i = (p_min / p_i) ** beta_t over their fp64 leaves p_i (p_min: smallest nonzero */
+/*       leaf of the batch; a zero leaf gets w = 0), beta_t = min(1, beta0 + (1 - beta0) * */
+/*       t / beta_updates) with t = *step (the optimizer's device step counter).  w_out    */
+/*       [n] fp32, w64_out [n] fp64 or NULL.                                               */
+/*   rb200_per_priority_update  TD-error priorities written back IN ORDER:                */
+/*       p_i = ((double)|q_selected_i - td_target_i| + eps) ** alpha -> p_out [n], then    */
+/*       SumTree.set(idx_i, p_i) for i = 0..n-1 as rb200_sumtree_set_device.  A priority   */
+/*       that is not finite applies none of them and sets status 3.                        */
 /* status words are sticky error flags the host wrapper turns into the reference's        */
-/* exceptions: 1 = "Max sample attempts", 2 = negative priority.                          */
+/* exceptions: 1 = "Max sample attempts", 2 = negative priority, 3 = non-finite PER       */
+/* priority (a non-finite TD error).                                                      */
 /* ------------------------------------------------------------------------- */
 typedef struct rb200_replay_dev {
   int64_t* state;             /* [4] device: add_count, transitions in the current episode,
@@ -617,6 +628,7 @@ typedef struct rb200_add_args {
   const double* priority_in;          /* [n] or NULL */
   int32_t n_rows;                     /* other keys: src = staging [n,row_bytes], dst = store */
   rb200_gather_spec_t rows[RB200_MAX_GATHER_SPECS];
+  int32_t priority_from_max;          /* 1: a NaN priority_in means *rb.max_priority (PER) */
 } rb200_add_args_t;
 
 typedef struct rb200_per_draw_args {
@@ -637,6 +649,13 @@ int rb200_replay_add_device(const rb200_add_args_t* args, void* stream);
 int rb200_sumtree_set_device(double* tree, int32_t depth, const int64_t* idx, const double* val,
                              int32_t n, double* max_recorded, int32_t* status, void* stream);
 int rb200_per_draw_indices(const rb200_per_draw_args_t* args, void* stream);
+int rb200_per_weights(const double* tree, int32_t depth, const int64_t* idx, int32_t n,
+                      const int64_t* step, double beta0, double beta_updates, float* w_out,
+                      double* w64_out, void* stream);
+int rb200_per_priority_update(double* tree, int32_t depth, const int64_t* idx,
+                              const float* td_target, const float* q_selected, int32_t n,
+                              double alpha, double eps, double* p_out, double* max_recorded,
+                              int32_t* status, void* stream);
 
 /* ------------------------------------------------------------------------- */
 /* Peer-memory plumbing of the fused data-parallel step (one process per GPU).  The    */

@@ -62,6 +62,7 @@ class DqnArgsT(C.Structure):
         ("loss_partials", _vp),
         ("loss", _vp),
         ("tile_counter", _vp),
+        ("sample_weight", _vp),
     ]
 
 
@@ -203,7 +204,7 @@ class ReplayDevT(C.Structure):
 class AddArgsT(C.Structure):
     _fields_ = [("rb", ReplayDevT), ("n", C.c_int32), ("terminal_in", _vp), ("reward_in", _vp),
                 ("priority_in", _vp), ("n_rows", C.c_int32),
-                ("rows", GatherSpecT * MAX_GATHER_SPECS)]
+                ("rows", GatherSpecT * MAX_GATHER_SPECS), ("priority_from_max", C.c_int32)]
 
 
 class PerDrawArgsT(C.Structure):
@@ -303,6 +304,10 @@ def _declare(lib):
     lib.rb200_replay_add_device.argtypes = [C.POINTER(AddArgsT), _vp]
     lib.rb200_sumtree_set_device.argtypes = [_vp, C.c_int32, _vp, _vp, C.c_int32, _vp, _vp, _vp]
     lib.rb200_per_draw_indices.argtypes = [C.POINTER(PerDrawArgsT), _vp]
+    lib.rb200_per_weights.argtypes = [_vp, C.c_int32, _vp, C.c_int32, _vp, C.c_double, C.c_double,
+                                      _vp, _vp, _vp]
+    lib.rb200_per_priority_update.argtypes = [_vp, C.c_int32, _vp, _vp, _vp, C.c_int32, C.c_double,
+                                              C.c_double, _vp, _vp, _vp, _vp]
     lib.rb200_adam_blocks.argtypes = [C.c_int64]
     lib.rb200_dp_alloc.argtypes = [C.c_int64, C.POINTER(_vp)]
     lib.rb200_dp_free.argtypes = [_vp]

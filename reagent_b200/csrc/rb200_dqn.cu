@@ -21,7 +21,9 @@ struct DqnDev {
   int ld_in, ld_h, ld_q;
 };
 
-template <int NT, int TM, int KC>
+// kWeighted: prioritized-replay importance weights (a.sample_weight), a separate instantiation so
+// that the unweighted kernels stay exactly as they are
+template <int NT, int TM, int KC, bool kWeighted>
 __global__ void __launch_bounds__(NT, 1)
 dqn_td_rows_kernel(const Mlp q, const Mlp qt, const DqnDev p) {
   constexpr int R = (NT / 64) * TM;
@@ -107,6 +109,11 @@ dqn_td_rows_kernel(const Mlp q, const Mlp qt, const DqnDev p) {
         le = d * d;
         g = 2.f * invB * d;
       }
+      if (kWeighted) {
+        const float w = a.sample_weight[row];
+        le *= w;
+        g *= w;
+      }
       if (a.q_selected) a.q_selected[row] = qsel;
       const int lact = q.act[L - 1];
       for (int c = 0; c < A4; ++c) {
@@ -146,7 +153,7 @@ dqn_td_rows_kernel(const Mlp q, const Mlp qt, const DqnDev p) {
 
 #define RB200_LAUNCH_DQN(NT_, TM_, KC_, grid, smem, stream, ...)                                   \
   do {                                                                                        \
-    auto kfn = dqn_td_rows_kernel<NT_, TM_, KC_>;                                                  \
+    auto kfn = dqn_td_rows_kernel<NT_, TM_, KC_, kWeighted>;                                       \
     static SmemOptIn optin_ = {};                                                             \
     {                                                                                         \
       cudaError_t e_ = ensure_dynamic_smem(kfn, optin_, (size_t)(smem));                      \
@@ -160,6 +167,13 @@ static RowsCfg dqn_cfg(const rb200_mlp_t* q, int batch, int* ld_q) {
   *ld_q = round_up4(A) + 4;
   // 1 input tile, 3 hidden tiles, 3 q tiles + 2 scalars per row
   return pick_rows_cfg(batch, q->dims[0], mlp_max_hidden(q), 1, 3, 3 * (*ld_q) + 2, 0);
+}
+
+template <bool kWeighted>
+static int launch_dqn_rows(const RowsCfg& cfg, int grid, cudaStream_t st, const Mlp& q,
+                           const Mlp& qt, const DqnDev& p) {
+  RB200_DISPATCH_ROWS(cfg, RB200_LAUNCH_DQN, grid, cfg.smem_bytes, st, q, qt, p);
+  return check_cuda(cudaGetLastError(), "dqn_td_rows_kernel launch");
 }
 
 }  // namespace rb200
@@ -197,8 +211,8 @@ extern "C" int rb200_dqn_td_step(const rb200_mlp_t* q_net, const rb200_mlp_t* q_
   const Mlp q = make_mlp(q_net), qt = make_mlp(q_target);
   const int grid = ceil_div(args->batch, rows_per_tile(cfg));
   cudaStream_t st = (cudaStream_t)stream;
-  RB200_DISPATCH_ROWS(cfg, RB200_LAUNCH_DQN, grid, cfg.smem_bytes, st, q, qt, p);
-  return check_cuda(cudaGetLastError(), "dqn_td_rows_kernel launch");
+  return args->sample_weight ? launch_dqn_rows<true>(cfg, grid, st, q, qt, p)
+                             : launch_dqn_rows<false>(cfg, grid, st, q, qt, p);
 }
 
 extern "C" int rb200_num_row_tiles(int batch, int max_dim_in, int max_dim_hidden) {

@@ -144,6 +144,9 @@ __global__ void __launch_bounds__(256) dqn_tc_pack_kernel(const PackDev p) {
 __device__ __noinline__ float act_fwd_slow(float x, int act) { return act_fwd(x, act); }
 __device__ __noinline__ float act_bwd_slow(float y, int act) { return act_bwd_from_out(y, act); }
 
+// kWeighted: prioritized-replay importance weights (a.sample_weight), a separate instantiation so
+// that the unweighted kernel stays exactly as it is
+template <bool kWeighted>
 __global__ void __launch_bounds__(kQThreads, 1)
 dqn_td_tc_kernel(const Mlp q, const Mlp qt, const QDev p) {
   extern __shared__ __align__(128) unsigned char smem_raw[];
@@ -500,6 +503,11 @@ dqn_td_tc_kernel(const Mlp q, const Mlp qt, const QDev p) {
           le = d * d;
           g = 2.f * invB * d;
         }
+        if (kWeighted) {
+          const float w = a.sample_weight[row];
+          le *= w;
+          g *= w;
+        }
         if (sub == 0) {
           if (a.td_target) a.td_target[row] = tgt;
           if (a.next_action_idx) a.next_action_idx[row] = bi;
@@ -757,13 +765,19 @@ extern "C" int rb200_dqn_td_step_tc(const rb200_mlp_t* q_net, const rb200_mlp_t*
   pl.dev.ws = *ws;
   pl.dev.pack = static_cast<const unsigned char*>(pack_ws);
   cudaStream_t st = (cudaStream_t)stream;
-  static SmemOptIn optin = {};  // per device; raised outside graph capture by the first eager call
+  // per device; raised outside graph capture by the first eager call
+  static SmemOptIn optin = {}, optin_w = {};
+  const bool weighted = args->sample_weight != nullptr;
   {
-    cudaError_t e = ensure_dynamic_smem(dqn_td_tc_kernel, optin, pl.smem_bytes);
+    cudaError_t e = weighted ? ensure_dynamic_smem(dqn_td_tc_kernel<true>, optin_w, pl.smem_bytes)
+                             : ensure_dynamic_smem(dqn_td_tc_kernel<false>, optin, pl.smem_bytes);
     if (e != cudaSuccess) return check_cuda(e, "cudaFuncSetAttribute(dqn_td_tc)");
   }
   const Mlp q = make_mlp(q_net), qt = make_mlp(q_target);
   const int grid = ceil_div(args->batch, kQR);
-  dqn_td_tc_kernel<<<grid, kQThreads, pl.smem_bytes, st>>>(q, qt, pl.dev);
+  if (weighted)
+    dqn_td_tc_kernel<true><<<grid, kQThreads, pl.smem_bytes, st>>>(q, qt, pl.dev);
+  else
+    dqn_td_tc_kernel<false><<<grid, kQThreads, pl.smem_bytes, st>>>(q, qt, pl.dev);
   return check_cuda(cudaGetLastError(), "dqn_td_tc_kernel launch");
 }

@@ -16,8 +16,8 @@
 //   sum_tree.py:113,152): state kept ON THE DEVICE in CPython's own layout (624 words +
 //   position), uploaded from / downloaded to `random.getstate()` by the host wrapper.
 //
-// All three kernels are single-CTA: the work is a few microseconds of latency-bound
-// sequential-semantics bookkeeping that runs on a side stream underneath the TD kernel.
+// The add and draw kernels are single-CTA: the work is a few microseconds of latency-bound
+// sequential-semantics bookkeeping.  The batched SumTree.set runs one CTA per tree level.
 #include "rb200_common.cuh"
 
 namespace rb200 {
@@ -201,8 +201,8 @@ __global__ void __launch_bounds__(kDrawThreads) per_draw_indices_kernel(const Dr
 }
 
 // ---------------------------------------------------------------------------
-// SumTree.set for a batch, applied IN ORDER (sum_tree.py:164-189): one warp, lane l owns level
-// l of the root path, so the per-node order of the fp64 additions is the reference's
+// SumTree.set of ONE transition (sum_tree.py:164-189) by one warp, for the add kernel: lane l
+// owns level l of the root path
 // ---------------------------------------------------------------------------
 __device__ __forceinline__ void tree_set_warp(double* tree, int depth, long long leaf, double value,
                                               double* max_recorded, int lane) {
@@ -220,13 +220,241 @@ __device__ __forceinline__ void tree_set_warp(double* tree, int depth, long long
   __syncwarp();
 }
 
-__global__ void sumtree_set_kernel(double* tree, int depth, const long long* idx, const double* val,
-                                   int n, double* max_recorded, int* status) {
-  const int lane = threadIdx.x;
-  for (int i = 0; i < n; ++i) {
-    const double v = val[i];
-    if (v < 0.0) { if (lane == 0 && status) status[0] = 2; return; }  // "values should be nonnegative"
-    tree_set_warp(tree, depth, idx[i], v, max_recorded, lane);
+// ---------------------------------------------------------------------------
+// SumTree.set for a batch, applied IN ORDER (sum_tree.py:164-189), bit-equal to the sequential
+// loop.  Set k adds delta_k = v_k - (its leaf before set k) to every node on its root path, so a
+// node's final value is its old value plus ITS deltas folded in k order.  Nodes are independent,
+// which regroups the work without reassociating any fp64 sum:
+//   deltas  sort the sets by (leaf, k); one thread folds each leaf's run in k order
+//   levels  one CTA per inner level sorts the sets by (node, k) and folds each node's run
+// The levels kernel reads the leaves and the leaf kernel then writes them (with max_recorded and
+// the status word): two launches per chunk of kSetChunk sets, chunks in order.  The critical path
+// is the root's fold, one dependent fp64 add per set.
+// ---------------------------------------------------------------------------
+constexpr int kSetThreads = 1024;
+constexpr int kSetKBits = 12;
+constexpr int kSetChunk = 1 << kSetKBits;
+constexpr int kSetPer = kSetChunk / kSetThreads;
+constexpr size_t kSetSmem = (size_t)kSetChunk * (sizeof(unsigned long long) + sizeof(double));
+
+struct SetSrc {
+  const long long* idx;      // [n] leaf of set i
+  const double* val;         // [n] the values (set_priority), or NULL: PER priorities
+  const float* td_target;    // [n]  p_i = ((double)|q_selected_i - td_target_i| + eps) ** alpha
+  const float* q_selected;   // [n]
+  double alpha, eps;
+  double* p_out;             // [n] or NULL: the values, written by the leaf kernel
+  int n;
+};
+
+__device__ __forceinline__ double set_value(const SetSrc& s, int i) {
+  if (s.val) return s.val[i];
+  return pow(__dadd_rn((double)fabsf(__fsub_rn(s.q_selected[i], s.td_target[i])), s.eps), s.alpha);
+}
+
+// How many sets apply: all, up to the first negative value (sum_tree.py raises there, after the
+// earlier sets), or none when a PER priority is not finite.  *code = the status it sets (0, 2, 3).
+__device__ int sets_applied(const SetSrc& s, int* code) {
+  __shared__ int s_neg, s_bad;
+  if (threadIdx.x == 0) { s_neg = s.n; s_bad = 0; }
+  __syncthreads();
+  int neg = s.n;
+  bool bad = false;
+  for (int i = threadIdx.x; i < s.n; i += blockDim.x) {
+    const double v = set_value(s, i);
+    if (v < 0.0 && i < neg) neg = i;
+    if (!s.val && !isfinite(v)) bad = true;
+  }
+  if (neg < s.n) atomicMin(&s_neg, neg);
+  if (bad) s_bad = 1;
+  __syncthreads();
+  *code = s_bad ? 3 : (s_neg < s.n ? 2 : 0);
+  return s_bad ? 0 : s_neg;
+}
+
+// ascending bitonic sort of key[0, m) by the whole CTA (m <= kSetChunk)
+__device__ void block_sort_u64(unsigned long long* key, int m) {
+  int np = 1;
+  while (np < m) np <<= 1;
+  for (int i = m + threadIdx.x; i < np; i += blockDim.x) key[i] = ~0ull;
+  __syncthreads();
+  for (int size = 2; size <= np; size <<= 1) {
+    for (int stride = size >> 1; stride > 0; stride >>= 1) {
+      for (int t = threadIdx.x; t < np / 2; t += blockDim.x) {
+        const int lo = 2 * t - (t & (stride - 1)), hi = lo + stride;
+        const unsigned long long x = key[lo], y = key[hi];
+        if ((x > y) == ((lo & size) == 0)) { key[lo] = y; key[hi] = x; }
+      }
+      __syncthreads();
+    }
+  }
+}
+
+// end of the run of sorted key[j] that shares its group (key >> kSetKBits): binary search
+__device__ __forceinline__ int run_end(const unsigned long long* key, int j, int m) {
+  const unsigned long long lim = ((key[j] >> kSetKBits) + 1) << kSetKBits;
+  int lo = j + 1, hi = m;
+  while (lo < hi) {
+    const int mid = (lo + hi) >> 1;
+    if (key[mid] < lim) lo = mid + 1; else hi = mid;
+  }
+  return lo;
+}
+
+// Sets [c0, c0 + m) of the chunk: vals[k] <- delta_k (k = i - c0), each leaf's run folded in k
+// order from its value in the tree; with write_leaves the leaves take their final values
+__device__ void chunk_deltas(const SetSrc& s, double* leaves, int c0, int m,
+                             unsigned long long* key, double* vals, bool write_leaves) {
+  for (int k = threadIdx.x; k < m; k += blockDim.x) {
+    vals[k] = set_value(s, c0 + k);
+    key[k] = ((unsigned long long)s.idx[c0 + k] << kSetKBits) | (unsigned long long)k;
+  }
+  block_sort_u64(key, m);
+  for (int j = threadIdx.x; j < m; j += blockDim.x) {
+    const unsigned long long leaf = key[j] >> kSetKBits;
+    if (j > 0 && (key[j - 1] >> kSetKBits) == leaf) continue;
+    const int e = run_end(key, j, m);
+    double cur = leaves[leaf];
+    for (int r = j; r < e; ++r) {
+      const int k = (int)(key[r] & (kSetChunk - 1));
+      const double d = __dadd_rn(vals[k], -cur);  // sum_tree.py: delta = value - leaf
+      vals[k] = d;
+      cur = __dadd_rn(cur, d);
+    }
+    if (write_leaves) leaves[leaf] = cur;
+  }
+  __syncthreads();
+}
+
+__global__ void __launch_bounds__(kSetThreads) sumtree_levels_kernel(double* tree, int depth,
+                                                                     const SetSrc s, int c0) {
+  extern __shared__ __align__(16) unsigned long long set_smem[];
+  unsigned long long* key = set_smem;
+  double* vals = reinterpret_cast<double*>(set_smem + kSetChunk);
+  int code;
+  const int m = min(kSetChunk, sets_applied(s, &code) - c0);
+  if (m <= 0) return;
+  chunk_deltas(s, tree + ((1ll << depth) - 1), c0, m, key, vals, false);
+  const int lvl = blockIdx.x, shift = depth - lvl;
+  for (int k = threadIdx.x; k < m; k += blockDim.x)
+    key[k] = ((unsigned long long)(s.idx[c0 + k] >> shift) << kSetKBits) | (unsigned long long)k;
+  block_sort_u64(key, m);
+  // deltas into sorted order (all reads before any write), so that each fold reads a contiguous run
+  double dv[kSetPer];
+#pragma unroll
+  for (int u = 0; u < kSetPer; ++u) {
+    const int j = threadIdx.x + u * kSetThreads;
+    if (j < m) dv[u] = vals[key[j] & (kSetChunk - 1)];
+  }
+  __syncthreads();
+#pragma unroll
+  for (int u = 0; u < kSetPer; ++u) {
+    const int j = threadIdx.x + u * kSetThreads;
+    if (j < m) vals[j] = dv[u];
+  }
+  __syncthreads();
+  double* level = tree + ((1ll << lvl) - 1);
+  for (int j = threadIdx.x; j < m; j += blockDim.x) {
+    const unsigned long long node = key[j] >> kSetKBits;
+    if (j > 0 && (key[j - 1] >> kSetKBits) == node) continue;
+    const int e = run_end(key, j, m);
+    double acc = level[node];
+#pragma unroll 8
+    for (int r = j; r < e; ++r) acc = __dadd_rn(acc, vals[r]);
+    level[node] = acc;
+  }
+}
+
+__global__ void __launch_bounds__(kSetThreads) sumtree_leaves_kernel(double* tree, int depth,
+                                                                     const SetSrc s, int c0,
+                                                                     double* max_recorded,
+                                                                     int* status) {
+  extern __shared__ __align__(16) unsigned long long set_smem[];
+  unsigned long long* key = set_smem;
+  double* vals = reinterpret_cast<double*>(set_smem + kSetChunk);
+  __shared__ double s_best[kSetThreads / 32];
+  __shared__ int s_bestk[kSetThreads / 32];
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  int code;
+  const int applied = sets_applied(s, &code);
+  const int c1 = min(c0 + kSetChunk, s.n);
+  if (s.p_out)
+    for (int i = c0 + tid; i < c1; i += blockDim.x) s.p_out[i] = set_value(s, i);
+  if (c0 == 0 && code && status && tid == 0) status[0] = code;
+  const int m = min(kSetChunk, applied - c0);
+  if (m <= 0) return;
+  if (max_recorded) {
+    // the sequential "if value > max_recorded" keeps the FIRST set holding the largest value
+    double best = -INFINITY;
+    int bk = 0x7fffffff;
+    for (int k = tid; k < m; k += blockDim.x) {
+      const double v = set_value(s, c0 + k);
+      if (v > best) { best = v; bk = k; }
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+      const double ob = __shfl_xor_sync(0xffffffffu, best, o);
+      const int ok = __shfl_xor_sync(0xffffffffu, bk, o);
+      if (ok != 0x7fffffff && (bk == 0x7fffffff || ob > best || (ob == best && ok < bk))) { best = ob; bk = ok; }
+    }
+    if (lane == 0) { s_best[warp] = best; s_bestk[warp] = bk; }
+    __syncthreads();
+    if (tid == 0) {
+      for (int w = 1; w < kSetThreads / 32; ++w) {
+        const double ob = s_best[w];
+        const int ok = s_bestk[w];
+        if (ok != 0x7fffffff && (bk == 0x7fffffff || ob > best || (ob == best && ok < bk))) { best = ob; bk = ok; }
+      }
+      if (bk != 0x7fffffff && best > *max_recorded) *max_recorded = best;
+    }
+  }
+  chunk_deltas(s, tree + ((1ll << depth) - 1), c0, m, key, vals, true);
+}
+
+static int sumtree_update(double* tree, int depth, const SetSrc& s, double* max_recorded,
+                          int* status, cudaStream_t st) {
+  static SmemOptIn optin_levels = {}, optin_leaves = {};
+  cudaError_t e = ensure_dynamic_smem(sumtree_levels_kernel, optin_levels, kSetSmem);
+  if (e == cudaSuccess) e = ensure_dynamic_smem(sumtree_leaves_kernel, optin_leaves, kSetSmem);
+  if (e != cudaSuccess) return check_cuda(e, "cudaFuncSetAttribute(sumtree)");
+  for (int c0 = 0; c0 < s.n; c0 += kSetChunk) {
+    if (depth > 0) sumtree_levels_kernel<<<depth, kSetThreads, kSetSmem, st>>>(tree, depth, s, c0);
+    sumtree_leaves_kernel<<<1, kSetThreads, kSetSmem, st>>>(tree, depth, s, c0, max_recorded, status);
+  }
+  return check_cuda(cudaGetLastError(), "sumtree update launch");
+}
+
+// ---------------------------------------------------------------------------
+// PER importance weights (Schaul et al. 2016, normalised by the batch maximum as in Dopamine):
+// w_i = (p_min / p_i) ** beta_t over the drawn leaves p_i; a zero leaf gets weight 0 and no say
+// in p_min.  beta_t = min(1, beta0 + (1 - beta0) * t / beta_updates), t = *step.
+// ---------------------------------------------------------------------------
+constexpr int kWeightThreads = 1024;
+
+__global__ void __launch_bounds__(kWeightThreads) per_weights_kernel(
+    const double* tree, int depth, const long long* idx, int n, const long long* step,
+    double beta0, double beta_updates, float* w, double* w64) {
+  __shared__ double s_min[kWeightThreads / 32];
+  const double* leaves = tree + ((1ll << depth) - 1);
+  const int tid = threadIdx.x;
+  double mn = INFINITY;
+  for (int i = tid; i < n; i += kWeightThreads) {
+    const double p = leaves[idx[i]];
+    if (p > 0.0) mn = fmin(mn, p);
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) mn = fmin(mn, __shfl_xor_sync(0xffffffffu, mn, o));
+  if ((tid & 31) == 0) s_min[tid >> 5] = mn;
+  __syncthreads();
+  mn = s_min[0];
+  for (int k = 1; k < kWeightThreads / 32; ++k) mn = fmin(mn, s_min[k]);
+  const double t = (double)*step;
+  const double beta = fmin(1.0, __dadd_rn(beta0, __ddiv_rn(__dmul_rn(__dadd_rn(1.0, -beta0), t), beta_updates)));
+  for (int i = tid; i < n; i += kWeightThreads) {
+    const double p = leaves[idx[i]];
+    const double wi = p > 0.0 ? pow(__ddiv_rn(mn, p), beta) : 0.0;
+    w[i] = (float)wi;
+    if (w64) w64[i] = wi;
   }
 }
 
@@ -276,7 +504,10 @@ __global__ void __launch_bounds__(256) replay_add_kernel(const AddDev d) {
   // priorities: prioritized_replay_buffer.py:76-84 -> SumTree.set(cursor, priority), in order
   if (warp == 0 && rb.tree && a.priority_in) {
     for (int t = 0; t < a.n; ++t) {
-      const double v = a.priority_in[t];
+      double v = a.priority_in[t];
+      // Schaul et al.'s rule for a transition without a priority: the largest one recorded so
+      // far, read here, after the sets of the earlier transitions of this call
+      if (a.priority_from_max && isnan(v)) v = *rb.max_priority;
       if (v < 0.0) { if (lane == 0) rb.state[3] = 2; break; }
       tree_set_warp(rb.tree, rb.tree_depth, s_cur[t], v, rb.max_priority, lane);
     }
@@ -318,9 +549,38 @@ extern "C" int rb200_sumtree_set_device(double* tree, int32_t depth, const int64
                                         int32_t* status, void* stream) {
   if (!tree || !idx || !val || depth < 0 || depth > 31 || n < 0) { set_last_error("rb200_sumtree_set_device: bad argument"); return RB200_E_INVALID; }
   if (n == 0) return RB200_OK;
-  sumtree_set_kernel<<<1, 32, 0, (cudaStream_t)stream>>>(tree, depth, (const long long*)idx, val, n,
-                                                         max_recorded, status);
-  return check_cuda(cudaGetLastError(), "sumtree_set_kernel launch");
+  SetSrc s = {};
+  s.idx = (const long long*)idx;
+  s.val = val;
+  s.n = n;
+  return sumtree_update(tree, depth, s, max_recorded, status, (cudaStream_t)stream);
+}
+
+extern "C" int rb200_per_priority_update(double* tree, int32_t depth, const int64_t* idx,
+                                         const float* td_target, const float* q_selected,
+                                         int32_t n, double alpha, double eps, double* p_out,
+                                         double* max_recorded, int32_t* status, void* stream) {
+  if (!tree || !idx || !td_target || !q_selected || !p_out || !status) { set_last_error("rb200_per_priority_update: null argument"); return RB200_E_INVALID; }
+  if (depth < 0 || depth > 31 || n <= 0) { set_last_error("rb200_per_priority_update: bad depth/n"); return RB200_E_INVALID; }
+  SetSrc s = {};
+  s.idx = (const long long*)idx;
+  s.td_target = td_target;
+  s.q_selected = q_selected;
+  s.alpha = alpha;
+  s.eps = eps;
+  s.p_out = p_out;
+  s.n = n;
+  return sumtree_update(tree, depth, s, max_recorded, status, (cudaStream_t)stream);
+}
+
+extern "C" int rb200_per_weights(const double* tree, int32_t depth, const int64_t* idx, int32_t n,
+                                 const int64_t* step, double beta0, double beta_updates,
+                                 float* w_out, double* w64_out, void* stream) {
+  if (!tree || !idx || !step || !w_out) { set_last_error("rb200_per_weights: null argument"); return RB200_E_INVALID; }
+  if (depth < 0 || depth > 31 || n <= 0 || !(beta_updates > 0.0)) { set_last_error("rb200_per_weights: bad depth/n/beta_updates"); return RB200_E_INVALID; }
+  per_weights_kernel<<<1, kWeightThreads, 0, (cudaStream_t)stream>>>(
+      tree, depth, (const long long*)idx, n, (const long long*)step, beta0, beta_updates, w_out, w64_out);
+  return check_cuda(cudaGetLastError(), "per_weights_kernel launch");
 }
 
 extern "C" int rb200_replay_add_device(const rb200_add_args_t* a, void* stream) {
@@ -330,6 +590,7 @@ extern "C" int rb200_replay_add_device(const rb200_add_args_t* a, void* stream) 
   if (a->n <= 0 || a->n > kAddMax) { set_last_error("rb200_replay_add_device: n must be in [1, %d]", kAddMax); return RB200_E_INVALID; }
   if (a->rb.capacity <= 0 || a->rb.update_horizon <= 0 || a->n_rows < 0 || a->n_rows > RB200_MAX_GATHER_SPECS) { set_last_error("rb200_replay_add_device: bad capacity/horizon/rows"); return RB200_E_INVALID; }
   if (a->rb.tree && (a->rb.tree_depth < 0 || a->rb.tree_depth > 31)) { set_last_error("rb200_replay_add_device: bad tree depth"); return RB200_E_INVALID; }
+  if (a->priority_from_max && (!a->rb.tree || !a->rb.max_priority)) { set_last_error("rb200_replay_add_device: priority_from_max needs the tree and max_priority"); return RB200_E_INVALID; }
   AddDev d;
   d.a = *a;
   replay_add_kernel<<<1, 256, 0, (cudaStream_t)stream>>>(d);

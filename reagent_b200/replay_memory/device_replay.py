@@ -16,7 +16,9 @@ the whole step in one CUDA graph).  `sync_to_host()` brings the host mirrors (an
 `random` state) back, after which the buffer's ordinary host-side API continues the same
 streams bit for bit.
 """
+import math
 import random
+from dataclasses import dataclass
 from typing import Dict, Optional
 
 import numpy as np
@@ -25,6 +27,28 @@ import torch
 from .. import _lib
 
 MAX_ADD = 1024  # transitions per rb200_replay_add_device launch
+
+
+@dataclass(frozen=True)
+class PrioritizedUpdate:
+    """Prioritized experience replay (Schaul et al. 2016) for FusedDqnStep: after each update the
+    drawn transitions get p_i = (|TD error_i| + eps) ** alpha, and the update is weighted by
+    w_i = (p_min / p_i) ** beta_t (p over the drawn leaves, p_min their smallest nonzero one),
+    beta_t = min(1, beta0 + (1 - beta0) * t / beta_updates) with t the optimizer's step count."""
+    alpha: float = 0.6
+    beta0: float = 0.4
+    beta_updates: int = 100_000
+    eps: float = 1e-6
+
+    def __post_init__(self):
+        if not (math.isfinite(self.alpha) and self.alpha >= 0.0):
+            raise ValueError(f"alpha must be finite and >= 0, got {self.alpha}")
+        if not (math.isfinite(self.eps) and self.eps >= 0.0):
+            raise ValueError(f"eps must be finite and >= 0, got {self.eps}")
+        if not 0.0 <= self.beta0 <= 1.0:
+            raise ValueError(f"beta0 must lie in [0, 1], got {self.beta0}")
+        if not (math.isfinite(self.beta_updates) and self.beta_updates > 0):
+            raise ValueError(f"beta_updates must be positive, got {self.beta_updates}")
 
 
 class DeviceReplay:
@@ -94,15 +118,21 @@ class DeviceReplay:
             d.max_priority = self.max_priority.data_ptr()
         return d
 
-    def stage(self, row: int, slot: int = 0, **transition):
-        """Write one transition into row `row` of staging block `slot` (host only)."""
+    def stage(self, row: int, slot: int = 0, priority_from_max: bool = False, **transition):
+        """Write one transition into row `row` of staging block `slot` (host only).  With
+        `priority_from_max` (prioritized replay) a transition without `priority` is staged as NaN,
+        which an add launched with `priority_from_max` replaces by the largest priority recorded
+        so far, read on the device when it is inserted."""
         views = self.host_np[slot]
+        if priority_from_max and "priority" not in transition:
+            views["priority"][row] = np.nan
         for k, v in transition.items():
             views[k][row] = v
 
-    def launch_add(self, n: int, slot: int = 0):
+    def launch_add(self, n: int, slot: int = 0, priority_from_max: bool = False):
         """ONE host->device copy of staging block `slot` + the add kernel for its first `n`
-        rows, on the current stream (graph-capturable: fixed pinned / device addresses)."""
+        rows, on the current stream (graph-capturable: fixed pinned / device addresses).
+        `priority_from_max`: a NaN staged priority means the largest one recorded so far."""
         assert 1 <= n <= min(self.stage_rows, MAX_ADD) and 0 <= slot < self.stage_slots
         self.dev_raw[slot].copy_(self.host_raw[slot], non_blocking=True)
         base = self.dev_raw[slot].data_ptr()
@@ -119,6 +149,7 @@ class DeviceReplay:
             a.rows[j].row_bytes = md.row_bytes
             a.rows[j].which = 0
         a.n_rows = len(self._keys)
+        a.priority_from_max = int(bool(priority_from_max))
         _lib.check(_lib.lib().rb200_replay_add_device(a, _lib.cur_stream()), "rb200_replay_add_device")
         self.rb._valid_index_stale = True
 
@@ -155,6 +186,30 @@ class DeviceReplay:
             idx.numel(), self.max_priority.data_ptr(), self.status.data_ptr(), _lib.cur_stream())
         _lib.check(rc, "rb200_sumtree_set_device")
         self._keep = (idx, val)
+
+    def importance_weights(self, indices: torch.Tensor, step: torch.Tensor, per: PrioritizedUpdate,
+                           out: torch.Tensor, out64: Optional[torch.Tensor] = None):
+        """PER importance weights of the drawn `indices` from the current leaves (fp32 `out`,
+        optionally fp64 `out64`); `step` is the optimizer's int64 device step counter."""
+        rc = _lib.lib().rb200_per_weights(
+            self.tree.data_ptr(), self.rb.sum_tree.depth, indices.data_ptr(), indices.numel(),
+            step.data_ptr(), float(per.beta0), float(per.beta_updates), out.data_ptr(),
+            None if out64 is None else out64.data_ptr(), _lib.cur_stream())
+        _lib.check(rc, "rb200_per_weights")
+        return out
+
+    def write_back_priorities(self, indices: torch.Tensor, td_target: torch.Tensor,
+                              q_selected: torch.Tensor, per: PrioritizedUpdate,
+                              p_out: torch.Tensor):
+        """set_priority(indices, (|q_selected - td_target| + eps) ** alpha), in batch order; the
+        priorities also go to `p_out` (fp64).  A non-finite one applies none (status 3)."""
+        rc = _lib.lib().rb200_per_priority_update(
+            self.tree.data_ptr(), self.rb.sum_tree.depth, indices.data_ptr(), td_target.data_ptr(),
+            q_selected.data_ptr(), indices.numel(), float(per.alpha), float(per.eps),
+            p_out.data_ptr(), self.max_priority.data_ptr(), self.status.data_ptr(),
+            _lib.cur_stream())
+        _lib.check(rc, "rb200_per_priority_update")
+        return p_out
 
     # ---- index selection ---------------------------------------------------------------
     def upload_host_rng(self):
@@ -210,6 +265,10 @@ class DeviceReplay:
                 "for every stratum.".format(self.rb._max_sample_attempts))
         if code == 2:
             raise ValueError("Sum tree values should be nonnegative.")
+        if code == 3:
+            raise FloatingPointError(
+                "prioritized replay: a TD error was not finite, so its priority could not be "
+                "written back (no priority of that update was applied)")
 
     def sync_to_host(self):
         """Bring the host-side mirrors (counters, validity, terminal flags, sum tree, Python's

@@ -246,8 +246,10 @@ class DQNTrainer(DQNTrainerBaseLightning):
         self._tc_prepacked = True
         return True
 
-    def _td_step(self, batch: rlt.DiscreteDqnInput, do_backward: bool = True) -> torch.Tensor:
-        """Fused TD target + loss (+ backward).  Returns the device loss scalar (shape [])."""
+    def _td_step(self, batch: rlt.DiscreteDqnInput, do_backward: bool = True,
+                 sample_weight: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """Fused TD target + loss (+ backward).  Returns the device loss scalar (shape []).
+        `sample_weight`: [B] fp32 importance weights (loss = mean(w * loss_row), dZ row * w)."""
         state = _f32c(batch.state.float_features)
         if not state.is_cuda:
             raise _lib.Rb200Error(
@@ -299,6 +301,11 @@ class DQNTrainer(DQNTrainerBaseLightning):
         a.loss_partials = ws["loss_partials"].data_ptr()
         a.loss = ws["loss"].data_ptr()
         a.tile_counter = ws["counter"].data_ptr()
+        if sample_weight is not None:
+            if sample_weight.dtype != torch.float32 or sample_weight.shape != (B,):
+                raise ValueError(f"importance_weights must be a [{B}] float32 tensor, got "
+                                 f"{sample_weight.dtype} {tuple(sample_weight.shape)}")
+            a.sample_weight = P(sample_weight)
         self.q_network.arena.refresh()          # no-op for plain MLPs; folds a dueling head
         self.q_network_target.arena.refresh()
         qd, qtd = self.q_network.arena.desc(), self.q_network_target.arena.desc()
@@ -348,15 +355,18 @@ class DQNTrainer(DQNTrainerBaseLightning):
         yield self.soft_update_result()
 
     def train_batch(self, training_batch: rlt.DiscreteDqnInput, batch_idx: int = 0,
-                    process_group=None):
+                    process_group=None, importance_weights: Optional[torch.Tensor] = None):
         """Fast path: one full update in 3 launches, Polyak fused into the Adam kernel.
         Same arithmetic as driving train_step_gen with reagent_b200.training.loop.
+        `importance_weights` ([B] fp32 on the batch's device, prioritized replay): the TD loss
+        becomes mean_i(w_i * loss_i) and row i of dZ is scaled by w_i; the CPE losses stay
+        unweighted.
         With `process_group` (data parallel, one rank per GPU, equal shards): the flat
         gradient is summed over ranks and scaled by 1/world before Adam (every loss is a batch
         mean, SURVEY.md 8e) -- inside the Adam kernel over NVLink peer memory when
         data_parallel.enable_p2p(group) was called, else by ONE NCCL all-reduce."""
         opts = self.optimizers()
-        self._td_step(training_batch)
+        self._td_step(training_batch, sample_weight=importance_weights)
         tcp = self._tc_pack_in_adam() if self._last_td_call[-1] is not None else None
         from .data_parallel import dp_fused_step
 

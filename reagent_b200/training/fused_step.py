@@ -21,13 +21,14 @@ import numpy as np
 import torch
 
 from .. import _lib
+from ..replay_memory.device_replay import PrioritizedUpdate
 from ..replay_memory.prioritized_replay_buffer import PrioritizedReplayBuffer
 
 
 class FusedDqnStep:
     def __init__(self, trainer, replay_buffer, batch_size: int, process_group=None,
                  slots: int = 2, prefetch: bool = False, shard=None, rng: str = "host",
-                 online: bool = False):
+                 online: bool = False, per: Optional[PrioritizedUpdate] = None):
         """`shard = (rank, world)`: data-parallel strong scaling (SURVEY.md 8e).  `batch_size`
         is the GLOBAL minibatch; the replay buffer is replicated and every rank consumes the
         identical random stream, so all ranks select the same global indices, and this
@@ -40,7 +41,26 @@ class FusedDqnStep:
         `online=True` (needs rng="device"): `step(transition)` also ADDS one transition before
         drawing, the reference's online loop (reagent/gym/runners/gymrunner.py: one env step
         -> replay_buffer.add -> one update); the transition is the step's only host->device
-        traffic, staged in pinned memory and copied + inserted by the same graph replay."""
+        traffic, staged in pinned memory and copied + inserted by the same graph replay.
+        `per=PrioritizedUpdate(...)` (needs rng="device", prefetch=False): prioritized
+        experience replay.  Each update weights its TD loss by the importance weights of the
+        drawn rows and then writes their TD-error priorities back into the device tree, in
+        batch order, inside the same graph; the next draw sees them.  Online, a transition
+        staged without `priority` enters with the largest priority recorded so far."""
+        if per is not None:
+            from .dqn_trainer import DQNTrainer
+
+            if rng != "device":
+                raise ValueError("per needs rng='device': the priorities live in the device tree")
+            if prefetch:
+                raise ValueError("per needs prefetch=False: a prefetched draw would run before "
+                                 "the previous update's priority write-back")
+            if shard is not None or process_group is not None:
+                raise NotImplementedError("per is single-GPU: data-parallel write-back would need "
+                                          "every rank's TD errors")
+            if type(trainer) is not DQNTrainer:
+                raise NotImplementedError("per covers DQNTrainer; got " + type(trainer).__name__)
+        self.per = per
         if rng not in ("host", "device"):
             raise ValueError("rng must be 'host' or 'device'")
         if online and rng != "device":
@@ -84,6 +104,9 @@ class FusedDqnStep:
             self._status_np = self._status_host.numpy()
             self.h2d_bytes = self.dr.h2d_bytes_per_add if self.online else 0
             self.d2h_bytes = 4 + 8
+            if per is not None:
+                self.weights = torch.empty(self.B, dtype=torch.float32, device=self.dev)
+                self.priorities = torch.empty(self.B, dtype=torch.float64, device=self.dev)
         # warm-up outside capture (lazy allocations, cudaFuncSetAttribute, optimizer state)
         self._one_update(None)
         torch.cuda.synchronize()
@@ -140,7 +163,20 @@ class FusedDqnStep:
         batch = self._sample(rnd_dev)
         if forked:
             main.wait_stream(self._side)
+        if self.per is not None:
+            return self._per_train(batch)
         return self.trainer.train_batch(batch, process_group=self.pg)
+
+    def _per_train(self, batch):
+        """Importance weights of the drawn rows -> weighted update -> priority write-back."""
+        idx = self._idx_buf[0]
+        opt = self.trainer.optimizers()[0]
+        opt._ensure_state()
+        self.dr.importance_weights(idx, opt.step_t, self.per, self.weights)
+        loss = self.trainer.train_batch(batch, importance_weights=self.weights)
+        ws = self.trainer._ws
+        self.dr.write_back_priorities(idx, ws["td_target"], ws["q_sel"], self.per, self.priorities)
+        return loss
 
     def _prefetch_update(self, i, rnd_dev, overrides=None):
         """Update on batch set i; the sampler fills set 1-i concurrently (second stream)."""
@@ -218,8 +254,12 @@ class FusedDqnStep:
                 loss = self._prefetch_update(i, marker)
             else:
                 if self.online:
-                    self.dr.launch_add(1, slot=i)
-                loss = self.trainer.train_batch(self._device_sample(0, False), process_group=self.pg)
+                    self.dr.launch_add(1, slot=i, priority_from_max=self.per is not None)
+                batch = self._device_sample(0, False)
+                if self.per is not None:
+                    loss = self._per_train(batch)
+                else:
+                    loss = self.trainer.train_batch(batch, process_group=self.pg)
             loss_host.copy_(loss.reshape(1), non_blocking=True)
             self._status_host.copy_(self.dr.status, non_blocking=True)
         return {"graph": g, "loss_host": loss_host, "done": torch.cuda.Event(), "used": False}
@@ -258,7 +298,8 @@ class FusedDqnStep:
                     raise ValueError("online FusedDqnStep.step() needs the new transition")
                 # every slot's graph copies from its own pinned staging row; the slot's previous
                 # replay (and with it that H2D copy) was waited for above
-                self.dr.stage(0, (self.k - 1) % len(self.slots), **transition)
+                self.dr.stage(0, (self.k - 1) % len(self.slots),
+                              priority_from_max=self.per is not None, **transition)
             s["graph"].replay()
             s["done"].record()
             s["used"] = True
