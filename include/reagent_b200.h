@@ -290,9 +290,10 @@ typedef struct rb200_c51_args {
   float* dz_logits;                /* [B, A*N] */
   float* all_q_values;             /* [B,A] or NULL */
   int32_t* next_action_idx;        /* [B] or NULL */
-  float* loss_partials;            /* [B] */
+  float* loss_partials;            /* [B] per-row cross entropy, unweighted */
   float* loss;                     /* [1] */
   uint32_t* tile_counter;
+  const float* sample_weight;      /* [B] or NULL: loss = mean(w * loss_row), dz_logits row scaled by w */
 } rb200_c51_args_t;
 int rb200_c51_head(const rb200_c51_args_t* args, void* stream);
 
@@ -342,9 +343,10 @@ typedef struct rb200_qrdqn_args {
   float* dz_head;              /* [B, A*N] d loss / d head output */
   float* all_q_values;         /* [B, A] mean over atoms of q(s), or NULL */
   int32_t* next_action_idx;    /* [B] or NULL */
-  float* loss_partials;        /* [B] */
+  float* loss_partials;        /* [B] per-row quantile-Huber sum over the N*N pairs, unweighted */
   float* loss;                 /* [1] */
   uint32_t* tile_counter;      /* [1] zero-initialised, self-resetting */
+  const float* sample_weight;  /* [B] or NULL: loss = mean(w * loss_row), dz_head row scaled by w */
 } rb200_qrdqn_args_t;
 
 int rb200_linear_forward(const float* W, const float* b, int32_t act, int32_t K, int32_t N,
@@ -604,9 +606,13 @@ int rb200_valid_index_build(const uint8_t* valid, int64_t capacity, int32_t* cou
 /*       p_i = ((double)|q_selected_i - td_target_i| + eps) ** alpha -> p_out [n], then    */
 /*       SumTree.set(idx_i, p_i) for i = 0..n-1 as rb200_sumtree_set_device.  A priority   */
 /*       that is not finite applies none of them and sets status 3.                        */
+/*   rb200_per_priority_update_rows  the same write-back from per-row losses (the         */
+/*       distributional heads, which have no scalar TD error):                             */
+/*       p_i = ((double)|row_loss_i| / divisor + eps) ** alpha, divisor > 0 and finite      */
+/*       (N*N for the QR-DQN head's loss_partials, 1 for C51's).                           */
 /* status words are sticky error flags the host wrapper turns into the reference's        */
 /* exceptions: 1 = "Max sample attempts", 2 = negative priority, 3 = non-finite PER       */
-/* priority (a non-finite TD error).                                                      */
+/* priority (a non-finite TD error or row loss).                                          */
 /* ------------------------------------------------------------------------- */
 typedef struct rb200_replay_dev {
   int64_t* state;             /* [4] device: add_count, transitions in the current episode,
@@ -656,6 +662,10 @@ int rb200_per_priority_update(double* tree, int32_t depth, const int64_t* idx,
                               const float* td_target, const float* q_selected, int32_t n,
                               double alpha, double eps, double* p_out, double* max_recorded,
                               int32_t* status, void* stream);
+int rb200_per_priority_update_rows(double* tree, int32_t depth, const int64_t* idx,
+                                   const float* row_loss, int32_t n, double divisor, double alpha,
+                                   double eps, double* p_out, double* max_recorded,
+                                   int32_t* status, void* stream);
 
 /* ------------------------------------------------------------------------- */
 /* Peer-memory plumbing of the fused data-parallel step (one process per GPU).  The    */

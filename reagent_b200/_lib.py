@@ -173,7 +173,7 @@ class C51ArgsT(C.Structure):
                 ("qmax", C.c_float), ("scale_support", C.c_float), ("double_q", C.c_int32),
                 ("maxq", C.c_int32), ("dz_logits", _vp), ("all_q_values", _vp),
                 ("next_action_idx", _vp), ("loss_partials", _vp), ("loss", _vp),
-                ("tile_counter", _vp)]
+                ("tile_counter", _vp), ("sample_weight", _vp)]
 
 
 BC_ROWS_PER_BLOCK = 8  # rb200_bc_xent_head: loss_partials holds ceil(batch / 8) floats
@@ -222,6 +222,7 @@ class QrdqnArgsT(C.Structure):
         ("gamma", C.c_float), ("double_q", C.c_int32), ("maxq", C.c_int32),
         ("dz_head", _vp), ("all_q_values", _vp), ("next_action_idx", _vp),
         ("loss_partials", _vp), ("loss", _vp), ("tile_counter", _vp),
+        ("sample_weight", _vp),
     ]
 
 
@@ -308,6 +309,8 @@ def _declare(lib):
                                       _vp, _vp, _vp]
     lib.rb200_per_priority_update.argtypes = [_vp, C.c_int32, _vp, _vp, _vp, C.c_int32, C.c_double,
                                               C.c_double, _vp, _vp, _vp, _vp]
+    lib.rb200_per_priority_update_rows.argtypes = [_vp, C.c_int32, _vp, _vp, C.c_int32, C.c_double,
+                                                   C.c_double, C.c_double, _vp, _vp, _vp, _vp]
     lib.rb200_adam_blocks.argtypes = [C.c_int64]
     lib.rb200_dp_alloc.argtypes = [C.c_int64, C.POINTER(_vp)]
     lib.rb200_dp_free.argtypes = [_vp]

@@ -107,6 +107,11 @@ __device__ void c51_log_softmax(float* x, int A, int N) {
   }
 }
 
+// kWeighted: prioritized-replay importance weights (a.sample_weight), a separate instantiation so
+// that the unweighted kernel stays exactly as it is.  Row b's dz_logits is scaled by w_b and the
+// loss is mean_b(w_b * loss_partials[b]); loss_partials keeps the unweighted row cross entropies
+// (the priorities are computed from them).
+template <bool kWeighted>
 __global__ void __launch_bounds__(256) c51_head_kernel(const C51Dev d) {
   const rb200_c51_args_t& a = d.a;
   extern __shared__ float sm[];
@@ -198,11 +203,14 @@ __global__ void __launch_bounds__(256) c51_head_kernel(const C51Dev d) {
   for (int c = 0; c < N; ++c) msum += m[c];
   float le = 0.f;
   const float invB = 1.f / (float)a.batch;
+  const float w_row = kWeighted ? a.sample_weight[b] : 1.f;
   for (int i = tid; i < AN; i += blockDim.x) {
     const int r = i / N, c = i - r * N;
     const float aw = a.action[(size_t)b * A + r];
     le -= m[c] * lc[i] * aw;
-    a.dz_logits[(size_t)b * AN + i] = aw * (expf(lc[i]) * msum - m[c]) * invB;
+    float dz = aw * (expf(lc[i]) * msum - m[c]) * invB;
+    if (kWeighted) dz *= w_row;
+    a.dz_logits[(size_t)b * AN + i] = dz;
   }
   if (a.all_q_values) {
     for (int r = tid >> 5; r < A; r += blockDim.x >> 5) {
@@ -232,7 +240,10 @@ __global__ void __launch_bounds__(256) c51_head_kernel(const C51Dev d) {
     // `batch` dependent loads at the tail of the kernel
     __threadfence();
     float tot = 0.f;
-    for (unsigned i = tid; i < gridDim.x; i += blockDim.x) tot += ((volatile float*)a.loss_partials)[i];
+    for (unsigned i = tid; i < gridDim.x; i += blockDim.x) {
+      const float p = ((volatile float*)a.loss_partials)[i];
+      tot += kWeighted ? __fmul_rn(p, a.sample_weight[i]) : p;
+    }
     tot = warp_sum(tot);
     __syncthreads();
     if ((tid & 31) == 0) s_l[tid >> 5] = tot;
@@ -363,11 +374,16 @@ extern "C" int rb200_c51_head(const rb200_c51_args_t* a, void* stream) {
   d.a = *a;
   const size_t smem = ((size_t)3 * a->num_actions * a->num_atoms + 2 * a->num_atoms + a->num_actions) * sizeof(float);
   if (smem > 200 * 1024) { set_last_error("rb200_c51_head: too many atoms/actions for one CTA"); return RB200_E_SMEM; }
-  static SmemOptIn optin = {};
+  static SmemOptIn optin = {}, optin_w = {};
+  const bool weighted = a->sample_weight != nullptr;
   if (smem > 48 * 1024) {
-    cudaError_t e = ensure_dynamic_smem(c51_head_kernel, optin, smem);
+    cudaError_t e = weighted ? ensure_dynamic_smem(c51_head_kernel<true>, optin_w, smem)
+                             : ensure_dynamic_smem(c51_head_kernel<false>, optin, smem);
     if (e != cudaSuccess) return check_cuda(e, "cudaFuncSetAttribute(c51_head)");
   }
-  c51_head_kernel<<<a->batch, 256, smem, (cudaStream_t)stream>>>(d);
+  if (weighted)
+    c51_head_kernel<true><<<a->batch, 256, smem, (cudaStream_t)stream>>>(d);
+  else
+    c51_head_kernel<false><<<a->batch, 256, smem, (cudaStream_t)stream>>>(d);
   return check_cuda(cudaGetLastError(), "c51_head_kernel launch");
 }

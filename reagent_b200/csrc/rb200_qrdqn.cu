@@ -119,6 +119,11 @@ struct QrDev {
   rb200_qrdqn_args_t a;
 };
 
+// kWeighted: prioritized-replay importance weights (a.sample_weight), a separate instantiation so
+// that the unweighted kernel stays exactly as it is.  Row b's dz_head is scaled by w_b and the loss
+// is mean_b(w_b * loss_partials[b] / N^2); loss_partials keeps the unweighted row sums (the
+// priorities are computed from them).
+template <bool kWeighted>
 __global__ void __launch_bounds__(256) qr_head_kernel(const QrDev d) {
   const rb200_qrdqn_args_t& a = d.a;
   extern __shared__ __align__(16) float sm[];
@@ -203,6 +208,7 @@ __global__ void __launch_bounds__(256) qr_head_kernel(const QrDev d) {
   __syncthreads();
   // pairwise quantile-Huber (:152-155): td[i,b,j] = target[i] - current[j], weight |tau_j - 1[td<0]|
   const float norm = 1.f / ((float)N * (float)a.batch * (float)N);
+  const float w_row = kWeighted ? a.sample_weight[b] : 1.f;
   float lsum = 0.f;
   for (int j = tid; j < N; j += blockDim.x) {
     const float c = cq[j];
@@ -232,7 +238,8 @@ __global__ void __launch_bounds__(256) qr_head_kernel(const QrDev d) {
     }
     lsum += l2;
     g += g2;
-    const float dcur = -g * norm;   // d loss / d current[j]
+    float dcur = -g * norm;   // d loss / d current[j]
+    if (kWeighted) dcur *= w_row;
     // d loss / d head output [b, a, j] = action[b,a] * dcur  (linear head)
     for (int cact = 0; cact < A; ++cact)
       a.dz_head[base + (size_t)cact * N + j] = (staged ? s_act[cact] : a.action[(size_t)b * A + cact]) * dcur;
@@ -255,7 +262,10 @@ __global__ void __launch_bounds__(256) qr_head_kernel(const QrDev d) {
     // 4096 dependent loads by a single thread were ~20 us of kernel tail)
     __threadfence();
     float tot = 0.f;
-    for (unsigned i = tid; i < gridDim.x; i += blockDim.x) tot += ((volatile float*)a.loss_partials)[i];
+    for (unsigned i = tid; i < gridDim.x; i += blockDim.x) {
+      const float p = ((volatile float*)a.loss_partials)[i];
+      tot += kWeighted ? __fmul_rn(p, a.sample_weight[i]) : p;
+    }
     tot = warp_sum(tot);
     __syncthreads();
     if ((tid & 31) == 0) red[tid >> 5] = tot;
@@ -366,6 +376,9 @@ extern "C" int rb200_qrdqn_head(const rb200_qrdqn_args_t* a, void* stream) {
   d.a = *a;
   const size_t smem = (size_t)(2 * a->num_atoms + a->num_actions + 256) * sizeof(float);
   if (smem > 48 * 1024) { set_last_error("rb200_qrdqn_head: too many atoms/actions for one CTA"); return RB200_E_SMEM; }
-  qr_head_kernel<<<a->batch, 256, smem, (cudaStream_t)stream>>>(d);
+  if (a->sample_weight)
+    qr_head_kernel<true><<<a->batch, 256, smem, (cudaStream_t)stream>>>(d);
+  else
+    qr_head_kernel<false><<<a->batch, 256, smem, (cudaStream_t)stream>>>(d);
   return check_cuda(cudaGetLastError(), "qr_head_kernel launch");
 }

@@ -242,6 +242,8 @@ struct SetSrc {
   const double* val;         // [n] the values (set_priority), or NULL: PER priorities
   const float* td_target;    // [n]  p_i = ((double)|q_selected_i - td_target_i| + eps) ** alpha
   const float* q_selected;   // [n]
+  const float* row_loss;     // [n] or NULL:  p_i = ((double)|row_loss_i| / divisor + eps) ** alpha
+  double divisor;
   double alpha, eps;
   double* p_out;             // [n] or NULL: the values, written by the leaf kernel
   int n;
@@ -249,7 +251,9 @@ struct SetSrc {
 
 __device__ __forceinline__ double set_value(const SetSrc& s, int i) {
   if (s.val) return s.val[i];
-  return pow(__dadd_rn((double)fabsf(__fsub_rn(s.q_selected[i], s.td_target[i])), s.eps), s.alpha);
+  const double e = s.row_loss ? __ddiv_rn(fabs((double)s.row_loss[i]), s.divisor)
+                              : (double)fabsf(__fsub_rn(s.q_selected[i], s.td_target[i]));
+  return pow(__dadd_rn(e, s.eps), s.alpha);
 }
 
 // How many sets apply: all, up to the first negative value (sum_tree.py raises there, after the
@@ -566,6 +570,26 @@ extern "C" int rb200_per_priority_update(double* tree, int32_t depth, const int6
   s.idx = (const long long*)idx;
   s.td_target = td_target;
   s.q_selected = q_selected;
+  s.alpha = alpha;
+  s.eps = eps;
+  s.p_out = p_out;
+  s.n = n;
+  return sumtree_update(tree, depth, s, max_recorded, status, (cudaStream_t)stream);
+}
+
+extern "C" int rb200_per_priority_update_rows(double* tree, int32_t depth, const int64_t* idx,
+                                              const float* row_loss, int32_t n, double divisor,
+                                              double alpha, double eps, double* p_out,
+                                              double* max_recorded, int32_t* status, void* stream) {
+  const char* null_arg = !tree ? "tree" : !idx ? "idx" : !row_loss ? "row_loss"
+                         : !p_out ? "p_out" : !status ? "status" : nullptr;
+  if (null_arg) { set_last_error("rb200_per_priority_update_rows: %s is null", null_arg); return RB200_E_INVALID; }
+  if (depth < 0 || depth > 31 || n <= 0) { set_last_error("rb200_per_priority_update_rows: bad depth %d / n %d", depth, n); return RB200_E_INVALID; }
+  if (!(divisor > 0.0) || !isfinite(divisor)) { set_last_error("rb200_per_priority_update_rows: divisor must be positive and finite, got %g", divisor); return RB200_E_INVALID; }
+  SetSrc s = {};
+  s.idx = (const long long*)idx;
+  s.row_loss = row_loss;
+  s.divisor = divisor;
   s.alpha = alpha;
   s.eps = eps;
   s.p_out = p_out;

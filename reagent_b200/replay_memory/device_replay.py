@@ -211,6 +211,19 @@ class DeviceReplay:
         _lib.check(rc, "rb200_per_priority_update")
         return p_out
 
+    def write_back_row_priorities(self, indices: torch.Tensor, row_loss: torch.Tensor,
+                                  divisor: float, per: PrioritizedUpdate, p_out: torch.Tensor):
+        """set_priority(indices, (|row_loss| / divisor + eps) ** alpha), in batch order, for the
+        distributional heads, whose priority is the row's own loss (fp32 `row_loss`, fp64
+        arithmetic); the priorities also go to `p_out` (fp64).  A non-finite one applies none
+        (status 3)."""
+        rc = _lib.lib().rb200_per_priority_update_rows(
+            self.tree.data_ptr(), self.rb.sum_tree.depth, indices.data_ptr(), row_loss.data_ptr(),
+            indices.numel(), float(divisor), float(per.alpha), float(per.eps), p_out.data_ptr(),
+            self.max_priority.data_ptr(), self.status.data_ptr(), _lib.cur_stream())
+        _lib.check(rc, "rb200_per_priority_update_rows")
+        return p_out
+
     # ---- index selection ---------------------------------------------------------------
     def upload_host_rng(self):
         """Python's `random` state -> device (the device stream continues it).  The 624 words +
@@ -267,7 +280,8 @@ class DeviceReplay:
             raise ValueError("Sum tree values should be nonnegative.")
         if code == 3:
             raise FloatingPointError(
-                "prioritized replay: a TD error was not finite, so its priority could not be "
+                "prioritized replay: a TD error or row loss was not finite, so its priority "
+                "could not be "
                 "written back (no priority of that update was applied)")
 
     def sync_to_host(self):

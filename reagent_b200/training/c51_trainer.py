@@ -12,7 +12,8 @@ from ..core.parameters import RLParameters
 from ..optimizer import Optimizer__Union, SoftUpdate
 from .reagent_lightning_module import ReAgentLightningModule
 from .rl_trainer_pytorch import RLTrainerMixin
-from .workspace import NetWorkspace, head_backward_dx, param_grads, wgrad
+from .workspace import (NetWorkspace, check_sample_weight, head_backward_dx, param_grads,
+                        wgrad)
 
 
 def _f32c(t):
@@ -90,7 +91,10 @@ class C51Trainer(RLTrainerMixin, ReAgentLightningModule):
                                       h.data_ptr(), B, out.data_ptr(), st)
         _lib.check(rc, "rb200_linear_forward(head)")
 
-    def _c51_step(self, batch: rlt.DiscreteDqnInput) -> torch.Tensor:
+    def _c51_step(self, batch: rlt.DiscreteDqnInput,
+                  sample_weight: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """`sample_weight`: [B] fp32 importance weights (loss = mean(w * loss_row), dz_logits row
+        scaled by w; ws["loss_partials"] keeps the unweighted row cross entropies)."""
         state = _f32c(batch.state.float_features)
         if not state.is_cuda:
             raise _lib.Rb200Error("C51Trainer: training batch must be on the GPU (no CPU path)")
@@ -141,6 +145,7 @@ class C51Trainer(RLTrainerMixin, ReAgentLightningModule):
         a.loss_partials = ws["loss_partials"].data_ptr()
         a.loss = ws["loss"].data_ptr()
         a.tile_counter = ws["counter"].data_ptr()
+        a.sample_weight = P(check_sample_weight(sample_weight, B))
         _lib.check(lib.rb200_c51_head(a, st), "rb200_c51_head")
         if L > 1:
             head_backward_dx(qa, ws["net"], B, ws)
@@ -156,11 +161,15 @@ class C51Trainer(RLTrainerMixin, ReAgentLightningModule):
         yield self.fused_loss(loss)
         yield self.soft_update_result()
 
-    def train_batch(self, training_batch: rlt.DiscreteDqnInput, batch_idx: int = 0, process_group=None):
+    def train_batch(self, training_batch: rlt.DiscreteDqnInput, batch_idx: int = 0, process_group=None,
+                    importance_weights: Optional[torch.Tensor] = None):
+        """`importance_weights` ([B] fp32 on the batch's device, prioritized replay): the loss
+        becomes mean_b(w_b * loss_b) over the per-row cross entropies and row b of d loss /
+        d logits is scaled by w_b."""
         from .data_parallel import dp_fused_step
 
         opts = self.optimizers()
-        self._c51_step(training_batch)
+        self._c51_step(training_batch, sample_weight=importance_weights)
         dp_fused_step(opts[0], self.q_network.arena, process_group,
                       target=self.q_network_target.arena, tau=self.tau)
         self.all_batches_processed += 1

@@ -43,12 +43,18 @@ class FusedDqnStep:
         -> replay_buffer.add -> one update); the transition is the step's only host->device
         traffic, staged in pinned memory and copied + inserted by the same graph replay.
         `per=PrioritizedUpdate(...)` (needs rng="device", prefetch=False): prioritized
-        experience replay.  Each update weights its TD loss by the importance weights of the
-        drawn rows and then writes their TD-error priorities back into the device tree, in
-        batch order, inside the same graph; the next draw sees them.  Online, a transition
-        staged without `priority` enters with the largest priority recorded so far."""
+        experience replay for DQNTrainer, QRDQNTrainer and C51Trainer.  Each update weights
+        its loss by the importance weights of the drawn rows and then writes their priorities
+        back into the device tree, in batch order, inside the same graph; the next draw sees
+        them.  The priority is computed from the TD error for DQN, and from the row's own
+        distributional loss for QR-DQN (mean over the N^2 quantile pairs) and C51 (cross
+        entropy).  Online, a transition staged without `priority` enters with the largest
+        priority recorded so far."""
+        self._row_loss_divisor = None
         if per is not None:
+            from .c51_trainer import C51Trainer
             from .dqn_trainer import DQNTrainer
+            from .qrdqn_trainer import QRDQNTrainer
 
             if rng != "device":
                 raise ValueError("per needs rng='device': the priorities live in the device tree")
@@ -58,8 +64,14 @@ class FusedDqnStep:
             if shard is not None or process_group is not None:
                 raise NotImplementedError("per is single-GPU: data-parallel write-back would need "
                                           "every rank's TD errors")
-            if type(trainer) is not DQNTrainer:
-                raise NotImplementedError("per covers DQNTrainer; got " + type(trainer).__name__)
+            if type(trainer) not in (DQNTrainer, QRDQNTrainer, C51Trainer):
+                raise NotImplementedError("per covers DQNTrainer, QRDQNTrainer and C51Trainer; "
+                                          "got " + type(trainer).__name__)
+            # priority source: None = the TD error (DQN); else the head's per-row loss over D
+            if type(trainer) is QRDQNTrainer:
+                self._row_loss_divisor = float(trainer.num_atoms) * float(trainer.num_atoms)
+            elif type(trainer) is C51Trainer:
+                self._row_loss_divisor = 1.0
         self.per = per
         if rng not in ("host", "device"):
             raise ValueError("rng must be 'host' or 'device'")
@@ -144,8 +156,9 @@ class FusedDqnStep:
     def _refresh_tc_images(self):
         v = self._versions()
         if v != self._param_versions:
-            self.trainer._tc_images_state = None
-            self.trainer.tc_prepack()  # eager, on the current stream, before the replay
+            if hasattr(self.trainer, "tc_prepack"):  # only DQNTrainer keeps packed images
+                self.trainer._tc_images_state = None
+                self.trainer.tc_prepack()  # eager, on the current stream, before the replay
             self._param_versions = v
 
     # -- one update on the current stream ---------------------------------------
@@ -175,7 +188,12 @@ class FusedDqnStep:
         self.dr.importance_weights(idx, opt.step_t, self.per, self.weights)
         loss = self.trainer.train_batch(batch, importance_weights=self.weights)
         ws = self.trainer._ws
-        self.dr.write_back_priorities(idx, ws["td_target"], ws["q_sel"], self.per, self.priorities)
+        if self._row_loss_divisor is None:
+            self.dr.write_back_priorities(idx, ws["td_target"], ws["q_sel"], self.per,
+                                          self.priorities)
+        else:
+            self.dr.write_back_row_priorities(idx, ws["loss_partials"], self._row_loss_divisor,
+                                              self.per, self.priorities)
         return loss
 
     def _prefetch_update(self, i, rnd_dev, overrides=None):

@@ -19,7 +19,8 @@ from ..core.parameters import EvaluationParameters, RLParameters
 from ..optimizer import Optimizer__Union, SoftUpdate
 from .dqn_trainer import _f32c
 from .dqn_trainer_base import DQNTrainerBaseLightning
-from .workspace import NetWorkspace, head_backward_dx, param_grads, wgrad
+from .workspace import (NetWorkspace, check_sample_weight, head_backward_dx, param_grads,
+                        wgrad)
 
 
 class QRDQNTrainer(DQNTrainerBaseLightning):
@@ -114,7 +115,10 @@ class QRDQNTrainer(DQNTrainerBaseLightning):
             out.data_ptr(), st)
         _lib.check(rc, "rb200_linear_forward(head)")
 
-    def _qr_step(self, batch: rlt.DiscreteDqnInput) -> torch.Tensor:
+    def _qr_step(self, batch: rlt.DiscreteDqnInput,
+                 sample_weight: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """`sample_weight`: [B] fp32 importance weights (loss = mean(w * loss_row), dz_head row
+        scaled by w; ws["loss_partials"] keeps the unweighted row sums)."""
         state = _f32c(batch.state.float_features)
         if not state.is_cuda:
             raise _lib.Rb200Error("QRDQNTrainer: training batch must be on the GPU (no CPU path)")
@@ -167,6 +171,7 @@ class QRDQNTrainer(DQNTrainerBaseLightning):
         a.loss_partials = ws["loss_partials"].data_ptr()
         a.loss = ws["loss"].data_ptr()
         a.tile_counter = ws["counter"].data_ptr()
+        a.sample_weight = P(check_sample_weight(sample_weight, B))
         _lib.check(lib.rb200_qrdqn_head(a, st), "rb200_qrdqn_head")
         if L > 1:
             head_backward_dx(qa, ws["net"], B, ws)
@@ -193,9 +198,12 @@ class QRDQNTrainer(DQNTrainerBaseLightning):
         yield self.soft_update_result()
 
     def train_batch(self, training_batch: rlt.DiscreteDqnInput, batch_idx: int = 0,
-                    process_group=None):
+                    process_group=None, importance_weights: Optional[torch.Tensor] = None):
+        """`importance_weights` ([B] fp32 on the batch's device, prioritized replay): the loss
+        becomes mean_b(w_b * loss_b) over the per-row quantile-Huber losses and row b of the
+        head gradient is scaled by w_b."""
         opts = self.optimizers()
-        self._qr_step(training_batch)
+        self._qr_step(training_batch, sample_weight=importance_weights)
         from .data_parallel import dp_fused_step
 
         dp_fused_step(opts[0], self.q_network.arena, process_group,

@@ -23,6 +23,15 @@ class NetWorkspace:
         self.c.input = None if self.input is None else self.input.data_ptr()
 
 
+def check_sample_weight(w, batch: int):
+    """Prioritized-replay importance weights of a distributional head: None or a [batch] float32
+    tensor, with DQNTrainer's error for anything else."""
+    if w is not None and (w.dtype != torch.float32 or w.shape != (batch,)):
+        raise ValueError(f"importance_weights must be a [{batch}] float32 tensor, got "
+                         f"{w.dtype} {tuple(w.shape)}")
+    return w
+
+
 def ensure_gpart(arena: ParamArena, splits: int):
     """[splits, n] gradient partial slab (zeroed once: alignment padding is never written)."""
     flat = arena.flat
