@@ -414,6 +414,9 @@ typedef struct rb200_ac_args {
   float* log_prob_out;       /* [B] or NULL (unclamped sum of log-probs) */
   float* q1_value;           /* [B] or NULL */
   float* q2_value;           /* [B] or NULL */
+  /* prioritized replay (critic step only; the actor step ignores both) */
+  const float* sample_weight; /* [B] or NULL: critic losses mean(w * d^2), dz row scaled by w */
+  float* td_error_out;       /* [B] or NULL: max over critics of |q_c - td_target| */
 } rb200_ac_args_t;
 
 int rb200_ac_critic_step(const rb200_mlp_t* actor, const rb200_mlp_t* q1, const rb200_mlp_t* q2,

@@ -113,6 +113,7 @@ class AcArgsT(C.Structure):
         ("loss_partials", _vp), ("loss", _vp), ("tile_counter", _vp), ("alpha_grad", _vp),
         ("td_target", _vp), ("next_action_out", _vp), ("log_prob_out", _vp),
         ("q1_value", _vp), ("q2_value", _vp),
+        ("sample_weight", _vp), ("td_error_out", _vp),
     ]
 
 

@@ -50,7 +50,14 @@ __device__ __forceinline__ float gaussian_head_row(const float* __restrict__ out
 }
 
 // ---------------------------------------------------------------------------------------
-template <int NT, int TM, int KC>
+// kWeighted: prioritized replay, a separate instantiation so that the unweighted kernel keeps
+// its code.  Row b's loss element and dz are multiplied by a.sample_weight[b] (1 when that
+// pointer is NULL) as the last operation, so unit weights reproduce the unweighted update bit
+// for bit, and the row's TD error max_c |q_c(s,a) - y| (the twin-critic priority of Fujimoto,
+// Meger & Precup 2020) goes to a.td_error_out.  Only the critics are weighted: the importance
+// weights correct the bias of the critics' regression towards the TD target (Schaul et al.
+// 2016); the actor and alpha losses do not regress on the sampled targets.
+template <int NT, int TM, int KC, bool kWeighted>
 __global__ void __launch_bounds__(NT, 1)
 ac_critic_rows_kernel(const Mlp actor, const Mlp q1, const Mlp q2, const Mlp q1t, const Mlp q2t,
                       const AcDev p) {
@@ -143,6 +150,7 @@ ac_critic_rows_kernel(const Mlp actor, const Mlp q1, const Mlp q2, const Mlp q1t
     __syncthreads();
     if (p.ws_q1.input) tile_store_rows<NT, R>(cin, ld_c, p.ws_q1.input, D, D, row0, B);
   }
+  float td_err = 0.f;  // kWeighted: row tid's max_c |q_c - y|, kept across both critics
   for (int which = 0; which < (p.has_q2 ? 2 : 1); ++which) {
     const Mlp& q = which ? q2 : q1;
     const rb200_net_ws_t& ws = which ? p.ws_q2 : p.ws_q1;
@@ -153,11 +161,19 @@ ac_critic_rows_kernel(const Mlp actor, const Mlp q1, const Mlp q2, const Mlp q1t
       float le = 0.f, g = 0.f;
       if (row < B) {
         const float qv = v[r * 8];
-        const float d = qv - rowv[r];
+        const float d = __fsub_rn(qv, rowv[r]);
         le = d * d;                                   // F.mse_loss, mean over B
         g = 2.f / (float)B * d;
         const int lact = q.act[q.n_layers - 1];
         if (lact != RB200_ACT_LINEAR) g *= act_bwd_from_out(qv, lact);
+        if (kWeighted) {
+          const float w = a.sample_weight ? a.sample_weight[row] : 1.f;
+          le = __fmul_rn(le, w);
+          g = __fmul_rn(g, w);
+          // torch.maximum: a NaN from either critic propagates (status 3 on write-back)
+          const float e = fabsf(d);
+          td_err = (which == 0 || e > td_err || e != e) ? e : td_err;
+        }
         float* qo = which ? a.q2_value : a.q1_value;
         if (qo) qo[row] = qv;
       }
@@ -170,6 +186,7 @@ ac_critic_rows_kernel(const Mlp actor, const Mlp q1, const Mlp q2, const Mlp q1t
                              nullptr, 0, 0, 0);
     __syncthreads();
   }
+  if (kWeighted && a.td_error_out && tid < R && row0 + tid < B) a.td_error_out[row0 + tid] = td_err;
   if (tid == 0) {
     float s1 = 0.f, s2 = 0.f;
     for (int r = 0; r < R; ++r) { s1 += rowv[2 * R + r]; s2 += rowv[3 * R + r]; }
@@ -382,7 +399,7 @@ ac_actor_rows_kernel(const Mlp actor, const Mlp q1, const Mlp q2, const AcDev p)
 
 #define RB200_LAUNCH_ACC(NT_, TM_, KC_, grid, smem, stream, ...)                              \
   do {                                                                                        \
-    auto kfn = ac_critic_rows_kernel<NT_, TM_, KC_>;                                          \
+    auto kfn = ac_critic_rows_kernel<NT_, TM_, KC_, kWeighted>;                               \
     static SmemOptIn optin_ = {};                                                             \
     {                                                                                         \
       cudaError_t e_ = ensure_dynamic_smem(kfn, optin_, (size_t)(smem));                      \
@@ -431,6 +448,14 @@ static RowsCfg ac_cfg(const rb200_mlp_t* actor, const rb200_mlp_t* q1, const rb2
   return pick_rows_cfg(batch, q1->dims[0], hmax, 1, 3, n_out_tiles * (*ld_o) + 16 + 4, 0);
 }
 
+template <bool kWeighted>
+static int launch_ac_critic(const RowsCfg& cfg, int grid, cudaStream_t st, const Mlp& ma,
+                            const Mlp& m1, const Mlp& m2, const Mlp& t1, const Mlp& t2,
+                            const AcDev& p) {
+  RB200_DISPATCH_ROWS(cfg, RB200_LAUNCH_ACC, grid, cfg.smem_bytes, st, ma, m1, m2, t1, t2, p);
+  return check_cuda(cudaGetLastError(), "ac_critic_rows_kernel launch");
+}
+
 }  // namespace rb200
 
 using namespace rb200;
@@ -459,8 +484,10 @@ extern "C" int rb200_ac_critic_step(const rb200_mlp_t* actor, const rb200_mlp_t*
   const Mlp t1 = make_mlp(q1_target), t2 = make_mlp(q2 ? q2_target : q1_target);
   const int grid = ceil_div(args->batch, rows_per_tile(cfg));
   cudaStream_t st = (cudaStream_t)stream;
-  RB200_DISPATCH_ROWS(cfg, RB200_LAUNCH_ACC, grid, cfg.smem_bytes, st, ma, m1, m2, t1, t2, p);
-  return check_cuda(cudaGetLastError(), "ac_critic_rows_kernel launch");
+  // prioritized replay: weights and / or TD errors take the weighted instantiation
+  return (args->sample_weight || args->td_error_out)
+             ? launch_ac_critic<true>(cfg, grid, st, ma, m1, m2, t1, t2, p)
+             : launch_ac_critic<false>(cfg, grid, st, ma, m1, m2, t1, t2, p);
 }
 
 extern "C" int rb200_ac_actor_step(const rb200_mlp_t* actor, const rb200_mlp_t* q1,

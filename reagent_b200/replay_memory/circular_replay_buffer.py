@@ -676,6 +676,21 @@ class ReplayBuffer:
         batch.sampling_probabilities = t.get("sampling_probabilities")
         return batch
 
+    def _action_bounds(self, action_low, action_high, dev):
+        """Device copies of the action range, cached per value: the host->device copy happens
+        once, so a sampling launch with known bounds can be captured into a CUDA graph."""
+        lo = np.ascontiguousarray(np.asarray(action_low, dtype=np.float32).reshape(-1))
+        hi = np.ascontiguousarray(np.asarray(action_high, dtype=np.float32).reshape(-1))
+        key = (lo.tobytes(), hi.tobytes(), str(dev))
+        cache = self.__dict__.setdefault("_action_bounds_cache", {})
+        out = cache.get(key)
+        if out is None:
+            if len(cache) >= 16:
+                cache.clear()
+            out = (torch.from_numpy(lo.copy()).to(dev), torch.from_numpy(hi.copy()).to(dev))
+            cache[key] = out
+        return out
+
     def sample_policy_network_batch(self, batch_size, action_low, action_high, indices=None,
                                     **index_kwargs):
         """sample_transition_batch + PolicyNetworkInputMaker.__call__
@@ -688,9 +703,7 @@ class ReplayBuffer:
             raise NotImplementedError("continuous batches need a flat float32 action")
         args, t, keep = self._fused_common(batch_size, indices, index_kwargs)
         B, dev, A = batch_size, self._dev(), amd.shape[0]
-        lo = torch.as_tensor(np.asarray(action_low, dtype=np.float32)).reshape(-1).to(dev)
-        hi = torch.as_tensor(np.asarray(action_high, dtype=np.float32)).reshape(-1).to(dev)
-        keep += [lo, hi]
+        lo, hi = self._action_bounds(action_low, action_high, dev)
         action = self._alloc("action", B, A)
         next_action = self._alloc("next_action", B, A)
         args.action_f32 = self._store["action"].data_ptr()

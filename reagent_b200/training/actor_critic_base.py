@@ -8,7 +8,7 @@ from .. import _lib
 from ..core import types as rlt
 from .reagent_lightning_module import ReAgentLightningModule
 from .rl_trainer_pytorch import RLTrainerMixin
-from .workspace import NetWorkspace, param_grads, wgrad
+from .workspace import NetWorkspace, check_sample_weight, param_grads, wgrad
 
 
 def _f32c(t):
@@ -54,6 +54,8 @@ class ActorCriticBase(RLTrainerMixin, ReAgentLightningModule):
                 "q1_value": torch.empty(B, device=device),
                 "q2_value": torch.empty(B, device=device),
                 "log_prob": torch.empty(B, device=device),
+                # weighted critic step (prioritized replay): max_c |q_c(s, a) - td_target|
+                "td_error": torch.empty(B, device=device),
             }
             if ws["q2"] is not None:
                 ws["q2"].c.input = ws["q1"].input.data_ptr()
@@ -88,12 +90,22 @@ class ActorCriticBase(RLTrainerMixin, ReAgentLightningModule):
     def _desc(self, net):
         return None if net is None else net.arena.desc()
 
-    def _critic_step(self, batch, actor_net, q1t, q2t, fill):
+    def _critic_step(self, batch, actor_net, q1t, q2t, fill,
+                     sample_weight: Optional[torch.Tensor] = None):
+        """`sample_weight`: [B] fp32 importance weights of prioritized replay.  Each critic's
+        loss becomes mean(w * (q - y)^2) and row b of its dZ is scaled by w_b; the row's TD
+        error max_c |q_c - y| goes to the workspace's "td_error"."""
         state = batch.state.float_features
         B, dev = state.shape[0], state.device
+        check_sample_weight(sample_weight, B)
         ws = self._workspace(B, dev)
         keep = []
         a, state = self._base_args(batch, ws, keep)
+        if sample_weight is not None:
+            w = _lib.on_device(sample_weight.contiguous(), state.device)
+            keep.append(w)
+            a.sample_weight = w.data_ptr()
+            a.td_error_out = ws["td_error"].data_ptr()
         A = self.q1_network.arena.dims[0] - self.actor_network.arena.dims[0]
         nz = self._noise("next", B, A, dev)
         keep.append(nz)

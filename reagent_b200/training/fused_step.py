@@ -14,6 +14,9 @@ during update k-1 while the replay-sample kernel for update k+1 runs on a second
 does not depend on the parameters).  The host's random stream is consumed in the same order;
 the only observable difference is that a transition added between two `step()` calls can be
 sampled one update later.
+
+`FusedPolicyStep` is the device-resident online step for SACTrainer and TD3Trainer (continuous
+actions), with the same staging, draw, status words and optional prioritized replay.
 """
 from typing import Optional
 
@@ -176,9 +179,7 @@ class FusedDqnStep:
         batch = self._sample(rnd_dev)
         if forked:
             main.wait_stream(self._side)
-        if self.per is not None:
-            return self._per_train(batch)
-        return self.trainer.train_batch(batch, process_group=self.pg)
+        return self._train(batch)
 
     def _per_train(self, batch):
         """Importance weights of the drawn rows -> weighted update -> priority write-back."""
@@ -263,8 +264,16 @@ class FusedDqnStep:
             batch = self.rb.sample_discrete_dqn_batch(self.B, self.A, ranks_dev=rnd_dev)
         return batch
 
+    def _train(self, batch):
+        """The update on a drawn device-resident batch; returns the loss tensor."""
+        if self.per is not None:
+            return self._per_train(batch)
+        return self.trainer.train_batch(batch, process_group=self.pg)
+
+    _loss_width = 1  # elements of the loss copied to the pinned host tensor of a step
+
     def _capture_device(self, i=0):
-        loss_host = torch.zeros(1, dtype=torch.float32).pin_memory()
+        loss_host = torch.zeros(self._loss_width, dtype=torch.float32).pin_memory()
         g = torch.cuda.CUDAGraph()
         marker = torch.zeros(1, device=self.dev)  # non-None: "inside the captured step"
         with torch.cuda.graph(g):
@@ -274,11 +283,8 @@ class FusedDqnStep:
                 if self.online:
                     self.dr.launch_add(1, slot=i, priority_from_max=self.per is not None)
                 batch = self._device_sample(0, False)
-                if self.per is not None:
-                    loss = self._per_train(batch)
-                else:
-                    loss = self.trainer.train_batch(batch, process_group=self.pg)
-            loss_host.copy_(loss.reshape(1), non_blocking=True)
+                loss = self._train(batch)
+            loss_host.copy_(loss.reshape(self._loss_width), non_blocking=True)
             self._status_host.copy_(self.dr.status, non_blocking=True)
         return {"graph": g, "loss_host": loss_host, "done": torch.cuda.Event(), "used": False}
 
@@ -309,19 +315,7 @@ class FusedDqnStep:
             s["done"].synchronize()
         self._refresh_tc_images()
         if self.dr is not None:
-            if self._status_np[0] != 0:  # sticky device status of an earlier step
-                self.dr.raise_if_failed(self._status_host)
-            if self.online:
-                if transition is None:
-                    raise ValueError("online FusedDqnStep.step() needs the new transition")
-                # every slot's graph copies from its own pinned staging row; the slot's previous
-                # replay (and with it that H2D copy) was waited for above
-                self.dr.stage(0, (self.k - 1) % len(self.slots),
-                              priority_from_max=self.per is not None, **transition)
-            s["graph"].replay()
-            s["done"].record()
-            s["used"] = True
-            return s["loss_host"]
+            return self._replay_device(s, s["graph"], s["loss_host"], transition)
         # bring device mirrors up to date OUTSIDE the captured graph (adds / set_priority)
         self.rb._flush()
         if self.prioritized:
@@ -349,6 +343,158 @@ class FusedDqnStep:
         s["done"].record()
         s["used"] = True
         return s["loss_host"]
+
+    def _replay_device(self, s, graph, loss_host, transition):
+        """Device-resident step on slot `s` (already waited for): raise a sticky status of an
+        earlier step, stage the new transition (online), replay `graph`."""
+        if self._status_np[0] != 0:  # sticky device status of an earlier step
+            self.dr.raise_if_failed(self._status_host)
+        if self.online:
+            if transition is None:
+                raise ValueError(f"online {type(self).__name__}.step() needs the new transition")
+            # every slot's graph copies from its own pinned staging row; the slot's previous
+            # replay (and with it that H2D copy) was waited for above
+            self.dr.stage(0, (self.k - 1) % len(self.slots),
+                          priority_from_max=self.per is not None, **transition)
+        graph.replay()
+        s["done"].record()
+        s["used"] = True
+        return loss_host
+
+
+class FusedPolicyStep(FusedDqnStep):
+    """FusedDqnStep's device-resident step for the continuous-action trainers SACTrainer and
+    TD3Trainer: per `step(transition)` ONE graph replay adds the transition (online), draws the
+    batch with the device MT19937 stream, gathers it with `sample_policy_network_batch` (the
+    actions rescaled from [action_low, action_high]) and runs the whole `train_batch`.  SAC's
+    noise is drawn with torch.randn inside the graph (or comes from the trainer's `noise_hook`).
+
+    `per=PrioritizedUpdate(...)`: the critic losses are weighted by the importance weights of
+    the drawn rows (beta annealed with q1's Adam step count), and each row's priority
+    (max over the critics of |q_c(s, a) - y| + eps) ** alpha is written back into the device
+    tree, in batch order, inside the same graph.  The actor and alpha losses stay unweighted.
+
+    TD3 trains its actor on every `delayed_policy_update`-th batch only, a decision taken in
+    Python; one graph is captured per phase (and staging slot) and `step()` picks it from its
+    own update counter.  The constructor runs one eager warm-up update, which is batch 0.
+    `step()` returns the pinned host tensor that will hold [q1 loss, q2 loss] of the update."""
+
+    _loss_width = 2
+
+    def __init__(self, trainer, replay_buffer, batch_size: int, action_low, action_high,
+                 online: bool = True, per: Optional[PrioritizedUpdate] = None,
+                 rng: str = "device", prefetch: bool = False, slots: int = 2, shard=None,
+                 process_group=None):
+        from ..replay_memory.device_replay import DeviceReplay
+        from .sac_trainer import SACTrainer
+        from .td3_trainer import TD3Trainer
+
+        if type(trainer) not in (SACTrainer, TD3Trainer):
+            raise NotImplementedError("FusedPolicyStep covers SACTrainer and TD3Trainer; got "
+                                      + type(trainer).__name__)
+        if shard is not None or process_group is not None:
+            raise NotImplementedError("FusedPolicyStep is single-GPU: a data-parallel priority "
+                                      "write-back would need every rank's TD errors")
+        if rng != "device":
+            raise ValueError("FusedPolicyStep needs rng='device' (device-resident replay)")
+        if prefetch:
+            raise ValueError("FusedPolicyStep needs prefetch=False: a prefetched draw would run "
+                             "before the previous update's priority write-back")
+        if int(slots) < 1:
+            raise ValueError("slots must be >= 1")
+        if not isinstance(replay_buffer, PrioritizedReplayBuffer):
+            raise NotImplementedError("FusedPolicyStep covers the prioritized buffer")
+        self.trainer, self.rb, self.per = trainer, replay_buffer, per
+        self.rng, self.online, self.prefetch, self.pg = "device", bool(online), False, None
+        self.B = self.B_global = batch_size
+        self.row0 = 0
+        self.prioritized = True
+        self.dev = replay_buffer._dev()
+        self.action_low = np.asarray(action_low, dtype=np.float32).reshape(-1).copy()
+        self.action_high = np.asarray(action_high, dtype=np.float32).reshape(-1).copy()
+        replay_buffer._flush()
+        self.dr = getattr(replay_buffer, "_device_resident", None) or DeviceReplay(
+            replay_buffer, stage_rows=1, stage_slots=max(2, int(slots)))
+        if self.dr.stage_slots < int(slots):
+            self.dr._alloc_stage(self.dr.stage_rows, int(slots))
+        self._idx_buf = [torch.zeros(batch_size, dtype=torch.int64, device=self.dev)]
+        self._status_host = torch.zeros(2, dtype=torch.int32).pin_memory()
+        self._status_np = self._status_host.numpy()
+        self.h2d_bytes = self.dr.h2d_bytes_per_add if self.online else 0
+        self.d2h_bytes = 4 * self._loss_width + 8
+        if per is not None:
+            self.weights = torch.empty(batch_size, dtype=torch.float32, device=self.dev)
+            self.priorities = torch.empty(batch_size, dtype=torch.float64, device=self.dev)
+        # a batch_idx of each phase: TD3 with a delayed actor has two, SAC one
+        self._delay = int(getattr(trainer, "delayed_policy_update", 1))
+        self._phase_batch_idx = [0, 1] if (type(trainer) is TD3Trainer and self._delay != 1) else [0]
+        self._updates = 0
+        self.slots, self.k = [], 0
+        n0 = trainer.all_batches_processed
+        # warm-up outside capture (lazy allocations, cudaFuncSetAttribute, optimizer state and
+        # the device copies of the action bounds): update 0
+        self._one_update(None)
+        torch.cuda.synchronize()
+        for i in range(int(slots)):
+            self.slots.append(self._capture(i))
+        trainer.all_batches_processed = n0 + 1  # a capture runs the Python body, not an update
+
+    def _refresh_tc_images(self):
+        pass  # the actor-critic kernels read the parameters directly: nothing to rebuild
+
+    def _device_sample(self, slot: int, add: bool, stage_row: int = 0):
+        if add:
+            self.dr.launch_add(1, slot=stage_row)
+        idx = self.dr.draw_indices(self.B, out=self._idx_buf[slot])
+        return self.rb.sample_policy_network_batch(self.B, self.action_low, self.action_high,
+                                                   indices=idx)
+
+    def _one_update(self, rnd_dev):
+        """One eager update (draw + train) of the next batch_idx, on the current stream."""
+        self._batch_idx = self._updates
+        loss = self._train(self._device_sample(0, False))
+        self._updates += 1
+        return loss
+
+    def _train(self, batch):
+        if self.per is not None:
+            return self._per_train(batch)
+        closs, _ = self.trainer.train_batch(batch, self._batch_idx)
+        return closs
+
+    def _per_train(self, batch):
+        """Importance weights -> weighted critics -> twin-critic TD-error priority write-back."""
+        idx = self._idx_buf[0]
+        opt = self.trainer.optimizers()[0]  # q1's Adam: its step count anneals beta
+        opt._ensure_state()
+        self.dr.importance_weights(idx, opt.step_t, self.per, self.weights)
+        closs, _ = self.trainer.train_batch(batch, self._batch_idx,
+                                            importance_weights=self.weights)
+        self.dr.write_back_row_priorities(idx, self.trainer._ws["td_error"], 1.0, self.per,
+                                          self.priorities)
+        return closs
+
+    def _capture(self, i=0):
+        graphs, hosts = [], []
+        for b in self._phase_batch_idx:
+            self._batch_idx = b
+            c = self._capture_device(i)
+            graphs.append(c["graph"])
+            hosts.append(c["loss_host"])
+        return {"graphs": graphs, "loss_hosts": hosts, "done": torch.cuda.Event(), "used": False}
+
+    def step(self, transition=None) -> torch.Tensor:
+        """One full update (see FusedDqnStep.step); `transition` (online mode): dict of the add()
+        keyword arguments of the new transition."""
+        s = self.slots[self.k % len(self.slots)]
+        self.k += 1
+        if s["used"]:
+            s["done"].synchronize()
+        phase = 0 if self._updates % self._delay == 0 else len(self._phase_batch_idx) - 1
+        out = self._replay_device(s, s["graphs"][phase], s["loss_hosts"][phase], transition)
+        self._updates += 1
+        self.trainer.all_batches_processed += 1
+        return out
 
 
 def capture_device_only(trainer, rb, batch_size, steps, queries_dev, process_group=None,

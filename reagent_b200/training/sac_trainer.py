@@ -178,13 +178,16 @@ class SACTrainer(ActorCriticBase):
         yield result
 
     def train_batch(self, training_batch: rlt.PolicyNetworkInput, batch_idx: int = 0,
-                    process_group=None):
+                    process_group=None, importance_weights: Optional[torch.Tensor] = None):
         """Fast path: the whole update (same arithmetic as train_step_gen), Polyak updates
-        fused into the critics' Adam launches, exp(log_alpha) into the alpha launch."""
+        fused into the critics' Adam launches, exp(log_alpha) into the alpha launch.
+        `importance_weights` ([B] fp32 on the batch's device, prioritized replay): each critic
+        loss becomes mean_b(w_b * (q_b - y_b)^2); the actor and alpha losses stay unweighted."""
         opts = self.optimizers()
         i = 0
         closs = self._critic_step(training_batch, self.actor_network, self.q1_network_target,
-                                  self.q2_network_target, self._fill_critic)
+                                  self.q2_network_target, self._fill_critic,
+                                  sample_weight=importance_weights)
         self._dp_step(opts[i], self.q1_network.arena, self.q1_network_target.arena, process_group)
         i += 1
         if self.q2_network:

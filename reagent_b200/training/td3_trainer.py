@@ -102,12 +102,15 @@ class TD3Trainer(ActorCriticBase):
             yield None
 
     def train_batch(self, training_batch: rlt.PolicyNetworkInput, batch_idx: int = 0,
-                    process_group=None):
-        """Fast path; Polyak updates fused into the Adam launches on policy-update batches."""
+                    process_group=None, importance_weights: Optional[torch.Tensor] = None):
+        """Fast path; Polyak updates fused into the Adam launches on policy-update batches.
+        `importance_weights` ([B] fp32 on the batch's device, prioritized replay): each critic
+        loss becomes mean_b(w_b * (q_b - y_b)^2); the actor loss stays unweighted."""
         opts = self.optimizers()
         upd = batch_idx % self.delayed_policy_update == 0
         closs = self._critic_step(training_batch, self.actor_network_target,
-                                  self.q1_network_target, self.q2_network_target, self._fill)
+                                  self.q1_network_target, self.q2_network_target, self._fill,
+                                  sample_weight=importance_weights)
         i = 0
         self._dp_step(opts[i], self.q1_network.arena,
                       self.q1_network_target.arena if upd else None, process_group)
