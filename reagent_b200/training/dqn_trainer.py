@@ -21,7 +21,7 @@ from ..core import types as rlt
 from ..core.parameters import EvaluationParameters, RLParameters
 from ..optimizer import Optimizer__Union, SoftUpdate
 from .dqn_trainer_base import DQNTrainerBaseLightning
-from .workspace import NetWorkspace, param_grads, wgrad
+from .workspace import NetWorkspace, check_sample_weight, param_grads, wgrad
 
 
 @dataclass(frozen=True)
@@ -302,10 +302,7 @@ class DQNTrainer(DQNTrainerBaseLightning):
         a.loss = ws["loss"].data_ptr()
         a.tile_counter = ws["counter"].data_ptr()
         if sample_weight is not None:
-            if sample_weight.dtype != torch.float32 or sample_weight.shape != (B,):
-                raise ValueError(f"importance_weights must be a [{B}] float32 tensor, got "
-                                 f"{sample_weight.dtype} {tuple(sample_weight.shape)}")
-            a.sample_weight = P(sample_weight)
+            a.sample_weight = P(check_sample_weight(sample_weight, B))
         self.q_network.arena.refresh()          # no-op for plain MLPs; folds a dueling head
         self.q_network_target.arena.refresh()
         qd, qtd = self.q_network.arena.desc(), self.q_network_target.arena.desc()

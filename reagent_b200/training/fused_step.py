@@ -23,12 +23,37 @@ from typing import Optional
 import numpy as np
 import torch
 
-from .. import _lib
-from ..replay_memory.device_replay import PrioritizedUpdate
+from ..replay_memory.device_replay import DeviceReplay, PrioritizedUpdate
 from ..replay_memory.prioritized_replay_buffer import PrioritizedReplayBuffer
+from .c51_trainer import C51Trainer
+from .dqn_trainer import DQNTrainer
+from .qrdqn_trainer import QRDQNTrainer
+from .sac_trainer import SACTrainer
+from .td3_trainer import TD3Trainer
+
+# Prioritized replay: each trainer's priority source, keyed on the exact type (a subclass could
+# change what its per-row workspace values mean) -- the DeviceReplay write-back and a function of
+# (trainer, workspace) giving its inputs after the update.  DQN: the TD error; QR-DQN: the row's
+# loss over its N^2 quantile pairs; C51: its cross entropy; SAC / TD3: the larger critic TD error.
+_PRIORITY_SOURCES = {
+    DQNTrainer: (DeviceReplay.write_back_priorities, lambda t, ws: (ws["td_target"], ws["q_sel"])),
+    QRDQNTrainer: (DeviceReplay.write_back_row_priorities,
+                   lambda t, ws: (ws["loss_partials"], float(t.num_atoms) * float(t.num_atoms))),
+    C51Trainer: (DeviceReplay.write_back_row_priorities, lambda t, ws: (ws["loss_partials"], 1.0)),
+    SACTrainer: (DeviceReplay.write_back_row_priorities, lambda t, ws: (ws["td_error"], 1.0)),
+    TD3Trainer: (DeviceReplay.write_back_row_priorities, lambda t, ws: (ws["td_error"], 1.0)),
+}
+
+
+def _query_keyword(rb) -> str:
+    """sample_discrete_dqn_batch's keyword for the device random numbers of `rb`'s draw."""
+    return "query_dev" if isinstance(rb, PrioritizedReplayBuffer) else "ranks_dev"
 
 
 class FusedDqnStep:
+    _per_trainers = (DQNTrainer, QRDQNTrainer, C51Trainer)  # exact types `per` covers
+    _index_buffers = 2  # of a device draw: the prefetch path alternates two
+
     def __init__(self, trainer, replay_buffer, batch_size: int, process_group=None,
                  slots: int = 2, prefetch: bool = False, shard=None, rng: str = "host",
                  online: bool = False, per: Optional[PrioritizedUpdate] = None):
@@ -53,12 +78,7 @@ class FusedDqnStep:
         distributional loss for QR-DQN (mean over the N^2 quantile pairs) and C51 (cross
         entropy).  Online, a transition staged without `priority` enters with the largest
         priority recorded so far."""
-        self._row_loss_divisor = None
         if per is not None:
-            from .c51_trainer import C51Trainer
-            from .dqn_trainer import DQNTrainer
-            from .qrdqn_trainer import QRDQNTrainer
-
             if rng != "device":
                 raise ValueError("per needs rng='device': the priorities live in the device tree")
             if prefetch:
@@ -67,14 +87,9 @@ class FusedDqnStep:
             if shard is not None or process_group is not None:
                 raise NotImplementedError("per is single-GPU: data-parallel write-back would need "
                                           "every rank's TD errors")
-            if type(trainer) not in (DQNTrainer, QRDQNTrainer, C51Trainer):
+            if type(trainer) not in self._per_trainers:
                 raise NotImplementedError("per covers DQNTrainer, QRDQNTrainer and C51Trainer; "
                                           "got " + type(trainer).__name__)
-            # priority source: None = the TD error (DQN); else the head's per-row loss over D
-            if type(trainer) is QRDQNTrainer:
-                self._row_loss_divisor = float(trainer.num_atoms) * float(trainer.num_atoms)
-            elif type(trainer) is C51Trainer:
-                self._row_loss_divisor = 1.0
         self.per = per
         if rng not in ("host", "device"):
             raise ValueError("rng must be 'host' or 'device'")
@@ -93,8 +108,8 @@ class FusedDqnStep:
         self.B = batch_size
         self.pg = process_group
         self.prioritized = isinstance(replay_buffer, PrioritizedReplayBuffer)
+        self._query_kw = _query_keyword(replay_buffer)
         self.dev = replay_buffer._dev()
-        self.A = trainer.num_actions
         self.slots = []
         self.k = 0
         self.h2d_bytes = batch_size * 8
@@ -102,23 +117,23 @@ class FusedDqnStep:
         self._side2 = torch.cuda.Stream(device=self.dev)
         self.d2h_bytes = 4
         self.prefetch = bool(prefetch)
+        slots = 2 if self.prefetch else int(slots)  # prefetch alternates two batch sets
         replay_buffer._flush()
         self.dr = None
         if rng == "device":
-            from ..replay_memory.device_replay import DeviceReplay
-
             if not self.prioritized:
                 raise NotImplementedError("rng='device' covers the prioritized buffer")
+            # every slot's graph adds from its own staging block
             self.dr = getattr(replay_buffer, "_device_resident", None) or DeviceReplay(
-                replay_buffer, stage_rows=1, stage_slots=2)
-            if self.dr.stage_slots < 2:
-                self.dr._alloc_stage(self.dr.stage_rows, 2)
+                replay_buffer, stage_rows=1, stage_slots=max(2, slots))
+            if self.dr.stage_slots < slots:
+                self.dr._alloc_stage(self.dr.stage_rows, slots)
             self._idx_buf = [torch.zeros(self.B_global, dtype=torch.int64, device=self.dev)
-                             for _ in range(2)]
+                             for _ in range(self._index_buffers)]
             self._status_host = torch.zeros(2, dtype=torch.int32).pin_memory()
             self._status_np = self._status_host.numpy()
             self.h2d_bytes = self.dr.h2d_bytes_per_add if self.online else 0
-            self.d2h_bytes = 4 + 8
+            self.d2h_bytes = 4 * self._loss_width + 8
             if per is not None:
                 self.weights = torch.empty(self.B, dtype=torch.float32, device=self.dev)
                 self.priorities = torch.empty(self.B, dtype=torch.float64, device=self.dev)
@@ -135,12 +150,11 @@ class FusedDqnStep:
                 self._batches[0] = self._sample(None)
             with self.rb.output_buffers(self._pools[1]):
                 self._batches[1] = self.rb.sample_discrete_dqn_batch(
-                    self.B, self.A, indices=self._batches[0].indices.reshape(-1))
+                    self.B, trainer.num_actions, indices=self._batches[0].indices.reshape(-1))
             torch.cuda.synchronize()
-            slots = 2
         for i in range(slots):
             self.slots.append(self._capture(i))
-        self._param_versions = self._versions()
+        self._param_versions = self._versions() if hasattr(trainer, "tc_prepack") else None
 
     # -- parameters changed from outside (load_state_dict, manual edits) ----------------------
     def _versions(self):
@@ -157,11 +171,12 @@ class FusedDqnStep:
         self._param_versions = None
 
     def _refresh_tc_images(self):
+        if not hasattr(self.trainer, "tc_prepack"):  # only DQNTrainer keeps packed images
+            return
         v = self._versions()
         if v != self._param_versions:
-            if hasattr(self.trainer, "tc_prepack"):  # only DQNTrainer keeps packed images
-                self.trainer._tc_images_state = None
-                self.trainer.tc_prepack()  # eager, on the current stream, before the replay
+            self.trainer._tc_images_state = None
+            self.trainer.tc_prepack()  # eager, on the current stream, before the replay
             self._param_versions = v
 
     # -- one update on the current stream ---------------------------------------
@@ -181,20 +196,27 @@ class FusedDqnStep:
             main.wait_stream(self._side)
         return self._train(batch)
 
+    def _train_batch(self, batch, **weights):
+        """The trainer's update on `batch` (`importance_weights=` with per); returns the loss
+        tensor a step copies to the host."""
+        return self.trainer.train_batch(batch, process_group=self.pg, **weights)
+
+    def _train(self, batch):
+        """The update on a drawn batch; returns the loss tensor."""
+        if self.per is not None:
+            return self._per_train(batch)
+        return self._train_batch(batch)
+
     def _per_train(self, batch):
         """Importance weights of the drawn rows -> weighted update -> priority write-back."""
         idx = self._idx_buf[0]
-        opt = self.trainer.optimizers()[0]
+        opt = self.trainer.optimizers()[0]  # its Adam step count anneals beta
         opt._ensure_state()
         self.dr.importance_weights(idx, opt.step_t, self.per, self.weights)
-        loss = self.trainer.train_batch(batch, importance_weights=self.weights)
-        ws = self.trainer._ws
-        if self._row_loss_divisor is None:
-            self.dr.write_back_priorities(idx, ws["td_target"], ws["q_sel"], self.per,
-                                          self.priorities)
-        else:
-            self.dr.write_back_row_priorities(idx, ws["loss_partials"], self._row_loss_divisor,
-                                              self.per, self.priorities)
+        loss = self._train_batch(batch, importance_weights=self.weights)
+        write_back, inputs = _PRIORITY_SOURCES[type(self.trainer)]
+        write_back(self.dr, idx, *inputs(self.trainer, self.trainer._ws), self.per,
+                   self.priorities)
         return loss
 
     def _prefetch_update(self, i, rnd_dev, overrides=None):
@@ -210,14 +232,11 @@ class FusedDqnStep:
         with torch.cuda.stream(self._side), self.rb.output_buffers(self._pools[1 - i]):
             if self.dr is not None:
                 nxt = self._device_sample(1 - i, self.online and rnd_dev is not None, stage_row=i)
-            elif overrides is None:
-                nxt = self._sample(rnd_dev)
             else:
-                nxt = self.rb.sample_discrete_dqn_batch(self.B, self.A, query_dev=rnd_dev,
-                                                        overrides=overrides)
+                nxt = self._sample(rnd_dev, overrides)
         if forked:
             main.wait_stream(self._side2)
-        loss = self.trainer.train_batch(self._batches[i], process_group=self.pg)
+        loss = self._train_batch(self._batches[i])
         main.wait_stream(self._side)
         self._batches[1 - i] = nxt
         return loss
@@ -238,37 +257,27 @@ class FusedDqnStep:
         """Device-resident draw: (optionally insert the staged transition,) select the global
         indices with the device MT19937 stream, gather this rank's rows."""
         if add:
-            self.dr.launch_add(1, slot=stage_row)
-        idx = self.dr.draw_indices(self.B_global, out=self._idx_buf[slot])
-        return self.rb.sample_discrete_dqn_batch(self.B, self.A,
-                                                 indices=idx[self.row0:self.row0 + self.B])
+            self.dr.launch_add(1, slot=stage_row, priority_from_max=self.per is not None)
+        return self._gather(self.dr.draw_indices(self.B_global, out=self._idx_buf[slot]))
 
-    def _sample(self, rnd_dev):
+    def _gather(self, indices):
+        """This rank's rows of the drawn global `indices`, as the trainer's batch."""
+        return self.rb.sample_discrete_dqn_batch(self.B, self.trainer.num_actions,
+                                                 indices=indices[self.row0:self.row0 + self.B])
+
+    def _sample(self, rnd_dev, overrides=None):
         if self.dr is not None:
             return self._device_sample(0, False)
+        kw = {}
         if rnd_dev is None and self.B != self.B_global:
             q, pos, idxs = self._host_draw()
-            qd = torch.from_numpy(np.ascontiguousarray(q)).to(self.dev)
-            if self.prioritized:
-                kw = {"query_dev": qd}
-                if pos:
-                    kw["overrides"] = (pos, idxs)
-            else:
-                kw = {"ranks_dev": qd}
-            batch = self.rb.sample_discrete_dqn_batch(self.B, self.A, **kw)
-        elif rnd_dev is None:
-            batch = self.rb.sample_discrete_dqn_batch(self.B, self.A)
-        elif self.prioritized:
-            batch = self.rb.sample_discrete_dqn_batch(self.B, self.A, query_dev=rnd_dev)
-        else:
-            batch = self.rb.sample_discrete_dqn_batch(self.B, self.A, ranks_dev=rnd_dev)
-        return batch
-
-    def _train(self, batch):
-        """The update on a drawn device-resident batch; returns the loss tensor."""
-        if self.per is not None:
-            return self._per_train(batch)
-        return self.trainer.train_batch(batch, process_group=self.pg)
+            rnd_dev = torch.from_numpy(np.ascontiguousarray(q)).to(self.dev)
+            overrides = (pos, idxs) if pos else None
+        if overrides is not None:
+            kw["overrides"] = overrides
+        if rnd_dev is not None:
+            kw[self._query_kw] = rnd_dev
+        return self.rb.sample_discrete_dqn_batch(self.B, self.trainer.num_actions, **kw)
 
     _loss_width = 1  # elements of the loss copied to the pinned host tensor of a step
 
@@ -280,10 +289,7 @@ class FusedDqnStep:
             if self.prefetch:
                 loss = self._prefetch_update(i, marker)
             else:
-                if self.online:
-                    self.dr.launch_add(1, slot=i, priority_from_max=self.per is not None)
-                batch = self._device_sample(0, False)
-                loss = self._train(batch)
+                loss = self._train(self._device_sample(0, self.online, stage_row=i))
             loss_host.copy_(loss.reshape(self._loss_width), non_blocking=True)
             self._status_host.copy_(self.dr.status, non_blocking=True)
         return {"graph": g, "loss_host": loss_host, "done": torch.cuda.Event(), "used": False}
@@ -320,24 +326,20 @@ class FusedDqnStep:
         self.rb._flush()
         if self.prioritized:
             self.rb.sum_tree.device_heap(self.dev)
-        else:
-            self.rb._ensure_valid_index()
-        if self.prioritized:
             q, pos, idxs = self._host_draw()
             if pos:  # rare retry path: resolved on the host, run this update un-captured
                 qd = torch.from_numpy(q).to(self.dev)
                 if self.prefetch:
                     loss = self._prefetch_update((self.k - 1) % 2, qd, overrides=(pos, idxs))
                 else:
-                    batch = self.rb.sample_discrete_dqn_batch(self.B, self.A, query_dev=qd,
-                                                              overrides=(pos, idxs))
-                    loss = self.trainer.train_batch(batch, process_group=self.pg)
+                    loss = self._train(self._sample(qd, (pos, idxs)))
                 s["loss_host"].copy_(loss.reshape(1), non_blocking=True)
                 s["done"].record()
                 s["used"] = True
                 return s["loss_host"]
             s["host"].numpy()[:] = q
         else:
+            self.rb._ensure_valid_index()
             s["host"].copy_(torch.from_numpy(self._host_draw()[0]))
         s["graph"].replay()
         s["done"].record()
@@ -380,16 +382,14 @@ class FusedPolicyStep(FusedDqnStep):
     `step()` returns the pinned host tensor that will hold [q1 loss, q2 loss] of the update."""
 
     _loss_width = 2
+    _per_trainers = (SACTrainer, TD3Trainer)  # the exact types it covers, with or without per
+    _index_buffers = 1
 
     def __init__(self, trainer, replay_buffer, batch_size: int, action_low, action_high,
                  online: bool = True, per: Optional[PrioritizedUpdate] = None,
                  rng: str = "device", prefetch: bool = False, slots: int = 2, shard=None,
                  process_group=None):
-        from ..replay_memory.device_replay import DeviceReplay
-        from .sac_trainer import SACTrainer
-        from .td3_trainer import TD3Trainer
-
-        if type(trainer) not in (SACTrainer, TD3Trainer):
+        if type(trainer) not in self._per_trainers:
             raise NotImplementedError("FusedPolicyStep covers SACTrainer and TD3Trainer; got "
                                       + type(trainer).__name__)
         if shard is not None or process_group is not None:
@@ -404,75 +404,33 @@ class FusedPolicyStep(FusedDqnStep):
             raise ValueError("slots must be >= 1")
         if not isinstance(replay_buffer, PrioritizedReplayBuffer):
             raise NotImplementedError("FusedPolicyStep covers the prioritized buffer")
-        self.trainer, self.rb, self.per = trainer, replay_buffer, per
-        self.rng, self.online, self.prefetch, self.pg = "device", bool(online), False, None
-        self.B = self.B_global = batch_size
-        self.row0 = 0
-        self.prioritized = True
-        self.dev = replay_buffer._dev()
         self.action_low = np.asarray(action_low, dtype=np.float32).reshape(-1).copy()
         self.action_high = np.asarray(action_high, dtype=np.float32).reshape(-1).copy()
-        replay_buffer._flush()
-        self.dr = getattr(replay_buffer, "_device_resident", None) or DeviceReplay(
-            replay_buffer, stage_rows=1, stage_slots=max(2, int(slots)))
-        if self.dr.stage_slots < int(slots):
-            self.dr._alloc_stage(self.dr.stage_rows, int(slots))
-        self._idx_buf = [torch.zeros(batch_size, dtype=torch.int64, device=self.dev)]
-        self._status_host = torch.zeros(2, dtype=torch.int32).pin_memory()
-        self._status_np = self._status_host.numpy()
-        self.h2d_bytes = self.dr.h2d_bytes_per_add if self.online else 0
-        self.d2h_bytes = 4 * self._loss_width + 8
-        if per is not None:
-            self.weights = torch.empty(batch_size, dtype=torch.float32, device=self.dev)
-            self.priorities = torch.empty(batch_size, dtype=torch.float64, device=self.dev)
         # a batch_idx of each phase: TD3 with a delayed actor has two, SAC one
         self._delay = int(getattr(trainer, "delayed_policy_update", 1))
         self._phase_batch_idx = [0, 1] if (type(trainer) is TD3Trainer and self._delay != 1) else [0]
         self._updates = 0
-        self.slots, self.k = [], 0
         n0 = trainer.all_batches_processed
-        # warm-up outside capture (lazy allocations, cudaFuncSetAttribute, optimizer state and
-        # the device copies of the action bounds): update 0
-        self._one_update(None)
-        torch.cuda.synchronize()
-        for i in range(int(slots)):
-            self.slots.append(self._capture(i))
+        # its warm-up (which also puts the action bounds on the device) is update 0
+        super().__init__(trainer, replay_buffer, batch_size, slots=slots, rng="device",
+                         online=online, per=per)
         trainer.all_batches_processed = n0 + 1  # a capture runs the Python body, not an update
 
-    def _refresh_tc_images(self):
-        pass  # the actor-critic kernels read the parameters directly: nothing to rebuild
-
-    def _device_sample(self, slot: int, add: bool, stage_row: int = 0):
-        if add:
-            self.dr.launch_add(1, slot=stage_row)
-        idx = self.dr.draw_indices(self.B, out=self._idx_buf[slot])
+    def _gather(self, indices):
         return self.rb.sample_policy_network_batch(self.B, self.action_low, self.action_high,
-                                                   indices=idx)
+                                                   indices=indices)
 
     def _one_update(self, rnd_dev):
-        """One eager update (draw + train) of the next batch_idx, on the current stream."""
+        """One eager update (draw + train) of the next batch_idx, on the current stream: the
+        constructor's warm-up, or an update run outside the captured graphs."""
         self._batch_idx = self._updates
-        loss = self._train(self._device_sample(0, False))
+        loss = super()._one_update(rnd_dev)
         self._updates += 1
         return loss
 
-    def _train(self, batch):
-        if self.per is not None:
-            return self._per_train(batch)
-        closs, _ = self.trainer.train_batch(batch, self._batch_idx)
-        return closs
-
-    def _per_train(self, batch):
-        """Importance weights -> weighted critics -> twin-critic TD-error priority write-back."""
-        idx = self._idx_buf[0]
-        opt = self.trainer.optimizers()[0]  # q1's Adam: its step count anneals beta
-        opt._ensure_state()
-        self.dr.importance_weights(idx, opt.step_t, self.per, self.weights)
-        closs, _ = self.trainer.train_batch(batch, self._batch_idx,
-                                            importance_weights=self.weights)
-        self.dr.write_back_row_priorities(idx, self.trainer._ws["td_error"], 1.0, self.per,
-                                          self.priorities)
-        return closs
+    def _train_batch(self, batch, **weights):
+        """Returns the critic losses; importance weights weight the critics only."""
+        return self.trainer.train_batch(batch, self._batch_idx, **weights)[0]
 
     def _capture(self, i=0):
         graphs, hosts = [], []
@@ -497,6 +455,9 @@ class FusedPolicyStep(FusedDqnStep):
         return out
 
 
+assert set(FusedDqnStep._per_trainers + FusedPolicyStep._per_trainers) == set(_PRIORITY_SOURCES)
+
+
 def capture_device_only(trainer, rb, batch_size, steps, queries_dev, process_group=None,
                         overlap_sampling=True):
     """`steps` consecutive updates in ONE graph with all random numbers already resident in
@@ -506,12 +467,10 @@ def capture_device_only(trainer, rb, batch_size, steps, queries_dev, process_gro
     k (the row-tile kernels leave ~20 SMs and most of HBM idle; sampling does not depend on
     the parameters, and no trainer of the path writes priorities back -- SURVEY.md fact 5)."""
     A = trainer.num_actions
-    prioritized = isinstance(rb, PrioritizedReplayBuffer)
+    kw = _query_keyword(rb)
 
     def sample(k):
-        if prioritized:
-            return rb.sample_discrete_dqn_batch(batch_size, A, query_dev=queries_dev[k])
-        return rb.sample_discrete_dqn_batch(batch_size, A, ranks_dev=queries_dev[k])
+        return rb.sample_discrete_dqn_batch(batch_size, A, **{kw: queries_dev[k]})
 
     g = torch.cuda.CUDAGraph()
     keep = []  # every batch stays alive until the capture ends: no cross-stream block reuse
