@@ -773,11 +773,39 @@ extern "C" int rb200_dqn_td_step_tc(const rb200_mlp_t* q_net, const rb200_mlp_t*
                              : ensure_dynamic_smem(dqn_td_tc_kernel<false>, optin, pl.smem_bytes);
     if (e != cudaSuccess) return check_cuda(e, "cudaFuncSetAttribute(dqn_td_tc)");
   }
+  // Launched at the device's greatest priority.  A CTA of this kernel needs nearly a whole SM
+  // (~210 KB of shared memory, 9 warps at ~160 registers), so when an independent kernel becomes
+  // ready at the same time -- the next update's replay sample in a captured training loop --
+  // and its CTAs are placed first, K2's CTAs wait for them to drain and the whole chain of K2
+  // slips (config 2: 80 us instead of 61 us per launch on an H100).  With the higher priority
+  // the block scheduler places K2's CTAs first and the other kernel fills what is left.  The
+  // priority is recorded in captured graph nodes; it takes effect where the graph is
+  // instantiated with cudaGraphInstantiateFlagUseNodePriority, as torch.cuda.CUDAGraph does.
+  static int greatest[64] = {};
+  static bool have_greatest[64] = {};
+  int dev = 0;
+  if (cudaError_t e = cudaGetDevice(&dev)) return check_cuda(e, "cudaGetDevice");
+  int prio = 0;
+  if (dev >= 0 && dev < 64 && have_greatest[dev]) {
+    prio = greatest[dev];
+  } else {
+    int least = 0;
+    if (cudaError_t e = cudaDeviceGetStreamPriorityRange(&least, &prio))
+      return check_cuda(e, "cudaDeviceGetStreamPriorityRange");
+    if (dev >= 0 && dev < 64) { greatest[dev] = prio; have_greatest[dev] = true; }
+  }
   const Mlp q = make_mlp(q_net), qt = make_mlp(q_target);
-  const int grid = ceil_div(args->batch, kQR);
-  if (weighted)
-    dqn_td_tc_kernel<true><<<grid, kQThreads, pl.smem_bytes, st>>>(q, qt, pl.dev);
-  else
-    dqn_td_tc_kernel<false><<<grid, kQThreads, pl.smem_bytes, st>>>(q, qt, pl.dev);
-  return check_cuda(cudaGetLastError(), "dqn_td_tc_kernel launch");
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3((unsigned)ceil_div(args->batch, kQR));
+  cfg.blockDim = dim3(kQThreads);
+  cfg.dynamicSmemBytes = pl.smem_bytes;
+  cfg.stream = st;
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributePriority;
+  attr[0].val.priority = prio;
+  cfg.attrs = attr;
+  cfg.numAttrs = 1;
+  const cudaError_t e = weighted ? cudaLaunchKernelEx(&cfg, dqn_td_tc_kernel<true>, q, qt, pl.dev)
+                                 : cudaLaunchKernelEx(&cfg, dqn_td_tc_kernel<false>, q, qt, pl.dev);
+  return check_cuda(e, "dqn_td_tc_kernel launch");
 }
