@@ -190,21 +190,10 @@ ac_critic_rows_kernel(const Mlp actor, const Mlp q1, const Mlp q2, const Mlp q1t
   if (tid == 0) {
     float s1 = 0.f, s2 = 0.f;
     for (int r = 0; r < R; ++r) { s1 += rowv[2 * R + r]; s2 += rowv[3 * R + r]; }
-    a.loss_partials[2 * blockIdx.x] = s1;
-    a.loss_partials[2 * blockIdx.x + 1] = s2;
-    __threadfence();
-    const unsigned done = atomicAdd(a.tile_counter, 1u);
-    if (done == gridDim.x - 1) {
-      __threadfence();
-      float t1 = 0.f, t2 = 0.f;
-      for (unsigned i = 0; i < gridDim.x; ++i) {
-        t1 += ((volatile float*)a.loss_partials)[2 * i];
-        t2 += ((volatile float*)a.loss_partials)[2 * i + 1];
-      }
-      a.loss[0] = t1 / (float)B;
-      a.loss[1] = t2 / (float)B;
-      *a.tile_counter = 0u;
-    }
+    finish_serial<2>(a.loss_partials, a.tile_counter, {s1, s2}, [&](const float (&tot)[2]) {
+      a.loss[0] = tot[0] / (float)B;
+      a.loss[1] = tot[1] / (float)B;
+    });
   }
 }
 
@@ -375,49 +364,16 @@ ac_actor_rows_kernel(const Mlp actor, const Mlp q1, const Mlp q2, const AcDev p)
       if (sac && row0 + r < B)
         ent += fminf(fmaxf(rowv[r], kLogProbMin), kLogProbMax) + a.target_entropy;
     }
-    a.loss_partials[2 * blockIdx.x] = s;
-    a.loss_partials[2 * blockIdx.x + 1] = ent;
-    __threadfence();
-    const unsigned done = atomicAdd(a.tile_counter, 1u);
-    if (done == gridDim.x - 1) {
-      __threadfence();
-      float t1 = 0.f, t2 = 0.f;
-      for (unsigned i = 0; i < gridDim.x; ++i) {
-        t1 += ((volatile float*)a.loss_partials)[2 * i];
-        t2 += ((volatile float*)a.loss_partials)[2 * i + 1];
-      }
-      a.loss[0] = t1 * invB;
+    finish_serial<2>(a.loss_partials, a.tile_counter, {s, ent}, [&](const float (&tot)[2]) {
+      a.loss[0] = tot[0] * invB;
       if (sac && a.alpha_grad) {
-        const float m = t2 * invB;            // mean(clamp(logp) + target_entropy)
+        const float m = tot[1] * invB;        // mean(clamp(logp) + target_entropy)
         a.alpha_grad[0] = -m;                 // d/d log_alpha of -(log_alpha * m)
         if (a.log_alpha) a.loss[1] = -((*a.log_alpha) * m);
       }
-      *a.tile_counter = 0u;
-    }
+    });
   }
 }
-
-#define RB200_LAUNCH_ACC(NT_, TM_, KC_, grid, smem, stream, ...)                              \
-  do {                                                                                        \
-    auto kfn = ac_critic_rows_kernel<NT_, TM_, KC_, kWeighted>;                               \
-    static SmemOptIn optin_ = {};                                                             \
-    {                                                                                         \
-      cudaError_t e_ = ensure_dynamic_smem(kfn, optin_, (size_t)(smem));                      \
-      if (e_ != cudaSuccess) return check_cuda(e_, "cudaFuncSetAttribute(ac_critic)");                                       \
-    }                                                                                         \
-    kfn<<<grid, NT_, smem, stream>>>(__VA_ARGS__);                                            \
-  } while (0)
-
-#define RB200_LAUNCH_ACA(NT_, TM_, KC_, grid, smem, stream, ...)                              \
-  do {                                                                                        \
-    auto kfn = ac_actor_rows_kernel<NT_, TM_, KC_>;                                           \
-    static SmemOptIn optin_ = {};                                                             \
-    {                                                                                         \
-      cudaError_t e_ = ensure_dynamic_smem(kfn, optin_, (size_t)(smem));                      \
-      if (e_ != cudaSuccess) return check_cuda(e_, "cudaFuncSetAttribute(ac_actor)");                                       \
-    }                                                                                         \
-    kfn<<<grid, NT_, smem, stream>>>(__VA_ARGS__);                                            \
-  } while (0)
 
 static int ac_common_checks(const rb200_mlp_t* actor, const rb200_mlp_t* q1, const rb200_mlp_t* q2,
                             const rb200_ac_args_t* a) {
@@ -446,14 +402,6 @@ static RowsCfg ac_cfg(const rb200_mlp_t* actor, const rb200_mlp_t* q1, const rb2
   const int NO = actor->dims[actor->n_layers];
   *ld_o = round_up4(NO > 8 ? NO : 8) + 12;  // room for a 1-wide dz quad + an A-wide gradient
   return pick_rows_cfg(batch, q1->dims[0], hmax, 1, 3, n_out_tiles * (*ld_o) + 16 + 4, 0);
-}
-
-template <bool kWeighted>
-static int launch_ac_critic(const RowsCfg& cfg, int grid, cudaStream_t st, const Mlp& ma,
-                            const Mlp& m1, const Mlp& m2, const Mlp& t1, const Mlp& t2,
-                            const AcDev& p) {
-  RB200_DISPATCH_ROWS(cfg, RB200_LAUNCH_ACC, grid, cfg.smem_bytes, st, ma, m1, m2, t1, t2, p);
-  return check_cuda(cudaGetLastError(), "ac_critic_rows_kernel launch");
 }
 
 }  // namespace rb200
@@ -485,9 +433,15 @@ extern "C" int rb200_ac_critic_step(const rb200_mlp_t* actor, const rb200_mlp_t*
   const int grid = ceil_div(args->batch, rows_per_tile(cfg));
   cudaStream_t st = (cudaStream_t)stream;
   // prioritized replay: weights and / or TD errors take the weighted instantiation
-  return (args->sample_weight || args->td_error_out)
-             ? launch_ac_critic<true>(cfg, grid, st, ma, m1, m2, t1, t2, p)
-             : launch_ac_critic<false>(cfg, grid, st, ma, m1, m2, t1, t2, p);
+  const bool weighted = args->sample_weight || args->td_error_out;
+  return dispatch_rows(cfg, [&](auto NT, auto KC) {
+    const char* what = "ac_critic_rows_kernel launch";
+    return weighted
+               ? launch<ac_critic_rows_kernel<NT(), 4, KC(), true>>(grid, NT(), cfg.smem_bytes, st,
+                                                                     what, ma, m1, m2, t1, t2, p)
+               : launch<ac_critic_rows_kernel<NT(), 4, KC(), false>>(grid, NT(), cfg.smem_bytes, st,
+                                                                      what, ma, m1, m2, t1, t2, p);
+  });
 }
 
 extern "C" int rb200_ac_actor_step(const rb200_mlp_t* actor, const rb200_mlp_t* q1,
@@ -510,6 +464,8 @@ extern "C" int rb200_ac_actor_step(const rb200_mlp_t* actor, const rb200_mlp_t* 
   const Mlp ma = make_mlp(actor), m1 = make_mlp(q1), m2 = make_mlp(q2 ? q2 : q1);
   const int grid = ceil_div(args->batch, rows_per_tile(cfg));
   cudaStream_t st = (cudaStream_t)stream;
-  RB200_DISPATCH_ROWS(cfg, RB200_LAUNCH_ACA, grid, cfg.smem_bytes, st, ma, m1, m2, p);
-  return check_cuda(cudaGetLastError(), "ac_actor_rows_kernel launch");
+  return dispatch_rows(cfg, [&](auto NT, auto KC) {
+    return launch<ac_actor_rows_kernel<NT(), 4, KC()>>(grid, NT(), cfg.smem_bytes, st,
+                                                       "ac_actor_rows_kernel launch", ma, m1, m2, p);
+  });
 }

@@ -117,26 +117,93 @@ __device__ __forceinline__ void warp_row_max_sumexp(const Row& x, int n, float& 
   sum = warp_sum(s);
 }
 
-// Dynamic shared-memory opt-in of a kernel, remembered PER DEVICE (the attribute is per device
-// and per function): a high-water mark indexed by the current device id, so the first launch on
-// a second GPU of the same process opts in as well.  Racing threads at worst set the attribute
-// twice.  Raised outside CUDA-graph capture by the first eager call.
-struct SmemOptIn {
-  size_t configured[64];
-};
-template <typename Kernel>
-inline cudaError_t ensure_dynamic_smem(Kernel kernel, SmemOptIn& st, size_t bytes) {
-  int dev = 0;
-  cudaError_t e = cudaGetDevice(&dev);
-  if (e != cudaSuccess) return e;
-  if (dev >= 0 && dev < 64 && st.configured[dev] >= bytes) return cudaSuccess;
-  e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
-  if (e == cudaSuccess && dev >= 0 && dev < 64) st.configured[dev] = bytes;
-  return e;
+// ----------------------------------------------------------------------------
+// deterministic loss means
+// ----------------------------------------------------------------------------
+// A loss kernel's mean over the batch: every block publishes its partial(s) to `partials`, and
+// the last block to take `counter` sums them in a fixed order, hands the totals to `fin` and
+// re-arms the counter for the next launch.  There are two summation orders, and each kernel keeps
+// the one it has, since another order changes the loss bits:
+//   finish_serial, called by ONE thread of each block: kCh partials per block at
+//     partials[kCh * block + c]; the last block's thread adds each channel in block order.
+//   finish_block, called by ALL threads (one CTA per batch row, so grids of thousands of
+//     blocks): `mine` is read from thread 0; the last block's thread t adds load(i, partials[i])
+//     over i = t, t + blockDim, ..., the warps combine with warp_sum, and thread 0 adds the warp
+//     sums in order into s_warp[blockDim / 32] (the caller's shared memory).  One thread walking
+//     4096 dependent loads instead cost ~20 us of kernel tail.
+template <int kCh, typename Fin>
+__device__ __forceinline__ void finish_serial(float* partials, uint32_t* counter,
+                                              const float (&mine)[kCh], Fin fin) {
+#pragma unroll
+  for (int c = 0; c < kCh; ++c) partials[kCh * blockIdx.x + c] = mine[c];
+  __threadfence();
+  if (atomicAdd(counter, 1u) == gridDim.x - 1) {
+    __threadfence();
+    float tot[kCh] = {};
+    for (unsigned i = 0; i < gridDim.x; ++i) {
+#pragma unroll
+      for (int c = 0; c < kCh; ++c) tot[c] += ((volatile float*)partials)[kCh * i + c];
+    }
+    fin(tot);
+    *counter = 0u;
+  }
+}
+
+template <typename Load, typename Fin>
+__device__ __forceinline__ void finish_block(float* partials, uint32_t* counter, float mine,
+                                             float* s_warp, bool& s_last, Load load, Fin fin) {
+  const unsigned tid = threadIdx.x;
+  if (tid == 0) {
+    partials[blockIdx.x] = mine;
+    __threadfence();
+    s_last = atomicAdd(counter, 1u) == gridDim.x - 1;
+  }
+  __syncthreads();
+  if (s_last) {
+    __threadfence();
+    float tot = 0.f;
+    for (unsigned i = tid; i < gridDim.x; i += blockDim.x) tot += load(i, ((volatile float*)partials)[i]);
+    tot = warp_sum(tot);
+    __syncthreads();
+    if ((tid & 31) == 0) s_warp[tid >> 5] = tot;
+    __syncthreads();
+    if (tid == 0) {
+      float t2 = 0.f;
+      for (int w = 0; w < (int)(blockDim.x >> 5); ++w) t2 += s_warp[w];
+      fin(t2);
+      *counter = 0u;
+    }
+  }
 }
 
 // Error plumbing shared by the C-ABI translation units.
 void set_last_error(const char* fmt, ...);
 int check_cuda(cudaError_t e, const char* what);
+
+// Dynamic shared-memory opt-in of `Kernel`, remembered PER DEVICE (the attribute is per device
+// and per function): a high-water mark indexed by the current device id, so the first launch on
+// a second GPU of the same process opts in as well.  Racing threads at worst set the attribute
+// twice.  Raised outside CUDA-graph capture by the first eager call.
+template <auto Kernel>
+inline cudaError_t opt_in_smem(size_t bytes) {
+  static size_t configured[64] = {};
+  int dev = 0;
+  cudaError_t e = cudaGetDevice(&dev);
+  if (e != cudaSuccess) return e;
+  if (dev >= 0 && dev < 64 && configured[dev] >= bytes) return cudaSuccess;
+  e = cudaFuncSetAttribute(Kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
+  if (e == cudaSuccess && dev >= 0 && dev < 64) configured[dev] = bytes;
+  return e;
+}
+
+// Opts `Kernel` in to `smem` bytes of dynamic shared memory and launches it; errors of either
+// step are reported under `what`.
+template <auto Kernel, typename... Args>
+inline int launch(dim3 grid, dim3 block, size_t smem, cudaStream_t st, const char* what,
+                  Args... args) {
+  if (cudaError_t e = opt_in_smem<Kernel>(smem)) return check_cuda(e, what);
+  Kernel<<<grid, block, smem, st>>>(args...);
+  return check_cuda(cudaGetLastError(), what);
+}
 
 }  // namespace rb200

@@ -87,22 +87,11 @@ __global__ void __launch_bounds__(256) cpe_heads_kernel(const CpeDev d) {
   if (threadIdx.x == 0) {
     float r = 0.f, q = 0.f;
     for (int w = 0; w < 8; ++w) { r += s_r[w]; q += s_q[w]; }
-    a.loss_partials[2 * blockIdx.x] = r;
-    a.loss_partials[2 * blockIdx.x + 1] = q;
-    __threadfence();
-    const unsigned fin = atomicAdd(a.tile_counter, 1u);
-    if (fin == gridDim.x - 1) {
-      __threadfence();
-      float tr = 0.f, tq = 0.f;
-      for (unsigned i = 0; i < gridDim.x; ++i) {
-        tr += ((volatile float*)a.loss_partials)[2 * i];
-        tq += ((volatile float*)a.loss_partials)[2 * i + 1];
-      }
+    finish_serial<2>(a.loss_partials, a.tile_counter, {r, q}, [&](const float (&tot)[2]) {
       const float inv = 1.f / ((float)a.batch * (float)M);
-      a.loss[0] = tr * inv;
-      a.loss[1] = tq * inv;
-      *a.tile_counter = 0u;
-    }
+      a.loss[0] = tot[0] * inv;
+      a.loss[1] = tot[1] * inv;
+    });
   }
 }
 

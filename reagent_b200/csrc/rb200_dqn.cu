@@ -133,16 +133,8 @@ dqn_td_rows_kernel(const Mlp q, const Mlp qt, const DqnDev p) {
   if (tid == 0) {
     float s = 0.f;
     for (int r = 0; r < R; ++r) s += rowv[R + r];
-    a.loss_partials[blockIdx.x] = s;
-    __threadfence();
-    const unsigned done = atomicAdd(a.tile_counter, 1u);
-    if (done == gridDim.x - 1) {
-      __threadfence();
-      float tot = 0.f;
-      for (unsigned i = 0; i < gridDim.x; ++i) tot += ((volatile float*)a.loss_partials)[i];
-      *a.loss = tot / (float)B;
-      *a.tile_counter = 0u;
-    }
+    finish_serial<1>(a.loss_partials, a.tile_counter, {s},
+                     [&](const float (&tot)[1]) { *a.loss = tot[0] / (float)B; });
   }
 
   // ---- backward: dZ chain of q_network ----
@@ -151,29 +143,11 @@ dqn_td_rows_kernel(const Mlp q, const Mlp qt, const DqnDev p) {
                          nullptr, 0, 0, 0);
 }
 
-#define RB200_LAUNCH_DQN(NT_, TM_, KC_, grid, smem, stream, ...)                                   \
-  do {                                                                                        \
-    auto kfn = dqn_td_rows_kernel<NT_, TM_, KC_, kWeighted>;                                       \
-    static SmemOptIn optin_ = {};                                                             \
-    {                                                                                         \
-      cudaError_t e_ = ensure_dynamic_smem(kfn, optin_, (size_t)(smem));                      \
-      if (e_ != cudaSuccess) return check_cuda(e_, "cudaFuncSetAttribute(dqn)");                                       \
-    }                                                                                         \
-    kfn<<<grid, NT_, smem, stream>>>(__VA_ARGS__);                                       \
-  } while (0)
-
 static RowsCfg dqn_cfg(const rb200_mlp_t* q, int batch, int* ld_q) {
   const int A = q->dims[q->n_layers];
   *ld_q = round_up4(A) + 4;
   // 1 input tile, 3 hidden tiles, 3 q tiles + 2 scalars per row
   return pick_rows_cfg(batch, q->dims[0], mlp_max_hidden(q), 1, 3, 3 * (*ld_q) + 2, 0);
-}
-
-template <bool kWeighted>
-static int launch_dqn_rows(const RowsCfg& cfg, int grid, cudaStream_t st, const Mlp& q,
-                           const Mlp& qt, const DqnDev& p) {
-  RB200_DISPATCH_ROWS(cfg, RB200_LAUNCH_DQN, grid, cfg.smem_bytes, st, q, qt, p);
-  return check_cuda(cudaGetLastError(), "dqn_td_rows_kernel launch");
 }
 
 }  // namespace rb200
@@ -211,8 +185,15 @@ extern "C" int rb200_dqn_td_step(const rb200_mlp_t* q_net, const rb200_mlp_t* q_
   const Mlp q = make_mlp(q_net), qt = make_mlp(q_target);
   const int grid = ceil_div(args->batch, rows_per_tile(cfg));
   cudaStream_t st = (cudaStream_t)stream;
-  return args->sample_weight ? launch_dqn_rows<true>(cfg, grid, st, q, qt, p)
-                             : launch_dqn_rows<false>(cfg, grid, st, q, qt, p);
+  const bool weighted = args->sample_weight != nullptr;
+  return dispatch_rows(cfg, [&](auto NT, auto KC) {
+    const char* what = "dqn_td_rows_kernel launch";
+    return weighted
+               ? launch<dqn_td_rows_kernel<NT(), 4, KC(), true>>(grid, NT(), cfg.smem_bytes, st,
+                                                                  what, q, qt, p)
+               : launch<dqn_td_rows_kernel<NT(), 4, KC(), false>>(grid, NT(), cfg.smem_bytes, st,
+                                                                   what, q, qt, p);
+  });
 }
 
 extern "C" int rb200_num_row_tiles(int batch, int max_dim_in, int max_dim_hidden) {

@@ -568,16 +568,8 @@ dqn_td_tc_kernel(const Mlp q, const Mlp qt, const QDev p) {
     if (tid == 0) {
       float loss_partial = 0.f;
       for (int w = 0; w < kQEpiThreads / 32; ++w) loss_partial += scal_s[kQR * 4 + w];
-      a.loss_partials[blockIdx.x] = loss_partial;
-      __threadfence();
-      const unsigned fin = atomicAdd(a.tile_counter, 1u);
-      if (fin == gridDim.x - 1) {
-        __threadfence();
-        float tot = 0.f;
-        for (unsigned i = 0; i < gridDim.x; ++i) tot += ((volatile float*)a.loss_partials)[i];
-        *a.loss = tot / (float)B;
-        *a.tile_counter = 0u;
-      }
+      finish_serial<1>(a.loss_partials, a.tile_counter, {loss_partial},
+                       [&](const float (&tot)[1]) { *a.loss = tot[0] / (float)B; });
     }
   }
 }
@@ -765,14 +757,10 @@ extern "C" int rb200_dqn_td_step_tc(const rb200_mlp_t* q_net, const rb200_mlp_t*
   pl.dev.ws = *ws;
   pl.dev.pack = static_cast<const unsigned char*>(pack_ws);
   cudaStream_t st = (cudaStream_t)stream;
-  // per device; raised outside graph capture by the first eager call
-  static SmemOptIn optin = {}, optin_w = {};
   const bool weighted = args->sample_weight != nullptr;
-  {
-    cudaError_t e = weighted ? ensure_dynamic_smem(dqn_td_tc_kernel<true>, optin_w, pl.smem_bytes)
-                             : ensure_dynamic_smem(dqn_td_tc_kernel<false>, optin, pl.smem_bytes);
-    if (e != cudaSuccess) return check_cuda(e, "cudaFuncSetAttribute(dqn_td_tc)");
-  }
+  if (cudaError_t e = weighted ? opt_in_smem<dqn_td_tc_kernel<true>>(pl.smem_bytes)
+                               : opt_in_smem<dqn_td_tc_kernel<false>>(pl.smem_bytes))
+    return check_cuda(e, "cudaFuncSetAttribute(dqn_td_tc)");
   // Launched at the device's greatest priority.  A CTA of this kernel needs nearly a whole SM
   // (~210 KB of shared memory, 9 warps at ~160 registers), so when an independent kernel becomes
   // ready at the same time -- the next update's replay sample in a captured training loop --

@@ -70,16 +70,8 @@ __global__ void __launch_bounds__(256) pdqn_head_kernel(const PdqnDev d) {
   if (threadIdx.x == 0) {
     float t = 0.f;
     for (int w = 0; w < 8; ++w) t += s_l[w];
-    a.loss_partials[blockIdx.x] = t;
-    __threadfence();
-    const unsigned fin = atomicAdd(a.tile_counter, 1u);
-    if (fin == gridDim.x - 1) {
-      __threadfence();
-      float tot = 0.f;
-      for (unsigned i = 0; i < gridDim.x; ++i) tot += ((volatile float*)a.loss_partials)[i];
-      *a.loss = tot / (float)a.batch;
-      *a.tile_counter = 0u;
-    }
+    finish_serial<1>(a.loss_partials, a.tile_counter, {t},
+                     [&](const float (&tot)[1]) { *a.loss = tot[0] / (float)a.batch; });
   }
 }
 
@@ -225,36 +217,13 @@ __global__ void __launch_bounds__(256) c51_head_kernel(const C51Dev d) {
   le = warp_sum(le);
   if ((tid & 31) == 0) s_l[tid >> 5] = le;
   __syncthreads();
-  if (tid == 0) {
-    float t = 0.f;
+  float t = 0.f;
+  if (tid == 0)
     for (int w = 0; w < (int)(blockDim.x >> 5); ++w) t += s_l[w];
-    a.loss_partials[b] = t;
-    __threadfence();
-    const unsigned fin = atomicAdd(a.tile_counter, 1u);
-    s_last = fin == gridDim.x - 1;
-  }
-  __syncthreads();
-  if (s_last) {
-    // one CTA per row: the last one adds the per-row partials with all its threads (thread t
-    // takes rows t, t + blockDim, ...; fixed combination order) instead of one thread walking
-    // `batch` dependent loads at the tail of the kernel
-    __threadfence();
-    float tot = 0.f;
-    for (unsigned i = tid; i < gridDim.x; i += blockDim.x) {
-      const float p = ((volatile float*)a.loss_partials)[i];
-      tot += kWeighted ? __fmul_rn(p, a.sample_weight[i]) : p;
-    }
-    tot = warp_sum(tot);
-    __syncthreads();
-    if ((tid & 31) == 0) s_l[tid >> 5] = tot;
-    __syncthreads();
-    if (tid == 0) {
-      float t2 = 0.f;
-      for (int w = 0; w < (int)(blockDim.x >> 5); ++w) t2 += s_l[w];
-      *a.loss = t2 * invB;
-      *a.tile_counter = 0u;
-    }
-  }
+  finish_block(
+      a.loss_partials, a.tile_counter, t, s_l, s_last,
+      [&](unsigned i, float p) { return kWeighted ? __fmul_rn(p, a.sample_weight[i]) : p; },
+      [&](float t2) { *a.loss = t2 * invB; });
 }
 
 // ---------------------------------------------------------------------------
@@ -301,36 +270,17 @@ __global__ void __launch_bounds__(32 * kBcRowsPerBlock) bc_xent_head_kernel(cons
       }
     }
   }
-  // deterministic mean: per-block partial of the rows in warp order, then the last block to
-  // finish adds the partials in block order (pdqn_head_kernel's pattern)
+  // deterministic mean: per-block partial of the rows in warp order, then finish_block
   __shared__ float s_l[kBcRowsPerBlock];
   __shared__ bool s_last;
   if (lane == 0) s_l[warp] = le;
   __syncthreads();
-  if (tid == 0) {
-    float t = 0.f;
+  float t = 0.f;
+  if (tid == 0)
     for (int w = 0; w < kBcRowsPerBlock; ++w) t += s_l[w];
-    a.loss_partials[blockIdx.x] = t;
-    __threadfence();
-    const unsigned fin = atomicAdd(a.tile_counter, 1u);
-    s_last = fin == gridDim.x - 1;
-  }
-  __syncthreads();
-  if (s_last) {
-    __threadfence();
-    float tot = 0.f;
-    for (unsigned i = tid; i < gridDim.x; i += blockDim.x) tot += ((volatile float*)a.loss_partials)[i];
-    tot = warp_sum(tot);
-    __syncthreads();
-    if (lane == 0) s_l[warp] = tot;
-    __syncthreads();
-    if (tid == 0) {
-      float t2 = 0.f;
-      for (int w = 0; w < kBcRowsPerBlock; ++w) t2 += s_l[w];
-      *a.loss = t2 / (float)a.batch;
-      *a.tile_counter = 0u;
-    }
-  }
+  finish_block(
+      a.loss_partials, a.tile_counter, t, s_l, s_last, [](unsigned, float p) { return p; },
+      [&](float t2) { *a.loss = t2 / (float)a.batch; });
 }
 
 }  // namespace rb200
@@ -374,16 +324,8 @@ extern "C" int rb200_c51_head(const rb200_c51_args_t* a, void* stream) {
   d.a = *a;
   const size_t smem = ((size_t)3 * a->num_actions * a->num_atoms + 2 * a->num_atoms + a->num_actions) * sizeof(float);
   if (smem > 200 * 1024) { set_last_error("rb200_c51_head: too many atoms/actions for one CTA"); return RB200_E_SMEM; }
-  static SmemOptIn optin = {}, optin_w = {};
-  const bool weighted = a->sample_weight != nullptr;
-  if (smem > 48 * 1024) {
-    cudaError_t e = weighted ? ensure_dynamic_smem(c51_head_kernel<true>, optin_w, smem)
-                             : ensure_dynamic_smem(c51_head_kernel<false>, optin, smem);
-    if (e != cudaSuccess) return check_cuda(e, "cudaFuncSetAttribute(c51_head)");
-  }
-  if (weighted)
-    c51_head_kernel<true><<<a->batch, 256, smem, (cudaStream_t)stream>>>(d);
-  else
-    c51_head_kernel<false><<<a->batch, 256, smem, (cudaStream_t)stream>>>(d);
-  return check_cuda(cudaGetLastError(), "c51_head_kernel launch");
+  cudaStream_t st = (cudaStream_t)stream;
+  const char* what = "c51_head_kernel launch";
+  return a->sample_weight ? launch<c51_head_kernel<true>>(a->batch, 256, smem, st, what, d)
+                          : launch<c51_head_kernel<false>>(a->batch, 256, smem, st, what, d);
 }

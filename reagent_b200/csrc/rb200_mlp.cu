@@ -48,17 +48,6 @@ __global__ void __launch_bounds__(NT, 1) mlp_fwd_rows_kernel(const Mlp net, cons
   tile_store_rows<NT, R>(xo, p.ld_o, p.out, DO, DO, row0, p.batch);
 }
 
-#define RB200_LAUNCH_FWD(NT_, TM_, KC_, grid, smem, stream, ...)                                   \
-  do {                                                                                        \
-    auto kfn = mlp_fwd_rows_kernel<NT_, TM_, KC_>;                                                 \
-    static SmemOptIn optin_ = {};                                                             \
-    {                                                                                         \
-      cudaError_t e_ = ensure_dynamic_smem(kfn, optin_, (size_t)(smem));                      \
-      if (e_ != cudaSuccess) return check_cuda(e_, "cudaFuncSetAttribute(mlp_fwd)");                                       \
-    }                                                                                         \
-    kfn<<<grid, NT_, smem, stream>>>(__VA_ARGS__);                                       \
-  } while (0)
-
 }  // namespace rb200
 
 using namespace rb200;
@@ -87,6 +76,8 @@ extern "C" int rb200_mlp_forward(const rb200_mlp_t* net, const float* in0, int32
   const Mlp m = make_mlp(net);
   const int grid = ceil_div(batch, rows_per_tile(cfg));
   cudaStream_t st = (cudaStream_t)stream;
-  RB200_DISPATCH_ROWS(cfg, RB200_LAUNCH_FWD, grid, cfg.smem_bytes, st, m, p);
-  return check_cuda(cudaGetLastError(), "mlp_fwd_rows_kernel launch");
+  return dispatch_rows(cfg, [&](auto NT, auto KC) {
+    return launch<mlp_fwd_rows_kernel<NT(), 4, KC()>>(grid, NT(), cfg.smem_bytes, st,
+                                                      "mlp_fwd_rows_kernel launch", m, p);
+  });
 }

@@ -247,36 +247,13 @@ __global__ void __launch_bounds__(256) qr_head_kernel(const QrDev d) {
   lsum = warp_sum(lsum);
   if ((tid & 31) == 0) red[tid >> 5] = lsum;
   __syncthreads();
-  if (tid == 0) {
-    float s = 0.f;
+  float s = 0.f;
+  if (tid == 0)
     for (int i = 0; i < (int)blockDim.x / 32; ++i) s += red[i];
-    a.loss_partials[b] = s;
-    __threadfence();
-    const unsigned done = atomicAdd(a.tile_counter, 1u);
-    s_last = done == gridDim.x - 1;
-  }
-  __syncthreads();
-  if (s_last) {
-    // the last row's CTA adds the per-row partials: thread t takes rows t, t + 256, ... and the
-    // block combines them in a fixed order (deterministic, and off one thread's critical path:
-    // 4096 dependent loads by a single thread were ~20 us of kernel tail)
-    __threadfence();
-    float tot = 0.f;
-    for (unsigned i = tid; i < gridDim.x; i += blockDim.x) {
-      const float p = ((volatile float*)a.loss_partials)[i];
-      tot += kWeighted ? __fmul_rn(p, a.sample_weight[i]) : p;
-    }
-    tot = warp_sum(tot);
-    __syncthreads();
-    if ((tid & 31) == 0) red[tid >> 5] = tot;
-    __syncthreads();
-    if (tid == 0) {
-      float t2 = 0.f;
-      for (int i = 0; i < (int)blockDim.x / 32; ++i) t2 += red[i];
-      *a.loss = t2 * norm;
-      *a.tile_counter = 0u;
-    }
-  }
+  finish_block(
+      a.loss_partials, a.tile_counter, s, red, s_last,
+      [&](unsigned i, float p) { return kWeighted ? __fmul_rn(p, a.sample_weight[i]) : p; },
+      [&](float t2) { *a.loss = t2 * norm; });
   // mean over atoms of q(s) for reporting (all_q_values, :146)
   if (a.all_q_values) {
     for (int act = tid >> 5; act < A; act += 8) {
@@ -285,26 +262,6 @@ __global__ void __launch_bounds__(256) qr_head_kernel(const QrDev d) {
     }
   }
 }
-
-#define RB200_LAUNCH_GENERIC(KERN, TAG)                                                         \
-  template <int NT_, int TM_, int KC_, typename... Args>                                        \
-  static int launch_##TAG(dim3 grid, size_t smem, cudaStream_t st, Args... args) {              \
-    auto kfn = KERN<NT_, TM_, KC_>;                                                             \
-    static SmemOptIn optin_ = {};                                                               \
-    {                                                                                           \
-      cudaError_t e_ = ensure_dynamic_smem(kfn, optin_, smem);                                  \
-      if (e_ != cudaSuccess) return check_cuda(e_, "cudaFuncSetAttribute(" #TAG ")");           \
-    }                                                                                           \
-    kfn<<<grid, NT_, smem, st>>>(args...);                                                      \
-    return RB200_OK;                                                                            \
-  }
-RB200_LAUNCH_GENERIC(linear_fwd_wide_kernel, linfwd)
-RB200_LAUNCH_GENERIC(linear_bwd_wide_kernel, linbwd)
-RB200_LAUNCH_GENERIC(mlp_bwd_rows_kernel, mlpbwd)
-
-#define RB200_DISPATCH_FN(cfg, FN, ...)                                                         \
-  ((cfg).nt == 512 ? ((cfg).kc == 32 ? FN<512, 4, 32>(__VA_ARGS__) : FN<512, 4, 16>(__VA_ARGS__)) \
-                   : ((cfg).kc == 32 ? FN<256, 4, 32>(__VA_ARGS__) : FN<256, 4, 16>(__VA_ARGS__)))
 
 }  // namespace rb200
 
@@ -326,9 +283,10 @@ extern "C" int rb200_linear_forward(const float* W, const float* b, int32_t act,
   if (cfg.tm == 0) { set_last_error("rb200_linear_forward: tile does not fit in shared memory"); return RB200_E_SMEM; }
   p.ld_in = cfg.ld_in;
   dim3 grid(ceil_div(batch, rows_per_tile(cfg)), ceil_div(N, kColBlock));
-  int rc = RB200_DISPATCH_FN(cfg, launch_linfwd, grid, cfg.smem_bytes, (cudaStream_t)stream, p);
-  if (rc) return rc;
-  return check_cuda(cudaGetLastError(), "linear_fwd_wide_kernel launch");
+  return dispatch_rows(cfg, [&](auto NT, auto KC) {
+    return launch<linear_fwd_wide_kernel<NT(), 4, KC()>>(grid, NT(), cfg.smem_bytes, (cudaStream_t)stream,
+                                                         "linear_fwd_wide_kernel launch", p);
+  });
 }
 
 extern "C" int rb200_linear_backward_dx(const float* W, int32_t K, int32_t N, const float* dz,
@@ -340,9 +298,10 @@ extern "C" int rb200_linear_backward_dx(const float* W, int32_t K, int32_t N, co
   if (cfg.tm == 0) { set_last_error("rb200_linear_backward_dx: tile does not fit in shared memory"); return RB200_E_SMEM; }
   p.ld_z = cfg.ld_in;
   dim3 grid(ceil_div(batch, rows_per_tile(cfg)));
-  int rc = RB200_DISPATCH_FN(cfg, launch_linbwd, grid, cfg.smem_bytes, (cudaStream_t)stream, p);
-  if (rc) return rc;
-  return check_cuda(cudaGetLastError(), "linear_bwd_wide_kernel launch");
+  return dispatch_rows(cfg, [&](auto NT, auto KC) {
+    return launch<linear_bwd_wide_kernel<NT(), 4, KC()>>(grid, NT(), cfg.smem_bytes, (cudaStream_t)stream,
+                                                         "linear_bwd_wide_kernel launch", p);
+  });
 }
 
 extern "C" int rb200_mlp_backward(const rb200_mlp_t* net, const float* dz_last, int32_t batch,
@@ -361,9 +320,10 @@ extern "C" int rb200_mlp_backward(const rb200_mlp_t* net, const float* dz_last, 
   p.ld_h = cfg.ld_h;
   const Mlp m = make_mlp(net);
   dim3 grid(ceil_div(batch, rows_per_tile(cfg)));
-  int rc = RB200_DISPATCH_FN(cfg, launch_mlpbwd, grid, cfg.smem_bytes, (cudaStream_t)stream, m, p);
-  if (rc) return rc;
-  return check_cuda(cudaGetLastError(), "mlp_bwd_rows_kernel launch");
+  return dispatch_rows(cfg, [&](auto NT, auto KC) {
+    return launch<mlp_bwd_rows_kernel<NT(), 4, KC()>>(grid, NT(), cfg.smem_bytes, (cudaStream_t)stream,
+                                                      "mlp_bwd_rows_kernel launch", m, p);
+  });
 }
 
 extern "C" int rb200_qrdqn_head(const rb200_qrdqn_args_t* a, void* stream) {

@@ -417,9 +417,8 @@ __global__ void __launch_bounds__(kSetThreads) sumtree_leaves_kernel(double* tre
 
 static int sumtree_update(double* tree, int depth, const SetSrc& s, double* max_recorded,
                           int* status, cudaStream_t st) {
-  static SmemOptIn optin_levels = {}, optin_leaves = {};
-  cudaError_t e = ensure_dynamic_smem(sumtree_levels_kernel, optin_levels, kSetSmem);
-  if (e == cudaSuccess) e = ensure_dynamic_smem(sumtree_leaves_kernel, optin_leaves, kSetSmem);
+  cudaError_t e = opt_in_smem<sumtree_levels_kernel>(kSetSmem);
+  if (e == cudaSuccess) e = opt_in_smem<sumtree_leaves_kernel>(kSetSmem);
   if (e != cudaSuccess) return check_cuda(e, "cudaFuncSetAttribute(sumtree)");
   for (int c0 = 0; c0 < s.n; c0 += kSetChunk) {
     if (depth > 0) sumtree_levels_kernel<<<depth, kSetThreads, kSetSmem, st>>>(tree, depth, s, c0);

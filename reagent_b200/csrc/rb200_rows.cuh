@@ -3,6 +3,8 @@
 #include <stdio.h>
 #include <stdlib.h>
 
+#include <type_traits>
+
 #include "rb200_tile.cuh"
 
 namespace rb200 {
@@ -57,12 +59,15 @@ inline int mlp_max_hidden(const rb200_mlp_t* m) {
   return h;
 }
 
-#define RB200_DISPATCH_ROWS(cfg, KERNEL, ...)                                        \
-  do {                                                                               \
-    if ((cfg).nt == 512 && (cfg).kc == 32) { KERNEL(512, 4, 32, __VA_ARGS__); }      \
-    else if ((cfg).nt == 512 && (cfg).kc == 16) { KERNEL(512, 4, 16, __VA_ARGS__); } \
-    else if ((cfg).nt == 256 && (cfg).kc == 32) { KERNEL(256, 4, 32, __VA_ARGS__); } \
-    else { KERNEL(256, 4, 16, __VA_ARGS__); }                                        \
-  } while (0)
+// Calls f(NT, KC) with the tile of `cfg` as std::integral_constant<int, ...> arguments, so that
+// a call site instantiates its kernel once per tile of pick_rows_cfg (TM is 4 on every tile).
+template <typename F>
+inline auto dispatch_rows(const RowsCfg& cfg, F&& f) {
+  using std::integral_constant;
+  if (cfg.nt == 512 && cfg.kc == 32) return f(integral_constant<int, 512>{}, integral_constant<int, 32>{});
+  if (cfg.nt == 512 && cfg.kc == 16) return f(integral_constant<int, 512>{}, integral_constant<int, 16>{});
+  if (cfg.nt == 256 && cfg.kc == 32) return f(integral_constant<int, 256>{}, integral_constant<int, 32>{});
+  return f(integral_constant<int, 256>{}, integral_constant<int, 16>{});
+}
 
 }  // namespace rb200

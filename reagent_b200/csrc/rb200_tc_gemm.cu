@@ -266,11 +266,8 @@ extern "C" int rb200_linear_backward_dx_tc(const float* W, int32_t K, int32_t N,
   if ((reinterpret_cast<uintptr_t>(scratch) & 15) || (reinterpret_cast<uintptr_t>(out) & 15) ||
       (h_prev && (reinterpret_cast<uintptr_t>(h_prev) & 15))) { set_last_error("rb200_linear_backward_dx_tc: buffers must be 16-byte aligned"); return RB200_E_INVALID; }
   cudaStream_t st = (cudaStream_t)stream;
-  static SmemOptIn optin = {};
-  {
-    cudaError_t e = ensure_dynamic_smem(tc_linear_fwd_kernel, optin, (size_t)kTcSmemBytes);
-    if (e != cudaSuccess) return check_cuda(e, "cudaFuncSetAttribute(tc_linear_fwd)");
-  }
+  if (cudaError_t e = opt_in_smem<tc_linear_fwd_kernel>(kTcSmemBytes))
+    return check_cuda(e, "cudaFuncSetAttribute(tc_linear_fwd)");
   float* Wt = static_cast<float*>(scratch);
   float* partial = Wt + pl.wt_floats;
   tc_transpose_kernel<<<dim3(ceil_div(N, 32), ceil_div(K, 32)), 256, 0, st>>>(W, N, K, Wt);
@@ -288,13 +285,8 @@ extern "C" int rb200_linear_forward_tc(const float* W, const float* b, int32_t a
                                        int32_t N, const float* in, int32_t batch, float* out,
                                        void* stream) {
   if (!W || !in || !out || K <= 0 || N <= 0 || batch <= 0) { set_last_error("rb200_linear_forward_tc: bad argument"); return RB200_E_INVALID; }
-  static SmemOptIn optin = {};
-  {
-    cudaError_t e = ensure_dynamic_smem(tc_linear_fwd_kernel, optin, (size_t)kTcSmemBytes);
-    if (e != cudaSuccess) return check_cuda(e, "cudaFuncSetAttribute(tc_linear_fwd)");
-  }
   TcDev p{in, W, b, out, batch, K, N, act, 0};
   dim3 grid(ceil_div(batch, kTcM), ceil_div(N, kTcN));
-  tc_linear_fwd_kernel<<<grid, kTcThreads, kTcSmemBytes, (cudaStream_t)stream>>>(p);
-  return check_cuda(cudaGetLastError(), "tc_linear_fwd_kernel launch");
+  return launch<tc_linear_fwd_kernel>(grid, kTcThreads, kTcSmemBytes, (cudaStream_t)stream,
+                                      "tc_linear_fwd_kernel launch", p);
 }

@@ -269,12 +269,7 @@ int rb200_wgrad_tc_launch(const rb200_mlp_t* net, const float* net_input, int32_
     jobs += L.tiles_m * L.tiles_k;
   }
   for (int l = net->n_layers; l < kMaxLayers; ++l) p.L[l].job_start = 1 << 30;
-  static SmemOptIn optin = {};
-  {
-    cudaError_t e = ensure_dynamic_smem(wgrad_tc_kernel, optin, (size_t)kWtSmem);
-    if (e != cudaSuccess) return check_cuda(e, "cudaFuncSetAttribute(wgrad_tc)");
-  }
   dim3 grid(jobs, splits);
-  wgrad_tc_kernel<<<grid, kWtThreads, kWtSmem, (cudaStream_t)stream>>>(p);
-  return check_cuda(cudaGetLastError(), "wgrad_tc_kernel launch");
+  return launch<wgrad_tc_kernel>(grid, kWtThreads, kWtSmem, (cudaStream_t)stream,
+                                 "wgrad_tc_kernel launch", p);
 }
