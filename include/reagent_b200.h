@@ -446,8 +446,8 @@ int rb200_grad_reduce(const float* gpart, int32_t splits, int64_t n, float* g, v
 
 /* ------------------------------------------------------------------------- */
 /* K3: fused Adam + soft target update over flat arenas.                        */
-/* Replaces torch.optim.Adam.step (reagent/optimizer/optimizer.py:64-85,        */
-/* uninferrable_optimizers.py:23-33) and SoftUpdate.step                        */
+/* Replaces torch.optim.Adam.step / AdamW.step (reagent/optimizer/optimizer.py: */
+/* 64-85, uninferrable_optimizers.py:23-33, 70-78) and SoftUpdate.step          */
 /* (reagent/optimizer/soft_update.py:47-71) in this order per element:          */
 /* Adam on the source, then target = tau*new_source + (1-tau)*target.           */
 /* `step` is a device int64 counter incremented by the kernel (graph friendly). */
@@ -492,6 +492,15 @@ typedef struct rb200_adam_args {
   uint32_t* const* dp_flags;
   int64_t dp_stride;           /* >= n */
   int32_t dp_max_blocks;       /* >= the grid this call launches (rb200_adam_blocks(n)) */
+  /* Optional: torch.optim.AdamW / AMSGrad (torch/optim/adam.py, _single_tensor_adam).  All zero
+   * is Adam as above.
+   *   decoupled_weight_decay = 1: p = p * float(1 - lr*weight_decay) before the moment updates,
+   *     in place of the coupled g += weight_decay * p.
+   *   amsgrad = 1: max_exp_avg_sq = maximum(max_exp_avg_sq, exp_avg_sq) (NaN propagates, as
+   *     torch.maximum), and the step's denominator is built from it instead of exp_avg_sq. */
+  int32_t decoupled_weight_decay;  /* 0 or 1 */
+  int32_t amsgrad;                 /* 0 or 1 */
+  float* max_exp_avg_sq;           /* [n]; needed when amsgrad = 1 */
 } rb200_adam_args_t;
 int rb200_adam_blocks(int64_t n);
 int rb200_adam_soft_update(const rb200_adam_args_t* a, void* stream);

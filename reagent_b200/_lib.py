@@ -96,6 +96,9 @@ class AdamArgsT(C.Structure):
         ("dp_flags", _vp),
         ("dp_stride", C.c_int64),
         ("dp_max_blocks", C.c_int32),
+        ("decoupled_weight_decay", C.c_int32),
+        ("amsgrad", C.c_int32),
+        ("max_exp_avg_sq", _vp),
     ]
 
 

@@ -198,6 +198,10 @@ __global__ void grad_reduce_kernel(const float* __restrict__ gpart, int splits, 
 //   bc1 = 1 - b1^t, bc2 = 1 - b2^t (double), step_size = lr/bc1
 //   p  -= step_size * m / (sqrt(v)/sqrt(bc2) + eps)
 // then target = tau*p + (1-tau)*target  (SoftUpdate.step on the updated source).
+// kDecoupled (AdamW): no wd term in g; instead p *= float(1 - lr*wd) (double, like Python)
+// before the moment updates.  kAmsgrad: vmax = maximum(vmax, v) with NaN propagating like
+// torch.maximum, and the denominator uses vmax.  Adam is <false, false>: no per-element work
+// is added to it.
 // ---------------------------------------------------------------------------
 struct AdamDev {
   rb200_adam_args_t a;
@@ -221,6 +225,14 @@ __device__ __forceinline__ void adam_pack_weight(const TcPackView& pv, long long
   }
 }
 
+// maximum that returns NaN when either input is NaN (fmaxf returns the other input)
+__device__ __forceinline__ float fmax_nan(float a, float b) {
+  float r;
+  asm("max.NaN.f32 %0, %1, %2;" : "=f"(r) : "f"(a), "f"(b));
+  return r;
+}
+
+template <bool kDecoupled, bool kAmsgrad>
 __global__ void __launch_bounds__(256) adam_soft_kernel(const AdamDev d) {
   const rb200_adam_args_t& a = d.a;
   // bias corrections in double like torch (Python floats), once per block
@@ -245,6 +257,7 @@ __global__ void __launch_bounds__(256) adam_soft_kernel(const AdamDev d) {
   const float b2 = (float)a.beta2;
   const float w2 = (float)(1.0 - a.beta2);
   const float wd = (float)a.weight_decay;
+  const float decay = kDecoupled ? (float)(1.0 - a.lr * a.weight_decay) : 1.f;
   const long long n = a.n;
   const long long stride = (long long)gridDim.x * blockDim.x;
   // split-K partials: loads issued 8 at a time, summed in slab order (deterministic)
@@ -310,7 +323,11 @@ __global__ void __launch_bounds__(256) adam_soft_kernel(const AdamDev d) {
     }
     g *= a.grad_scale;
     float p = a.params[i];
-    if (wd != 0.f) g = fmaf(wd, p, g);
+    if (kDecoupled) {
+      if (wd != 0.f) p = __fmul_rn(p, decay);
+    } else if (wd != 0.f) {
+      g = fmaf(wd, p, g);
+    }
     float m = a.exp_avg[i];
     float v = a.exp_avg_sq[i];
     // rounding mirrors ATen's CPU kernels:
@@ -323,7 +340,12 @@ __global__ void __launch_bounds__(256) adam_soft_kernel(const AdamDev d) {
     const float gm = __fsub_rn(g, m);
     m = w1_small ? fmaf(w1, gm, m) : fmaf(w1m1, gm, g);
     v = __fadd_rn(__fmul_rn(v, b2), __fmul_rn(__fmul_rn(w2, g), g));
-    const float denom = __fadd_rn(__fdiv_rn(__fsqrt_rn(v), bc2_sqrt), eps);
+    float vd = v;
+    if (kAmsgrad) {
+      vd = fmax_nan(a.max_exp_avg_sq[i], v);
+      a.max_exp_avg_sq[i] = vd;
+    }
+    const float denom = __fadd_rn(__fdiv_rn(__fsqrt_rn(vd), bc2_sqrt), eps);
     p = __fadd_rn(p, __fdiv_rn(__fmul_rn(-step_size, m), denom));
     a.params[i] = p;
     a.exp_avg[i] = m;
@@ -447,6 +469,11 @@ extern "C" int rb200_adam_soft_update(const rb200_adam_args_t* a, void* stream) 
     set_last_error("rb200_adam_soft_update: null argument"); return RB200_E_INVALID;
   }
   if (a->n <= 0 || a->splits <= 0) { set_last_error("rb200_adam_soft_update: bad n/splits"); return RB200_E_INVALID; }
+  if ((a->decoupled_weight_decay != 0 && a->decoupled_weight_decay != 1) ||
+      (a->amsgrad != 0 && a->amsgrad != 1)) {
+    set_last_error("rb200_adam_soft_update: decoupled_weight_decay and amsgrad must be 0 or 1"); return RB200_E_INVALID;
+  }
+  if (a->amsgrad && !a->max_exp_avg_sq) { set_last_error("rb200_adam_soft_update: amsgrad needs max_exp_avg_sq"); return RB200_E_INVALID; }
   AdamDev d;
   d.a = *a;
   d.a.tc_net = nullptr;  // host pointer: not for the device
@@ -477,7 +504,10 @@ extern "C" int rb200_adam_soft_update(const rb200_adam_args_t* a, void* stream) 
   } else {
     d.a.dp_world = 1;
   }
-  adam_soft_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(d);
+  void (*kernel)(const AdamDev) =
+      a->decoupled_weight_decay ? (a->amsgrad ? adam_soft_kernel<true, true> : adam_soft_kernel<true, false>)
+                                : (a->amsgrad ? adam_soft_kernel<false, true> : adam_soft_kernel<false, false>);
+  kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(d);
   return check_cuda(cudaGetLastError(), "adam_soft_kernel launch");
 }
 

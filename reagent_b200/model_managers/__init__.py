@@ -1,6 +1,7 @@
 """Model managers: `build_trainer(normalization_data_map, use_gpu, reward_options=None)` with
 the reference's flow (reagent/model_managers/model_manager.py:84-96 and
-discrete/discrete_dqn.py:63-116, discrete/discrete_qrdqn.py:73-121, actor_critic/sac.py:80-113,
+discrete/discrete_dqn.py:63-116, discrete/discrete_qrdqn.py:73-121,
+discrete/discrete_c51dqn.py:43-88, actor_critic/sac.py:80-113,
 actor_critic/td3.py:70-102): build the networks from the net builders, copy the target, hand
 everything to the trainer.  Policies, serving modules, data modules and reporters are out of
 scope (SURVEY.md section 2 rows 8, 12, 15, 16)."""
@@ -9,10 +10,11 @@ from typing import Union, Dict, List, Optional
 
 from ..core.parameters import (EvaluationParameters, NormalizationData, NormalizationKey,
                                RLParameters)
-from ..net_builder import (ActorFullyConnected, Dueling, DuelingQuantile, FullyConnected,
-                           GaussianFullyConnected, ParametricFullyConnected, Quantile)
+from ..net_builder import (ActorFullyConnected, Categorical, Dueling, DuelingQuantile,
+                           FullyConnected, GaussianFullyConnected, ParametricFullyConnected,
+                           Quantile)
 from ..optimizer import Optimizer__Union
-from ..training import DQNTrainer, QRDQNTrainer, SACTrainer, TD3Trainer
+from ..training import C51Trainer, DQNTrainer, QRDQNTrainer, SACTrainer, TD3Trainer
 
 
 def _device(use_gpu: bool):
@@ -106,6 +108,37 @@ class DiscreteQRDQN(_DiscretePolicyMixin):
             rl=self.rl, double_q_learning=self.double_q_learning, num_atoms=self.num_atoms,
             minibatch_size=self.minibatch_size, optimizer=self.optimizer,
             evaluation=self.eval_parameters).to(dev)
+
+
+@dataclass
+class DiscreteC51DQN(_DiscretePolicyMixin):
+    actions: List[str]
+    rl: RLParameters = field(default_factory=RLParameters)
+    double_q_learning: bool = True
+    num_atoms: int = 51
+    qmin: float = -100
+    qmax: float = 200
+    minibatch_size: int = 1024
+    optimizer: Optimizer__Union = field(default_factory=Optimizer__Union.default)
+    net_builder: Categorical = field(default_factory=Categorical)
+
+    def __post_init__(self):
+        # discrete_c51dqn.py:43-48
+        assert len(self.actions) > 1, "DiscreteC51DQN needs at least 2 actions"
+        assert self.minibatch_size % 8 == 0, (
+            "The minibatch size must be divisible by 8 for performance reasons.")
+
+    def build_trainer(self, normalization_data_map, use_gpu: bool, reward_options=None):
+        dev = _device(use_gpu)
+        q_network = self.net_builder.build_q_network(
+            normalization_data_map[NormalizationKey.STATE], len(self.actions), self.num_atoms,
+            self.qmin, self.qmax).to(dev)
+        q_network_target = q_network.get_target_network()
+        return C51Trainer(
+            q_network=q_network, q_network_target=q_network_target, actions=self.actions,
+            rl=self.rl, double_q_learning=self.double_q_learning,
+            minibatch_size=self.minibatch_size, num_atoms=self.num_atoms, qmin=self.qmin,
+            qmax=self.qmax, optimizer=self.optimizer).to(dev)
 
 
 @dataclass

@@ -5,8 +5,8 @@ from dataclasses import dataclass, field
 from typing import List
 
 from ..core.parameters import NormalizationData
-from ..models import (DuelingQNetwork, FullyConnectedActor, FullyConnectedCritic,
-                      FullyConnectedDQN, GaussianFullyConnectedActor)
+from ..models import (CategoricalDQN, DuelingQNetwork, FullyConnectedActor,
+                      FullyConnectedCritic, FullyConnectedDQN, GaussianFullyConnectedActor)
 from ..preprocessing.normalization import get_num_output_features
 
 
@@ -76,6 +76,24 @@ class DuelingQuantile:
         return DuelingQNetwork.make_fully_connected(
             _dim(state_normalization_data), output_dim, layers=self.sizes,
             activations=self.activations, num_atoms=num_atoms)
+
+
+@dataclass
+class Categorical:
+    """reagent/net_builder/categorical_dqn/categorical.py:15-49"""
+    sizes: List[int] = field(default_factory=lambda: [256, 128])
+    activations: List[str] = field(default_factory=lambda: ["relu", "relu"])
+
+    def __post_init__(self):
+        assert len(self.sizes) == len(self.activations), (
+            f"Must have the same numbers of sizes and activations; got: {self.sizes}, {self.activations}")
+
+    def build_q_network(self, state_normalization_data: NormalizationData, output_dim: int,
+                        num_atoms: int, qmin: float, qmax: float):
+        dist = FullyConnectedDQN(state_dim=_dim(state_normalization_data), action_dim=output_dim,
+                                 sizes=self.sizes, activations=self.activations,
+                                 num_atoms=num_atoms)
+        return CategoricalDQN(dist, qmin=qmin, qmax=qmax, num_atoms=num_atoms)
 
 
 @dataclass

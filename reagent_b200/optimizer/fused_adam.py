@@ -1,4 +1,4 @@
-"""Adam over a flat parameter arena, one fused CUDA launch per step (K3).
+"""Adam and AdamW over a flat parameter arena, one fused CUDA launch per step (K3).
 
 Numerics follow torch.optim.Adam's single-tensor path, which is what the reference gets
 from `Optimizer__Union.default()` -> `torch.optim.Adam(lr=1e-3, betas=(0.9, 0.999),
@@ -6,6 +6,10 @@ eps=1e-8, weight_decay=0, amsgrad=False)` (reagent/optimizer/optimizer.py:64-85,
 reagent/optimizer/uninferrable_optimizers.py:23-33).  Gradients are NOT read from
 `p.grad`: the trainer's fused backward leaves split-K partials in `arena.gpart`, which the
 kernel sums in a fixed order (deterministic) before the update.
+
+FusedAdamW is the counterpart of torch.optim.AdamW (decoupled weight decay, optional AMSGrad),
+which the reference's CartPole QR-DQN / C51 configurations select with
+`AdamW: {lr: 0.001, amsgrad: true}` (reagent/optimizer/uninferrable_optimizers.py:70-78).
 """
 from typing import Optional
 
@@ -17,15 +21,22 @@ from ..models.arena import ParamArena, ScalarArena, arena_of
 
 _TORCH_FLAGS = dict(amsgrad=False, maximize=False, foreach=None, capturable=False,
                     differentiable=False, fused=None, decoupled_weight_decay=False)
-# group flags of torch.optim.Adam that change the update rule; the kernel has none of them
+# group flags of torch.optim.Adam that change the update rule; FusedAdam has none of them
+# (FusedAdamW has decoupled_weight_decay and amsgrad)
 _UNSUPPORTED_FLAGS = ("amsgrad", "maximize", "decoupled_weight_decay")
 
 
 class FusedAdam(torch.optim.Optimizer):
+    _decoupled = False  # AdamW's decoupled weight decay (FusedAdamW)
+
     def __init__(self, params, lr=1e-3, betas=(0.9, 0.999), eps=1e-8, weight_decay=0.0,
                  amsgrad=False, maximize=False, **unused):
         if amsgrad:
-            raise NotImplementedError("amsgrad has no fused kernel (reference default is False)")
+            raise NotImplementedError("FusedAdam has no amsgrad (reference default is False); "
+                                      "FusedAdamW has")
+        self._setup(params, lr, betas, eps, weight_decay, amsgrad, maximize)
+
+    def _setup(self, params, lr, betas, eps, weight_decay, amsgrad, maximize):
         if maximize:
             raise NotImplementedError("maximize has no fused kernel (reference default is False)")
         if not 0.0 <= lr:
@@ -35,12 +46,15 @@ class FusedAdam(torch.optim.Optimizer):
         if not 0.0 <= betas[0] < 1.0 or not 0.0 <= betas[1] < 1.0:
             raise ValueError(f"Invalid beta parameters: {betas}")
         params = list(params)
-        # torch.optim.Adam's group keys, with the values this kernel implements, so that
-        # checkpoints move between the two optimizers in either direction
-        defaults = dict(lr=lr, betas=betas, eps=eps, weight_decay=weight_decay, **_TORCH_FLAGS)
+        # torch.optim.Adam's (AdamW's) group keys, with the values this kernel implements, so
+        # that checkpoints move between the two optimizers in either direction
+        defaults = dict(lr=lr, betas=betas, eps=eps, weight_decay=weight_decay,
+                        **dict(_TORCH_FLAGS, amsgrad=bool(amsgrad),
+                               decoupled_weight_decay=self._decoupled))
         super().__init__(params, defaults)
         if len(self.param_groups) != 1:
-            raise NotImplementedError("FusedAdam takes one parameter group (one network)")
+            raise NotImplementedError(f"{type(self).__name__} takes one parameter group (one network)")
+        self.amsgrad = bool(amsgrad)
         ps = self.param_groups[0]["params"]
         if len(ps) == 1 and getattr(ps[0], "_rb200_arena", None) is None:
             ScalarArena(ps[0])  # stand-alone parameter such as SAC's log_alpha
@@ -55,6 +69,8 @@ class FusedAdam(torch.optim.Optimizer):
         dev = flat.device
         self.exp_avg = torch.zeros_like(flat)
         self.exp_avg_sq = torch.zeros_like(flat)
+        # AMSGrad's running maximum of exp_avg_sq, with the arena's layout
+        self.max_exp_avg_sq = torch.zeros_like(flat) if self.amsgrad else None
         self.step_t = torch.zeros(1, dtype=torch.int64, device=dev)
         self._counter = torch.zeros(1, dtype=torch.int32, device=dev)
 
@@ -62,11 +78,13 @@ class FusedAdam(torch.optim.Optimizer):
         flat = self.arena.flat
         if flat.data_ptr() != self._flat_id:
             # the model was moved (e.g. .cuda()) after the optimizer was built: follow it
-            old = (self.exp_avg, self.exp_avg_sq, self.step_t)
+            old = (self.exp_avg, self.exp_avg_sq, self.step_t, self.max_exp_avg_sq)
             self._alloc_state()
             self.exp_avg.copy_(old[0].to(flat.device))
             self.exp_avg_sq.copy_(old[1].to(flat.device))
             self.step_t.copy_(old[2].to(flat.device))
+            if self.amsgrad:
+                self.max_exp_avg_sq.copy_(old[3].to(flat.device))
 
     @property
     def num_steps(self) -> int:
@@ -88,7 +106,7 @@ class FusedAdam(torch.optim.Optimizer):
         if grad is None:
             if a.gpart is None or not a.grad_ready:
                 raise _lib.Rb200Error(
-                    "FusedAdam.step(): no gradient partials for this network -- run the "
+                    f"{type(self).__name__}.step(): no gradient partials for this network -- run the "
                     "trainer's train_step_gen/next() (fused backward) first")
             grad = a.gpart
         splits = grad.shape[0] if grad.dim() == 2 else 1
@@ -107,6 +125,9 @@ class FusedAdam(torch.optim.Optimizer):
         args.eps = float(g["eps"])
         args.weight_decay = float(g["weight_decay"])
         args.grad_scale = float(grad_scale)
+        args.decoupled_weight_decay = int(self._decoupled)
+        args.amsgrad = int(self.amsgrad)
+        args.max_exp_avg_sq = self.max_exp_avg_sq.data_ptr() if self.amsgrad else None
         if target is not None:
             if target.n != a.n:
                 raise ValueError("target / source arenas differ in size")
@@ -157,7 +178,7 @@ class FusedAdam(torch.optim.Optimizer):
         for p in self.param_groups[0]["params"]:
             p.grad = None
 
-    # state_dict in torch.optim.Adam's shape: per-parameter views of the flat moments
+    # state_dict in torch.optim.Adam's (AdamW's) shape: per-parameter views of the flat moments
     def state_dict(self):
         self._ensure_state()
         sd = super().state_dict()
@@ -174,16 +195,21 @@ class FusedAdam(torch.optim.Optimizer):
                 "exp_avg": self.exp_avg[off:off + n].view_as(p).clone(),
                 "exp_avg_sq": self.exp_avg_sq[off:off + n].view_as(p).clone(),
             }
+            if self.amsgrad:
+                state[i]["max_exp_avg_sq"] = self.max_exp_avg_sq[off:off + n].view_as(p).clone()
         sd["state"] = state
         return sd
 
+    def _check_group_flags(self, group):
+        for k in _UNSUPPORTED_FLAGS:
+            if group.get(k, False):
+                raise NotImplementedError(
+                    f"state dict has {k}=True, which has no fused kernel (reference default "
+                    "is False)")
+
     def load_state_dict(self, state_dict):
         for group in state_dict.get("param_groups", []):
-            for k in _UNSUPPORTED_FLAGS:
-                if group.get(k, False):
-                    raise NotImplementedError(
-                        f"state dict has {k}=True, which has no fused kernel (reference default "
-                        "is False)")
+            self._check_group_flags(group)
         self._ensure_state()
         ps = self.param_groups[0]["params"]
         base = self.arena.flat.data_ptr()
@@ -195,7 +221,29 @@ class FusedAdam(torch.optim.Optimizer):
             n = p.numel()
             self.exp_avg[off:off + n].copy_(st[i]["exp_avg"].reshape(-1))
             self.exp_avg_sq[off:off + n].copy_(st[i]["exp_avg_sq"].reshape(-1))
+            if self.amsgrad:
+                self.max_exp_avg_sq[off:off + n].copy_(st[i]["max_exp_avg_sq"].reshape(-1))
             self.step_t.fill_(int(st[i]["step"]))
         for k in ("lr", "betas", "eps", "weight_decay"):
             if state_dict.get("param_groups"):
                 self.param_groups[0][k] = state_dict["param_groups"][0].get(k, self.param_groups[0][k])
+
+
+class FusedAdamW(FusedAdam):
+    """torch.optim.AdamW (decoupled weight decay, weight_decay=0.01 by default, optional
+    AMSGrad) on the fused K3 kernel.  `maximize` has no kernel and raises."""
+    _decoupled = True
+
+    def __init__(self, params, lr=1e-3, betas=(0.9, 0.999), eps=1e-8, weight_decay=1e-2,
+                 amsgrad=False, maximize=False, **unused):
+        self._setup(params, lr, betas, eps, weight_decay, amsgrad, maximize)
+
+    def _check_group_flags(self, group):
+        if group.get("maximize", False):
+            raise NotImplementedError("state dict has maximize=True, which has no fused kernel")
+        if not group.get("decoupled_weight_decay", False):
+            raise ValueError("state dict has decoupled_weight_decay=False (torch.optim.Adam's); "
+                             "load it into FusedAdam")
+        if bool(group.get("amsgrad", False)) != self.amsgrad:
+            raise ValueError(f"state dict has amsgrad={group.get('amsgrad')}, this optimizer "
+                             f"was built with amsgrad={self.amsgrad}")
