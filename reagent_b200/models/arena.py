@@ -58,6 +58,11 @@ class ParamArena:
         o = self.dims[l + 1]
         return flat[self.b_off[l]: self.b_off[l] + o]
 
+    def layer_ptrs(self, l):
+        """Device pointers of layer l's weight and bias in the current flat buffer."""
+        f = self.flat.data_ptr()
+        return f + 4 * self.w_off[l], f + 4 * self.b_off[l]
+
     def desc(self, n_layers=None) -> _lib.MlpT:
         """ctypes descriptor for the current flat buffer (optionally only the first
         `n_layers` layers, e.g. the trunk below a wide head)."""
@@ -74,6 +79,42 @@ class ParamArena:
         d.params = self.flat.data_ptr()
         d.n_params = self.n
         return d
+
+    # -- launches (the library is looked up per call, so a wrapped entry point takes effect) --
+    def forward(self, x, out, *, n_layers=None, x1=None, save=None):
+        """out = MLP(cat(x, x1)) over the first `n_layers` layers as one fused launch; `save`
+        (a NetWorkspace) keeps the activations the backward reads."""
+        run_mlp(self.desc(n_layers), x, out, x1=x1, save=save)
+
+    def forward_wide(self, x, out, trunk_out, save=None):
+        """out = MLP(x) for a head too wide for the fused row tiles: the trunk (all layers but
+        the last) as one fused launch into `trunk_out` [B, dims[-2]] (None for a one-layer
+        network), then the last layer as a 2-D tiled linear."""
+        L = len(self.acts)
+        h = x
+        if L > 1:
+            self.forward(x, trunk_out, n_layers=L - 1, save=save)
+            h = trunk_out
+        W, b = self.layer_ptrs(L - 1)
+        rc = _lib.lib().rb200_linear_forward(W, b, self.acts[L - 1], self.dims[L - 1], self.dims[L],
+                                             h.data_ptr(), x.shape[0], out.data_ptr(),
+                                             _lib.cur_stream())
+        _lib.check(rc, "rb200_linear_forward(head)")
+
+    def backward(self, ws, batch: int, n_layers=None):
+        """dZ chain of the first `n_layers` layers from the dZ of the last of them (in `ws`)."""
+        L = len(self.acts) if n_layers is None else n_layers
+        rc = _lib.lib().rb200_mlp_backward(self.desc(n_layers), ws.dz[L - 1].data_ptr(), batch,
+                                           ws.c, _lib.cur_stream())
+        _lib.check(rc, "rb200_mlp_backward")
+
+
+def run_mlp(desc: _lib.MlpT, x, out, x1=None, save=None):
+    """One fused MLP forward over `desc`: out = MLP(cat(x, x1)) for the x.shape[0] rows of x."""
+    rc = _lib.lib().rb200_mlp_forward(desc, x.data_ptr(), x.shape[1], _lib.ptr(x1),
+                                      0 if x1 is None else x1.shape[1], x.shape[0], out.data_ptr(),
+                                      None if save is None else save.c, _lib.cur_stream())
+    _lib.check(rc, "rb200_mlp_forward")
 
 
 def flatten_linears(linears: List[nn.Linear], arena: ParamArena, device=None) -> torch.Tensor:

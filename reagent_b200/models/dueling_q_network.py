@@ -25,7 +25,7 @@ import torch
 
 from .. import _lib
 from ..core import types as rlt
-from .arena import ParamArena, _align4
+from .arena import ParamArena, _align4, run_mlp
 from .base import ModelBase, require_cuda
 from .dqn import FullyConnectedDQN
 
@@ -75,12 +75,10 @@ class DuelingArena(ParamArena):
         return sc
 
     def refresh(self):
-        f = self.flat
-        p = f.data_ptr()
-        L = len(self.acts)
+        p = self.flat.data_ptr()
+        W, b = self.layer_ptrs(len(self.acts) - 1)
         rc = _lib.lib().rb200_dueling_fold(p + 4 * self.o_wa, p + 4 * self.o_ba, p + 4 * self.o_wv,
-                                           p + 4 * self.o_bv, self.A, self.N, self.H,
-                                           p + 4 * self.w_off[L - 1], p + 4 * self.b_off[L - 1],
+                                           p + 4 * self.o_bv, self.A, self.N, self.H, W, b,
                                            self._scratch_for(1).data_ptr(), _lib.cur_stream())
         _lib.check(rc, "rb200_dueling_fold")
 
@@ -228,9 +226,7 @@ class DuelingQNetwork(ModelBase):
 
     def _run(self, desc, x, out_dim):
         out = torch.empty(x.shape[0], out_dim, dtype=torch.float32, device=x.device)
-        rc = _lib.lib().rb200_mlp_forward(desc, x.data_ptr(), x.shape[1], None, 0, x.shape[0],
-                                          out.data_ptr(), None, _lib.cur_stream())
-        _lib.check(rc, "rb200_mlp_forward")
+        run_mlp(desc, x, out)
         return out
 
     def _get_values(self, state: rlt.FeatureData):
@@ -260,20 +256,10 @@ class DuelingQNetwork(ModelBase):
         R = ar.A * ar.N
         out = torch.empty(x.shape[0], R, dtype=torch.float32, device=x.device)
         if R > 256:  # wide head (atoms): fused trunk + 2-D tiled head, as FullyConnectedDQN does
-            L = len(ar.acts)
-            h = torch.empty(x.shape[0], ar.dims[L - 1], dtype=torch.float32, device=x.device)
-            rc = _lib.lib().rb200_mlp_forward(ar.desc(L - 1), x.data_ptr(), x.shape[1], None, 0,
-                                              x.shape[0], h.data_ptr(), None, _lib.cur_stream())
-            _lib.check(rc, "rb200_mlp_forward(trunk)")
-            f = ar.flat.data_ptr()
-            rc = _lib.lib().rb200_linear_forward(f + 4 * ar.w_off[L - 1], f + 4 * ar.b_off[L - 1],
-                                                 ar.acts[L - 1], ar.dims[L - 1], R, h.data_ptr(),
-                                                 x.shape[0], out.data_ptr(), _lib.cur_stream())
-            _lib.check(rc, "rb200_linear_forward(head)")
+            h = torch.empty(x.shape[0], ar.dims[-2], dtype=torch.float32, device=x.device)
+            ar.forward_wide(x, out, h)
         else:
-            rc = _lib.lib().rb200_mlp_forward(ar.desc(), x.data_ptr(), x.shape[1], None, 0,
-                                              x.shape[0], out.data_ptr(), None, _lib.cur_stream())
-            _lib.check(rc, "rb200_mlp_forward")
+            ar.forward(x, out)
         if self.num_atoms is not None:
             out = out.view(-1, ar.A, ar.N)
         if possible_actions_mask is not None:

@@ -117,28 +117,14 @@ class FullyConnectedNetwork(ModelBase):
             x1 = x1.contiguous().float()
         B = x0.shape[0]
         out = torch.empty(B, self.layers[-1], dtype=torch.float32, device=x0.device)
-        a = self._arena
-        L = len(a.acts)
         if self.layers[-1] <= 1024:
-            rc = _lib.lib().rb200_mlp_forward(
-                a.desc(), x0.data_ptr(), x0.shape[1], _lib.ptr(x1),
-                0 if x1 is None else x1.shape[1], B, out.data_ptr(), None, _lib.cur_stream())
-            _lib.check(rc, "rb200_mlp_forward")
+            self._arena.forward(x0, out, x1=x1)
             return out
         # wide head (e.g. QR-DQN's A*N outputs): trunk as one fused launch, head 2-D tiled
         h = x0 if x1 is None else torch.cat((x0, x1), dim=1)
-        if L > 1:
-            hh = torch.empty(B, self.layers[-2], dtype=torch.float32, device=x0.device)
-            rc = _lib.lib().rb200_mlp_forward(a.desc(L - 1), h.data_ptr(), h.shape[1], None, 0, B,
-                                              hh.data_ptr(), None, _lib.cur_stream())
-            _lib.check(rc, "rb200_mlp_forward(trunk)")
-            h = hh
-        flat = a.flat
-        rc = _lib.lib().rb200_linear_forward(
-            flat.data_ptr() + 4 * a.w_off[L - 1], flat.data_ptr() + 4 * a.b_off[L - 1],
-            a.acts[L - 1], a.dims[L - 1], a.dims[L], h.data_ptr(), B, out.data_ptr(),
-            _lib.cur_stream())
-        _lib.check(rc, "rb200_linear_forward")
+        trunk = (torch.empty(B, self.layers[-2], dtype=torch.float32, device=x0.device)
+                 if len(self.layers) > 2 else None)
+        self._arena.forward_wide(h, out, trunk)
         return out
 
     def forward(self, input: torch.Tensor) -> torch.Tensor:

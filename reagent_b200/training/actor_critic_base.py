@@ -8,15 +8,8 @@ from .. import _lib
 from ..core import types as rlt
 from .reagent_lightning_module import ReAgentLightningModule
 from .rl_trainer_pytorch import RLTrainerMixin
-from .workspace import NetWorkspace, check_sample_weight, param_grads, wgrad
-
-
-def _f32c(t):
-    if t is None:
-        return None
-    if t.dtype != torch.float32:
-        t = t.float()
-    return t.contiguous()
+from .workspace import (NetWorkspace, Pins, batch_device, check_sample_weight, param_grads,
+                        wgrad, ws_fits)
 
 
 class ActorCriticBase(RLTrainerMixin, ReAgentLightningModule):
@@ -29,15 +22,14 @@ class ActorCriticBase(RLTrainerMixin, ReAgentLightningModule):
         self.noise_hook = None
         self._kernel_events = None
 
-    def _noise(self, name, B, A, device):
+    def _noise(self, name, B, A, pins):
+        """Device pointer of a [B, A] standard normal draw (kept alive in `pins`)."""
         if self.noise_hook is not None:
-            t = self.noise_hook(name, (B, A), device)
-            return _f32c(t.to(device))
-        return torch.randn(B, A, device=device)
+            return pins(self.noise_hook(name, (B, A), pins.device))
+        return pins(torch.randn(B, A, device=pins.device))
 
     def _workspace(self, B, device):
-        ws = self._ws
-        if ws is None or ws["B"] != B or ws["dev"] != device:
+        if not ws_fits(self._ws, B, device):
             ntiles = (B + 15) // 16
             q2 = self.q2_network
             ws = {
@@ -60,28 +52,20 @@ class ActorCriticBase(RLTrainerMixin, ReAgentLightningModule):
             if ws["q2"] is not None:
                 ws["q2"].c.input = ws["q1"].input.data_ptr()
             self._ws = ws
-        return ws
+        return self._ws
 
-    def _base_args(self, batch: rlt.PolicyNetworkInput, ws, keep):
-        state = _f32c(batch.state.float_features)
-        if not state.is_cuda:
-            raise _lib.Rb200Error(
-                f"{type(self).__name__}: training batch must be on the GPU (no CPU path)")
-        _lib.require_current_device(state.device)
+    def _base_args(self, batch: rlt.PolicyNetworkInput, ws, pins):
+        """(args, state): the fields both fused steps read, `state` as the fp32 tensor handed
+        to them."""
         a = _lib.AcArgsT()
-
-        def P(t):
-            t = _lib.on_device(_f32c(t), state.device)
-            keep.append(t)
-            return _lib.ptr(t, state.device)
-
+        state = pins.tensor(batch.state.float_features)
         a.batch = state.shape[0]
         a.algo = self.ALGO
-        a.state = P(state)
-        a.action = P(batch.action.float_features)
-        a.next_state = P(batch.next_state.float_features)
-        a.reward = P(batch.reward.reshape(-1))
-        a.not_terminal = P(batch.not_terminal.reshape(-1))
+        a.state = state.data_ptr()
+        a.action = pins(batch.action.float_features)
+        a.next_state = pins(batch.next_state.float_features)
+        a.reward = pins(batch.reward.reshape(-1))
+        a.not_terminal = pins(batch.not_terminal.reshape(-1))
         a.gamma = float(self.gamma)
         a.loss_partials = ws["loss_partials"].data_ptr()
         a.tile_counter = ws["counter"].data_ptr()
@@ -95,27 +79,22 @@ class ActorCriticBase(RLTrainerMixin, ReAgentLightningModule):
         """`sample_weight`: [B] fp32 importance weights of prioritized replay.  Each critic's
         loss becomes mean(w * (q - y)^2) and row b of its dZ is scaled by w_b; the row's TD
         error max_c |q_c - y| goes to the workspace's "td_error"."""
-        state = batch.state.float_features
-        B, dev = state.shape[0], state.device
+        B = batch.state.float_features.shape[0]
         check_sample_weight(sample_weight, B)
-        ws = self._workspace(B, dev)
-        keep = []
-        a, state = self._base_args(batch, ws, keep)
+        pins = Pins(batch_device(batch.state.float_features, type(self).__name__))
+        ws = self._workspace(B, pins.device)
+        a, _ = self._base_args(batch, ws, pins)
         if sample_weight is not None:
-            w = _lib.on_device(sample_weight.contiguous(), state.device)
-            keep.append(w)
-            a.sample_weight = w.data_ptr()
+            a.sample_weight = pins(sample_weight)
             a.td_error_out = ws["td_error"].data_ptr()
         A = self.q1_network.arena.dims[0] - self.actor_network.arena.dims[0]
-        nz = self._noise("next", B, A, dev)
-        keep.append(nz)
-        a.noise_next = nz.data_ptr()
+        a.noise_next = self._noise("next", B, A, pins)
         a.loss = ws["critic_loss"].data_ptr()
         a.td_target = ws["td_target"].data_ptr()
         a.q1_value = ws["q1_value"].data_ptr()
         a.q2_value = ws["q2_value"].data_ptr()
         a.log_prob_out = ws["log_prob"].data_ptr()
-        fill(a, keep)
+        fill(a, pins)
         q2 = self.q2_network
         ev = self._kernel_events
         if ev is not None:
@@ -135,14 +114,13 @@ class ActorCriticBase(RLTrainerMixin, ReAgentLightningModule):
         return ws["critic_loss"]
 
     def _actor_step(self, batch, fill):
-        state = batch.state.float_features
-        B, dev = state.shape[0], state.device
-        ws = self._workspace(B, dev)
-        keep = []
-        a, state = self._base_args(batch, ws, keep)
+        B = batch.state.float_features.shape[0]
+        pins = Pins(batch_device(batch.state.float_features, type(self).__name__))
+        ws = self._workspace(B, pins.device)
+        a, state = self._base_args(batch, ws, pins)
         a.loss = ws["actor_loss"].data_ptr()
         a.log_prob_out = ws["log_prob"].data_ptr()
-        fill(a, keep)
+        fill(a, pins)
         q2 = self.q2_network
         rc = _lib.lib().rb200_ac_actor_step(
             self._desc(self.actor_network), self._desc(self.q1_network), self._desc(q2), a,

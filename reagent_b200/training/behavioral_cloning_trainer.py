@@ -18,11 +18,7 @@ from .. import _lib
 from ..core import types as rlt
 from ..optimizer import Optimizer__Union
 from .reagent_lightning_module import ReAgentLightningModule
-from .workspace import NetWorkspace, param_grads, wgrad
-
-
-def _f32c(t: torch.Tensor, device) -> torch.Tensor:
-    return _lib.on_device(t.float().contiguous(), device)
+from .workspace import NetWorkspace, Pins, backward_wgrad, batch_device, param_grads, ws_fits
 
 
 class BehavioralCloningTrainer(ReAgentLightningModule):
@@ -45,56 +41,45 @@ class BehavioralCloningTrainer(ReAgentLightningModule):
 
     # ------------------------------------------------------------------
     def _workspace(self, B: int, device):
-        ws = self._ws
-        if ws is None or ws["B"] != B or ws["dev"] != device:
-            ws = {"B": B, "dev": device,
-                  "net": NetWorkspace(self.bc_net.arena, B, device),
-                  "scores": torch.empty(B, self.bc_net.action_dim, device=device),
-                  "loss_partials": torch.zeros(-(-B // _lib.BC_ROWS_PER_BLOCK), device=device),
-                  "loss": torch.zeros(1, device=device),
-                  "counter": torch.zeros(1, dtype=torch.int32, device=device)}
-            self._ws = ws
-        return ws
+        if not ws_fits(self._ws, B, device):
+            self._ws = {"B": B, "dev": device,
+                        "net": NetWorkspace(self.bc_net.arena, B, device),
+                        "scores": torch.empty(B, self.bc_net.action_dim, device=device),
+                        "loss_partials": torch.zeros(-(-B // _lib.BC_ROWS_PER_BLOCK),
+                                                     device=device),
+                        "loss": torch.zeros(1, device=device),
+                        "counter": torch.zeros(1, dtype=torch.int32, device=device)}
+        return self._ws
 
     def _step(self, batch: rlt.BehavioralCloningModelInput, do_backward: bool = True) -> torch.Tensor:
         """Forward, loss head (and backward into the gradient partials).  Returns the device
         loss scalar (shape []); no host synchronisation."""
-        state = batch.state.float_features.float().contiguous()
-        if not state.is_cuda:
-            raise _lib.Rb200Error("BehavioralCloningTrainer: training batch must be on the GPU "
-                                  "(reagent_b200 has no CPU path)")
-        dev = state.device
-        _lib.require_current_device(dev)
+        pins = Pins(batch_device(batch.state.float_features, type(self).__name__))
+        state = pins.tensor(batch.state.float_features)
         ar = self.bc_net.arena
         B, A = state.shape[0], self.bc_net.action_dim
         if state.shape[1] != ar.dims[0]:
             raise ValueError(f"state has {state.shape[1]} features, bc_net expects {ar.dims[0]}")
         if batch.possible_actions_mask is None:
             raise TypeError("BehavioralCloningTrainer needs possible_actions_mask")
-        labels = _f32c(batch.action, dev)
-        mask = _f32c(batch.possible_actions_mask, dev)
+        labels = pins.tensor(batch.action)
+        mask = pins.tensor(batch.possible_actions_mask)
         for name, t in (("action", labels), ("possible_actions_mask", mask)):
             if tuple(t.shape) != (B, A):
                 raise ValueError(f"{name} has shape {tuple(t.shape)}, expected {(B, A)}")
-        ws = self._workspace(B, dev)
+        ws = self._workspace(B, pins.device)
         net = ws["net"]
-        lib, st = _lib.lib(), _lib.cur_stream()
-        rc = lib.rb200_mlp_forward(ar.desc(), state.data_ptr(), ar.dims[0], None, 0, B,
-                                   ws["scores"].data_ptr(), net.c if do_backward else None, st)
-        _lib.check(rc, "rb200_mlp_forward")
-        L = len(ar.acts)
+        ar.forward(state, ws["scores"], save=net if do_backward else None)
         a = _lib.BcXentArgsT()
         a.batch, a.num_actions = B, A
         a.logits, a.labels, a.mask = ws["scores"].data_ptr(), labels.data_ptr(), mask.data_ptr()
-        a.dz = net.dz[L - 1].data_ptr() if do_backward else None
+        a.dz = net.dz[-1].data_ptr() if do_backward else None
         a.loss_partials = ws["loss_partials"].data_ptr()
         a.loss = ws["loss"].data_ptr()
         a.tile_counter = ws["counter"].data_ptr()
-        _lib.check(lib.rb200_bc_xent_head(a, st), "rb200_bc_xent_head")
+        _lib.check(_lib.lib().rb200_bc_xent_head(a, _lib.cur_stream()), "rb200_bc_xent_head")
         if do_backward:
-            rc = lib.rb200_mlp_backward(ar.desc(), net.dz[L - 1].data_ptr(), B, net.c, st)
-            _lib.check(rc, "rb200_mlp_backward")
-            wgrad(ar, net, state, B)
+            backward_wgrad(ar, net, state, B)
         return ws["loss"].reshape(())
 
     # ------------------------------------------------------------------

@@ -21,20 +21,13 @@ from ..core import types as rlt
 from ..core.parameters import EvaluationParameters, RLParameters
 from ..optimizer import Optimizer__Union, SoftUpdate
 from .dqn_trainer_base import DQNTrainerBaseLightning
-from .workspace import NetWorkspace, check_sample_weight, param_grads, wgrad
+from .workspace import (NetWorkspace, Pins, batch_device, check_sample_weight, discount_source,
+                        param_grads, wgrad, ws_fits)
 
 
 @dataclass(frozen=True)
 class BCQConfig:
     drop_threshold: float = 0.1
-
-
-def _f32c(t: Optional[torch.Tensor]) -> Optional[torch.Tensor]:
-    if t is None:
-        return None
-    if t.dtype != torch.float32:
-        t = t.float()
-    return t.contiguous()
 
 
 class DQNTrainer(DQNTrainerBaseLightning):
@@ -123,13 +116,11 @@ class DQNTrainer(DQNTrainerBaseLightning):
 
     # ------------------------------------------------------------------
     def _workspace(self, B: int, device):
-        ws = self._ws
-        if ws is None or ws["B"] != B or ws["dev"] != device:
-            arena = self.q_network.arena
+        if not ws_fits(self._ws, B, device):
             ntiles = (B + 15) // 16
             ws = {
                 "B": B, "dev": device,
-                "net": NetWorkspace(arena, B, device),
+                "net": NetWorkspace(self.q_network.arena, B, device),
                 "scores": torch.empty(B, self.num_actions, device=device),
                 "td_target": torch.empty(B, device=device),
                 "q_sel": torch.empty(B, device=device),
@@ -142,7 +133,7 @@ class DQNTrainer(DQNTrainerBaseLightning):
                 ws["bcq_logits"] = torch.empty(B, self.num_actions, device=device)
                 ws["bcq_mask"] = torch.empty(B, self.num_actions, device=device)
             self._ws = ws
-        return ws
+        return self._ws
 
     def _bcq_filter(self, x: torch.Tensor, mask_in, logits, mask_out) -> torch.Tensor:
         """mask_out = mask_in * (r >= drop_threshold), r = softmax(imitator(x)) / its row max
@@ -152,14 +143,10 @@ class DQNTrainer(DQNTrainerBaseLightning):
         if im.arena.flat.device != mask_out.device:
             raise _lib.Rb200Error(f"DQNTrainer: the BCQ imitator lives on {im.arena.flat.device}, "
                                   f"the batch on {mask_out.device} (call trainer.to(device))")
-        lib, st = _lib.lib(), _lib.cur_stream()
-        B = x.shape[0]
-        rc = lib.rb200_mlp_forward(im.arena.desc(), x.data_ptr(), x.shape[1], None, 0, B,
-                                   logits.data_ptr(), None, st)
-        _lib.check(rc, "rb200_mlp_forward(imitator)")
-        rc = lib.rb200_bcq_filter(logits.data_ptr(), B, self.num_actions,
-                                  float(self.bcq_drop_threshold), mask_in, mask_out.data_ptr(),
-                                  None, None, st)
+        im.arena.forward(x, logits)
+        rc = _lib.lib().rb200_bcq_filter(logits.data_ptr(), x.shape[0], self.num_actions,
+                                         float(self.bcq_drop_threshold), mask_in,
+                                         mask_out.data_ptr(), None, None, _lib.cur_stream())
         _lib.check(rc, "rb200_bcq_filter")
         return mask_out
 
@@ -250,45 +237,27 @@ class DQNTrainer(DQNTrainerBaseLightning):
                  sample_weight: Optional[torch.Tensor] = None) -> torch.Tensor:
         """Fused TD target + loss (+ backward).  Returns the device loss scalar (shape []).
         `sample_weight`: [B] fp32 importance weights (loss = mean(w * loss_row), dZ row * w)."""
-        state = _f32c(batch.state.float_features)
-        if not state.is_cuda:
-            raise _lib.Rb200Error(
-                "DQNTrainer: training batch must be on the GPU (reagent_b200 has no CPU path)")
-        _lib.require_current_device(state.device)
+        pins = Pins(batch_device(batch.state.float_features, type(self).__name__))
+        state = pins.tensor(batch.state.float_features)
+        next_state = pins.tensor(batch.next_state.float_features)  # the imitator reads it too
         B = state.shape[0]
-        ws = self._workspace(B, state.device)
+        ws = self._workspace(B, pins.device)
         a = _lib.DqnArgsT()
-        keep = []
-
-        def P(t):
-            t = _lib.on_device(_f32c(t), state.device)
-            keep.append(t)
-            return _lib.ptr(t, state.device)
-
         a.batch = B
-        a.state = P(state)
-        a.next_state = P(batch.next_state.float_features)
-        next_state = keep[-1]  # the fp32 contiguous tensor handed to K2 (the imitator reads it too)
-        a.action = P(batch.action)
-        a.next_action = P(batch.next_action)
-        a.reward = P(batch.reward.reshape(-1))
-        a.not_terminal = P(batch.not_terminal.reshape(-1))
-        a.possible_next_actions_mask = P(batch.possible_next_actions_mask)
+        a.state, a.next_state = state.data_ptr(), next_state.data_ptr()
+        a.action = pins(batch.action)
+        a.next_action = pins(batch.next_action)
+        a.reward = pins(batch.reward.reshape(-1))
+        a.not_terminal = pins(batch.not_terminal.reshape(-1))
+        a.possible_next_actions_mask = pins(batch.possible_next_actions_mask)
         if self.bcq and self.maxq_learning:  # the SARSA branch ignores BCQ (dqn_trainer.py:221-227)
             self.bcq_next_actions_mask = self._bcq_filter(
                 next_state, a.possible_next_actions_mask, ws["bcq_logits"], ws["bcq_mask"])
             a.possible_next_actions_mask = ws["bcq_mask"].data_ptr()
-        a.discount_src = None
-        a.discount_mode = _lib.DISCOUNT_CONST
-        if self.use_seq_num_diff_as_time_diff:
-            assert self.multi_steps is None
-            a.discount_src = P(batch.time_diff.reshape(-1))
-            a.discount_mode = _lib.DISCOUNT_POW
-        if self.multi_steps is not None:
-            assert batch.step is not None
-            a.discount_src = P(batch.step.reshape(-1))
-            a.discount_mode = _lib.DISCOUNT_POW
-        a.reward_boost = P(self.reward_boosts.reshape(-1)) if self._has_reward_boost else None
+        src = discount_source(self, batch)
+        a.discount_src = pins(src)
+        a.discount_mode = _lib.DISCOUNT_CONST if src is None else _lib.DISCOUNT_POW
+        a.reward_boost = pins(self.reward_boosts.reshape(-1)) if self._has_reward_boost else None
         a.gamma = float(self.gamma)
         a.double_q = int(bool(self.double_q_learning))
         a.maxq = int(bool(self.maxq_learning))
@@ -302,7 +271,7 @@ class DQNTrainer(DQNTrainerBaseLightning):
         a.loss = ws["loss"].data_ptr()
         a.tile_counter = ws["counter"].data_ptr()
         if sample_weight is not None:
-            a.sample_weight = P(check_sample_weight(sample_weight, B))
+            a.sample_weight = pins(check_sample_weight(sample_weight, B))
         self.q_network.arena.refresh()          # no-op for plain MLPs; folds a dueling head
         self.q_network_target.arena.refresh()
         qd, qtd = self.q_network.arena.desc(), self.q_network_target.arena.desc()
@@ -323,7 +292,8 @@ class DQNTrainer(DQNTrainerBaseLightning):
         else:
             rc = _lib.lib().rb200_dqn_td_step(qd, qtd, a, ws["net"].c, _lib.cur_stream())
             _lib.check(rc, "rb200_dqn_td_step")
-        self._last_td_call = (qd, qtd, a, ws["net"].c, keep, pack)  # profiling hook (re-launch)
+        # profiling hook (re-launch)
+        self._last_td_call = (qd, qtd, a, ws["net"].c, pins.keep, pack)
         if ev is not None:
             e1.record()
             ev.append((e0, e1))
@@ -398,8 +368,8 @@ class DQNTrainer(DQNTrainerBaseLightning):
         mask = (training_batch.possible_actions_mask if self.maxq_learning
                 else training_batch.action)
         if self.bcq and self.maxq_learning:  # dqn_trainer.py:287-291, without writing the batch
-            state, mask = _f32c(training_batch.state.float_features), _f32c(mask)
-            mask = self._bcq_filter(state, _lib.ptr(mask, state.device),
+            pins = Pins(training_batch.state.float_features.device)
+            mask = self._bcq_filter(pins.tensor(training_batch.state.float_features), pins(mask),
                                     torch.empty_like(scores), torch.empty_like(scores))
         model_action_idxs = self.get_max_q_values(scores, mask.float())[1]
         extras = training_batch.extras

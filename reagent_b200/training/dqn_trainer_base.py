@@ -4,7 +4,7 @@ heads (reward network, q_network_cpe, `_calculate_cpes`, :243-452): two extra ML
 by the generic forward / backward / weight-gradient kernels with rb200_cpe_heads in between.
 The offline evaluation machinery behind them (Evaluator, EvaluationDataPage, :454-509) is
 reporting, not training, and stays out of scope."""
-from typing import Dict, List, Optional
+from typing import List, Optional
 
 import torch
 
@@ -13,6 +13,8 @@ from ..core import types as rlt
 from ..core.parameters import EvaluationParameters, RLParameters
 from .reagent_lightning_module import ReAgentLightningModule
 from .rl_trainer_pytorch import RLTrainerMixin
+from .workspace import (NetWorkspace, Pins, backward_wgrad, batch_device, discount_source,
+                        loss_kind, register_reward_boosts, ws_fits)
 
 
 class DQNTrainerMixin:
@@ -55,30 +57,14 @@ class DQNTrainerBaseLightning(DQNTrainerMixin, RLTrainerMixin, ReAgentLightningM
             evaluation_parameters and evaluation_parameters.calc_cpe_in_training)
         assert actions is not None
         self._actions: List[str] = actions
-        if rl_parameters.q_network_loss == "mse":
-            self.q_network_loss_kind = _lib.LOSS_MSE
-        elif rl_parameters.q_network_loss == "huber":
-            self.q_network_loss_kind = _lib.LOSS_HUBER
-        else:
-            raise Exception(
-                "Q-Network loss type {} not valid loss.".format(rl_parameters.q_network_loss))
+        self.q_network_loss_kind = loss_kind(rl_parameters.q_network_loss)
         if metrics_to_score:
             self.metrics_to_score = metrics_to_score + ["reward"]
         else:
             self.metrics_to_score = ["reward"]
-        self._init_reward_boosts(rl_parameters.reward_boost)
+        register_reward_boosts(self, self._actions, rl_parameters.reward_boost)
         # mirror of the reference's host-syncing `.any()` input check; off by default
         self.strict_input_checks = False
-
-    def _init_reward_boosts(self, rl_reward_boost: Optional[Dict[str, float]]) -> None:
-        reward_boosts = torch.zeros([1, len(self._actions)])
-        self._has_reward_boost = False
-        if rl_reward_boost is not None:
-            for k in rl_reward_boost.keys():
-                i = self._actions.index(k)
-                reward_boosts[0, i] = rl_reward_boost[k]
-                self._has_reward_boost = True
-        self.register_buffer("reward_boosts", reward_boosts)
 
     def _initialize_cpe(self, reward_network, q_network_cpe, q_network_cpe_target, optimizer):
         """dqn_trainer_base.py:243-311: store the reward / CPE networks and the offsets of
@@ -112,12 +98,9 @@ class DQNTrainerBaseLightning(DQNTrainerMixin, RLTrainerMixin, ReAgentLightningM
         return target_params, source_params, optimizers
 
     def _cpe_workspace(self, B: int, device):
-        from .workspace import NetWorkspace
-
-        ws = self._cpe_ws
-        if ws is None or ws["B"] != B or ws["dev"] != device:
+        if not ws_fits(self._cpe_ws, B, device):
             MA = len(self.metrics_to_score) * self.num_actions
-            ws = {
+            self._cpe_ws = {
                 "B": B, "dev": device,
                 "reward": NetWorkspace(self.reward_network.arena, B, device),
                 "qcpe": NetWorkspace(self.q_network_cpe.arena, B, device),
@@ -130,8 +113,7 @@ class DQNTrainerBaseLightning(DQNTrainerMixin, RLTrainerMixin, ReAgentLightningM
                 "loss": torch.zeros(2, device=device),
                 "counter": torch.zeros(1, dtype=torch.int32, device=device),
             }
-            self._cpe_ws = ws
-        return ws
+        return self._cpe_ws
 
     def _calculate_cpes(self, training_batch: rlt.DiscreteDqnInput,
                         next_actions_mask: Optional[torch.Tensor] = None):
@@ -141,30 +123,19 @@ class DQNTrainerBaseLightning(DQNTrainerMixin, RLTrainerMixin, ReAgentLightningM
         (all_next_action_scores is evaluated after `yield td_loss`, dqn_trainer.py:266-268).
         `next_actions_mask` replaces the batch's next-action mask of the model propensities
         (DQNTrainer with BCQ passes its filtered mask)."""
-        from .workspace import wgrad
-
-        lib, st = _lib.lib(), _lib.cur_stream()
-        state = training_batch.state.float_features.float().contiguous()
-        next_state = training_batch.next_state.float_features.float().contiguous()
-        B, dev = state.shape[0], state.device
-        _lib.require_current_device(dev)
-        ws = self._cpe_workspace(B, dev)
-        keep = [state, next_state]
-
-        def P(t):
-            t = _lib.on_device(t.float().contiguous(), dev)
-            keep.append(t)
-            return _lib.ptr(t, dev)
+        pins = Pins(batch_device(training_batch.state.float_features, type(self).__name__))
+        state = pins.tensor(training_batch.state.float_features)
+        next_state = pins.tensor(training_batch.next_state.float_features)
+        B = state.shape[0]
+        ws = self._cpe_workspace(B, pins.device)
 
         def fwd(net, x, out, save=None):
             net.arena.refresh()
-            rc = lib.rb200_mlp_forward(net.arena.desc(), x.data_ptr(), x.shape[1], None, 0, B,
-                                       out.data_ptr(), save, st)
-            _lib.check(rc, "rb200_mlp_forward")
+            net.arena.forward(x, out, save=save)
 
         fwd(self.q_network, next_state, ws["next_scores"])
-        fwd(self.reward_network, state, ws["reward_est"], ws["reward"].c)
-        fwd(self.q_network_cpe, state, ws["qcpe_out"], ws["qcpe"].c)
+        fwd(self.reward_network, state, ws["reward_est"], ws["reward"])
+        fwd(self.q_network_cpe, state, ws["qcpe_out"], ws["qcpe"])
         fwd(self.q_network_cpe_target, next_state, ws["qcpe_t_next"])
         metrics = training_batch.extras.metrics if training_batch.extras is not None else None
         mrc = training_batch.reward if metrics is None else torch.cat((training_batch.reward, metrics), dim=1)
@@ -177,17 +148,15 @@ class DQNTrainerBaseLightning(DQNTrainerMixin, RLTrainerMixin, ReAgentLightningM
                 else training_batch.next_action)
         if next_actions_mask is not None:
             mask = next_actions_mask
-        a.mask = P(mask)
+        a.mask = pins(mask)
         a.temperature = float(self.rl_temperature)
-        a.action = P(training_batch.action)
-        a.metrics_reward = P(mrc)
+        a.action = pins(training_batch.action)
+        a.metrics_reward = pins(mrc)
         a.gamma = float(self.gamma)
-        a.discount_mode = _lib.DISCOUNT_CONST
-        if self.use_seq_num_diff_as_time_diff:
-            a.discount_src, a.discount_mode = P(training_batch.time_diff.reshape(-1)), _lib.DISCOUNT_POW
-        if self.multi_steps is not None:
-            a.discount_src, a.discount_mode = P(training_batch.step.reshape(-1)), _lib.DISCOUNT_POW
-        a.not_terminal = P(training_batch.not_terminal.reshape(-1))
+        src = discount_source(self, training_batch)
+        a.discount_src = pins(src)
+        a.discount_mode = _lib.DISCOUNT_CONST if src is None else _lib.DISCOUNT_POW
+        a.not_terminal = pins(training_batch.not_terminal.reshape(-1))
         a.reward_est = ws["reward_est"].data_ptr()
         a.qcpe = ws["qcpe_out"].data_ptr()
         a.qcpe_target_next = ws["qcpe_t_next"].data_ptr()
@@ -199,14 +168,10 @@ class DQNTrainerBaseLightning(DQNTrainerMixin, RLTrainerMixin, ReAgentLightningM
         a.loss_partials = ws["loss_partials"].data_ptr()
         a.loss = ws["loss"].data_ptr()
         a.tile_counter = ws["counter"].data_ptr()
-        _lib.check(lib.rb200_cpe_heads(a, st), "rb200_cpe_heads")
+        _lib.check(_lib.lib().rb200_cpe_heads(a, _lib.cur_stream()), "rb200_cpe_heads")
         for net, w in ((self.reward_network, ws["reward"]), (self.q_network_cpe, ws["qcpe"])):
-            ar = net.arena
-            L = len(ar.acts)
-            rc = lib.rb200_mlp_backward(ar.desc(), w.dz[L - 1].data_ptr(), B, w.c, st)
-            _lib.check(rc, "rb200_mlp_backward")
-            wgrad(ar, w, state, B)
-            ar.finish_grads()
+            backward_wgrad(net.arena, w, state, B)
+            net.arena.finish_grads()
         self.model_propensities_next_states = ws["prop_next"]
         return ws["loss"]
 

@@ -14,7 +14,8 @@ from ..core.parameters import RLParameters
 from ..optimizer import Optimizer__Union, SoftUpdate
 from .reagent_lightning_module import ReAgentLightningModule
 from .rl_trainer_pytorch import RLTrainerMixin
-from .workspace import NetWorkspace, param_grads, wgrad
+from .workspace import (NetWorkspace, Pins, backward_wgrad, batch_device, discount_source,
+                        loss_kind, param_grads, ws_fits)
 
 
 class ParametricDQNTrainer(RLTrainerMixin, ReAgentLightningModule):
@@ -31,15 +32,9 @@ class ParametricDQNTrainer(RLTrainerMixin, ReAgentLightningModule):
         self.reward_network = reward_network
         self.optimizer = Optimizer__Union.default() if optimizer is None else optimizer
         self.log_tensorboard = log_tensorboard
-        loss = self.rl_parameters.q_network_loss
-        if loss == "mse":
-            self.q_network_loss_kind = _lib.LOSS_MSE
-        elif loss == "huber":
-            self.q_network_loss_kind = _lib.LOSS_HUBER
-        elif loss == "bce_with_logits":
+        if self.rl_parameters.q_network_loss == "bce_with_logits":
             raise NotImplementedError("bce_with_logits (gamma == 0 only) has no fused head")
-        else:
-            raise Exception("Q-Network loss type {} not valid loss.".format(loss))
+        self.q_network_loss_kind = loss_kind(self.rl_parameters.q_network_loss)
         self._ws = None
 
     def configure_optimizers(self):
@@ -60,50 +55,30 @@ class ParametricDQNTrainer(RLTrainerMixin, ReAgentLightningModule):
 
     # ------------------------------------------------------------------
     def _workspace(self, B, device):
-        ws = self._ws
-        if ws is None or ws["B"] != B or ws["dev"] != device:
-            ws = {"B": B, "dev": device,
-                  "q": NetWorkspace(self.q_network.arena, B, device),
-                  "r": (None if self.reward_network is None
-                        else NetWorkspace(self.reward_network.arena, B, device)),
-                  "q_values": torch.empty(B, 1, device=device),
-                  "td_target": torch.empty(B, device=device),
-                  "loss_partials": torch.zeros((B + 255) // 256, device=device),
-                  "loss": torch.zeros(1, device=device),
-                  "r_loss": torch.zeros(1, device=device),
-                  "counter": torch.zeros(1, dtype=torch.int32, device=device)}
-            self._ws = ws
-        return ws
+        if not ws_fits(self._ws, B, device):
+            self._ws = {"B": B, "dev": device,
+                        "q": NetWorkspace(self.q_network.arena, B, device),
+                        "r": (None if self.reward_network is None
+                              else NetWorkspace(self.reward_network.arena, B, device)),
+                        "q_values": torch.empty(B, 1, device=device),
+                        "td_target": torch.empty(B, device=device),
+                        "loss_partials": torch.zeros((B + 255) // 256, device=device),
+                        "loss": torch.zeros(1, device=device),
+                        "r_loss": torch.zeros(1, device=device),
+                        "counter": torch.zeros(1, dtype=torch.int32, device=device)}
+        return self._ws
 
     @staticmethod
-    def _fwd(net, x, save=None):
+    def _fwd(net, x):
         out = torch.empty(x.shape[0], net.arena.dims[-1], device=x.device)
-        rc = _lib.lib().rb200_mlp_forward(net.arena.desc(), x.data_ptr(), x.shape[1], None, 0,
-                                          x.shape[0], out.data_ptr(), save, _lib.cur_stream())
-        _lib.check(rc, "rb200_mlp_forward")
+        net.arena.forward(x, out)
         return out
 
-    def _backward(self, net, w, x, B):
-        ar = net.arena
-        L = len(ar.acts)
-        rc = _lib.lib().rb200_mlp_backward(ar.desc(), w.dz[L - 1].data_ptr(), B, w.c, _lib.cur_stream())
-        _lib.check(rc, "rb200_mlp_backward")
-        wgrad(ar, w, x, B)
-
     def _td_step(self, batch: rlt.ParametricDqnInput) -> torch.Tensor:
+        pins = Pins(batch_device(batch.state.float_features, type(self).__name__))
         state = batch.state.float_features.float().contiguous()
-        if not state.is_cuda:
-            raise _lib.Rb200Error("ParametricDQNTrainer: training batch must be on the GPU (no CPU path)")
-        dev, B = state.device, state.shape[0]
-        _lib.require_current_device(dev)
-        ws = self._workspace(B, dev)
-        keep = []
-
-        def P(t):
-            t = _lib.on_device(t.float().contiguous(), dev)
-            keep.append(t)
-            return _lib.ptr(t, dev)
-
+        B = state.shape[0]
+        ws = self._workspace(B, pins.device)
         a = _lib.PdqnArgsT()
         a.batch = B
         next_state = batch.next_state.float_features.float()
@@ -116,43 +91,37 @@ class ParametricDQNTrainer(RLTrainerMixin, ReAgentLightningModule):
             x_next = torch.cat((next_state.repeat_interleave(M, dim=0), pna), dim=1).contiguous()
             nq_t = self._fwd(self.q_network_target, x_next)
             nq = self._fwd(self.q_network, x_next) if self.double_q_learning else None
-            keep += [x_next, nq_t, nq]
+            pins.keep += [x_next, nq_t, nq]
             a.max_num_action = M
             a.next_q = None if nq is None else nq.data_ptr()
             a.next_q_target = nq_t.data_ptr()
-            a.mask = P(batch.possible_next_actions_mask)
+            a.mask = pins(batch.possible_next_actions_mask)
         else:  # SARSA on the target network
             x_next = torch.cat((next_state, batch.next_action.float_features.float()), dim=1).contiguous()
             nq_t = self._fwd(self.q_network_target, x_next)
-            keep += [x_next, nq_t]
+            pins.keep += [x_next, nq_t]
             a.max_num_action = 0
             a.next_q_target = nq_t.data_ptr()
-        a.reward = P(batch.reward.reshape(-1))
-        a.not_terminal = P(batch.not_terminal.reshape(-1))
+        a.reward = pins(batch.reward.reshape(-1))
+        a.not_terminal = pins(batch.not_terminal.reshape(-1))
         a.gamma = float(self.gamma)
-        a.discount_mode = _lib.DISCOUNT_CONST
-        if self.use_seq_num_diff_as_time_diff:
-            assert self.multi_steps is None
-            a.discount_src, a.discount_mode = P(batch.time_diff.reshape(-1)), _lib.DISCOUNT_POW
-        if self.multi_steps is not None:
-            a.discount_src, a.discount_mode = P(batch.step.reshape(-1)), _lib.DISCOUNT_POW
+        src = discount_source(self, batch)
+        a.discount_src = pins(src)
+        a.discount_mode = _lib.DISCOUNT_CONST if src is None else _lib.DISCOUNT_POW
         a.double_q = int(bool(self.double_q_learning))
         a.loss_kind = self.q_network_loss_kind
         x = torch.cat((state, batch.action.float_features.float()), dim=1).contiguous()
         self._x = x
         qv = ws["q_values"]
-        rc = _lib.lib().rb200_mlp_forward(self.q_network.arena.desc(), x.data_ptr(), x.shape[1], None, 0,
-                                          B, qv.data_ptr(), ws["q"].c, _lib.cur_stream())
-        _lib.check(rc, "rb200_mlp_forward")
-        L = len(self.q_network.arena.acts)
+        self.q_network.arena.forward(x, qv, save=ws["q"])
         a.q_values = qv.data_ptr()
-        a.dz = ws["q"].dz[L - 1].data_ptr()
+        a.dz = ws["q"].dz[-1].data_ptr()
         a.td_target = ws["td_target"].data_ptr()
         a.loss_partials = ws["loss_partials"].data_ptr()
         a.loss = ws["loss"].data_ptr()
         a.tile_counter = ws["counter"].data_ptr()
         _lib.check(_lib.lib().rb200_pdqn_head(a, _lib.cur_stream()), "rb200_pdqn_head")
-        self._backward(self.q_network, ws["q"], x, B)
+        backward_wgrad(self.q_network.arena, ws["q"], x, B)
         return ws["loss"].reshape(())
 
     def _reward_step(self, batch: rlt.ParametricDqnInput) -> torch.Tensor:
@@ -163,14 +132,11 @@ class ParametricDQNTrainer(RLTrainerMixin, ReAgentLightningModule):
         mrc = batch.reward if metrics is None else torch.cat((batch.reward, metrics), dim=1)
         w = ws["r"]
         est = torch.empty(B, self.reward_network.arena.dims[-1], device=x.device)
-        rc = _lib.lib().rb200_mlp_forward(self.reward_network.arena.desc(), x.data_ptr(), x.shape[1],
-                                          None, 0, B, est.data_ptr(), w.c, _lib.cur_stream())
-        _lib.check(rc, "rb200_mlp_forward")
+        self.reward_network.arena.forward(x, est, save=w)
         diff = est - mrc.float()
-        L = len(self.reward_network.arena.acts)
-        w.dz[L - 1].copy_(diff * (2.0 / diff.numel()))
+        w.dz[-1].copy_(diff * (2.0 / diff.numel()))
         ws["r_loss"].copy_((diff * diff).mean().reshape(1))
-        self._backward(self.reward_network, w, x, B)
+        backward_wgrad(self.reward_network.arena, w, x, B)
         return ws["r_loss"].reshape(())
 
     # ------------------------------------------------------------------

@@ -118,7 +118,7 @@ class SACTrainer(ActorCriticBase):
         return optimizers
 
     # ---- kernel argument fillers --------------------------------------------------
-    def _fill_critic(self, a, keep):
+    def _fill_critic(self, a, pins):
         dev = self._ws["dev"]
         if self._alpha_dev.device != dev:  # trainer built from CUDA networks, never .cuda()'d
             self._alpha_dev = self._alpha_dev.to(dev)
@@ -130,14 +130,11 @@ class SACTrainer(ActorCriticBase):
         a.target_entropy = float(self.target_entropy)
         a.backprop_through_log_prob = int(bool(self.backprop_through_log_prob))
 
-    def _fill_actor(self, a, keep):
-        self._fill_critic(a, keep)
+    def _fill_actor(self, a, pins):
+        self._fill_critic(a, pins)
         ws = self._ws
-        B = ws["B"]
         A = self.q1_network.arena.dims[0] - self.actor_network.arena.dims[0]
-        nz = self._noise("cur", B, A, ws["dev"])
-        keep.append(nz)
-        a.noise_cur = nz.data_ptr()
+        a.noise_cur = self._noise("cur", ws["B"], A, pins)
         if self.alpha_optimizer is not None:
             a.alpha_grad = ws["alpha_grad"].data_ptr()
             a.log_alpha = _lib.ptr(self.log_alpha.data, ws["dev"])

@@ -81,7 +81,7 @@ class TD3Trainer(ActorCriticBase):
             SoftUpdate.make_optimizer_scheduler(target_params, source_params, tau=self.tau))
         return optimizers
 
-    def _fill(self, a, keep):
+    def _fill(self, a, pins):
         a.noise_variance = float(self.noise_variance)
         a.noise_clip = float(self.noise_clip_range[1])
 

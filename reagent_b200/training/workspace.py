@@ -1,8 +1,78 @@
-"""Device workspaces for the fused trainers (activations, dZ, gradient partials)."""
+"""Device workspaces for the fused trainers (activations, dZ, gradient partials) and the
+marshalling every trainer does around the C entry points."""
 import torch
 
 from .. import _lib
 from ..models.arena import ParamArena
+
+
+class Pins:
+    """The tensors of one C call: `pins(t)` makes `t` fp32, contiguous and resident on `device`,
+    keeps that tensor alive in `keep` until the launch is enqueued and returns its device
+    pointer (None -> NULL); `pins.tensor(t)` returns the tensor itself."""
+
+    def __init__(self, device):
+        self.device = device
+        self.keep = []
+
+    def tensor(self, t):
+        if t is None:
+            return None
+        if t.dtype != torch.float32:
+            t = t.float()
+        t = _lib.on_device(t.contiguous(), self.device)
+        self.keep.append(t)
+        return t
+
+    def __call__(self, t):
+        return _lib.ptr(self.tensor(t), self.device)
+
+
+def batch_device(state: torch.Tensor, who: str):
+    """The device of a training batch (given its state features): a GPU, the current one."""
+    if not state.is_cuda:
+        raise _lib.Rb200Error(f"{who}: training batch must be on the GPU "
+                              "(reagent_b200 has no CPU path)")
+    _lib.require_current_device(state.device)
+    return state.device
+
+
+def discount_source(trainer, batch):
+    """The per-row exponent of gamma -- the batch's time_diff with use_seq_num_diff_as_time_diff,
+    its step with multi_steps -- or None for a constant gamma."""
+    if trainer.use_seq_num_diff_as_time_diff:
+        assert trainer.multi_steps is None
+        return batch.time_diff.reshape(-1)
+    if trainer.multi_steps is not None:
+        assert batch.step is not None
+        return batch.step.reshape(-1)
+    return None
+
+
+def loss_kind(q_network_loss: str) -> int:
+    """The kernels' code of RLParameters.q_network_loss."""
+    if q_network_loss == "mse":
+        return _lib.LOSS_MSE
+    if q_network_loss == "huber":
+        return _lib.LOSS_HUBER
+    raise Exception("Q-Network loss type {} not valid loss.".format(q_network_loss))
+
+
+def register_reward_boosts(module, actions, reward_boost) -> None:
+    """The [1, A] `reward_boosts` buffer of RLParameters.reward_boost ({action name: boost}) and
+    `_has_reward_boost`, which tells the kernels whether to read it."""
+    boosts = torch.zeros([1, len(actions)])
+    module._has_reward_boost = False
+    if reward_boost is not None:
+        for k in reward_boost.keys():
+            boosts[0, actions.index(k)] = reward_boost[k]
+            module._has_reward_boost = True
+    module.register_buffer("reward_boosts", boosts)
+
+
+def ws_fits(ws, B: int, device) -> bool:
+    """Whether a cached workspace dict was built for batch size B on `device`."""
+    return ws is not None and ws["B"] == B and ws["dev"] == device
 
 
 class NetWorkspace:
@@ -50,6 +120,13 @@ def wgrad(arena: ParamArena, ws: NetWorkspace, net_input, batch: int):
     arena.grad_ready = True
 
 
+def backward_wgrad(arena: ParamArena, ws: NetWorkspace, net_input, batch: int):
+    """The whole backward of one network from the dZ of its last layer: dZ chain, then the
+    weight gradients."""
+    arena.backward(ws, batch)
+    wgrad(arena, ws, net_input, batch)
+
+
 def head_backward_dx(arena: ParamArena, ws: NetWorkspace, batch: int, cache: dict):
     """dZ of the layer below a wide head: dz[L-2] = (dz[L-1] . W_head) * act'(h[L-2])
     (torch.nn.functional.linear's backward w.r.t. its input).  Wide heads (QR-DQN: A*N atoms,
@@ -57,7 +134,7 @@ def head_backward_dx(arena: ParamArena, ws: NetWorkspace, batch: int, cache: dic
     lib, st = _lib.lib(), _lib.cur_stream()
     L = len(arena.acts)
     K, N = arena.dims[L - 1], arena.dims[L]
-    W = arena.flat.data_ptr() + 4 * arena.w_off[L - 1]
+    W, _ = arena.layer_ptrs(L - 1)
     dz, h, out = ws.dz[L - 1], ws.hidden[L - 2], ws.dz[L - 2]
     key = ("dx_scratch", K, N, batch)
     if key not in cache:
