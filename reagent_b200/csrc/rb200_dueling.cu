@@ -77,7 +77,7 @@ __global__ void dueling_fold_apply_kernel(const float* __restrict__ Wa, const fl
   }
 }
 
-// per slab: dW_a, db_a from the folded gradient; the folded gradient is cleared
+// per slab: dW_a, db_a from the folded gradient; the folded gradient (dW_q and db_q) is cleared
 __global__ void dueling_unfold_apply_kernel(float* __restrict__ g, long long slab_stride, int R,
                                             int N, int H, long long o_wq, long long o_bq,
                                             long long o_wa, long long o_ba,
@@ -95,6 +95,7 @@ __global__ void dueling_unfold_apply_kernel(float* __restrict__ g, long long sla
     } else {
       const int r = (int)(i - total);
       s[o_ba + r] = s[o_bq + r] - sm[2 * H] * invR;
+      s[o_bq + r] = 0.f;
     }
   }
 }

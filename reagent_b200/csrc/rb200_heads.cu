@@ -169,22 +169,29 @@ __global__ void __launch_bounds__(256) c51_head_kernel(const C51Dev d) {
     }
     const float disc = (a.discount_src) ? powf(a.gamma, a.discount_src[b]) : a.gamma;
     const float nt = a.not_terminal[b];
-    for (int j = 0; j < N; ++j) {
+    // position b of atom j's target on the support grid and its neighbours l, u.  A NaN target
+    // keeps b NaN (fminf / fmaxf would clamp it to qmin) and lands on atom 0, so that m, the
+    // row's cross entropy and the loss turn NaN.  In float32 (qmax - qmin) / scale_support can
+    // exceed N - 1 by an ulp; b is clamped so that u stays inside m.
+    const auto project = [&](int j, int& l, int& u) {
       float tq = rew + (disc * nt) * a.support[j];
+      if (tq != tq) { l = u = 0; return tq; }
       tq = fminf(fmaxf(tq, a.qmin), a.qmax);
-      const float bb = (tq - a.qmin) / a.scale_support;
-      long long l = (long long)floorf(bb), u = (long long)ceilf(bb);
+      const float bb = fminf((tq - a.qmin) / a.scale_support, (float)(N - 1));
+      l = (int)floorf(bb);
+      u = (int)ceilf(bb);
       if (u > 0 && l == u) l -= 1;
       if (l < N - 1 && l == u) u += 1;
+      return bb;
+    };
+    for (int j = 0; j < N; ++j) {
+      int l, u;
+      const float bb = project(j, l, u);
       m[l] += nd[j] * ((float)u - bb);
     }
     for (int j = 0; j < N; ++j) {
-      float tq = rew + (disc * nt) * a.support[j];
-      tq = fminf(fmaxf(tq, a.qmin), a.qmax);
-      const float bb = (tq - a.qmin) / a.scale_support;
-      long long l = (long long)floorf(bb), u = (long long)ceilf(bb);
-      if (u > 0 && l == u) l -= 1;
-      if (l < N - 1 && l == u) u += 1;
+      int l, u;
+      const float bb = project(j, l, u);
       m[u] += nd[j] * (bb - (float)l);
     }
   }

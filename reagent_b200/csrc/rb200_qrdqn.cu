@@ -188,6 +188,7 @@ __global__ void __launch_bounds__(256) qr_head_kernel(const QrDev d) {
   }
   const float disc = a.discount_src ? powf(a.gamma, a.discount_src[b]) : a.gamma;
   const float nd = a.not_terminal[b];
+  bool finite = true;
   for (int n = tid; n < N; n += blockDim.x) {
     float nq;
     if (a.maxq) {
@@ -198,6 +199,7 @@ __global__ void __launch_bounds__(256) qr_head_kernel(const QrDev d) {
         nq += a.q_next_target[base + (size_t)c * N + n] * (staged ? s_nact[c] : a.next_action[(size_t)b * A + c]);
     }
     tq[n] = rew + disc * nd * nq;                                       // :142
+    finite = finite && isfinite(tq[n]);
     float cur = 0.f;                                                    // :149
     for (int c = 0; c < A; ++c) {
       const float w = staged ? s_act[c] : a.action[(size_t)b * A + c];
@@ -205,7 +207,7 @@ __global__ void __launch_bounds__(256) qr_head_kernel(const QrDev d) {
     }
     cq[n] = cur;
   }
-  __syncthreads();
+  const bool tq_finite = __syncthreads_and(finite);
   // pairwise quantile-Huber (:152-155): td[i,b,j] = target[i] - current[j], weight |tau_j - 1[td<0]|
   const float norm = 1.f / ((float)N * (float)a.batch * (float)N);
   const float w_row = kWeighted ? a.sample_weight[b] : 1.f;
@@ -238,6 +240,13 @@ __global__ void __launch_bounds__(256) qr_head_kernel(const QrDev d) {
     }
     lsum += l2;
     g += g2;
+    // fminf / fmaxf turn a NaN td into a derivative of 1; autograd keeps the NaN.  A NaN td
+    // needs a non-finite target or current value, so only such columns look for one.
+    if (!(tq_finite && isfinite(c)))
+      for (int i2 = 0; i2 < N; ++i2) {
+        const float td = tq[i2] - c;
+        if (td != td) g = td;
+      }
     float dcur = -g * norm;   // d loss / d current[j]
     if (kWeighted) dcur *= w_row;
     // d loss / d head output [b, a, j] = action[b,a] * dcur  (linear head)
@@ -330,15 +339,16 @@ extern "C" int rb200_qrdqn_head(const rb200_qrdqn_args_t* a, void* stream) {
   if (!a || a->batch <= 0 || a->num_actions <= 0 || a->num_atoms <= 0) { set_last_error("rb200_qrdqn_head: bad argument"); return RB200_E_INVALID; }
   if (!a->q_next_target || !a->q_cur || !a->action || !a->reward || !a->not_terminal || !a->dz_head ||
       !a->loss_partials || !a->loss || !a->tile_counter) { set_last_error("rb200_qrdqn_head: required pointer is null"); return RB200_E_INVALID; }
-  if (a->double_q && a->maxq && !a->q_next_online) { set_last_error("double-Q needs q_next_online"); return RB200_E_INVALID; }
+  // the atom means are read from q_next_online whenever double_q is set, SARSA included
+  if (a->double_q && !a->q_next_online) { set_last_error("double-Q needs q_next_online"); return RB200_E_INVALID; }
   if (!a->maxq && !a->next_action) { set_last_error("SARSA update needs next_action"); return RB200_E_INVALID; }
   QrDev d;
   d.a = *a;
   const size_t smem = (size_t)(2 * a->num_atoms + a->num_actions + 256) * sizeof(float);
   if (smem > 48 * 1024) { set_last_error("rb200_qrdqn_head: too many atoms/actions for one CTA"); return RB200_E_SMEM; }
-  if (a->sample_weight)
-    qr_head_kernel<true><<<a->batch, 256, smem, (cudaStream_t)stream>>>(d);
-  else
-    qr_head_kernel<false><<<a->batch, 256, smem, (cudaStream_t)stream>>>(d);
-  return check_cuda(cudaGetLastError(), "qr_head_kernel launch");
+  // opted in: the kernel's static shared memory comes on top of the 48 KB of dynamic
+  cudaStream_t st = (cudaStream_t)stream;
+  const char* what = "qr_head_kernel launch";
+  return a->sample_weight ? launch<qr_head_kernel<true>>(a->batch, 256, smem, st, what, d)
+                          : launch<qr_head_kernel<false>>(a->batch, 256, smem, st, what, d);
 }

@@ -336,11 +336,21 @@ def test_online_captured_equals_eager(kind, with_per):
 
 
 def test_online_per_qrdqn_nan_reward_raises():
+    _online_per_nan_reward_raises("qrdqn")
+
+
+def test_online_per_c51_nan_reward_raises():
+    """C51's projection must keep a NaN target (a clamp with fminf / fmaxf turned it into qmin
+    and the step trained on the transition without reporting it)."""
+    _online_per_nan_reward_raises("c51")
+
+
+def _online_per_nan_reward_raises(kind):
     from reagent_b200.replay_memory import PrioritizedUpdate
     from reagent_b200.training.fused_step import FusedDqnStep
 
-    cfg = _cfg("qrdqn")
-    rb, t = _setup("qrdqn", _stream(3000, cfg["S"], cfg["A"], 5))
+    cfg = _cfg(kind)
+    rb, t = _setup(kind, _stream(3000, cfg["S"], cfg["A"], 5))
     random.seed(1)
     fused = FusedDqnStep(t, rb, cfg["B"], rng="device", online=True, per=PrioritizedUpdate())
     extra = _stream(10, cfg["S"], cfg["A"], 6)
