@@ -114,6 +114,21 @@ int rb200_mlp_forward(const rb200_mlp_t* net, const float* in0, int32_t d0, cons
                       int32_t d1, int32_t batch, float* out, const rb200_net_ws_t* save_hidden,
                       void* stream);
 
+/* Tiled forward of the max-Q target of ParametricDQNTrainer (reagent/training/
+ * parametric_dqn_trainer.py:101-110, FeatureData.get_tiled_batch): for each of the
+ * batch * num_tiled rows r, out_n[r] = net_n(cat(state[r / num_tiled], actions[r])).
+ * state [batch, state_dim]; actions [batch * num_tiled, action_dim]; out0 / out1
+ * [batch * num_tiled, dims[L]].  net1 (with out1) is optional and must have net0's dims and
+ * activations; both networks run over one input tile built in shared memory, so the tiled
+ * input is never written to HBM.  Every output is bit-equal to rb200_mlp_forward on the
+ * materialised cat(state.repeat_interleave(num_tiled), actions).  RB200_E_INVALID on null
+ * pointers, differing descriptors, widths that do not sum to dims[0] or batch * num_tiled
+ * past int32; RB200_E_SMEM where rb200_mlp_forward's tile would not fit. */
+int rb200_mlp_forward_tiled(const rb200_mlp_t* net0, const rb200_mlp_t* net1,
+                            const float* state, int32_t state_dim, const float* actions,
+                            int32_t action_dim, int32_t batch, int32_t num_tiled, float* out0,
+                            float* out1, void* stream);
+
 /* ------------------------------------------------------------------------- */
 /* Dueling head folded into a Linear (rb200_dueling.cu).  Replaces the head arithmetic of     */
 /* DuelingQNetwork._get_values (reagent/models/dueling_q_network.py:92-103), with atoms:       */

@@ -265,6 +265,8 @@ def _declare(lib):
                                          C.POINTER(NetWsT), _vp, C.c_int64, C.c_int32, _vp]
     lib.rb200_mlp_forward.argtypes = [C.POINTER(MlpT), _vp, C.c_int32, _vp, C.c_int32, C.c_int32,
                                       _vp, C.POINTER(NetWsT), _vp]
+    lib.rb200_mlp_forward_tiled.argtypes = [C.POINTER(MlpT), C.POINTER(MlpT), _vp, C.c_int32, _vp,
+                                            C.c_int32, C.c_int32, C.c_int32, _vp, _vp, _vp]
     lib.rb200_linear_forward.argtypes = [_vp, _vp, C.c_int32, C.c_int32, C.c_int32, _vp,
                                          C.c_int32, _vp, _vp]
     lib.rb200_linear_backward_dx.argtypes = [_vp, C.c_int32, C.c_int32, _vp, _vp, C.c_int32,

@@ -48,6 +48,59 @@ __global__ void __launch_bounds__(NT, 1) mlp_fwd_rows_kernel(const Mlp net, cons
   tile_store_rows<NT, R>(xo, p.ld_o, p.out, DO, DO, row0, p.batch);
 }
 
+// Tiled forward of ParametricDQN's max-Q target: row r of the B*M rows is
+// cat(state[r / M], actions[r]) (FeatureData.get_tiled_batch + the possible next actions),
+// built in shared memory by the loader, so the tiled input never exists in HBM.  Every network
+// of the launch (online and target: same dims / act) runs over the SAME input tile.  The tile,
+// its shared-memory layout and the grid mapping are those of mlp_fwd_rows_kernel on the
+// materialised [B*M, S+K] input, and so are the bits of every output.
+struct TiledFwdDev {
+  const float* state; int S;     // [B, S]
+  const float* actions; int K;   // [B*M, K]
+  float* out[2];                 // [B*M, dims[L]] per network
+  int n_nets, rows, M;           // rows = B*M
+  int ld_in, ld_h, ld_o;
+};
+
+template <int NT, int TM, int KC>
+__global__ void __launch_bounds__(NT, 1) mlp_fwd_tiled_kernel(const Mlp net0, const Mlp net1,
+                                                              const TiledFwdDev p) {
+  constexpr int R = (NT / 64) * TM;
+  extern __shared__ __align__(16) float smem[];
+  tile_smem_zero_all<NT>(smem);
+  float* Wst = smem;
+  float* xin = Wst + 2 * wstage_floats<KC>();
+  float* hA = xin + R * p.ld_in;
+  float* hB = hA + R * p.ld_h;
+  float* xo = hB + R * p.ld_h;
+  const int row0 = blockIdx.x * R;
+  const int D = p.S + p.K, D4 = round_up4(D);
+  for (int idx = threadIdx.x; idx < R * D4; idx += NT) {
+    const int r = idx / D4, c = idx - r * D4;
+    const int gr = row0 + r;
+    float v = 0.f;
+    if (gr < p.rows) {
+      if (c < p.S) v = p.state[(size_t)(gr / p.M) * p.S + c];
+      else if (c < D) v = p.actions[(size_t)gr * p.K + (c - p.S)];
+    }
+    xin[r * p.ld_in + c] = v;
+  }
+  __syncthreads();
+  const int DO = net0.dims[net0.n_layers];
+  tile_mlp_fwd<NT, TM, KC>(net0, xin, p.ld_in, hA, hB, p.ld_h, xo, p.ld_o, Wst, nullptr, row0,
+                           p.rows);
+  tile_store_rows<NT, R>(xo, p.ld_o, p.out[0], DO, DO, row0, p.rows);
+  if (p.n_nets < 2) return;
+  // the second network starts from the state the first one saw: hidden and output tiles zero
+  // (their padding columns feed the MMA against zero weights), the input tile untouched
+  __syncthreads();
+  for (int i = threadIdx.x; i < R * (2 * p.ld_h + p.ld_o); i += NT) hA[i] = 0.f;
+  __syncthreads();
+  tile_mlp_fwd<NT, TM, KC>(net1, xin, p.ld_in, hA, hB, p.ld_h, xo, p.ld_o, Wst, nullptr, row0,
+                           p.rows);
+  tile_store_rows<NT, R>(xo, p.ld_o, p.out[1], DO, DO, row0, p.rows);
+}
+
 }  // namespace rb200
 
 using namespace rb200;
@@ -79,5 +132,64 @@ extern "C" int rb200_mlp_forward(const rb200_mlp_t* net, const float* in0, int32
   return dispatch_rows(cfg, [&](auto NT, auto KC) {
     return launch<mlp_fwd_rows_kernel<NT(), 4, KC()>>(grid, NT(), cfg.smem_bytes, st,
                                                       "mlp_fwd_rows_kernel launch", m, p);
+  });
+}
+
+extern "C" int rb200_mlp_forward_tiled(const rb200_mlp_t* net0, const rb200_mlp_t* net1,
+                                       const float* state, int32_t state_dim,
+                                       const float* actions, int32_t action_dim, int32_t batch,
+                                       int32_t num_tiled, float* out0, float* out1,
+                                       void* stream) {
+  if (!net0 || !state || !actions || !out0 || (net1 != nullptr) != (out1 != nullptr)) {
+    set_last_error("rb200_mlp_forward_tiled: null argument (net1 and out1 go together)");
+    return RB200_E_INVALID;
+  }
+  if (int rc = validate_mlp(net0, "net0")) return rc;
+  if (net1) {
+    if (int rc = validate_mlp(net1, "net1")) return rc;
+    bool same = net1->n_layers == net0->n_layers;
+    for (int l = 0; same && l <= net0->n_layers; ++l) same = net1->dims[l] == net0->dims[l];
+    for (int l = 0; same && l < net0->n_layers; ++l) same = net1->act[l] == net0->act[l];
+    if (!same) {
+      set_last_error("rb200_mlp_forward_tiled: net0 and net1 differ in dims or activations");
+      return RB200_E_INVALID;
+    }
+  }
+  if (batch <= 0 || num_tiled <= 0) {
+    set_last_error("rb200_mlp_forward_tiled: batch %d and num_tiled %d must be positive", batch,
+                   num_tiled);
+    return RB200_E_INVALID;
+  }
+  if ((long long)batch * num_tiled > INT32_MAX) {
+    set_last_error("rb200_mlp_forward_tiled: batch * num_tiled = %lld overflows int32",
+                   (long long)batch * num_tiled);
+    return RB200_E_INVALID;
+  }
+  if (state_dim <= 0 || action_dim <= 0 || state_dim + action_dim != net0->dims[0]) {
+    set_last_error("rb200_mlp_forward_tiled: input width %d + %d != dims[0]=%d", state_dim,
+                   action_dim, net0->dims[0]);
+    return RB200_E_INVALID;
+  }
+  const int rows = batch * num_tiled;
+  TiledFwdDev p;
+  p.state = state; p.S = state_dim; p.actions = actions; p.K = action_dim;
+  p.out[0] = out0; p.out[1] = out1; p.n_nets = net1 ? 2 : 1;
+  p.rows = rows; p.M = num_tiled;
+  const int DO = net0->dims[net0->n_layers];
+  const int hmax = mlp_max_hidden(net0);
+  p.ld_o = round_up4(DO) + 4;
+  if (p.ld_o > 1024 + 4) { set_last_error("rb200_mlp_forward_tiled: output width %d too large for the row-tile kernel", DO); return RB200_E_SMEM; }
+  // the tile of rb200_mlp_forward on the materialised [rows, S+K] input: the k-chunk rotation
+  // of tile_linear_fwd depends on the tile and the CTA, so this keeps every output bit-equal
+  RowsCfg cfg = pick_rows_cfg(rows, net0->dims[0], hmax, 1, 2, p.ld_o, 0);
+  if (cfg.tm == 0) { set_last_error("rb200_mlp_forward_tiled: tile does not fit in shared memory"); return RB200_E_SMEM; }
+  p.ld_in = cfg.ld_in; p.ld_h = cfg.ld_h;
+  const Mlp m0 = make_mlp(net0);
+  const Mlp m1 = make_mlp(net1 ? net1 : net0);
+  const int grid = ceil_div(rows, rows_per_tile(cfg));
+  cudaStream_t st = (cudaStream_t)stream;
+  return dispatch_rows(cfg, [&](auto NT, auto KC) {
+    return launch<mlp_fwd_tiled_kernel<NT(), 4, KC()>>(grid, NT(), cfg.smem_bytes, st,
+                                                       "mlp_fwd_tiled_kernel launch", m0, m1, p);
   });
 }

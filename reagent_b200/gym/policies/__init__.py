@@ -2,13 +2,15 @@
 then an action sampler -- the reference's Policy = scorer o sampler composition.
 
   discrete_dqn_scorer        reagent/gym/policies/scorers/discrete_scorer.py:16-48
+  parametric_dqn_scorer      reagent/gym/policies/scorers/discrete_scorer.py:65-87
   Greedy / EpsilonGreedy / Softmax samplers
                              reagent/gym/policies/samplers/discrete_sampler.py:14-183
   Policy                     reagent/gym/policies/policy.py:13-43
   ActorPolicyWrapper         reagent/model_managers/actor_critic_base.py:51-64 (continuous actors)
 
 The scorer runs `q_network(obs)` (ONE fused launch, rb200_mlp_forward; a QR-DQN head is
-averaged over atoms) on the GPU; the samplers are index / probability arithmetic on the (B, A)
+averaged over atoms) on the GPU -- for a parametric q network, q(obs, a) of every one-hot action
+a in one rb200_mlp_forward_tiled launch; the samplers are index / probability arithmetic on the (B, A)
 score tensor with torch's own RNG, so a seeded draw reproduces the reference's draw.
 """
 from typing import Any, Optional
@@ -46,6 +48,37 @@ def discrete_dqn_scorer(q_network):
         assert scores.dim() == 2, f"{scores.shape} isn't (batchsize, num_actions)."
         q_network.train(was_training or True)  # the reference always switches back to train()
         return apply_possible_actions_mask(scores, possible_actions_mask)
+
+    return score
+
+
+def parametric_dqn_scorer(max_num_actions: int, q_network):
+    """Scores (n, max_num_actions) of q_network(obs[i], e_a) for every one-hot action e_a, the
+    reference's get_parametric_input (obs.get_tiled_batch + get_possible_actions_for_gym).  The
+    repeated observations are built per row tile inside the forward kernel and never exist in
+    memory; the (n * max_num_actions, max_num_actions) identity tiling is a device tensor,
+    cached for the last n."""
+    from ...models.arena import run_mlp_tiled
+
+    eyes = {}
+
+    @torch.no_grad()
+    def score(preprocessed_obs: rlt.FeatureData) -> torch.Tensor:
+        obs = preprocessed_obs.float_features
+        assert obs.dim() == 2, f"{obs.shape} is not (batch_size, state_dim)."
+        arena = q_network.arena
+        dev = arena.flat.device
+        obs = obs.to(dev, torch.float32).contiguous()
+        n = obs.shape[0]
+        key = (n, str(dev))
+        if key not in eyes:
+            eyes.clear()
+            eyes[key] = torch.eye(max_num_actions, device=dev).repeat(n, 1)
+        q_network.eval()
+        out = torch.empty(n * max_num_actions, arena.dims[-1], device=dev)
+        run_mlp_tiled([arena], obs, eyes[key], max_num_actions, [out])
+        q_network.train()
+        return out.view(-1, max_num_actions)
 
     return score
 

@@ -1,10 +1,11 @@
 """Model managers: `build_trainer(normalization_data_map, use_gpu, reward_options=None)` with
 the reference's flow (reagent/model_managers/model_manager.py:84-96 and
 discrete/discrete_dqn.py:63-116, discrete/discrete_qrdqn.py:73-121,
-discrete/discrete_c51dqn.py:43-88, actor_critic/sac.py:80-113,
-actor_critic/td3.py:70-102): build the networks from the net builders, copy the target, hand
-everything to the trainer.  Policies, serving modules, data modules and reporters are out of
-scope (SURVEY.md section 2 rows 8, 12, 15, 16)."""
+discrete/discrete_c51dqn.py:43-88, parametric/parametric_dqn.py:45-81,
+actor_critic/sac.py:80-113, actor_critic/td3.py:70-102): build the networks from the net
+builders, copy the target, hand everything to the trainer; `create_policy` gives the online
+act-time policy.  Serving modules, data modules and reporters are out of scope (SURVEY.md
+section 2 rows 8, 12, 15, 16)."""
 from dataclasses import dataclass, field
 from typing import Union, Dict, List, Optional
 
@@ -14,7 +15,8 @@ from ..net_builder import (ActorFullyConnected, Categorical, Dueling, DuelingQua
                            FullyConnected, GaussianFullyConnected, ParametricFullyConnected,
                            Quantile)
 from ..optimizer import Optimizer__Union
-from ..training import C51Trainer, DQNTrainer, QRDQNTrainer, SACTrainer, TD3Trainer
+from ..training import (C51Trainer, DQNTrainer, ParametricDQNTrainer, QRDQNTrainer, SACTrainer,
+                        TD3Trainer)
 
 
 def _device(use_gpu: bool):
@@ -139,6 +141,54 @@ class DiscreteC51DQN(_DiscretePolicyMixin):
             rl=self.rl, double_q_learning=self.double_q_learning,
             minibatch_size=self.minibatch_size, num_atoms=self.num_atoms, qmin=self.qmin,
             qmax=self.qmax, optimizer=self.optimizer).to(dev)
+
+
+@dataclass
+class ParametricDQN:
+    """reagent/model_managers/parametric/parametric_dqn.py with its `trainer_param`
+    (ParametricDQNTrainerParameters) flattened into the manager, as DiscreteC51DQN does."""
+    rl: RLParameters = field(default_factory=RLParameters)
+    double_q_learning: bool = True
+    minibatches_per_step: int = 1
+    optimizer: Optimizer__Union = field(default_factory=Optimizer__Union.default)
+    net_builder: ParametricFullyConnected = field(default_factory=ParametricFullyConnected)
+    # reagent/model_managers/parametric_dqn_base.py:55: EvaluationParameters() by default
+    eval_parameters: EvaluationParameters = field(default_factory=EvaluationParameters)
+
+    @property
+    def rl_parameters(self) -> RLParameters:
+        return self.rl
+
+    def build_trainer(self, normalization_data_map, use_gpu: bool,
+                      reward_options=None) -> ParametricDQNTrainer:
+        """parametric_dqn.py:45-81: the q network, a reward network with one output for the
+        reward and one per metric to score (get_metrics_to_score: the sorted keys of
+        `reward_options.metric_reward_values`), the target as a copy of the q network."""
+        dev = _device(use_gpu)
+        s, a = (normalization_data_map[NormalizationKey.STATE],
+                normalization_data_map[NormalizationKey.ACTION])
+        q_network = self.net_builder.build_q_network(s, a).to(dev)
+        metric_values = getattr(reward_options, "metric_reward_values", None)
+        metrics_to_score = sorted(metric_values) if metric_values else []
+        reward_network = self.net_builder.build_q_network(
+            s, a, output_dim=len(metrics_to_score) + 1).to(dev)
+        q_network_target = q_network.get_target_network()
+        return ParametricDQNTrainer(
+            q_network=q_network, q_network_target=q_network_target,
+            reward_network=reward_network, rl=self.rl,
+            double_q_learning=self.double_q_learning,
+            minibatches_per_step=self.minibatches_per_step, optimizer=self.optimizer).to(dev)
+
+    def create_policy(self, trainer_module, serving: bool = False, normalization_data_map=None):
+        """parametric_dqn_base.py:73-103: softmax over the scores of every one-hot action at
+        temperature rl.temperature.  Serving modules are out of scope."""
+        if serving:
+            raise NotImplementedError("serving modules are out of scope of reagent_b200")
+        from ..gym.policies import Policy, SoftmaxActionSampler, parametric_dqn_scorer
+
+        action_dim = trainer_module.q_network.action_dim
+        return Policy(scorer=parametric_dqn_scorer(action_dim, trainer_module.q_network),
+                      sampler=SoftmaxActionSampler(temperature=self.rl.temperature))
 
 
 @dataclass

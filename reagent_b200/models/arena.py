@@ -117,6 +117,34 @@ def run_mlp(desc: _lib.MlpT, x, out, x1=None, save=None):
     _lib.check(rc, "rb200_mlp_forward")
 
 
+def run_mlp_tiled(arenas, state, actions, num_tiled: int, outs):
+    """outs[n][r] = arenas[n](cat(state[r // num_tiled], actions[r])) for one or two arenas of
+    identical shape (online and target), as ONE launch over a shared input tile; bit-equal to
+    run_mlp on the materialised cat(state.repeat_interleave(num_tiled), actions)."""
+    assert len(arenas) == len(outs) in (1, 2)
+    # the C ABI takes no row count for `actions` or the outputs: check every shape here
+    B, M = state.shape[0], int(num_tiled)
+    dev = state.device
+    named = [("state", state), ("actions", actions)] + [(f"outs[{i}]", o) for i, o in enumerate(outs)]
+    for name, t in named:
+        assert t.dim() == 2 and t.dtype == torch.float32 and t.is_cuda and t.device == dev, (
+            f"{name}: expected a 2-D float32 CUDA tensor on {dev}, "
+            f"got {t.dtype} {tuple(t.shape)} on {t.device}")
+        assert t.is_contiguous(), f"{name} must be contiguous"
+    assert M >= 1 and actions.shape[0] == B * M, (
+        f"actions has {actions.shape[0]} rows, expected batch {B} * num_tiled {M}")
+    assert state.shape[1] + actions.shape[1] == arenas[0].dims[0], (
+        f"state width {state.shape[1]} + action width {actions.shape[1]} != {arenas[0].dims[0]}")
+    for i, (a, o) in enumerate(zip(arenas, outs)):
+        assert tuple(o.shape) == (B * M, a.dims[-1]), f"outs[{i}] shape {tuple(o.shape)}"
+    d1 = arenas[1].desc() if len(arenas) == 2 else None
+    rc = _lib.lib().rb200_mlp_forward_tiled(
+        arenas[0].desc(), d1, state.data_ptr(), state.shape[1], actions.data_ptr(),
+        actions.shape[1], state.shape[0], num_tiled, outs[0].data_ptr(),
+        None if d1 is None else outs[1].data_ptr(), _lib.cur_stream())
+    _lib.check(rc, "rb200_mlp_forward_tiled")
+
+
 def flatten_linears(linears: List[nn.Linear], arena: ParamArena, device=None) -> torch.Tensor:
     """Move the Linear parameters into one flat buffer (keeping their values) and re-point
     `.data` at views of it.  Returns the flat tensor."""

@@ -131,6 +131,8 @@ class ReplayBuffer:
         self._decays_dev = None
         # optional fused normalisation of `observation` (set_state_preprocessor)
         self._preproc = None
+        # (B*A, A) identity tilings of sample_parametric_dqn_batch, per (B, A)
+        self._tiled_eye_cache: Dict[tuple, torch.Tensor] = {}
 
     # ------------------------------------------------------------------ init
     def _dev(self):
@@ -622,18 +624,29 @@ class ReplayBuffer:
             self._ones_cache = (key, torch.ones(B, A, device=self._dev()))
         return self._ones_cache[1]
 
-    def sample_discrete_dqn_batch(self, batch_size, num_actions, indices=None, **index_kwargs):
-        """sample_transition_batch + DiscreteDqnInputMaker.__call__
-        (gym/preprocessors/trainer_preprocessor.py:100-158) as ONE launch: returns an
-        rlt.DiscreteDqnInput of device tensors (masks are ones, step carries the n-step
-        length as float, time_diff None)."""
-        from ..core import types as rlt
+    def _tiled_eye(self, B, A):
+        """get_possible_actions_for_gym (trainer_preprocessor.py:357-367): the (B*A, A) tiling of
+        the A x A identity, one cached device constant per shape, so a sampling launch that
+        returns it can be captured into a CUDA graph."""
+        # never evicted: a captured graph keeps reading the constant of its shape, and a
+        # workload samples a handful of (batch size, action count) shapes
+        t = self._tiled_eye_cache.get((B, A))
+        if t is None:
+            t = torch.eye(A, device=self._dev()).repeat(B, 1)
+            self._tiled_eye_cache[(B, A)] = t
+        return t
 
+    def _sample_onehot(self, batch_size, num_actions, indices, index_kwargs, stored_masks):
+        """The ONE rb200_replay_sample launch behind the discrete-action batches: state,
+        next state, reward, not_terminal, the one-hot action and next action (zeroed on
+        terminal rows, one_hot_actions of trainer_preprocessor.py:72-97), the stored `log_prob`
+        and, with `stored_masks`, the stored `possible_actions_mask` and its next twin.
+        Returns (tensors, action, next_action, action_probability | None, masks | None)."""
         amd = self._key_to_replay_elem["action"].metadata
         if amd.dtype != np.int64 or amd.shape != ():
             raise NotImplementedError("discrete batches need an int64 scalar action")
         args, t, keep = self._fused_common(batch_size, indices, index_kwargs)
-        B, dev = batch_size, self._dev()
+        B = batch_size
         action = self._alloc("action", B, num_actions)
         next_action = self._alloc("next_action", B, num_actions)
         args.action_i64 = self._store["action"].data_ptr()
@@ -655,23 +668,59 @@ class ReplayBuffer:
 
         if "log_prob" in self._store:
             prob = spec("log_prob", "log_prob", 0, 1)
-        # DiscreteDqnInputMaker :131-139: masks come from the `possible_actions_mask` extra
-        # (and its `next_` twin) when the buffer stores one, else ones
-        pam = pnam = self._ones(B, num_actions)
-        if "possible_actions_mask" in self._store:
+        masks = None
+        if stored_masks and "possible_actions_mask" in self._store:
             md = self._key_to_replay_elem["possible_actions_mask"].metadata
             if md.dtype != np.float32 or md.shape != (num_actions,):
                 raise NotImplementedError("possible_actions_mask must be float32 [num_actions]")
-            pam = spec("possible_actions_mask", "possible_actions_mask", 0, num_actions)
-            pnam = spec("possible_actions_mask", "possible_next_actions_mask", 1, num_actions)
+            masks = (spec("possible_actions_mask", "possible_actions_mask", 0, num_actions),
+                     spec("possible_actions_mask", "possible_next_actions_mask", 1, num_actions))
         args.n_specs = ns
         _lib.check(_lib.lib().rb200_replay_sample(args, _lib.cur_stream()), "rb200_replay_sample")
+        return t, action, next_action, None if prob is None else prob.exp(), masks
+
+    def sample_discrete_dqn_batch(self, batch_size, num_actions, indices=None, **index_kwargs):
+        """sample_transition_batch + DiscreteDqnInputMaker.__call__
+        (gym/preprocessors/trainer_preprocessor.py:100-158) as ONE launch: returns an
+        rlt.DiscreteDqnInput of device tensors (masks are ones, step carries the n-step
+        length as float, time_diff None)."""
+        from ..core import types as rlt
+
+        t, action, next_action, prob, masks = self._sample_onehot(
+            batch_size, num_actions, indices, index_kwargs, stored_masks=True)
+        # DiscreteDqnInputMaker :131-139: masks come from the `possible_actions_mask` extra
+        # (and its `next_` twin) when the buffer stores one, else ones
+        pam, pnam = masks if masks is not None else (self._ones(batch_size, num_actions),) * 2
         batch = rlt.DiscreteDqnInput(
             state=rlt.FeatureData(t["state"]), next_state=rlt.FeatureData(t["next_state"]),
             reward=t["reward"], time_diff=None, step=t["step"], not_terminal=t["not_terminal"],
             action=action, next_action=next_action, possible_actions_mask=pam,
-            possible_next_actions_mask=pnam,
-            extras=rlt.ExtraData(action_probability=None if prob is None else prob.exp()))
+            possible_next_actions_mask=pnam, extras=rlt.ExtraData(action_probability=prob))
+        batch.indices = t["indices"]
+        batch.sampling_probabilities = t.get("sampling_probabilities")
+        return batch
+
+    def sample_parametric_dqn_batch(self, batch_size, num_actions, indices=None,
+                                    **index_kwargs):
+        """sample_transition_batch + ParametricDqnInputMaker.__call__
+        (gym/preprocessors/trainer_preprocessor.py:370-413) as ONE launch: returns an
+        rlt.ParametricDqnInput of device tensors.  The actions are one-hot FeatureData (the next
+        action zeroed on terminal rows); the possible (next) actions are the (B*A, A) identity
+        tiling and both masks are ones, cached device constants; step and time_diff are None,
+        as the reference's input maker passes them.  A stored `possible_actions_mask` extra is
+        ignored, as the reference ignores it."""
+        from ..core import types as rlt
+
+        t, action, next_action, prob, _ = self._sample_onehot(
+            batch_size, num_actions, indices, index_kwargs, stored_masks=False)
+        tiled = rlt.FeatureData(self._tiled_eye(batch_size, num_actions))
+        ones = self._ones(batch_size, num_actions)
+        batch = rlt.ParametricDqnInput(
+            state=rlt.FeatureData(t["state"]), next_state=rlt.FeatureData(t["next_state"]),
+            reward=t["reward"], time_diff=None, step=None, not_terminal=t["not_terminal"],
+            action=rlt.FeatureData(action), next_action=rlt.FeatureData(next_action),
+            possible_actions=tiled, possible_actions_mask=ones, possible_next_actions=tiled,
+            possible_next_actions_mask=ones, extras=rlt.ExtraData(action_probability=prob))
         batch.indices = t["indices"]
         batch.sampling_probabilities = t.get("sampling_probabilities")
         return batch

@@ -15,6 +15,10 @@ does not depend on the parameters).  The host's random stream is consumed in the
 the only observable difference is that a transition added between two `step()` calls can be
 sampled one update later.
 
+`FusedDqnStep` drives DQNTrainer, QRDQNTrainer and C51Trainer on sample_discrete_dqn_batch and
+ParametricDQNTrainer on sample_parametric_dqn_batch (one-hot actions as features, the identity
+tiling of the possible actions); the latter without `per` and on one GPU.
+
 `FusedPolicyStep` is the device-resident online step for SACTrainer and TD3Trainer (continuous
 actions), with the same staging, draw, status words and optional prioritized replay.
 """
@@ -27,6 +31,7 @@ from ..replay_memory.device_replay import DeviceReplay, PrioritizedUpdate
 from ..replay_memory.prioritized_replay_buffer import PrioritizedReplayBuffer
 from .c51_trainer import C51Trainer
 from .dqn_trainer import DQNTrainer
+from .parametric_dqn_trainer import ParametricDQNTrainer
 from .qrdqn_trainer import QRDQNTrainer
 from .sac_trainer import SACTrainer
 from .td3_trainer import TD3Trainer
@@ -78,6 +83,17 @@ class FusedDqnStep:
         distributional loss for QR-DQN (mean over the N^2 quantile pairs) and C51 (cross
         entropy).  Online, a transition staged without `priority` enters with the largest
         priority recorded so far."""
+        if isinstance(trainer, ParametricDQNTrainer):
+            if per is not None:
+                raise NotImplementedError("per does not cover ParametricDQNTrainer: its loss head "
+                                          "has no importance weights")
+            if shard is not None or process_group is not None:
+                raise NotImplementedError("the ParametricDQNTrainer step is single-GPU; "
+                                          "train_batch(process_group=...) runs data-parallel")
+        # ParametricDqnInputMaker's batch (one-hot actions as features, the identity tiling of
+        # the possible actions) for ParametricDQNTrainer, DiscreteDqnInputMaker's for the rest
+        self._sampler = ("sample_parametric_dqn_batch" if isinstance(trainer, ParametricDQNTrainer)
+                         else "sample_discrete_dqn_batch")
         if per is not None:
             if rng != "device":
                 raise ValueError("per needs rng='device': the priorities live in the device tree")
@@ -149,8 +165,8 @@ class FusedDqnStep:
             with self.rb.output_buffers(self._pools[0]):
                 self._batches[0] = self._sample(None)
             with self.rb.output_buffers(self._pools[1]):
-                self._batches[1] = self.rb.sample_discrete_dqn_batch(
-                    self.B, trainer.num_actions, indices=self._batches[0].indices.reshape(-1))
+                self._batches[1] = self._sample_batch(
+                    self.B, indices=self._batches[0].indices.reshape(-1))
             torch.cuda.synchronize()
         for i in range(slots):
             self.slots.append(self._capture(i))
@@ -260,10 +276,14 @@ class FusedDqnStep:
             self.dr.launch_add(1, slot=stage_row, priority_from_max=self.per is not None)
         return self._gather(self.dr.draw_indices(self.B_global, out=self._idx_buf[slot]))
 
+    def _sample_batch(self, batch_size, **kw):
+        """The trainer's replay batch: sample_parametric_dqn_batch for ParametricDQNTrainer,
+        sample_discrete_dqn_batch for the discrete-action trainers."""
+        return getattr(self.rb, self._sampler)(batch_size, self.trainer.num_actions, **kw)
+
     def _gather(self, indices):
         """This rank's rows of the drawn global `indices`, as the trainer's batch."""
-        return self.rb.sample_discrete_dqn_batch(self.B, self.trainer.num_actions,
-                                                 indices=indices[self.row0:self.row0 + self.B])
+        return self._sample_batch(self.B, indices=indices[self.row0:self.row0 + self.B])
 
     def _sample(self, rnd_dev, overrides=None):
         if self.dr is not None:
@@ -277,7 +297,7 @@ class FusedDqnStep:
             kw["overrides"] = overrides
         if rnd_dev is not None:
             kw[self._query_kw] = rnd_dev
-        return self.rb.sample_discrete_dqn_batch(self.B, self.trainer.num_actions, **kw)
+        return self._sample_batch(self.B, **kw)
 
     _loss_width = 1  # elements of the loss copied to the pinned host tensor of a step
 

@@ -1,9 +1,11 @@
 """ParametricDQNTrainer (reagent/training/parametric_dqn_trainer.py:22-214) on the generic
 kernels of this library: the critic-shaped q_network(state, action) is evaluated by
-rb200_mlp_forward (on the tiled possible next actions for max-Q learning), rb200_pdqn_head turns
-the values into the TD loss and d loss / d q, rb200_mlp_backward + rb200_mlp_wgrad produce the
-parameter gradients, FusedAdam / SoftUpdate apply them.  The tiling and the concatenation of
-(state, action) are torch plumbing on device tensors."""
+rb200_mlp_forward, and for max-Q learning by rb200_mlp_forward_tiled, which scores every
+(next state, possible next action) pair of both networks in one launch without writing the
+tiled input to HBM.  rb200_pdqn_head turns the values into the TD loss and d loss / d q,
+rb200_mlp_backward + rb200_mlp_wgrad produce the parameter gradients, FusedAdam / SoftUpdate
+apply them.  The concatenation of (state, action) for the current-state and SARSA forwards is
+torch plumbing on device tensors."""
 from typing import Optional
 
 import torch
@@ -11,6 +13,7 @@ import torch
 from .. import _lib
 from ..core import types as rlt
 from ..core.parameters import RLParameters
+from ..models.arena import run_mlp_tiled
 from ..optimizer import Optimizer__Union, SoftUpdate
 from .reagent_lightning_module import ReAgentLightningModule
 from .rl_trainer_pytorch import RLTrainerMixin
@@ -36,6 +39,12 @@ class ParametricDQNTrainer(RLTrainerMixin, ReAgentLightningModule):
             raise NotImplementedError("bce_with_logits (gamma == 0 only) has no fused head")
         self.q_network_loss_kind = loss_kind(self.rl_parameters.q_network_loss)
         self._ws = None
+
+    @property
+    def num_actions(self) -> int:
+        """Width of the q network's action input: the one-hot width of replay batches
+        (ReplayBuffer.sample_parametric_dqn_batch) and of the act-time policy."""
+        return self.q_network.action_dim
 
     def configure_optimizers(self):
         """[Adam(q_network), (Adam(reward_network),) SoftUpdate] -- :66-86."""
@@ -83,15 +92,22 @@ class ParametricDQNTrainer(RLTrainerMixin, ReAgentLightningModule):
         a.batch = B
         next_state = batch.next_state.float_features.float()
         if self.maxq_learning:
-            pna = batch.possible_next_actions.float_features.float()
+            pna = pins.tensor(batch.possible_next_actions.float_features)
             product = pna.shape[0]
             assert product % B == 0, f"batch_size * max_num_action {product} is not divisible by batch_size {B}"
             M = product // B
-            # FeatureData.get_tiled_batch: row i repeated M times, then cat with the actions
-            x_next = torch.cat((next_state.repeat_interleave(M, dim=0), pna), dim=1).contiguous()
-            nq_t = self._fwd(self.q_network_target, x_next)
-            nq = self._fwd(self.q_network, x_next) if self.double_q_learning else None
-            pins.keep += [x_next, nq_t, nq]
+            # FeatureData.get_tiled_batch + cat with the possible next actions, built per row
+            # tile in shared memory; both networks score the same tile in one launch
+            ns = pins.tensor(next_state)
+            nq_t = torch.empty(product, self.q_network_target.arena.dims[-1], device=pins.device)
+            arenas, outs = [self.q_network_target.arena], [nq_t]
+            nq = None
+            if self.double_q_learning:
+                nq = torch.empty_like(nq_t)
+                arenas.append(self.q_network.arena)
+                outs.append(nq)
+            run_mlp_tiled(arenas, ns, pna, M, outs)
+            pins.keep += [nq_t, nq]
             a.max_num_action = M
             a.next_q = None if nq is None else nq.data_ptr()
             a.next_q_target = nq_t.data_ptr()
