@@ -429,10 +429,26 @@ typedef struct rb200_ac_args {
   float* log_prob_out;       /* [B] or NULL (unclamped sum of log-probs) */
   float* q1_value;           /* [B] or NULL */
   float* q2_value;           /* [B] or NULL */
+  /* SAC state-value network V(s) (sac_trainer.py:109-113, :214-217, :254-283, :329-343);
+     ahead of the prioritized-replay pair, which stays last */
+  const rb200_mlp_t* value_target; /* critic step: non-NULL -> target r + gamma*V'(s')*not_terminal,
+                                      no actor forward on s', no noise_next, no q targets */
+  const rb200_mlp_t* value_net;    /* actor step with CRR: the current V [S -> 1] */
+  float* min_q_out;          /* [B] or NULL: actor step writes min_c q_c(s, pi(s)); the value
+                                step reads it (and log_prob_out) for its target */
+  int32_t crr_mode;          /* RB200_CRR_*: actor loss mean(-clamp(log_prob) * w(advantage)) */
+  float crr_threshold;       /* RB200_CRR_INDICATOR: w = (advantage >= threshold) */
+  float crr_beta;            /* RB200_CRR_EXPONENT: w = exp(advantage / beta) ... */
+  float crr_clamp;           /* ... clamped to [0, crr_clamp] when crr_clamp > 0 */
+  int32_t logged_action_uniform_prior; /* value step: target min_q (1) or
+                                          min_q - alpha * clamp(log_prob) (0) */
   /* prioritized replay (critic step only; the actor step ignores both) */
   const float* sample_weight; /* [B] or NULL: critic losses mean(w * d^2), dz row scaled by w */
   float* td_error_out;       /* [B] or NULL: max over critics of |q_c - td_target| */
 } rb200_ac_args_t;
+#define RB200_CRR_NONE 0
+#define RB200_CRR_INDICATOR 1
+#define RB200_CRR_EXPONENT 2
 
 int rb200_ac_critic_step(const rb200_mlp_t* actor, const rb200_mlp_t* q1, const rb200_mlp_t* q2,
                          const rb200_mlp_t* q1_target, const rb200_mlp_t* q2_target,
@@ -441,6 +457,11 @@ int rb200_ac_critic_step(const rb200_mlp_t* actor, const rb200_mlp_t* q1, const 
 int rb200_ac_actor_step(const rb200_mlp_t* actor, const rb200_mlp_t* q1, const rb200_mlp_t* q2,
                         const rb200_ac_args_t* args, const rb200_net_ws_t* ws_actor,
                         const rb200_net_ws_t* ws_q1, const rb200_net_ws_t* ws_q2, void* stream);
+/* value step (SAC with a value network, after the alpha step): V(s) against min_q_out, or    */
+/*   min_q_out - alpha * clamp(log_prob_out) with the post-update alpha; MSE loss -> loss[0],  */
+/*   dZ chain of the value network into ws_value (weight gradients: rb200_mlp_wgrad).          */
+int rb200_ac_value_step(const rb200_mlp_t* value, const rb200_ac_args_t* args,
+                        const rb200_net_ws_t* ws_value, void* stream);
 
 /* ------------------------------------------------------------------------- */
 /* Weight gradients: dW_l = dZ_l^T . A_{l-1}, db_l = sum_b dZ_l, split over    */

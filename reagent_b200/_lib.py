@@ -103,6 +103,7 @@ class AdamArgsT(C.Structure):
 
 
 ALGO_SAC, ALGO_TD3 = 0, 1
+CRR_NONE, CRR_INDICATOR, CRR_EXPONENT = 0, 1, 2
 
 
 class AcArgsT(C.Structure):
@@ -116,6 +117,9 @@ class AcArgsT(C.Structure):
         ("loss_partials", _vp), ("loss", _vp), ("tile_counter", _vp), ("alpha_grad", _vp),
         ("td_target", _vp), ("next_action_out", _vp), ("log_prob_out", _vp),
         ("q1_value", _vp), ("q2_value", _vp),
+        ("value_target", C.POINTER(MlpT)), ("value_net", C.POINTER(MlpT)), ("min_q_out", _vp),
+        ("crr_mode", C.c_int32), ("crr_threshold", C.c_float), ("crr_beta", C.c_float),
+        ("crr_clamp", C.c_float), ("logged_action_uniform_prior", C.c_int32),
         ("sample_weight", _vp), ("td_error_out", _vp),
     ]
 
@@ -296,6 +300,7 @@ def _declare(lib):
     lib.rb200_ac_actor_step.argtypes = [C.POINTER(MlpT), C.POINTER(MlpT), C.POINTER(MlpT),
                                         C.POINTER(AcArgsT), C.POINTER(NetWsT), C.POINTER(NetWsT),
                                         C.POINTER(NetWsT), _vp]
+    lib.rb200_ac_value_step.argtypes = [C.POINTER(MlpT), C.POINTER(AcArgsT), C.POINTER(NetWsT), _vp]
     lib.rb200_wgrad_splits.argtypes = [C.c_int]
     lib.rb200_wgrad_splits_for.argtypes = [C.POINTER(MlpT), C.c_int32]
     lib.rb200_mlp_wgrad.argtypes = [C.POINTER(MlpT), _vp, C.c_int32, C.POINTER(NetWsT), _vp,

@@ -57,7 +57,12 @@ __device__ __forceinline__ float gaussian_head_row(const float* __restrict__ out
 // Meger & Precup 2020) goes to a.td_error_out.  Only the critics are weighted: the importance
 // weights correct the bias of the critics' regression towards the TD target (Schaul et al.
 // 2016); the actor and alpha losses do not regress on the sampled targets.
-template <int NT, int TM, int KC, bool kWeighted>
+//
+// kValueTarget: SAC with a state-value network (sac_trainer.py:214-217).  q1t is then the
+// value-network target V' [S -> 1]; its forward on the s' columns replaces the actor forward
+// on s', both target critics and the entropy term (no noise_next is read).  Everything from
+// the TD target on is the same code.
+template <int NT, int TM, int KC, bool kWeighted, bool kValueTarget = false>
 __global__ void __launch_bounds__(NT, 1)
 ac_critic_rows_kernel(const Mlp actor, const Mlp q1, const Mlp q2, const Mlp q1t, const Mlp q2t,
                       const AcDev p) {
@@ -81,6 +86,24 @@ ac_critic_rows_kernel(const Mlp actor, const Mlp q1, const Mlp q2, const Mlp q1t
   const int A = q1.dims[0] - S;
   const bool sac = a.algo == RB200_ALGO_SAC;
 
+  if constexpr (kValueTarget) {
+    // ---- V'(s'): the value-network target on next_state ----
+    tile_load_rows<NT, R>(cin, ld_c, a.next_state, S, S, row0, B);
+    __syncthreads();
+    tile_mlp_fwd<NT, TM, KC>(q1t, cin, ld_c, hA, hB, ld_h, v1, 8, Wst, nullptr, row0, B);
+    if (tid < R) {
+      const int r = tid, row = row0 + r;
+      float tgt = 0.f;
+      if (row < B) {
+        tgt = a.gamma > 0.f
+                  ? __fadd_rn(a.reward[row], __fmul_rn(__fmul_rn(a.gamma, v1[r * 8]), a.not_terminal[row]))
+                  : a.reward[row];                                    // :233-239
+        if (a.td_target) a.td_target[row] = tgt;
+      }
+      rowv[r] = tgt;
+    }
+    __syncthreads();
+  } else {
   // ---- next action from the (target) actor on next_state ----
   tile_load_rows<NT, R>(cin, ld_c, a.next_state, S, S, row0, B);
   __syncthreads();
@@ -134,6 +157,7 @@ ac_critic_rows_kernel(const Mlp actor, const Mlp q1, const Mlp q2, const Mlp q1t
     rowv[r] = tgt;
   }
   __syncthreads();
+  }  // !kValueTarget
 
   // ---- critics on (s, a): loss + backward ----
   {
@@ -198,9 +222,13 @@ ac_critic_rows_kernel(const Mlp actor, const Mlp q1, const Mlp q2, const Mlp q1t
 }
 
 // ---------------------------------------------------------------------------------------
-template <int NT, int TM, int KC>
+// kCrr: Critic Regularized Regression weighting of the SAC actor loss (sac_trainer.py:23-48,
+// :265-276).  vn is the current value network V [S -> 1]; the row's loss element is
+// -clamp(lp) * w(min_q - V(s)), w detached, so the only gradient is through log_prob and the
+// input-gradient pass through the critics is skipped (dact stays zero).
+template <int NT, int TM, int KC, bool kCrr = false>
 __global__ void __launch_bounds__(NT, 1)
-ac_actor_rows_kernel(const Mlp actor, const Mlp q1, const Mlp q2, const AcDev p) {
+ac_actor_rows_kernel(const Mlp actor, const Mlp q1, const Mlp q2, const Mlp vn, const AcDev p) {
   constexpr int R = (NT / 64) * TM;
   extern __shared__ __align__(16) float smem[];
   const rb200_ac_args_t& a = p.a;
@@ -251,16 +279,21 @@ ac_actor_rows_kernel(const Mlp actor, const Mlp q1, const Mlp q2, const AcDev p)
   const bool use_q2 = sac && p.has_q2;  // TD3's actor loss uses q1 only (td3_trainer.py:183-184)
   if (use_q2)
     tile_mlp_fwd<NT, TM, KC>(q2, cin, ld_c, hA, hB, ld_h, v2, 8, Wst, p.ws_q2.hidden, row0, B);
+  // V(s) on the state columns of cin.  Exact despite the action columns after S: the staged
+  // weights are zero for k >= S and the actions are finite.
+  if constexpr (kCrr)
+    tile_mlp_fwd<NT, TM, KC>(vn, cin, ld_c, hA, hB, ld_h, dtmp, ld_o, Wst, nullptr, row0, B);
   if (tid < R) {
     const int r = tid, row = row0 + r;
     float w1 = 0.f, w2 = 0.f, le = 0.f;
     if (row < B) {
       const float qa = v1[r * 8];
+      float minq = qa;
       if (use_q2) {
         // torch.min(a, b) backward: ties split the gradient evenly
         const float qb = v2[r * 8];
         if (qa < qb) w1 = 1.f; else if (qa > qb) w2 = 1.f; else { w1 = 0.5f; w2 = 0.5f; }
-        const float minq = fminf(qa, qb);
+        minq = fminf(qa, qb);
         const float lpc = fminf(fmaxf(rowv[r], kLogProbMin), kLogProbMax);
         le = __fsub_rn(__fmul_rn(*a.alpha, lpc), minq);       // sac_trainer.py:278
       } else if (sac) {
@@ -271,6 +304,18 @@ ac_actor_rows_kernel(const Mlp actor, const Mlp q1, const Mlp q2, const AcDev p)
         w1 = 1.f;
         le = -qa;                                             // td3_trainer.py:184
       }
+      if (a.min_q_out) a.min_q_out[row] = minq;
+      if constexpr (kCrr) {
+        // CRRWeightFn.get_weight_from_advantage (sac_trainer.py:38-48); w1 carries w
+        const float adv = __fsub_rn(minq, dtmp[r * ld_o]);
+        if (a.crr_mode == RB200_CRR_INDICATOR) {
+          w1 = adv >= a.crr_threshold ? 1.f : 0.f;
+        } else {
+          w1 = expf(__fdiv_rn(adv, a.crr_beta));
+          if (a.crr_clamp > 0.f) w1 = fminf(fmaxf(w1, 0.f), a.crr_clamp);
+        }
+        le = -__fmul_rn(fminf(fmaxf(rowv[r], kLogProbMin), kLogProbMax), w1);
+      }
     }
     rowv[R + r] = w1;
     rowv[2 * R + r] = w2;
@@ -279,7 +324,7 @@ ac_actor_rows_kernel(const Mlp actor, const Mlp q1, const Mlp q2, const AcDev p)
   __syncthreads();
 
   // ---- d loss / d action through the critics: loss = mean(... - minQ) ----
-  for (int which = 0; which < (use_q2 ? 2 : 1); ++which) {
+  for (int which = 0; which < (kCrr ? 0 : (use_q2 ? 2 : 1)); ++which) {
     const Mlp& q = which ? q2 : q1;
     const rb200_net_ws_t& ws = which ? p.ws_q2 : p.ws_q1;
     const float* v = which ? v2 : v1;
@@ -317,7 +362,8 @@ ac_actor_rows_kernel(const Mlp actor, const Mlp q1, const Mlp q2, const AcDev p)
       if (sac) {
         const float lp = rowv[r];
         const bool in_clamp = (lp >= kLogProbMin) && (lp <= kLogProbMax);
-        const float glp = (a.backprop_through_log_prob && in_clamp) ? (*a.alpha) * invB : 0.f;
+        float glp = (a.backprop_through_log_prob && in_clamp) ? (*a.alpha) * invB : 0.f;
+        if constexpr (kCrr) glp = in_clamp ? -(rowv[R + r] * invB) : 0.f;
         const float* nz = a.noise_cur + (size_t)row * A;
         for (int j = 0; j < A; ++j) {
           const float loc = aout[r * ld_o + j];
@@ -375,6 +421,73 @@ ac_actor_rows_kernel(const Mlp actor, const Mlp q1, const Mlp q2, const AcDev p)
   }
 }
 
+// ---------------------------------------------------------------------------------------
+// Value step (sac_trainer.py:329-343): V(s) forward with the hidden activations saved, the
+// per-row target min_q (logged_action_uniform_prior) or min_q - alpha * clamp(log_prob) with
+// the post-update alpha, MSE against the detached target and the value network's dZ chain.
+template <int NT, int TM, int KC>
+__global__ void __launch_bounds__(NT, 1)
+ac_value_rows_kernel(const Mlp vn, const AcDev p) {
+  constexpr int R = (NT / 64) * TM;
+  extern __shared__ __align__(16) float smem[];
+  const rb200_ac_args_t& a = p.a;
+  const int tid = threadIdx.x;
+  const int ld_c = p.ld_c, ld_h = p.ld_h;
+  tile_smem_zero_all<NT>(smem);
+  float* Wst = smem;
+  float* cin = Wst + 2 * wstage_floats<KC>();  // [R, ld_c] state
+  float* hA = cin + R * ld_c;
+  float* hB = hA + R * ld_h;
+  float* hC = hB + R * ld_h;
+  float* v = hC + R * ld_h;                     // [R, 8] V(s), then its dz
+  float* rowv = v + R * 8;                      // [R] loss element
+  const int B = a.batch, row0 = blockIdx.x * R;
+  const int S = vn.dims[0];
+  const rb200_net_ws_t& ws = p.ws_q1;
+
+  tile_load_rows<NT, R>(cin, ld_c, a.state, S, S, row0, B);
+  __syncthreads();
+  tile_mlp_fwd<NT, TM, KC>(vn, cin, ld_c, hA, hB, ld_h, v, 8, Wst, ws.hidden, row0, B);
+  if (tid < R) {
+    const int r = tid, row = row0 + r;
+    float le = 0.f, g = 0.f;
+    if (row < B) {
+      const float sv = v[r * 8];
+      float tgt = a.min_q_out[row];
+      if (!a.logged_action_uniform_prior) {
+        const float lpc = fminf(fmaxf(a.log_prob_out[row], kLogProbMin), kLogProbMax);
+        tgt = __fsub_rn(tgt, __fmul_rn(*a.alpha, lpc));
+      }
+      const float d = __fsub_rn(sv, tgt);
+      le = d * d;                                     // F.mse_loss, mean over B
+      g = 2.f / (float)B * d;
+      const int lact = vn.act[vn.n_layers - 1];
+      if (lact != RB200_ACT_LINEAR) g *= act_bwd_from_out(sv, lact);
+    }
+    v[r * 8] = g;                                     // dz of the (1-wide) last layer
+    rowv[r] = le;
+  }
+  __syncthreads();
+  tile_mlp_bwd<NT, TM, KC>(vn, v, 8, hA, hB, hC, ld_h, Wst, ws.hidden, ws.dz, row0, B,
+                           nullptr, 0, 0, 0);
+  if (tid == 0) {
+    float s = 0.f;
+    for (int r = 0; r < R; ++r) s += rowv[r];
+    finish_serial<1>(a.loss_partials, a.tile_counter, {s}, [&](const float (&tot)[1]) {
+      a.loss[0] = tot[0] / (float)B;
+    });
+  }
+}
+
+// A state-value network V [S -> 1] for the step that `who` names.
+static int check_value_net(const rb200_mlp_t* v, int S, const rb200_ac_args_t* a, const char* who) {
+  if (!v) { set_last_error("%s: value network descriptor is null", who); return RB200_E_INVALID; }
+  if (int rc = validate_mlp(v, who)) return rc;
+  if (v->dims[0] != S || v->dims[v->n_layers] != 1) { set_last_error("%s: value network must map the state (%d wide) to 1 output (got %d -> %d)", who, S, v->dims[0], v->dims[v->n_layers]); return RB200_E_INVALID; }
+  if (a->algo != RB200_ALGO_SAC) { set_last_error("%s: a value network needs SAC (TD3 has none)", who); return RB200_E_INVALID; }
+  return RB200_OK;
+}
+
 static int ac_common_checks(const rb200_mlp_t* actor, const rb200_mlp_t* q1, const rb200_mlp_t* q2,
                             const rb200_ac_args_t* a) {
   if (!actor || !q1 || !a) { set_last_error("actor-critic step: null argument"); return RB200_E_INVALID; }
@@ -393,12 +506,15 @@ static int ac_common_checks(const rb200_mlp_t* actor, const rb200_mlp_t* q1, con
   return RB200_OK;
 }
 
+// `value`: the value network the launch runs (critic step: the value target; actor step with
+// CRR: the value network), or NULL.
 static RowsCfg ac_cfg(const rb200_mlp_t* actor, const rb200_mlp_t* q1, const rb200_mlp_t* q2,
-                      int batch, int n_out_tiles, int* ld_o) {
+                      const rb200_mlp_t* value, int batch, int n_out_tiles, int* ld_o) {
   int hmax = mlp_max_hidden(actor);
   const int h1 = mlp_max_hidden(q1);
   hmax = h1 > hmax ? h1 : hmax;
   if (q2) { const int h2 = mlp_max_hidden(q2); hmax = h2 > hmax ? h2 : hmax; }
+  if (value) { const int hv = mlp_max_hidden(value); hmax = hv > hmax ? hv : hmax; }
   const int NO = actor->dims[actor->n_layers];
   *ld_o = round_up4(NO > 8 ? NO : 8) + 12;  // room for a 1-wide dz quad + an A-wide gradient
   return pick_rows_cfg(batch, q1->dims[0], hmax, 1, 3, n_out_tiles * (*ld_o) + 16 + 4, 0);
@@ -414,28 +530,44 @@ extern "C" int rb200_ac_critic_step(const rb200_mlp_t* actor, const rb200_mlp_t*
                                     const rb200_net_ws_t* ws_q1, const rb200_net_ws_t* ws_q2,
                                     void* stream) {
   if (int rc = ac_common_checks(actor, q1, q2, args)) return rc;
-  if (!q1_target || (q2 && !q2_target) || !ws_q1 || (q2 && !ws_q2)) { set_last_error("critic step: target nets / workspaces required"); return RB200_E_INVALID; }
-  if (int rc = validate_mlp(q1_target, "q1_network_target")) return rc;
-  if (q2) if (int rc = validate_mlp(q2_target, "q2_network_target")) return rc;
-  if (!args->action || !args->next_state || !args->reward || !args->not_terminal || !args->noise_next) { set_last_error("critic step: batch pointer is null"); return RB200_E_INVALID; }
+  const rb200_mlp_t* vt = args->value_target;
+  if (vt) {
+    // the value target replaces the actor forward on s' and both q targets
+    if (int rc = check_value_net(vt, actor->dims[0], args, "value_network_target")) return rc;
+    if (!ws_q1 || (q2 && !ws_q2)) { set_last_error("critic step: workspaces required"); return RB200_E_INVALID; }
+    if (!args->action || !args->next_state || !args->reward || !args->not_terminal) { set_last_error("critic step: batch pointer is null"); return RB200_E_INVALID; }
+  } else {
+    if (!q1_target || (q2 && !q2_target) || !ws_q1 || (q2 && !ws_q2)) { set_last_error("critic step: target nets / workspaces required"); return RB200_E_INVALID; }
+    if (int rc = validate_mlp(q1_target, "q1_network_target")) return rc;
+    if (q2) if (int rc = validate_mlp(q2_target, "q2_network_target")) return rc;
+    if (!args->action || !args->next_state || !args->reward || !args->not_terminal || !args->noise_next) { set_last_error("critic step: batch pointer is null"); return RB200_E_INVALID; }
+  }
   AcDev p;
   p.a = *args;
   p.ws_q1 = *ws_q1;
   p.ws_q2 = q2 ? *ws_q2 : *ws_q1;
   p.ws_actor = *ws_q1;
   p.has_q2 = q2 ? 1 : 0;
-  RowsCfg cfg = ac_cfg(actor, q1, q2, args->batch, 1, &p.ld_o);
+  RowsCfg cfg = ac_cfg(actor, q1, q2, vt, args->batch, 1, &p.ld_o);
   if (cfg.tm == 0) { set_last_error("actor-critic tile does not fit in shared memory"); return RB200_E_SMEM; }
   p.ld_c = cfg.ld_in;
   p.ld_h = cfg.ld_h;
   const Mlp ma = make_mlp(actor), m1 = make_mlp(q1), m2 = make_mlp(q2 ? q2 : q1);
-  const Mlp t1 = make_mlp(q1_target), t2 = make_mlp(q2 ? q2_target : q1_target);
+  // with a value network, t1 carries the value target (t2 is unused)
+  const Mlp t1 = make_mlp(vt ? vt : q1_target);
+  const Mlp t2 = make_mlp(vt ? vt : (q2 ? q2_target : q1_target));
   const int grid = ceil_div(args->batch, rows_per_tile(cfg));
   cudaStream_t st = (cudaStream_t)stream;
   // prioritized replay: weights and / or TD errors take the weighted instantiation
   const bool weighted = args->sample_weight || args->td_error_out;
   return dispatch_rows(cfg, [&](auto NT, auto KC) {
     const char* what = "ac_critic_rows_kernel launch";
+    if (vt)
+      return weighted
+                 ? launch<ac_critic_rows_kernel<NT(), 4, KC(), true, true>>(
+                       grid, NT(), cfg.smem_bytes, st, what, ma, m1, m2, t1, t2, p)
+                 : launch<ac_critic_rows_kernel<NT(), 4, KC(), false, true>>(
+                       grid, NT(), cfg.smem_bytes, st, what, ma, m1, m2, t1, t2, p);
     return weighted
                ? launch<ac_critic_rows_kernel<NT(), 4, KC(), true>>(grid, NT(), cfg.smem_bytes, st,
                                                                      what, ma, m1, m2, t1, t2, p)
@@ -451,21 +583,58 @@ extern "C" int rb200_ac_actor_step(const rb200_mlp_t* actor, const rb200_mlp_t* 
   if (int rc = ac_common_checks(actor, q1, q2, args)) return rc;
   if (!ws_actor || !ws_q1 || (q2 && !ws_q2)) { set_last_error("actor step: workspaces required"); return RB200_E_INVALID; }
   if (args->algo == RB200_ALGO_SAC && !args->noise_cur) { set_last_error("SAC actor step needs noise_cur"); return RB200_E_INVALID; }
+  const bool crr = args->crr_mode != RB200_CRR_NONE;
+  if (crr) {
+    if (args->crr_mode != RB200_CRR_INDICATOR && args->crr_mode != RB200_CRR_EXPONENT) { set_last_error("actor step: unknown crr_mode %d", args->crr_mode); return RB200_E_INVALID; }
+    if (!args->value_net) { set_last_error("actor step: CRR needs a value network"); return RB200_E_INVALID; }
+    if (int rc = check_value_net(args->value_net, actor->dims[0], args, "value_network")) return rc;
+    if (!args->backprop_through_log_prob) { set_last_error("actor step: the CRR loss has no gradient without backprop_through_log_prob"); return RB200_E_INVALID; }
+    if (args->crr_mode == RB200_CRR_EXPONENT && !(args->crr_beta > 0.f)) { set_last_error("actor step: crr_beta must be > 0"); return RB200_E_INVALID; }
+  }
   AcDev p;
   p.a = *args;
   p.ws_actor = *ws_actor;
   p.ws_q1 = *ws_q1;
   p.ws_q2 = q2 ? *ws_q2 : *ws_q1;
   p.has_q2 = q2 ? 1 : 0;
-  RowsCfg cfg = ac_cfg(actor, q1, q2, args->batch, 3, &p.ld_o);
+  RowsCfg cfg = ac_cfg(actor, q1, q2, crr ? args->value_net : nullptr, args->batch, 3, &p.ld_o);
   if (cfg.tm == 0) { set_last_error("actor-critic tile does not fit in shared memory"); return RB200_E_SMEM; }
   p.ld_c = cfg.ld_in;
   p.ld_h = cfg.ld_h;
   const Mlp ma = make_mlp(actor), m1 = make_mlp(q1), m2 = make_mlp(q2 ? q2 : q1);
+  const Mlp mv = make_mlp(crr ? args->value_net : q1);
   const int grid = ceil_div(args->batch, rows_per_tile(cfg));
   cudaStream_t st = (cudaStream_t)stream;
   return dispatch_rows(cfg, [&](auto NT, auto KC) {
-    return launch<ac_actor_rows_kernel<NT(), 4, KC()>>(grid, NT(), cfg.smem_bytes, st,
-                                                       "ac_actor_rows_kernel launch", ma, m1, m2, p);
+    const char* what = "ac_actor_rows_kernel launch";
+    return crr ? launch<ac_actor_rows_kernel<NT(), 4, KC(), true>>(grid, NT(), cfg.smem_bytes, st,
+                                                                   what, ma, m1, m2, mv, p)
+               : launch<ac_actor_rows_kernel<NT(), 4, KC()>>(grid, NT(), cfg.smem_bytes, st, what,
+                                                             ma, m1, m2, mv, p);
+  });
+}
+
+extern "C" int rb200_ac_value_step(const rb200_mlp_t* value, const rb200_ac_args_t* args,
+                                   const rb200_net_ws_t* ws_value, void* stream) {
+  if (!args) { set_last_error("value step: null argument"); return RB200_E_INVALID; }
+  if (!value) { set_last_error("value step: value network descriptor is null"); return RB200_E_INVALID; }
+  if (int rc = check_value_net(value, value->dims[0], args, "value_network")) return rc;
+  if (!ws_value || args->batch <= 0 || !args->state || !args->min_q_out || !args->loss_partials || !args->loss || !args->tile_counter) { set_last_error("value step: required pointer is null"); return RB200_E_INVALID; }
+  if (!args->logged_action_uniform_prior && (!args->log_prob_out || !args->alpha)) { set_last_error("value step: the entropy target needs log_prob_out and alpha"); return RB200_E_INVALID; }
+  AcDev p;
+  p.a = *args;
+  p.ws_actor = p.ws_q1 = p.ws_q2 = *ws_value;
+  p.has_q2 = 0;
+  p.ld_o = 8;
+  RowsCfg cfg = pick_rows_cfg(args->batch, value->dims[0], mlp_max_hidden(value), 1, 3, 8 + 1, 0);
+  if (cfg.tm == 0) { set_last_error("value tile does not fit in shared memory"); return RB200_E_SMEM; }
+  p.ld_c = cfg.ld_in;
+  p.ld_h = cfg.ld_h;
+  const Mlp mv = make_mlp(value);
+  const int grid = ceil_div(args->batch, rows_per_tile(cfg));
+  cudaStream_t st = (cudaStream_t)stream;
+  return dispatch_rows(cfg, [&](auto NT, auto KC) {
+    return launch<ac_value_rows_kernel<NT(), 4, KC()>>(grid, NT(), cfg.smem_bytes, st,
+                                                       "ac_value_rows_kernel launch", mv, p);
   });
 }

@@ -13,10 +13,10 @@ from ..core.parameters import (EvaluationParameters, NormalizationData, Normaliz
                                RLParameters)
 from ..net_builder import (ActorFullyConnected, Categorical, Dueling, DuelingQuantile,
                            FullyConnected, GaussianFullyConnected, ParametricFullyConnected,
-                           Quantile)
+                           Quantile, ValueFullyConnected)
 from ..optimizer import Optimizer__Union
-from ..training import (C51Trainer, DQNTrainer, ParametricDQNTrainer, QRDQNTrainer, SACTrainer,
-                        TD3Trainer)
+from ..training import (C51Trainer, CRRWeightFn, DQNTrainer, ParametricDQNTrainer, QRDQNTrainer,
+                        SACTrainer, TD3Trainer)
 
 
 def _device(use_gpu: bool):
@@ -193,16 +193,25 @@ class ParametricDQN:
 
 @dataclass
 class SAC(_ActorPolicyMixin):
+    """The reference manager with `trainer_param` flattened.  `value_net_builder` defaults to
+    None here, so SAC() builds no state-value network; the reference's default builds one
+    (value FullyConnected, [256, 128] relu).  Configurations that name a value_net_builder,
+    such as the reference's Pendulum SAC and CRR configurations, get one either way."""
     rl: RLParameters = field(default_factory=RLParameters)
     actor_net_builder: GaussianFullyConnected = field(default_factory=GaussianFullyConnected)
     critic_net_builder: ParametricFullyConnected = field(default_factory=ParametricFullyConnected)
+    value_net_builder: Optional[ValueFullyConnected] = None
     use_2_q_functions: bool = True
     minibatch_size: int = 1024
     entropy_temperature: float = 0.01
+    logged_action_uniform_prior: bool = True
     target_entropy: float = -1.0
     q_network_optimizer: Optimizer__Union = field(default_factory=Optimizer__Union.default)
+    value_network_optimizer: Optimizer__Union = field(default_factory=Optimizer__Union.default)
     actor_network_optimizer: Optimizer__Union = field(default_factory=Optimizer__Union.default)
     alpha_optimizer: Optional[Optimizer__Union] = field(default_factory=Optimizer__Union.default)
+    crr_config: Optional[CRRWeightFn] = None
+    backprop_through_log_prob: bool = True
 
     def build_trainer(self, normalization_data_map, use_gpu: bool, reward_options=None):
         dev = _device(use_gpu)
@@ -211,13 +220,18 @@ class SAC(_ActorPolicyMixin):
         actor = self.actor_net_builder.build_actor(None, s, a).to(dev)
         q1 = self.critic_net_builder.build_q_network(s, a).to(dev)
         q2 = self.critic_net_builder.build_q_network(s, a).to(dev) if self.use_2_q_functions else None
+        value = (None if self.value_net_builder is None
+                 else self.value_net_builder.build_value_network(s).to(dev))
         return SACTrainer(
-            actor_network=actor, q1_network=q1, q2_network=q2, value_network=None, rl=self.rl,
+            actor_network=actor, q1_network=q1, q2_network=q2, value_network=value, rl=self.rl,
             q_network_optimizer=self.q_network_optimizer,
+            value_network_optimizer=self.value_network_optimizer,
             actor_network_optimizer=self.actor_network_optimizer,
             alpha_optimizer=self.alpha_optimizer, minibatch_size=self.minibatch_size,
             entropy_temperature=self.entropy_temperature,
-            target_entropy=self.target_entropy).to(dev)
+            logged_action_uniform_prior=self.logged_action_uniform_prior,
+            target_entropy=self.target_entropy, crr_config=self.crr_config,
+            backprop_through_log_prob=self.backprop_through_log_prob).to(dev)
 
 
 @dataclass

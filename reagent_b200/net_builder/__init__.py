@@ -7,6 +7,7 @@ from typing import List
 from ..core.parameters import NormalizationData
 from ..models import (CategoricalDQN, DuelingQNetwork, FullyConnectedActor,
                       FullyConnectedCritic, FullyConnectedDQN, GaussianFullyConnectedActor)
+from ..models.fully_connected_network import FloatFeatureFullyConnected
 from ..preprocessing.normalization import get_num_output_features
 
 
@@ -147,3 +148,21 @@ class ActorFullyConnected:
             sizes=self.sizes, activations=self.activations, use_batch_norm=self.use_batch_norm,
             action_activation=self.action_activation,
             exploration_variance=self.exploration_variance)
+
+
+@dataclass
+class ValueFullyConnected:
+    """reagent/net_builder/value/fully_connected.py:16-44 (the SAC state-value network)"""
+    sizes: List[int] = field(default_factory=lambda: [256, 128])
+    activations: List[str] = field(default_factory=lambda: ["relu", "relu"])
+    use_layer_norm: bool = False
+
+    def __post_init__(self):
+        assert len(self.sizes) == len(self.activations), (
+            f"Must have the same numbers of sizes and activations; got: {self.sizes}, {self.activations}")
+
+    def build_value_network(self, state_normalization_data: NormalizationData,
+                            output_dim: int = 1):
+        return FloatFeatureFullyConnected(
+            state_dim=_dim(state_normalization_data), output_dim=output_dim, sizes=self.sizes,
+            activations=self.activations, use_layer_norm=self.use_layer_norm)

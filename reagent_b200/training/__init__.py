@@ -5,5 +5,5 @@ from .loop import run_update  # noqa: F401
 from .parametric_dqn_trainer import ParametricDQNTrainer  # noqa: F401
 from .qrdqn_trainer import QRDQNTrainer  # noqa: F401
 from .reagent_lightning_module import ReAgentLightningModule  # noqa: F401
-from .sac_trainer import SACTrainer  # noqa: F401
+from .sac_trainer import CRRWeightFn, SACTrainer  # noqa: F401
 from .td3_trainer import TD3Trainer  # noqa: F401

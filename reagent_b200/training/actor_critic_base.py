@@ -32,6 +32,7 @@ class ActorCriticBase(RLTrainerMixin, ReAgentLightningModule):
         if not ws_fits(self._ws, B, device):
             ntiles = (B + 15) // 16
             q2 = self.q2_network
+            value = getattr(self, "value_network", None)
             ws = {
                 "B": B, "dev": device,
                 "actor": NetWorkspace(self.actor_network.arena, B, device),
@@ -48,6 +49,10 @@ class ActorCriticBase(RLTrainerMixin, ReAgentLightningModule):
                 "log_prob": torch.empty(B, device=device),
                 # weighted critic step (prioritized replay): max_c |q_c(s, a) - td_target|
                 "td_error": torch.empty(B, device=device),
+                # SAC with a value network: min_c q_c(s, pi(s)) from the actor step, V's loss
+                "value": None if value is None else NetWorkspace(value.arena, B, device),
+                "min_q": torch.empty(B, device=device),
+                "value_loss": torch.zeros(1, device=device),
             }
             if ws["q2"] is not None:
                 ws["q2"].c.input = ws["q1"].input.data_ptr()
@@ -87,8 +92,10 @@ class ActorCriticBase(RLTrainerMixin, ReAgentLightningModule):
         if sample_weight is not None:
             a.sample_weight = pins(sample_weight)
             a.td_error_out = ws["td_error"].data_ptr()
-        A = self.q1_network.arena.dims[0] - self.actor_network.arena.dims[0]
-        a.noise_next = self._noise("next", B, A, pins)
+        if getattr(self, "value_network", None) is None:
+            # with a value network the target is V'(s'): no actor forward on s', no draw
+            A = self.q1_network.arena.dims[0] - self.actor_network.arena.dims[0]
+            a.noise_next = self._noise("next", B, A, pins)
         a.loss = ws["critic_loss"].data_ptr()
         a.td_target = ws["td_target"].data_ptr()
         a.q1_value = ws["q1_value"].data_ptr()

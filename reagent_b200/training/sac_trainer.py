@@ -1,16 +1,21 @@
 """SACTrainer with the reference's constructor, optimizer order and generator protocol
-(reagent/training/sac_trainer.py:50-385) for the in-scope configuration: twin (or single)
-critics, no value network, learnable or fixed entropy temperature.
+(reagent/training/sac_trainer.py:50-385): twin (or single) critics, learnable or fixed entropy
+temperature, an optional state-value network and CRR weighting of the actor loss.
 
 Launch sequence of one update (value_network=None):
   rb200_ac_critic_step  target + q1/q2 losses + critic dZ chains     sac_trainer.py:214-248
   rb200_mlp_wgrad x2, Adam(q1), Adam(q2) [+ fused Polyak]            optimizer.py / soft_update.py
   rb200_ac_actor_step   actor + alpha losses, backward through the UPDATED critics  :254-322
   rb200_mlp_wgrad, Adam(actor), Adam(log_alpha) -> entropy_temperature = exp(log_alpha)
+With a value network the critic step's target is r + gamma * V'(s') (no actor forward on s',
+one noise draw per update), the actor step also writes min_c q_c(s, pi(s)), and after the
+alpha step rb200_ac_value_step, rb200_mlp_wgrad and Adam(value) [+ fused Polyak into the value
+target] train V(s) against it (:329-343).  Only the value target is soft-updated then.
 Sequential dependence of the reference is kept (SURVEY.md facts 3-4): the actor step sees the
-post-update critics; the new temperature takes effect in the next batch.
+post-update critics; the new temperature takes effect in the value step and the next batch.
 """
 import copy
+from dataclasses import dataclass
 from typing import List, Optional
 
 import numpy as np
@@ -22,8 +27,46 @@ from ..core.parameters import RLParameters
 from ..models.arena import ScalarArena
 from ..optimizer import Optimizer__Union, SoftUpdate
 from .actor_critic_base import ActorCriticBase
+from .workspace import Pins, batch_device, wgrad
 
 _DEFAULT = object()
+
+
+@dataclass
+class CRRWeightFn:
+    """Critic Regularized Regression weight of the advantage (sac_trainer.py:23-48): the
+    indicator advantage >= indicator_fn_threshold, or exp(advantage / exponent_beta), clamped
+    to [0, exponent_clamp] when exponent_clamp is set."""
+    indicator_fn_threshold: Optional[float] = None
+    exponent_beta: Optional[float] = None
+    exponent_clamp: Optional[float] = None
+
+    def __post_init__(self):
+        assert self.exponent_beta or self.indicator_fn_threshold
+        assert not (self.exponent_beta and self.indicator_fn_threshold)
+        if self.exponent_beta:
+            assert self.exponent_beta > 1e-6
+        if self.exponent_clamp:
+            assert self.exponent_clamp > 1e-6
+
+    def get_weight_from_advantage(self, advantage):
+        if self.indicator_fn_threshold:
+            return (advantage >= self.indicator_fn_threshold).float()
+        if self.exponent_beta:
+            exp = torch.exp(advantage / self.exponent_beta)
+            if self.exponent_clamp:
+                exp = torch.clamp(exp, 0.0, self.exponent_clamp)
+            return exp
+
+    def fill(self, a):
+        """The kernels' CRR fields of rb200_ac_args_t."""
+        if self.indicator_fn_threshold:
+            a.crr_mode = _lib.CRR_INDICATOR
+            a.crr_threshold = float(self.indicator_fn_threshold)
+        else:
+            a.crr_mode = _lib.CRR_EXPONENT
+            a.crr_beta = float(self.exponent_beta)
+            a.crr_clamp = float(self.exponent_clamp) if self.exponent_clamp else 0.0
 
 
 class SACTrainer(ActorCriticBase):
@@ -53,18 +96,25 @@ class SACTrainer(ActorCriticBase):
     ) -> None:
         super().__init__()
         self._ac_init()
-        if value_network is not None:
-            raise NotImplementedError("SAC with a value network is out of scope (SURVEY.md T7)")
-        if crr_config is not None or action_embedding_kld_weight:
-            raise NotImplementedError("CRR weighting / action-embedding KLD are out of scope")
+        if action_embedding_kld_weight:
+            raise NotImplementedError("action-embedding KLD is out of scope")
+        if crr_config is not None:
+            assert value_network is not None  # sac_trainer.py:142-144
+            if not backprop_through_log_prob:
+                # the CRR loss -clamp(log_prob) * w has no other path to the actor
+                raise ValueError("crr_config needs backprop_through_log_prob=True: without it "
+                                 "the actor loss has no gradient")
         self.rl_parameters = RLParameters() if rl is None else rl
         self.q1_network = q1_network
         self.q2_network = q2_network
         self.q_network_optimizer = q_network_optimizer or Optimizer__Union.default()
-        self.value_network = None
+        self.value_network = value_network
         self.value_network_optimizer = value_network_optimizer or Optimizer__Union.default()
-        self.q1_network_target = copy.deepcopy(self.q1_network)
-        self.q2_network_target = copy.deepcopy(self.q2_network)
+        if self.value_network is not None:
+            self.value_network_target = copy.deepcopy(self.value_network)
+        else:
+            self.q1_network_target = copy.deepcopy(self.q1_network)
+            self.q2_network_target = copy.deepcopy(self.q2_network)
         self.actor_network = actor_network
         self.actor_network_optimizer = actor_network_optimizer or Optimizer__Union.default()
         self.entropy_temperature = entropy_temperature
@@ -84,7 +134,7 @@ class SACTrainer(ActorCriticBase):
         self.register_load_state_dict_post_hook(SACTrainer._rederive_alpha)
         self.logged_action_uniform_prior = logged_action_uniform_prior
         self.add_kld_to_loss = False
-        self.crr_config = None
+        self.crr_config = crr_config
         self.backprop_through_log_prob = backprop_through_log_prob
         self.minibatch_size = minibatch_size
 
@@ -96,7 +146,7 @@ class SACTrainer(ActorCriticBase):
             module.entropy_temperature = module._alpha_dev
 
     def configure_optimizers(self):
-        """q1, q2, actor, alpha, SoftUpdate (sac_trainer.py:148-193)."""
+        """q1, q2, actor, alpha, value, SoftUpdate (sac_trainer.py:148-193)."""
         optimizers = []
         optimizers.append(
             self.q_network_optimizer.make_optimizer_scheduler(self.q1_network.parameters()))
@@ -108,11 +158,17 @@ class SACTrainer(ActorCriticBase):
                 self.actor_network.parameters()))
         if self.alpha_optimizer is not None:
             optimizers.append(self.alpha_optimizer.make_optimizer_scheduler([self.log_alpha]))
-        target_params = list(self.q1_network_target.parameters())
-        source_params = list(self.q1_network.parameters())
-        if self.q2_network:
-            target_params += list(self.q2_network_target.parameters())
-            source_params += list(self.q2_network.parameters())
+        if self.value_network:
+            optimizers.append(self.value_network_optimizer.make_optimizer_scheduler(
+                self.value_network.parameters()))
+            target_params = list(self.value_network_target.parameters())
+            source_params = list(self.value_network.parameters())
+        else:
+            target_params = list(self.q1_network_target.parameters())
+            source_params = list(self.q1_network.parameters())
+            if self.q2_network:
+                target_params += list(self.q2_network_target.parameters())
+                source_params += list(self.q2_network.parameters())
         optimizers.append(
             SoftUpdate.make_optimizer_scheduler(target_params, source_params, tau=self.tau))
         return optimizers
@@ -129,6 +185,8 @@ class SACTrainer(ActorCriticBase):
         a.alpha = _lib.ptr(self._alpha_dev, dev)
         a.target_entropy = float(self.target_entropy)
         a.backprop_through_log_prob = int(bool(self.backprop_through_log_prob))
+        if self.value_network is not None:
+            a.value_target = self._desc_ptr(self.value_network_target, pins)
 
     def _fill_actor(self, a, pins):
         self._fill_critic(a, pins)
@@ -138,6 +196,42 @@ class SACTrainer(ActorCriticBase):
         if self.alpha_optimizer is not None:
             a.alpha_grad = ws["alpha_grad"].data_ptr()
             a.log_alpha = _lib.ptr(self.log_alpha.data, ws["dev"])
+        if self.value_network is not None:
+            a.value_target = None
+            a.min_q_out = ws["min_q"].data_ptr()
+            if self.crr_config is not None:
+                a.value_net = self._desc_ptr(self.value_network, pins)
+                self.crr_config.fill(a)
+
+    @staticmethod
+    def _desc_ptr(net, pins):
+        d = net.arena.desc()
+        pins.keep.append(d)
+        return _lib.C.pointer(d)
+
+    def _value_step(self, batch):
+        """V(s) against min_q (minus alpha * clamp(log_prob) without the uniform prior), with
+        the log-probs and min-of-critics the actor step of this update wrote
+        (sac_trainer.py:329-343), then V's weight gradients."""
+        B = batch.state.float_features.shape[0]
+        pins = Pins(batch_device(batch.state.float_features, type(self).__name__))
+        ws = self._workspace(B, pins.device)
+        a, state = self._base_args(batch, ws, pins)
+        a.loss = ws["value_loss"].data_ptr()
+        a.min_q_out = ws["min_q"].data_ptr()
+        a.log_prob_out = ws["log_prob"].data_ptr()
+        a.alpha = _lib.ptr(self._alpha_dev, ws["dev"])
+        a.logged_action_uniform_prior = int(bool(self.logged_action_uniform_prior))
+        rc = _lib.lib().rb200_ac_value_step(self._desc(self.value_network), a, ws["value"].c,
+                                            _lib.cur_stream())
+        _lib.check(rc, "rb200_ac_value_step")
+        wgrad(self.value_network.arena, ws["value"], state, B)
+        return ws["value_loss"]
+
+    def _critic_targets(self):
+        if self.value_network is not None:
+            return None, None
+        return self.q1_network_target, self.q2_network_target
 
     def _alpha_arena(self):
         arena = getattr(self.log_alpha, "_rb200_arena", None)
@@ -149,8 +243,8 @@ class SACTrainer(ActorCriticBase):
     def train_step_gen(self, training_batch: rlt.PolicyNetworkInput, batch_idx: int):
         """IMPORTANT: the input action is assumed to match the actor's output range."""
         assert isinstance(training_batch, rlt.PolicyNetworkInput)
-        closs = self._critic_step(training_batch, self.actor_network, self.q1_network_target,
-                                  self.q2_network_target, self._fill_critic)
+        closs = self._critic_step(training_batch, self.actor_network, *self._critic_targets(),
+                                  self._fill_critic)
         yield self.fused_loss(closs[0])
         if self.q2_network:
             yield self.fused_loss(closs[1])
@@ -164,6 +258,8 @@ class SACTrainer(ActorCriticBase):
             # sac_trainer.py:322 (runs after the alpha step, used from the next batch on)
             self._alpha_dev.copy_(self.log_alpha.data.exp())
             self.entropy_temperature = self._alpha_dev
+        if self.value_network is not None:
+            yield self.fused_loss(self._value_step(training_batch)[0])
         if self.logger:
             self.logger.log_metrics(
                 {"td_loss": closs[0], "q1_value": self._ws["q1_value"].mean(),
@@ -179,16 +275,18 @@ class SACTrainer(ActorCriticBase):
         """Fast path: the whole update (same arithmetic as train_step_gen), Polyak updates
         fused into the critics' Adam launches, exp(log_alpha) into the alpha launch.
         `importance_weights` ([B] fp32 on the batch's device, prioritized replay): each critic
-        loss becomes mean_b(w_b * (q_b - y_b)^2); the actor and alpha losses stay unweighted."""
+        loss becomes mean_b(w_b * (q_b - y_b)^2); the actor, alpha and value losses stay
+        unweighted."""
         opts = self.optimizers()
         i = 0
-        closs = self._critic_step(training_batch, self.actor_network, self.q1_network_target,
-                                  self.q2_network_target, self._fill_critic,
-                                  sample_weight=importance_weights)
-        self._dp_step(opts[i], self.q1_network.arena, self.q1_network_target.arena, process_group)
+        q1t, q2t = self._critic_targets()
+        closs = self._critic_step(training_batch, self.actor_network, q1t, q2t,
+                                  self._fill_critic, sample_weight=importance_weights)
+        self._dp_step(opts[i], self.q1_network.arena, None if q1t is None else q1t.arena,
+                      process_group)
         i += 1
         if self.q2_network:
-            self._dp_step(opts[i], self.q2_network.arena, self.q2_network_target.arena,
+            self._dp_step(opts[i], self.q2_network.arena, None if q2t is None else q2t.arena,
                           process_group)
             i += 1
         aloss = self._actor_step(training_batch, self._fill_actor)
@@ -200,6 +298,11 @@ class SACTrainer(ActorCriticBase):
             arena.grad_ready = True
             self._dp_step(opts[i], arena, None, process_group, exp_out=self._alpha_dev)
             self.entropy_temperature = self._alpha_dev
+            i += 1
+        if self.value_network is not None:
+            self._value_step(training_batch)
+            self._dp_step(opts[i], self.value_network.arena, self.value_network_target.arena,
+                          process_group)
         self.all_batches_processed += 1
         return closs, aloss
 
