@@ -331,6 +331,73 @@ typedef struct rb200_bc_xent_args {
 } rb200_bc_xent_args_t;
 int rb200_bc_xent_head(const rb200_bc_xent_args_t* args, void* stream);
 
+/* Loss heads of DiscreteCRRTrainer (rb200_crr.cu), reagent/training/                 */
+/* discrete_crr_trainer.py, one warp per row, 1 <= num_actions <= 1024.  The actor's    */
+/* logits are FullyConnectedActor.forward's output (reagent/models/actor.py:90-110):    */
+/*   l = actor_out                            without exploration noise (noise NULL)    */
+/*   l = clamp(actor_out + noise, -1, 1)      with it; `noise` is the draw, scaled      */
+/* Both heads are deterministic (fixed-order means) and allocate nothing                */
+/* (graph-capturable); loss_partials holds 2 * ceil(B / RB200_CRR_ROWS_PER_BLOCK)       */
+/* floats.                                                                              */
+/* critic head: compute_target_q_values + compute_td_loss (:198-218, :304-326)          */
+/*   r  = reward + sum_a action * reward_boost              (boost_rewards)             */
+/*   V' = sum_a softmax(l')_a * q1_target(s')_a, min with q2's when q2 is given         */
+/*   y  = r + gamma * V' * not_terminal                                                 */
+/*   loss[c] = mean_b (q_c(s, a) - y)^2,  q_c(s, a) = sum_a q_c * action                */
+/*   dz_qc = 2 * (q_c(s, a) - y) / B * action               (d loss[c] / d q_c)         */
+#define RB200_CRR_ROWS_PER_BLOCK 16
+typedef struct rb200_crr_critic_args {
+  int32_t batch, num_actions;
+  const float* actor_next;         /* [B,A] actor (or target actor) output on next_state, before noise */
+  const float* noise_next;         /* [B,A] or NULL */
+  const float* q1_target_next;     /* [B,A] q1_network_target(next_state) */
+  const float* q2_target_next;     /* [B,A], with q2 only */
+  const float* q1;                 /* [B,A] q1_network(state) */
+  const float* q2;                 /* [B,A] q2_network(state) or NULL: single critic */
+  const float* action;             /* [B,A] one-hot logged action */
+  const float* reward;             /* [B] */
+  const float* reward_boost;       /* [A] or NULL */
+  const float* not_terminal;       /* [B] */
+  float gamma;
+  float* td_target;                /* [B] y */
+  float* q1_selected;              /* [B] q1(s, a) */
+  float* q2_selected;              /* [B], with q2 only */
+  float* dz_q1;                    /* [B,A] */
+  float* dz_q2;                    /* [B,A], with q2 only */
+  float* loss_partials;
+  float* loss;                     /* [2]: q1 loss, q2 loss (0 without q2) */
+  uint32_t* tile_counter;          /* [1] zero-initialised, self-resetting */
+} rb200_crr_critic_args_t;
+int rb200_crr_critic_head(const rb200_crr_critic_args_t* args, void* stream);
+
+/* actor head: compute_actor_loss (:220-288), a = first arg max of the action row       */
+/*   pi = softmax(l),  V = sum_a pi_a * q1_a,  weight = clamp(exp((q1[a] - V) * inv_beta), */
+/*   0, max_weight)  (a constant of the gradient),  log_pi = log_softmax(l)[a]          */
+/*   loss[0] = mean_b(-log_pi * weight)                      actor_loss_without_reg     */
+/*   loss[1] = loss[0] + entropy_coeff * mean_b(ratio * log_pi) when entropy_coeff > 0,  */
+/*             ratio = clip(pi[a] / action_probability, 1e-4, clip_limit)               */
+/*   dz = d loss[1] / d z for the PRE-activation z of the actor's last layer            */
+/*        (actor_out = act(z)), which is what rb200_mlp_backward / rb200_mlp_wgrad take: */
+/*        the gradient flows through log_pi and through the ratio where it is not        */
+/*        clipped, is zero where actor_out + noise lies outside [-1, 1] (noise given),   */
+/*        and is multiplied by act'(z) computed from actor_out.                          */
+typedef struct rb200_crr_actor_args {
+  int32_t batch, num_actions;
+  const float* actor_out;          /* [B,A] actor output on state, before noise */
+  const float* noise;              /* [B,A] or NULL */
+  const float* q1;                 /* [B,A] q1_network(state), after q1's update */
+  const float* action;             /* [B,A] one-hot logged action */
+  const float* action_probability; /* [B] logged propensities; required iff entropy_coeff > 0 */
+  float inv_beta, max_weight, entropy_coeff, clip_limit;
+  int32_t action_activation;       /* RB200_ACT_* of the actor's last layer */
+  float* weight;                   /* [B] or NULL */
+  float* dz;                       /* [B,A], or NULL: losses only */
+  float* loss_partials;
+  float* loss;                     /* [2] */
+  uint32_t* tile_counter;          /* [1] zero-initialised, self-resetting */
+} rb200_crr_actor_args_t;
+int rb200_crr_actor_head(const rb200_crr_actor_args_t* args, void* stream);
+
 /* ------------------------------------------------------------------------- */
 /* QR-DQN (reagent/training/qrdqn_trainer.py:108-194).  The [hidden -> A*N] head  */
 /* is too wide for a row tile, so it runs as 2-D tiled launches:                   */

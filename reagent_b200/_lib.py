@@ -10,6 +10,7 @@ import os
 MAX_LAYERS = 8
 
 ACT = {"linear": 0, "relu": 1, "tanh": 2, "leaky_relu": 3, "sigmoid": 4, "softplus": 5}
+E_SMEM = -3  # RB200_E_SMEM: a row tile does not fit in shared memory
 LOSS_MSE, LOSS_HUBER = 0, 1
 DISCOUNT_CONST, DISCOUNT_POW = 0, 1
 
@@ -193,6 +194,26 @@ class BcXentArgsT(C.Structure):
                 ("loss", _vp), ("tile_counter", _vp)]
 
 
+CRR_ROWS_PER_BLOCK = 16  # rb200_crr_*_head: loss_partials holds 2 * ceil(batch / 16) floats
+
+
+class CrrCriticArgsT(C.Structure):
+    _fields_ = [("batch", C.c_int32), ("num_actions", C.c_int32), ("actor_next", _vp),
+                ("noise_next", _vp), ("q1_target_next", _vp), ("q2_target_next", _vp),
+                ("q1", _vp), ("q2", _vp), ("action", _vp), ("reward", _vp),
+                ("reward_boost", _vp), ("not_terminal", _vp), ("gamma", C.c_float),
+                ("td_target", _vp), ("q1_selected", _vp), ("q2_selected", _vp), ("dz_q1", _vp),
+                ("dz_q2", _vp), ("loss_partials", _vp), ("loss", _vp), ("tile_counter", _vp)]
+
+
+class CrrActorArgsT(C.Structure):
+    _fields_ = [("batch", C.c_int32), ("num_actions", C.c_int32), ("actor_out", _vp),
+                ("noise", _vp), ("q1", _vp), ("action", _vp), ("action_probability", _vp),
+                ("inv_beta", C.c_float), ("max_weight", C.c_float), ("entropy_coeff", C.c_float),
+                ("clip_limit", C.c_float), ("action_activation", C.c_int32), ("weight", _vp),
+                ("dz", _vp), ("loss_partials", _vp), ("loss", _vp), ("tile_counter", _vp)]
+
+
 class CpeArgsT(C.Structure):
     _fields_ = [("batch", C.c_int32), ("num_actions", C.c_int32), ("num_metrics", C.c_int32),
                 ("next_scores", _vp), ("mask", _vp), ("temperature", C.c_float), ("action", _vp),
@@ -313,6 +334,8 @@ def _declare(lib):
     lib.rb200_pdqn_head.argtypes = [C.POINTER(PdqnArgsT), _vp]
     lib.rb200_c51_head.argtypes = [C.POINTER(C51ArgsT), _vp]
     lib.rb200_bc_xent_head.argtypes = [C.POINTER(BcXentArgsT), _vp]
+    lib.rb200_crr_critic_head.argtypes = [C.POINTER(CrrCriticArgsT), _vp]
+    lib.rb200_crr_actor_head.argtypes = [C.POINTER(CrrActorArgsT), _vp]
     lib.rb200_replay_add_device.argtypes = [C.POINTER(AddArgsT), _vp]
     lib.rb200_sumtree_set_device.argtypes = [_vp, C.c_int32, _vp, _vp, C.c_int32, _vp, _vp, _vp]
     lib.rb200_per_draw_indices.argtypes = [C.POINTER(PerDrawArgsT), _vp]

@@ -2,7 +2,7 @@
 the reference's flow (reagent/model_managers/model_manager.py:84-96 and
 discrete/discrete_dqn.py:63-116, discrete/discrete_qrdqn.py:73-121,
 discrete/discrete_c51dqn.py:43-88, parametric/parametric_dqn.py:45-81,
-actor_critic/sac.py:80-113, actor_critic/td3.py:70-102): build the networks from the net
+actor_critic/sac.py:80-113, actor_critic/td3.py:70-102, discrete/discrete_crr.py:104-179): build the networks from the net
 builders, copy the target, hand everything to the trainer; `create_policy` gives the online
 act-time policy.  Serving modules, data modules and reporters are out of scope (SURVEY.md
 section 2 rows 8, 12, 15, 16)."""
@@ -11,12 +11,12 @@ from typing import Union, Dict, List, Optional
 
 from ..core.parameters import (EvaluationParameters, NormalizationData, NormalizationKey,
                                RLParameters)
-from ..net_builder import (ActorFullyConnected, Categorical, Dueling, DuelingQuantile,
-                           FullyConnected, GaussianFullyConnected, ParametricFullyConnected,
+from ..net_builder import (ActorFullyConnected, Categorical, DiscreteActorFullyConnected,
+                           Dueling, DuelingQuantile, FullyConnected, GaussianFullyConnected, ParametricFullyConnected,
                            Quantile, ValueFullyConnected)
 from ..optimizer import Optimizer__Union
-from ..training import (C51Trainer, CRRWeightFn, DQNTrainer, ParametricDQNTrainer, QRDQNTrainer,
-                        SACTrainer, TD3Trainer)
+from ..training import (C51Trainer, CRRWeightFn, DiscreteCRRTrainer, DQNTrainer,
+                        ParametricDQNTrainer, QRDQNTrainer, SACTrainer, TD3Trainer)
 
 
 def _device(use_gpu: bool):
@@ -141,6 +141,77 @@ class DiscreteC51DQN(_DiscretePolicyMixin):
             rl=self.rl, double_q_learning=self.double_q_learning,
             minibatch_size=self.minibatch_size, num_atoms=self.num_atoms, qmin=self.qmin,
             qmax=self.qmax, optimizer=self.optimizer).to(dev)
+
+
+@dataclass
+class DiscreteCRR(_ActorPolicyMixin):
+    """reagent/model_managers/discrete/discrete_crr.py with its `trainer_param`
+    (CRRTrainerParameters) flattened into the manager.  The policy is the actor's forward
+    (:181-195)."""
+    actions: List[str] = field(default_factory=list)
+    rl: RLParameters = field(default_factory=RLParameters)
+    double_q_learning: bool = True
+    q_network_optimizer: Optimizer__Union = field(default_factory=Optimizer__Union.default)
+    actor_network_optimizer: Optimizer__Union = field(default_factory=Optimizer__Union.default)
+    use_target_actor: bool = False
+    delayed_policy_update: int = 1
+    beta: float = 1.0
+    entropy_coeff: float = 0.0
+    clip_limit: float = 10.0
+    max_weight: float = 20.0
+    actor_net_builder: DiscreteActorFullyConnected = field(
+        default_factory=DiscreteActorFullyConnected)
+    critic_net_builder: Union[Dueling, FullyConnected] = field(default_factory=Dueling)
+    cpe_net_builder: Union[Dueling, FullyConnected] = field(default_factory=FullyConnected)
+    eval_parameters: EvaluationParameters = field(default_factory=EvaluationParameters)
+    metrics_to_score: Optional[List[str]] = None
+
+    def __post_init__(self):
+        # :90-94
+        assert len(self.actions) > 1, (
+            f"DiscreteCRRModel needs at least 2 actions. Got {self.actions}.")
+
+    @property
+    def action_names(self) -> List[str]:
+        return self.actions
+
+    @property
+    def rl_parameters(self) -> RLParameters:
+        return self.rl
+
+    def build_trainer(self, normalization_data_map: Dict[str, NormalizationData], use_gpu: bool,
+                      reward_options=None) -> DiscreteCRRTrainer:
+        """:104-179: the actor, one or two critics, the reward / CPE networks with one block of
+        outputs per metric to score, every target a copy of its network."""
+        dev = _device(use_gpu)
+        s_norm = normalization_data_map[NormalizationKey.STATE]
+        A = len(self.actions)
+        actor = self.actor_net_builder.build_actor(s_norm, A).to(dev)
+        q1 = self.critic_net_builder.build_q_network(None, s_norm, A).to(dev)
+        q2 = q2_target = None
+        if self.double_q_learning:
+            q2 = self.critic_net_builder.build_q_network(None, s_norm, A).to(dev)
+            q2_target = q2.get_target_network()
+        metrics = list(self.metrics_to_score or [])
+        reward_network = q_network_cpe = q_network_cpe_target = None
+        if self.eval_parameters.calc_cpe_in_training:
+            n_out = (len(metrics) + 1) * A  # metrics + reward
+            reward_network = self.cpe_net_builder.build_q_network(None, s_norm, n_out).to(dev)
+            q_network_cpe = self.cpe_net_builder.build_q_network(None, s_norm, n_out).to(dev)
+            q_network_cpe_target = q_network_cpe.get_target_network()
+        return DiscreteCRRTrainer(
+            actor_network=actor, actor_network_target=actor.get_target_network(),
+            q1_network=q1, q1_network_target=q1.get_target_network(),
+            reward_network=reward_network, q2_network=q2, q2_network_target=q2_target,
+            q_network_cpe=q_network_cpe, q_network_cpe_target=q_network_cpe_target,
+            metrics_to_score=metrics, evaluation=self.eval_parameters, rl=self.rl,
+            double_q_learning=self.double_q_learning,
+            q_network_optimizer=self.q_network_optimizer,
+            actor_network_optimizer=self.actor_network_optimizer,
+            use_target_actor=self.use_target_actor, actions=self.actions,
+            delayed_policy_update=self.delayed_policy_update, beta=self.beta,
+            entropy_coeff=self.entropy_coeff, clip_limit=self.clip_limit,
+            max_weight=self.max_weight).to(dev)
 
 
 @dataclass

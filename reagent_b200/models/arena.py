@@ -106,7 +106,38 @@ class ParamArena:
         L = len(self.acts) if n_layers is None else n_layers
         rc = _lib.lib().rb200_mlp_backward(self.desc(n_layers), ws.dz[L - 1].data_ptr(), batch,
                                            ws.c, _lib.cur_stream())
+        if rc == _lib.E_SMEM:
+            # hidden layers too wide for the fused row tile (it keeps three of them in shared
+            # memory; [1024, 1024] does not fit): the same chain one layer per launch.  Nothing
+            # was launched by the refused call.
+            cache = self.__dict__.setdefault("_dx_scratch", {})
+            for l in range(L - 1, 0, -1):
+                self.layer_backward_dx(l, ws, batch, cache)
+            return
         _lib.check(rc, "rb200_mlp_backward")
+
+    def layer_backward_dx(self, l: int, ws, batch: int, cache: dict):
+        """dZ of layer l - 1 from the dZ of layer l: dz[l-1] = (dz[l] . W_l) * act'(h[l-1])
+        (torch.nn.functional.linear's backward w.r.t. its input).  Wide layers take the wgmma
+        split-K path, which needs a scratch buffer kept in `cache`."""
+        lib, st = _lib.lib(), _lib.cur_stream()
+        K, N = self.dims[l], self.dims[l + 1]
+        W, _ = self.layer_ptrs(l)
+        dz, h, out = ws.dz[l], ws.hidden[l - 1], ws.dz[l - 1]
+        key = ("dx_scratch", K, N, batch)
+        if key not in cache:
+            nbytes = int(lib.rb200_linear_backward_dx_tc_scratch_bytes(K, N, batch))
+            cache[key] = torch.empty(nbytes // 4, device=self.flat.device) if nbytes else None
+        scratch = cache[key]
+        if scratch is not None:
+            rc = lib.rb200_linear_backward_dx_tc(W, K, N, dz.data_ptr(), h.data_ptr(),
+                                                 self.acts[l - 1], batch, out.data_ptr(),
+                                                 scratch.data_ptr(), scratch.numel() * 4, st)
+            _lib.check(rc, "rb200_linear_backward_dx_tc")
+        else:
+            rc = lib.rb200_linear_backward_dx(W, K, N, dz.data_ptr(), h.data_ptr(),
+                                              self.acts[l - 1], batch, out.data_ptr(), st)
+            _lib.check(rc, "rb200_linear_backward_dx")
 
 
 def run_mlp(desc: _lib.MlpT, x, out, x1=None, save=None):

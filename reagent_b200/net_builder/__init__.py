@@ -151,6 +151,32 @@ class ActorFullyConnected:
 
 
 @dataclass
+class DiscreteActorFullyConnected:
+    """reagent/net_builder/discrete_actor/fully_connected.py:22-71: one logit per action (the
+    actor of DiscreteCRRTrainer)."""
+    sizes: List[int] = field(default_factory=lambda: [128, 64])
+    activations: List[str] = field(default_factory=lambda: ["relu", "relu"])
+    use_batch_norm: bool = False
+    use_layer_norm: bool = False
+    action_activation: str = "tanh"
+    exploration_variance: float = None
+
+    def __post_init__(self):
+        assert len(self.sizes) == len(self.activations), (
+            f"Must have the same numbers of sizes and activations; got: "
+            f"{self.sizes}, {self.activations}")
+        if self.use_layer_norm:
+            raise NotImplementedError("layer norm is out of scope of reagent_b200 (SURVEY.md M1)")
+
+    def build_actor(self, state_normalization_data: NormalizationData, num_actions: int):
+        return FullyConnectedActor(
+            state_dim=_dim(state_normalization_data), action_dim=num_actions, sizes=self.sizes,
+            activations=self.activations, use_batch_norm=self.use_batch_norm,
+            action_activation=self.action_activation,
+            exploration_variance=self.exploration_variance)
+
+
+@dataclass
 class ValueFullyConnected:
     """reagent/net_builder/value/fully_connected.py:16-44 (the SAC state-value network)"""
     sizes: List[int] = field(default_factory=lambda: [256, 128])

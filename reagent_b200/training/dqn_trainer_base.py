@@ -116,13 +116,19 @@ class DQNTrainerBaseLightning(DQNTrainerMixin, RLTrainerMixin, ReAgentLightningM
         return self._cpe_ws
 
     def _calculate_cpes(self, training_batch: rlt.DiscreteDqnInput,
-                        next_actions_mask: Optional[torch.Tensor] = None):
+                        next_actions_mask: Optional[torch.Tensor] = None,
+                        next_scores: Optional[torch.Tensor] = None,
+                        constant_discount: bool = False):
         """_calculate_cpes (:332-452) on the device: returns the [2] loss tensor (reward loss,
         CPE q-value loss) and leaves the gradient partials of both networks in their arenas.
         Runs AFTER the q-network step of the same batch, as in the reference's generator
         (all_next_action_scores is evaluated after `yield td_loss`, dqn_trainer.py:266-268).
         `next_actions_mask` replaces the batch's next-action mask of the model propensities
-        (DQNTrainer with BCQ passes its filtered mask)."""
+        (DQNTrainer with BCQ passes its filtered mask).  `next_scores` ([B, A] fp32 on the
+        batch's device) are the next-state scores the propensities come from, in place of a
+        forward of q_network on next_state; `constant_discount` discounts by gamma whatever the
+        batch's time_diff / step say.  DiscreteCRRTrainer passes q1_network_target(next_state)
+        from before its critic steps and a constant gamma (discrete_crr_trainer.py:308-367)."""
         pins = Pins(batch_device(training_batch.state.float_features, type(self).__name__))
         state = pins.tensor(training_batch.state.float_features)
         next_state = pins.tensor(training_batch.next_state.float_features)
@@ -133,7 +139,9 @@ class DQNTrainerBaseLightning(DQNTrainerMixin, RLTrainerMixin, ReAgentLightningM
             net.arena.refresh()
             net.arena.forward(x, out, save=save)
 
-        fwd(self.q_network, next_state, ws["next_scores"])
+        if next_scores is None:
+            fwd(self.q_network, next_state, ws["next_scores"])
+            next_scores = ws["next_scores"]
         fwd(self.reward_network, state, ws["reward_est"], ws["reward"])
         fwd(self.q_network_cpe, state, ws["qcpe_out"], ws["qcpe"])
         fwd(self.q_network_cpe_target, next_state, ws["qcpe_t_next"])
@@ -143,7 +151,7 @@ class DQNTrainerBaseLightning(DQNTrainerMixin, RLTrainerMixin, ReAgentLightningM
         assert mrc.shape[1] == M, f"reward + metrics have {mrc.shape[1]} columns, metrics_to_score {M}"
         a = _lib.CpeArgsT()
         a.batch, a.num_actions, a.num_metrics = B, self.num_actions, M
-        a.next_scores = ws["next_scores"].data_ptr()
+        a.next_scores = pins(next_scores)
         mask = (training_batch.possible_next_actions_mask if self.maxq_learning
                 else training_batch.next_action)
         if next_actions_mask is not None:
@@ -153,7 +161,7 @@ class DQNTrainerBaseLightning(DQNTrainerMixin, RLTrainerMixin, ReAgentLightningM
         a.action = pins(training_batch.action)
         a.metrics_reward = pins(mrc)
         a.gamma = float(self.gamma)
-        src = discount_source(self, training_batch)
+        src = None if constant_discount else discount_source(self, training_batch)
         a.discount_src = pins(src)
         a.discount_mode = _lib.DISCOUNT_CONST if src is None else _lib.DISCOUNT_POW
         a.not_terminal = pins(training_batch.not_terminal.reshape(-1))

@@ -17,7 +17,9 @@ sampled one update later.
 
 `FusedDqnStep` drives DQNTrainer, QRDQNTrainer and C51Trainer on sample_discrete_dqn_batch and
 ParametricDQNTrainer on sample_parametric_dqn_batch (one-hot actions as features, the identity
-tiling of the possible actions); the latter without `per` and on one GPU.
+tiling of the possible actions); the latter without `per` and on one GPU.  DiscreteCRRTrainer runs
+on sample_discrete_dqn_batch under the same two limits; its exploration noise is drawn with
+torch.randn inside the graph, and a step returns its q1 loss.
 
 `FusedPolicyStep` is the device-resident online step for SACTrainer and TD3Trainer (continuous
 actions), with the same staging, draw, status words and optional prioritized replay.
@@ -30,6 +32,7 @@ import torch
 from ..replay_memory.device_replay import DeviceReplay, PrioritizedUpdate
 from ..replay_memory.prioritized_replay_buffer import PrioritizedReplayBuffer
 from .c51_trainer import C51Trainer
+from .discrete_crr_trainer import DiscreteCRRTrainer
 from .dqn_trainer import DQNTrainer
 from .parametric_dqn_trainer import ParametricDQNTrainer
 from .qrdqn_trainer import QRDQNTrainer
@@ -90,6 +93,17 @@ class FusedDqnStep:
             if shard is not None or process_group is not None:
                 raise NotImplementedError("the ParametricDQNTrainer step is single-GPU; "
                                           "train_batch(process_group=...) runs data-parallel")
+        if isinstance(trainer, DiscreteCRRTrainer):
+            if per is not None:
+                raise NotImplementedError("per does not cover DiscreteCRRTrainer: its critic "
+                                          "head has no importance weights")
+            if shard is not None or process_group is not None:
+                raise NotImplementedError("the DiscreteCRRTrainer step is single-GPU; "
+                                          "train_batch(process_group=...) runs data-parallel")
+            if trainer.delayed_policy_update != 1:
+                raise NotImplementedError(
+                    "the DiscreteCRRTrainer step captures one graph, so every update trains the "
+                    "actor: delayed_policy_update must be 1 (train_batch takes batch_idx)")
         # ParametricDqnInputMaker's batch (one-hot actions as features, the identity tiling of
         # the possible actions) for ParametricDQNTrainer, DiscreteDqnInputMaker's for the rest
         self._sampler = ("sample_parametric_dqn_batch" if isinstance(trainer, ParametricDQNTrainer)
@@ -215,7 +229,9 @@ class FusedDqnStep:
     def _train_batch(self, batch, **weights):
         """The trainer's update on `batch` (`importance_weights=` with per); returns the loss
         tensor a step copies to the host."""
-        return self.trainer.train_batch(batch, process_group=self.pg, **weights)
+        out = self.trainer.train_batch(batch, process_group=self.pg, **weights)
+        # DiscreteCRRTrainer returns (critic losses [2], actor losses [2])
+        return out[0][:1] if isinstance(self.trainer, DiscreteCRRTrainer) else out
 
     def _train(self, batch):
         """The update on a drawn batch; returns the loss tensor."""

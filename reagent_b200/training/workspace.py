@@ -131,25 +131,7 @@ def head_backward_dx(arena: ParamArena, ws: NetWorkspace, batch: int, cache: dic
     """dZ of the layer below a wide head: dz[L-2] = (dz[L-1] . W_head) * act'(h[L-2])
     (torch.nn.functional.linear's backward w.r.t. its input).  Wide heads (QR-DQN: A*N atoms,
     C51: A*51) take the wgmma split-K path, which needs a scratch buffer kept in `cache`."""
-    lib, st = _lib.lib(), _lib.cur_stream()
-    L = len(arena.acts)
-    K, N = arena.dims[L - 1], arena.dims[L]
-    W, _ = arena.layer_ptrs(L - 1)
-    dz, h, out = ws.dz[L - 1], ws.hidden[L - 2], ws.dz[L - 2]
-    key = ("dx_scratch", K, N, batch)
-    if key not in cache:
-        nbytes = int(lib.rb200_linear_backward_dx_tc_scratch_bytes(K, N, batch))
-        cache[key] = torch.empty(nbytes // 4, device=arena.flat.device) if nbytes else None
-    scratch = cache[key]
-    if scratch is not None:
-        rc = lib.rb200_linear_backward_dx_tc(W, K, N, dz.data_ptr(), h.data_ptr(), arena.acts[L - 2],
-                                             batch, out.data_ptr(), scratch.data_ptr(),
-                                             scratch.numel() * 4, st)
-        _lib.check(rc, "rb200_linear_backward_dx_tc")
-    else:
-        rc = lib.rb200_linear_backward_dx(W, K, N, dz.data_ptr(), h.data_ptr(), arena.acts[L - 2],
-                                          batch, out.data_ptr(), st)
-        _lib.check(rc, "rb200_linear_backward_dx")
+    arena.layer_backward_dx(len(arena.acts) - 1, ws, batch, cache)
 
 
 def reduced_grad(arena: ParamArena) -> torch.Tensor:
