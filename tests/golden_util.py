@@ -5,6 +5,7 @@ import os
 import numpy as np
 import torch
 
+TOL = 1e-5  # the project's parity bar
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 
 
@@ -82,3 +83,31 @@ def grad_close(g_gpu, g_ref, what="grad", l2_tol=1e-3, max_tol=1e-2):
     assert l2 < l2_tol, (what, "rel L2", l2)
     assert mx < max_tol, (what, "rel max", mx)
     return l2, mx
+
+
+def _cmp_net(net, arrays, prefix, tol):
+    for i in range(len(net["W"])):
+        assert rel_err(net["W"][i], arrays[f"{prefix}.W{i}"]) < tol, f"{prefix}.W{i}"
+        assert rel_err(net["b"][i], arrays[f"{prefix}.b{i}"]) < tol, f"{prefix}.b{i}"
+
+
+def _cmp_losses(got, want, tol):
+    for g, w in zip(got, want):
+        if g is None:
+            assert np.isnan(w)
+        else:
+            assert abs(g - w) <= tol * max(1.0, abs(w)), (got, want)
+
+
+def _cmp_module(mod, arrays, prefix, tol=TOL):
+    for i, seq in enumerate(mod.fc.dnn):
+        assert rel_err(seq[0].weight, arrays[f"{prefix}.W{i}"]) < tol, f"{prefix}.W{i}"
+        assert rel_err(seq[0].bias, arrays[f"{prefix}.b{i}"]) < tol, f"{prefix}.b{i}"
+
+
+def _adam_close(w_gpu, w_ref, meta):
+    """Post-Adam parameters at config sizes: every element within the total step budget
+    (n_updates * 2 * lr) and the typical element within 2 % of one step."""
+    d = (w_gpu.detach().cpu().double() - w_ref.detach().double()).abs()
+    assert float(d.max()) <= 2.0 * meta["n_updates"] * meta["lr"] * 1.01
+    assert float(d.median()) < 0.02 * meta["lr"], float(d.median())

@@ -8,57 +8,11 @@ import torch
 
 from oracle import td_oracle as O
 from tests import golden_util as G
-from tests.test_oracle_golden import SAC_CASES, TD3_CASES
+from tests.builders import _build_sac, _build_td3, _inject, _net_arrays, _pbatch, _rand_net
+from tests.golden_cases import SAC_CASES, TD3_CASES
+from tests.golden_util import TOL, _adam_close, _cmp_module
 
 pytestmark = pytest.mark.gpu
-TOL = 1e-5
-
-
-def _pbatch(b):
-    from reagent_b200.core import types as rlt
-
-    return rlt.PolicyNetworkInput(
-        state=rlt.FeatureData(b["state"]), next_state=rlt.FeatureData(b["next_state"]),
-        action=rlt.FeatureData(b["action"]), next_action=rlt.FeatureData(b["next_action"]),
-        reward=b["reward"], not_terminal=b["not_terminal"], step=None, time_diff=None,
-        extras=rlt.ExtraData())
-
-
-def _cmp_module(mod, arrays, prefix, tol=TOL):
-    for i, seq in enumerate(mod.fc.dnn):
-        assert G.rel_err(seq[0].weight, arrays[f"{prefix}.W{i}"]) < tol, f"{prefix}.W{i}"
-        assert G.rel_err(seq[0].bias, arrays[f"{prefix}.b{i}"]) < tol, f"{prefix}.b{i}"
-
-
-def _build_sac(meta, arrays):
-    from reagent_b200.core.parameters import RLParameters
-    from reagent_b200.models import FullyConnectedCritic, GaussianFullyConnectedActor
-    from reagent_b200.optimizer import Optimizer__Union
-    from reagent_b200.training import SACTrainer
-
-    S, A = meta["S"], meta["A"]
-    actor = GaussianFullyConnectedActor(S, A, meta["sizes"], meta["acts"])
-    q1 = FullyConnectedCritic(S, A, meta["sizes"], meta["acts"])
-    q2 = FullyConnectedCritic(S, A, meta["sizes"], meta["acts"]) if meta["twin"] else None
-    G.load_into_module(arrays, "actor0", actor)
-    G.load_into_module(arrays, "q1_0", q1)
-    if q2 is not None:
-        G.load_into_module(arrays, "q2_0", q2)
-    opt = lambda: Optimizer__Union.default(lr=meta["lr"])  # noqa: E731
-    kw = {} if meta["learn_alpha"] else {"alpha_optimizer": None}
-    t = SACTrainer(actor, q1, q2, rl=RLParameters(gamma=meta["gamma"], target_update_rate=meta["tau"]),
-                   q_network_optimizer=opt(), actor_network_optimizer=opt(),
-                   minibatch_size=meta["B"], entropy_temperature=meta["entropy_temperature"],
-                   target_entropy=meta["target_entropy"],
-                   backprop_through_log_prob=meta["backprop"],
-                   **({"alpha_optimizer": opt()} if meta["learn_alpha"] else kw))
-    return t.cuda()
-
-
-def _inject(t, arrays, it):
-    def hook(name, shape, device):
-        return torch.from_numpy(arrays[f"noise{it}.{name}"]).to(device)
-    t.noise_hook = hook
 
 
 def _check_sac_final(t, arrays, meta):
@@ -118,28 +72,6 @@ def test_sac_fast_path_matches_reference(name):
     _check_sac_final(t, arrays, meta)
 
 
-def _build_td3(meta, arrays):
-    from reagent_b200.core.parameters import RLParameters
-    from reagent_b200.models import FullyConnectedActor, FullyConnectedCritic
-    from reagent_b200.optimizer import Optimizer__Union
-    from reagent_b200.training import TD3Trainer
-
-    S, A = meta["S"], meta["A"]
-    actor = FullyConnectedActor(S, A, meta["sizes"], meta["acts"])
-    q1 = FullyConnectedCritic(S, A, meta["sizes"], meta["acts"])
-    q2 = FullyConnectedCritic(S, A, meta["sizes"], meta["acts"]) if meta["twin"] else None
-    G.load_into_module(arrays, "actor0", actor)
-    G.load_into_module(arrays, "q1_0", q1)
-    if q2 is not None:
-        G.load_into_module(arrays, "q2_0", q2)
-    opt = lambda: Optimizer__Union.default(lr=meta["lr"])  # noqa: E731
-    t = TD3Trainer(actor, q1, q2, rl=RLParameters(gamma=meta["gamma"], target_update_rate=meta["tau"]),
-                   q_network_optimizer=opt(), actor_network_optimizer=opt(),
-                   minibatch_size=meta["B"], noise_variance=meta["noise_variance"],
-                   noise_clip=meta["noise_clip"], delayed_policy_update=meta["delay"])
-    return t.cuda()
-
-
 def _check_td3_final(t, arrays, meta):
     _cmp_module(t.actor_network, arrays, "actorN")
     _cmp_module(t.actor_network_target, arrays, "actort_N")
@@ -185,27 +117,6 @@ def test_td3_matches_reference(name, fast):
                     else:
                         assert abs(float(losses[oi].detach()) - r) <= TOL * max(1.0, abs(r))
     _check_td3_final(t, arrays, meta)
-
-
-def _adam_close(w_gpu, w_ref, meta):
-    """Post-Adam parameters at config sizes: every element within the total step budget
-    (n_updates * 2 * lr) and the typical element within 2 % of one step."""
-    d = (w_gpu.detach().cpu().double() - w_ref.detach().double()).abs()
-    assert float(d.max()) <= 2.0 * meta["n_updates"] * meta["lr"] * 1.01
-    assert float(d.median()) < 0.02 * meta["lr"], float(d.median())
-
-
-def _rand_net(dims, acts, gen, bias=0.05):
-    n = O.make_net(dims, acts, gen)
-    for b in n["b"]:
-        b.copy_(torch.randn(b.shape, generator=gen) * bias)
-    return n
-
-
-def _net_arrays(arrays, prefix, net):
-    for i in range(len(net["W"])):
-        arrays[f"{prefix}.W{i}"] = net["W"][i].detach().numpy().copy()
-        arrays[f"{prefix}.b{i}"] = net["b"][i].detach().numpy().copy()
 
 
 def test_sac_config4_shard_matches_oracle():

@@ -14,17 +14,11 @@ from oracle.adamw_oracle import AdamWState
 from reagent_b200.models import FullyConnectedNetwork
 from reagent_b200.optimizer import FusedAdam, FusedAdamW
 from tests import golden_util as G
-from tests.test_oracle_golden import _c51_kwargs, _cmp_losses, _cmp_net, _dqn_kwargs
+from tests.golden_cases import _c51_kwargs, _dqn_kwargs, batch_at
+from tests.golden_util import _cmp_losses, _cmp_net
 
 ADAMW_CASES = ["qrdqn_adamw_amsgrad_cartpole", "c51_adamw_amsgrad_cartpole", "dqn_adamw_decay"]
 SAC_ADAMW_CASES = ["sac_adamw_amsgrad"]
-
-
-def batch_at(arrays, it, device="cpu"):
-    """The batch of update `it` of a make_adamw_golden.py case."""
-    pre = f"batch{it}."
-    return {k[len(pre):]: torch.from_numpy(v.copy()).to(device)
-            for k, v in arrays.items() if k.startswith(pre)}
 
 
 def _adamw_kw(meta):

@@ -15,9 +15,10 @@ import torch
 
 from reagent_b200 import _lib
 from tests import golden_util as G
-from tests.test_adamw_cpu import batch_at
-from tests.test_layer_kernels_gpu import (BETAS, EPS, GRAD_SCALE, LR, NUM_SMS, TAU, _padded,
-                                          _record, _seq_sum)
+from tests.online_step import assert_captured_equals_eager, params, transition_stream
+from tests.builders import _batch, _build_trainer, _free_port, _inject, _pbatch, _record, _rlt_batch
+from tests.golden_cases import batch_at
+from tests.kernel_util import BETAS, EPS, GRAD_SCALE, LR, NUM_SMS, TAU, _padded, _seq_sum
 
 pytestmark = pytest.mark.gpu
 
@@ -299,7 +300,6 @@ def _discrete_trainer(meta, arrays):
                                   "dqn_adamw_decay"])
 def test_discrete_trainers_with_adamw_match_reference(name):
     from reagent_b200.optimizer import FusedAdamW
-    from tests.test_qrdqn_gpu import _batch
 
     arrays, meta = G.load(name)
     t, (q, qt) = _discrete_trainer(meta, arrays)
@@ -324,7 +324,6 @@ def test_sac_with_adamw_amsgrad_matches_reference():
     from reagent_b200.models import FullyConnectedCritic, GaussianFullyConnectedActor
     from reagent_b200.optimizer import FusedAdamW
     from reagent_b200.training import SACTrainer
-    from tests.test_actor_critic_gpu import _inject, _pbatch
 
     arrays, meta = G.load("sac_adamw_amsgrad")
     S, A = meta["S"], meta["A"]
@@ -362,7 +361,6 @@ def test_sac_with_adamw_amsgrad_matches_reference():
 @pytest.mark.parametrize("S,sizes,A", [(128, [256, 128], 16), (36, [300, 130, 20], 9)])
 def test_adamw_writes_the_same_weight_images_as_the_pack_kernel(S, sizes, A, amsgrad, monkeypatch):
     from reagent_b200.optimizer import Optimizer__Union, FusedAdamW
-    from tests.test_dqn_gpu import _build_trainer, _rlt_batch
 
     monkeypatch.setenv("RB200_ADAM_PACK", "1")
     B = 64
@@ -431,43 +429,24 @@ def test_cartpole_online_step_with_adamw_captured_equals_eager(kind, with_per):
     from reagent_b200.optimizer import FusedAdamW
     from reagent_b200.replay_memory import PrioritizedReplayBuffer, PrioritizedUpdate
     from reagent_b200.training.fused_step import FusedDqnStep
-    from tests.test_per_gpu import _stream
 
     n_steps = 30
-    base = _stream(3000, 4, 2, 7)
-    extra = _stream(n_steps, 4, 2, 8)
+    base = transition_stream(3000, 7, 4, 2)
     per = PrioritizedUpdate(alpha=0.6, beta0=0.4, beta_updates=10, eps=1e-6) if with_per else None
-    runs = []
-    for captured in (True, False):
+
+    def setup():
         t, B = _cartpole_trainer(kind)
         assert type(t.optimizers()[0]) is FusedAdamW and t.optimizers()[0].amsgrad
         rb = PrioritizedReplayBuffer(stack_size=1, replay_capacity=4096, batch_size=B)
         rb.add_batch(**base)
         random.seed(5)
-        fused = FusedDqnStep(t, rb, B, rng="device", online=True, per=per)
-        losses = []
-        for i in range(n_steps):
-            tr = {k: v[i] for k, v in extra.items()}
-            if with_per and i % 2:
-                del tr["priority"]
-            if captured:
-                out = fused.step(tr)
-                torch.cuda.current_stream().synchronize()
-                losses.append(float(out[0]))
-            else:
-                fused.dr.stage(0, 0, priority_from_max=with_per, **tr)
-                fused.dr.launch_add(1, slot=0, priority_from_max=with_per)
-                losses.append(float(fused._one_update(None)))
-        torch.cuda.synchronize()
-        fused.dr.raise_if_failed()
-        runs.append((losses, [p.detach().clone() for p in t.q_network.parameters()],
-                     [p.detach().clone() for p in t.q_network_target.parameters()],
-                     t.optimizers()[0].max_exp_avg_sq.clone()))
-    (l0, p0, t0, v0), (l1, p1, t1, v1) = runs
-    assert l0 == l1 and all(np.isfinite(l0))
-    assert all(torch.equal(a, b) for a, b in zip(p0, p1))
-    assert all(torch.equal(a, b) for a, b in zip(t0, t1))
-    assert torch.equal(v0, v1)
+        return FusedDqnStep(t, rb, B, rng="device", online=True, per=per), None
+
+    assert_captured_equals_eager(
+        setup, transition_stream(n_steps, 8, 4, 2), n_steps,
+        lambda f: [params(f.trainer.q_network), params(f.trainer.q_network_target),
+                   f.trainer.optimizers()[0].max_exp_avg_sq.clone()],
+        drop_priority=(lambda i: i % 2) if with_per else None)
 
 
 # ---------------------------------------------------------------------------
@@ -541,7 +520,6 @@ def test_two_rank_adamw_amsgrad_update_matches_full_batch(use_p2p):
         pytest.skip("needs 2 GPUs")
     import torch.multiprocessing as mp
 
-    from tests.test_dp_gpu import _free_port
 
     ctx = mp.get_context("spawn")
     out = ctx.Queue()

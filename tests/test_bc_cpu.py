@@ -11,13 +11,8 @@ from oracle import bc_oracle as BC
 from oracle import bcq_oracle as BO
 from oracle import td_oracle as O
 from tests import golden_util as G
-
-BC_CASES = ["bc_reference_4x4", "bc_a16_random_masks", "bc_a40_tanh_leaky"]
-
-
-def golden_batch(arrays, prefix, device="cpu"):
-    return {k: torch.from_numpy(arrays[f"{prefix}.{k}"].copy()).to(device)
-            for k in ("state", "action", "possible_actions_mask")}
+from tests.golden_cases import (BC_CASES, E2E, E2E_MAX_KEPT, E2E_MIN_BEHAVIOUR_KEPT, e2e_data,
+                                e2e_metrics, golden_batch)
 
 
 @pytest.mark.parametrize("name", BC_CASES)
@@ -58,34 +53,6 @@ def test_bc_oracle_labels_each_row_with_its_own_action():
 # ---------------------------------------------------------------------------
 # offline BCQ scenario: logged data from a deterministic behaviour rule -> BC -> BCQ filter
 # ---------------------------------------------------------------------------
-E2E = dict(S=16, A=6, B=512, sizes=[64, 64], lr=1e-2, steps=300, thr=0.3)
-# share of held-out rows on which the BCQ filter keeps the behaviour action: the CPU oracle
-# reaches 0.982 on these data (the misses are states next to a decision boundary of the rule);
-# the bound leaves room for another arithmetic's rounding to compound over 300 Adam steps
-E2E_MIN_BEHAVIOUR_KEPT = 0.95
-# and the filter does narrow the mask (the oracle keeps 0.17 of all (row, action) pairs)
-E2E_MAX_KEPT = 0.3
-
-
-def e2e_data(seed=0):
-    """(behaviour map, train batches, held-out states): the logged action of a state is
-    argmax(state @ Wb), every action is possible."""
-    g = torch.Generator().manual_seed(seed)
-    S, A, B = E2E["S"], E2E["A"], E2E["B"]
-    Wb = torch.randn(S, A, generator=g)
-    batches = []
-    for _ in range(E2E["steps"]):
-        x = torch.randn(B, S, generator=g)
-        batches.append(dict(state=x, action=torch.nn.functional.one_hot((x @ Wb).argmax(1), A).float(),
-                            possible_actions_mask=torch.ones(B, A)))
-    held_out = torch.randn(B, S, generator=g)
-    return Wb, batches, held_out
-
-
-def e2e_metrics(keep, Wb, states):
-    """(share of rows whose behaviour action the BCQ keep-mask holds, share of all pairs kept)."""
-    beh = (states @ Wb).argmax(1)
-    return float(keep[torch.arange(len(beh)), beh].mean()), float(keep.mean())
 
 
 def test_offline_bcq_scenario_on_the_oracle():

@@ -9,10 +9,11 @@ import torch
 
 from oracle import td_oracle as O
 from tests import golden_util as G
-from tests.test_bc_cpu import (BC_CASES, E2E, E2E_MAX_KEPT, E2E_MIN_BEHAVIOUR_KEPT, e2e_data,
-                               e2e_metrics, golden_batch)
-from tests.test_dp_gpu import _free_port
-from tests.test_dqn_gpu import CONFIG2_MAX_ADAM_OUTLIER_FRAC, CONFIG2_MAX_FLIPPED_ROWS, TOL, _record
+from tests.builders import (CONFIG2_MAX_ADAM_OUTLIER_FRAC, CONFIG2_MAX_FLIPPED_ROWS, _free_port,
+                            _record)
+from tests.golden_cases import (BC_CASES, E2E, E2E_MAX_KEPT, E2E_MIN_BEHAVIOUR_KEPT, e2e_data,
+                                e2e_metrics, golden_batch)
+from tests.golden_util import TOL
 
 pytestmark = pytest.mark.gpu
 

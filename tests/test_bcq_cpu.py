@@ -9,10 +9,7 @@ import torch
 from oracle import bcq_oracle as BO
 from oracle import td_oracle as O
 from tests import golden_util as G
-from tests.test_oracle_golden import _dqn_kwargs
-
-BCQ_DQN_CASES = ["dqn_bcq_huber_double", "dqn_bcq_cpe_mse_single",
-                 "dqn_bcq_dueling_multistep_boost"]
+from tests.golden_cases import BCQ_DQN_CASES, _dqn_kwargs
 
 
 def _imitator(arrays, meta):

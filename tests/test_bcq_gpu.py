@@ -12,60 +12,12 @@ import torch
 from oracle import bcq_oracle as BO
 from oracle import td_oracle as O
 from tests import golden_util as G
-from tests.test_bcq_cpu import BCQ_DQN_CASES
-from tests.test_dqn_gpu import K2_PATHS, TOL, _assert_k2, _record, _rlt_batch, _select_k2
+from tests.builders import (K2_PATHS, _assert_k2, _build_bcq, _golden_batch, _record, _rlt_batch,
+                            _select_k2)
+from tests.golden_cases import BCQ_DQN_CASES
+from tests.golden_util import TOL
 
 pytestmark = pytest.mark.gpu
-
-
-def _build(meta, arrays=None, imitator=None, dev="cuda"):
-    """DQNTrainer with BCQ (and CPE heads when meta["cpe_metrics"] is set) from golden weights."""
-    from reagent_b200.core.parameters import EvaluationParameters, RLParameters
-    from reagent_b200.models import DuelingQNetwork, FullyConnectedDQN, FullyConnectedNetwork
-    from reagent_b200.optimizer import Optimizer__Union
-    from reagent_b200.training import DQNTrainer
-    from reagent_b200.training.dqn_trainer import BCQConfig
-
-    S, A = meta["S"], meta["A"]
-    if meta.get("dueling"):
-        q = DuelingQNetwork.make_fully_connected(S, A, meta["sizes"], meta["acts"])
-    else:
-        q = FullyConnectedDQN(S, A, meta["sizes"], meta["acts"])
-    qt = q.get_target_network()
-    if imitator is None:
-        imitator = FullyConnectedNetwork([S] + meta["imitator_sizes"] + [A], meta["imitator_acts"])
-    nets, loads = (), [(q, "q0"), (qt, "qt0"), (imitator, "im")]
-    cpe = meta.get("cpe_metrics") is not None
-    if cpe:
-        n_out = (len(meta["cpe_metrics"]) + 1) * A
-        rn = FullyConnectedDQN(S, n_out, meta["sizes"], meta["acts"])
-        qc = FullyConnectedDQN(S, n_out, meta["sizes"], meta["acts"])
-        qct = qc.get_target_network()
-        nets = (rn, qc, qct)
-        loads += [(rn, "r0"), (qc, "c0"), (qct, "ct0")]
-    if arrays is not None:
-        for net, prefix in loads:
-            G.load_into_module(arrays, prefix, net)
-    rl = RLParameters(gamma=meta["gamma"], target_update_rate=meta["tau"],
-                      q_network_loss=meta["loss"], maxq_learning=meta["maxq"],
-                      multi_steps=meta["multi_steps"], temperature=meta.get("temperature", 0.01),
-                      use_seq_num_diff_as_time_diff=meta["time_diff"], reward_boost=meta["boost"])
-    t = DQNTrainer(q, qt, *nets, metrics_to_score=list(meta["cpe_metrics"]) if cpe else None,
-                   actions=[str(i) for i in range(A)], rl=rl, double_q_learning=meta["double_q"],
-                   minibatch_size=meta["B"], optimizer=Optimizer__Union.default(lr=meta["lr"]),
-                   evaluation=EvaluationParameters(calc_cpe_in_training=cpe), imitator=imitator,
-                   bcq=BCQConfig(meta["bcq"]))
-    return t.to(dev)
-
-
-def _golden_batch(arrays, meta):
-    from reagent_b200.core import types as rlt
-
-    b = G.batch_tensors(arrays, "cuda")
-    batch = _rlt_batch(b, meta)
-    batch.extras = rlt.ExtraData(action_probability=torch.ones_like(b["reward"]),
-                                 metrics=b.get("metrics"))
-    return b, batch
 
 
 def _close(got, want):
@@ -84,7 +36,7 @@ def test_bcq_dqn_matches_reference(name, path, fast, monkeypatch):
     _select_k2(monkeypatch, path)
     arrays, meta = G.load(name)
     cpe = meta["cpe_metrics"] is not None
-    t = _build(meta, arrays)
+    t = _build_bcq(meta, arrays)
     b, batch = _golden_batch(arrays, meta)
     masks_before = (b["possible_next_actions_mask"].clone(), b["possible_actions_mask"].clone())
     opts = t.optimizers()
@@ -140,7 +92,7 @@ def test_bcq_dqn_matches_reference(name, path, fast, monkeypatch):
 def test_bcq_compute_td_loss_only_uses_the_filter():
     """validation_step's loss (compute_td_loss_only) filters like the training step."""
     arrays, meta = G.load("dqn_bcq_huber_double")
-    t = _build(meta, arrays)
+    t = _build_bcq(meta, arrays)
     _, batch = _golden_batch(arrays, meta)
     loss = float(t.compute_td_loss_only(batch))
     assert torch.equal(t.bcq_next_actions_mask.cpu(), torch.from_numpy(arrays["bcq.next_mask0"]))
@@ -220,7 +172,7 @@ def test_bcq_config2_matches_oracle(path, monkeypatch):
              next_action=torch.nn.functional.one_hot(act, A).float() * nt,
              possible_actions_mask=torch.ones(B, A), possible_next_actions_mask=pnam)
     imitator = FullyConnectedNetwork([S, 256, 128, A], ["relu", "relu", "linear"])
-    t = _build(meta, arrays, imitator=imitator)
+    t = _build_bcq(meta, arrays, imitator=imitator)
     batch = _rlt_batch({k: (v.cuda() if v is not None else None) for k, v in b.items()}, meta)
     loss = float(t.compute_td_loss_only(batch))
     _assert_k2(t, path)

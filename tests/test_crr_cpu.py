@@ -15,42 +15,9 @@ from oracle import td_oracle as O
 from oracle.adamw_oracle import AdamWState
 from oracle.ref_harness import reference_available
 from tests import golden_util as G
-
-TOL = 1e-5
-CRR_CASES = ["crr_twin_default", "crr_single_target_actor", "crr_dueling_delayed",
-             "crr_entropy_clip", "crr_noise_saturated", "crr_cpe_boost", "crr_adamw_amsgrad",
-             "crr_odd_dims", "crr_cartpole_manager"]
-SOURCES = ("actor", "q1", "q2", "r", "c")  # the order the compact case seeds its networks in
-
-
-def net_names(meta):
-    """Golden prefixes of the trained networks and of their targets."""
-    src = ["actor", "q1"] + (["q2"] if meta["twin"] else [])
-    tgt = ["actor_t", "q1_t"] + (["q2_t"] if meta["twin"] else [])
-    if meta["cpe_metrics"] is not None:
-        src += ["r", "c"]
-        tgt += ["ct"]
-    return src, tgt
-
-
-def net_dims(meta, name):
-    A = meta["A"]
-    out = A if name in ("actor", "q1", "q2") else (len(meta["cpe_metrics"]) + 1) * A
-    return [meta["S"]] + meta["sizes"] + [out]
-
-
-def initial_tensors(arrays, meta, name):
-    """[W0, b0, W1, b1, ...] of network `name` before the first update (a target starts as a copy
-    of its network in the compact case, whose parameters are seeded rather than stored)."""
-    if not meta["compact"]:
-        return [torch.from_numpy(x.copy()) for pair in G.net_pairs(arrays, name + "0") for x in pair]
-    src = {"actor_t": "actor", "q1_t": "q1", "q2_t": "q2", "ct": "c"}.get(name, name)
-    dims = net_dims(meta, src)
-    shapes = []
-    for i in range(len(dims) - 1):
-        shapes += [torch.empty(dims[i + 1], dims[i]), torch.empty(dims[i + 1])]
-    present = [n for n in SOURCES if n in net_names(meta)[0]]
-    return CO.seeded_like(shapes, meta["seed"] + 100 + present.index(src))
+from tests.golden_cases import (CRR_CASES, check_grads, check_losses, check_params, initial_tensors,
+                                net_names, noise_of)
+from tests.golden_util import TOL
 
 
 def _acts(meta, name):
@@ -76,39 +43,6 @@ def update_kwargs(meta):
                 entropy_coeff=meta["entropy_coeff"], clip_limit=meta["clip_limit"],
                 max_weight=meta["max_weight"], reward_boost=boost,
                 temperature=meta["temperature"])
-
-
-def noise_of(arrays, it, which, device="cpu"):
-    k = f"noise{it}.{which}"
-    return torch.from_numpy(arrays[k].copy()).to(device) if k in arrays else None
-
-
-def check_params(arrays, meta, name, params, tol=TOL):
-    """`params` ([W0, b0, ...] tensors) against the golden's final values of network `name`."""
-    if meta["compact"]:
-        for i, p in enumerate(params):
-            assert G.rel_err(CO.digest(p), arrays[f"{name}N.digest{i}"]) < tol, (name, i)
-        return
-    ref = [x for pair in G.net_pairs(arrays, name + "N") for x in pair]
-    assert len(ref) == len(params)
-    for i, (p, r) in enumerate(zip(params, ref)):
-        assert G.rel_err(p, r) < tol, (name, i)
-
-
-def check_grads(arrays, meta, opt_idx, grads, tol=TOL):
-    for i, g in enumerate(grads):
-        ref = arrays[f"grad0.opt{opt_idx}.{i}"]
-        assert G.rel_err(CO.digest(g) if meta["compact"] else g, ref) < tol, (opt_idx, i)
-
-
-def check_losses(arrays, it, losses, tol=TOL):
-    ref = arrays["losses"][it]
-    assert len(losses) == len(ref)
-    for l, r in zip(losses, ref):
-        if np.isnan(r):
-            assert l is None
-        else:
-            assert abs(float(l) - r) <= tol * max(1.0, abs(r)), (it, float(l), r)
 
 
 @pytest.mark.parametrize("name", CRR_CASES)

@@ -8,8 +8,9 @@ import pytest
 import torch
 
 from tests import golden_util as G
-from tests.test_crr_cpu import (CRR_CASES, check_grads, check_losses, check_params,
-                                initial_tensors, net_names, noise_of)
+from tests.online_step import assert_captured_equals_eager, params
+from tests.golden_cases import (CRR_CASES, check_grads, check_losses, check_params, initial_tensors,
+                                net_names, noise_of)
 
 pytestmark = pytest.mark.gpu
 
@@ -328,29 +329,12 @@ def test_captured_online_step_matches_the_eager_one():
     run eagerly agree bit for bit."""
     from reagent_b200.training.fused_step import FusedDqnStep
 
-    extra = _stream(12, 11)
-    runs = []
-    for captured in (True, False):
+    def setup():
         rb, t = _setup(True)
         random.seed(5)
-        fused = FusedDqnStep(t, rb, B, rng="device", online=True)
-        losses = []
-        for i in range(12):
-            tr = {k: v[i] for k, v in extra.items()}
-            if captured:
-                lh = fused.step(tr)
-                torch.cuda.current_stream().synchronize()
-                losses.append(float(lh[0]))
-            else:
-                fused.dr.stage(0, 0, **tr)
-                fused.dr.launch_add(1, slot=0)
-                losses.append(float(fused._one_update(None)))
-        torch.cuda.synchronize()
-        fused.dr.raise_if_failed()
-        runs.append((losses, [p.detach().clone() for p in t.parameters()]))
-    (l0, p0), (l1, p1) = runs
-    assert l0 == l1 and all(np.isfinite(l0))
-    assert all(torch.equal(a, b) for a, b in zip(p0, p1))
+        return FusedDqnStep(t, rb, B, rng="device", online=True), None
+
+    assert_captured_equals_eager(setup, _stream(12, 11), 12, lambda f: params(f.trainer))
 
 
 def test_captured_online_step_draws_its_exploration_noise_inside_the_graph():

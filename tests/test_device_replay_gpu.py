@@ -8,7 +8,7 @@ import pytest
 import torch
 
 from tests import golden_util as G
-from tests.test_replay_gpu import _build
+from tests.builders import _build_replay
 
 pytestmark = pytest.mark.gpu
 
@@ -65,7 +65,7 @@ def test_device_add_and_draw_match_reference(name):
     st = {k: arrays[f"stream.{k}"] for k in keys}
     n0 = 3  # a few host-side adds first (buffer initialisation), the rest on the device
     head = dict(meta, n_add=n0)
-    rb = _build({f"stream.{k}": v[:n0] for k, v in st.items()}, head)
+    rb = _build_replay({f"stream.{k}": v[:n0] for k, v in st.items()}, head)
     dr = DeviceReplay(rb, stage_rows=64)
     dr.add_rows(**{k: v[n0:] for k, v in st.items()})
     dr.raise_if_failed()
@@ -82,7 +82,7 @@ def test_device_add_and_draw_match_reference(name):
         assert np.array_equal(batch.next_state.cpu().numpy()[~term], arrays[f"sample{s_i}.next_state"][~term])
     # back to the host API: identical state to a buffer built entirely on the host
     dr.sync_to_host()
-    host = _build(arrays, meta)
+    host = _build_replay(arrays, meta)
     host._flush()  # staged host rows -> device storage
     assert int(rb.add_count) == int(host.add_count) and rb.size == host.size
     assert np.array_equal(rb._is_index_valid.numpy(), host._is_index_valid.numpy())

@@ -3,20 +3,12 @@
 against one full-batch update on a single rank from identical parameters.  SURVEY.md 8e: every
 loss is a batch mean, so the mean of the shard gradients is the global gradient."""
 import os
-import socket
 
 import pytest
 import torch
+from tests.builders import _free_port
 
 pytestmark = pytest.mark.gpu
-
-
-def _free_port():
-    s = socket.socket()
-    s.bind(("127.0.0.1", 0))
-    p = s.getsockname()[1]
-    s.close()
-    return p
 
 
 def _worker(rank, world, port, algo, use_p2p, out):

@@ -6,70 +6,17 @@ import torch
 
 from oracle import td_oracle as O
 from tests import golden_util as G
-from tests.test_oracle_golden import DQN_CASES, _dqn_kwargs
+from tests.builders import (CONFIG2_DZ_TOL, CONFIG2_MAX_ADAM_OUTLIER_FRAC, CONFIG2_MAX_FLIPPED_ROWS,
+                            K2_PATHS, _assert_k2, _build_cpe_trainer, _build_trainer, _record,
+                            _rlt_batch, _select_k2)
+from tests.golden_cases import DQN_CASES, DQN_CPE_CASES
+from tests.golden_util import TOL
 
 pytestmark = pytest.mark.gpu
-TOL = 1e-5
 # the BASELINE configs[0]-shaped case has 49 k hidden elements and 8.9 k parameters: it gets the
 # size-aware post-Adam criterion of the config-2 test (test_dqn_config0_matches_reference)
 CONFIG0 = "dqn_cartpole_config0"
 DQN_CASES = [c for c in DQN_CASES if c != CONFIG0]
-# K2 has two implementations in the library: the warpgroup-MMA kernel (rb200_dqn_tc.cu,
-# preferred when the shapes fit; path id "tcgen05" is its historical name) and the mma.sync
-# row-tile kernel (rb200_dqn.cu); every golden case runs on both.
-K2_PATHS = ["tcgen05", "rows"]
-
-
-def _select_k2(monkeypatch, path):
-    if path == "rows":
-        monkeypatch.setenv("RB200_DISABLE_WGMMA", "1")
-    else:
-        monkeypatch.delenv("RB200_DISABLE_WGMMA", raising=False)
-
-
-def _assert_k2(t, path):
-    used_tc = t._last_td_call[-1] is not None
-    assert used_tc == (path == "tcgen05"), f"K2 ran on the wrong kernel (wanted {path})"
-
-
-def _build_trainer(meta, arrays=None, dev="cuda"):
-    from reagent_b200.core.parameters import EvaluationParameters, RLParameters
-    from reagent_b200.models import DuelingQNetwork, FullyConnectedDQN
-    from reagent_b200.optimizer import Optimizer__Union
-    from reagent_b200.training import DQNTrainer
-
-    if meta.get("dueling"):
-        q = DuelingQNetwork.make_fully_connected(meta["S"], meta["A"], meta["sizes"], meta["acts"])
-    else:
-        q = FullyConnectedDQN(meta["S"], meta["A"], meta["sizes"], meta["acts"])
-    qt = q.get_target_network()
-    if arrays is not None:
-        G.load_into_module(arrays, "q0", q)
-        G.load_into_module(arrays, "qt0", qt)
-    q, qt = q.to(dev), qt.to(dev)
-    rl = RLParameters(gamma=meta["gamma"], target_update_rate=meta["tau"],
-                      q_network_loss=meta["loss"], maxq_learning=meta["maxq"],
-                      multi_steps=meta["multi_steps"],
-                      use_seq_num_diff_as_time_diff=meta["time_diff"],
-                      reward_boost=meta["boost"])
-    t = DQNTrainer(q, qt, actions=[str(i) for i in range(meta["A"])], rl=rl,
-                   double_q_learning=meta["double_q"], minibatch_size=meta["B"],
-                   optimizer=Optimizer__Union.default(lr=meta["lr"]),
-                   evaluation=EvaluationParameters(calc_cpe_in_training=False))
-    return t.to(dev)
-
-
-def _rlt_batch(b, meta):
-    from reagent_b200.core import types as rlt
-
-    return rlt.DiscreteDqnInput(
-        state=rlt.FeatureData(b["state"]), next_state=rlt.FeatureData(b["next_state"]),
-        reward=b["reward"], time_diff=b["time_diff"],
-        step=b["step"] if meta["multi_steps"] is not None else None,
-        not_terminal=b["not_terminal"], action=b["action"], next_action=b["next_action"],
-        possible_actions_mask=b["possible_actions_mask"],
-        possible_next_actions_mask=b["possible_next_actions_mask"],
-        extras=rlt.ExtraData(action_probability=torch.ones_like(b["reward"])))
 
 
 def _check_against_golden(t, arrays, meta, losses):
@@ -128,26 +75,6 @@ def test_dqn_fast_path_matches_reference(name, path, monkeypatch):
     losses = [float(t.train_batch(batch, it)) for it in range(meta["n_updates"])]
     _assert_k2(t, path)
     _check_against_golden(t, arrays, meta, losses)
-
-
-def _record(name, **kv):
-    """Measurements the tolerances below are derived from, appended to
-    $RB200_TEST_RECORD_DIR/test_measurements.jsonl when that variable names a directory."""
-    import json, os
-    d = os.environ.get("RB200_TEST_RECORD_DIR")
-    if d and os.path.isdir(d):
-        with open(os.path.join(d, "test_measurements.jsonl"), "a") as f:
-            f.write(json.dumps({"test": name, **kv}) + "\n")
-
-
-# Bounds of test_dqn_config2_matches_oracle: a hidden unit within ~5e-6 of 0 may take the other
-# ReLU pattern than the oracle's, which moves its row's weight gradients; post-Adam elements
-# within fp32 noise of a zero gradient move by +-lr.  Both are counted against these bounds.
-CONFIG2_MAX_FLIPPED_ROWS = 8
-CONFIG2_MAX_ADAM_OUTLIER_FRAC = 1.2e-3
-# the mma.sync row-tile kernel (the library's second K2, taken when shapes do not fit the
-# wgmma kernel) accumulates its 3xTF32 products in a different order, so per-row dZ gets 2e-5
-CONFIG2_DZ_TOL = {"tcgen05": TOL, "rows": 2e-5}
 
 
 @pytest.mark.parametrize("path", K2_PATHS)
@@ -461,38 +388,10 @@ def test_dqn_config0_matches_reference(path, monkeypatch):
 # ---------------------------------------------------------------------------
 # CPE heads (calc_cpe_in_training=True, the reference default): dqn_trainer_base.py:243-452
 # ---------------------------------------------------------------------------
-CPE_CASES = ["dqn_cpe_huber", "dqn_cpe_mse_sarsa_multistep"]
-
-
-def _build_cpe_trainer(meta, arrays):
-    from reagent_b200.core.parameters import EvaluationParameters, RLParameters
-    from reagent_b200.models import FullyConnectedDQN
-    from reagent_b200.optimizer import Optimizer__Union
-    from reagent_b200.training import DQNTrainer
-
-    S, A = meta["S"], meta["A"]
-    n_out = (len(meta["cpe_metrics"]) + 1) * A
-    q = FullyConnectedDQN(S, A, meta["sizes"], meta["acts"])
-    qt = q.get_target_network()
-    rn = FullyConnectedDQN(S, n_out, meta["sizes"], meta["acts"])
-    qc = FullyConnectedDQN(S, n_out, meta["sizes"], meta["acts"])
-    qct = qc.get_target_network()
-    for net, prefix in ((q, "q0"), (qt, "qt0"), (rn, "r0"), (qc, "c0"), (qct, "ct0")):
-        G.load_into_module(arrays, prefix, net)
-    rl = RLParameters(gamma=meta["gamma"], target_update_rate=meta["tau"],
-                      q_network_loss=meta["loss"], maxq_learning=meta["maxq"],
-                      multi_steps=meta["multi_steps"], temperature=meta["temperature"],
-                      use_seq_num_diff_as_time_diff=meta["time_diff"], reward_boost=meta["boost"])
-    t = DQNTrainer(q.cuda(), qt.cuda(), rn.cuda(), qc.cuda(), qct.cuda(),
-                   metrics_to_score=list(meta["cpe_metrics"]),
-                   actions=[str(i) for i in range(A)], rl=rl, double_q_learning=meta["double_q"],
-                   minibatch_size=meta["B"], optimizer=Optimizer__Union.default(lr=meta["lr"]),
-                   evaluation=EvaluationParameters(calc_cpe_in_training=True))
-    return t.cuda()
 
 
 @pytest.mark.parametrize("fast", [False, True])
-@pytest.mark.parametrize("name", CPE_CASES)
+@pytest.mark.parametrize("name", DQN_CPE_CASES)
 def test_dqn_cpe_matches_reference(name, fast):
     from reagent_b200.core import types as rlt
     from reagent_b200.training import run_update

@@ -14,9 +14,7 @@ Random weights are scaled by 1/sqrt(fan_in), so every output row and column is O
 error confined to a ragged tail cannot hide under the tensor's maximum.  Measured errors are
 appended to $RB200_TEST_RECORD_DIR/test_measurements.jsonl when that directory exists.
 """
-import json
 import math
-import os
 
 import numpy as np
 import pytest
@@ -24,6 +22,8 @@ import torch
 
 from reagent_b200 import _lib
 from tests import golden_util as G
+from tests.builders import _record
+from tests.kernel_util import BETAS, EPS, GRAD_SCALE, LR, NAN, NUM_SMS, TAU, _padded, _seq_sum
 
 pytestmark = pytest.mark.gpu
 
@@ -40,19 +40,10 @@ def _tol(length):
 
 
 E_SMEM = -3
-NAN = float("nan")
 ACTS = ["linear", "relu", "tanh", "leaky_relu", "sigmoid", "softplus"]
 # pick_rows_cfg's four instances (threads, k-chunk) and the default choice
 CFGS = [None, (512, 32), (512, 16), (256, 32), (256, 16)]
-NUM_SMS = 132
 SMEM_FLOATS = 227 * 1024 // 4
-
-
-def _record(name, **kv):
-    d = os.environ.get("RB200_TEST_RECORD_DIR")
-    if d and os.path.isdir(d):
-        with open(os.path.join(d, "test_measurements.jsonl"), "a") as f:
-            f.write(json.dumps({"test": name, **kv}) + "\n")
 
 
 def _lib_():
@@ -90,14 +81,6 @@ def _fits(cfg, batch, din, hmax, n_in, n_h, extra_per_row):
         if 2 * stage + R * (n_in * ld_in + n_h * ld_h + extra_per_row) <= SMEM_FLOATS:
             return True
     return False
-
-
-def _padded(shape, offset=0, fill=NAN):
-    """A CUDA fp32 tensor of `shape` starting `offset` floats into its allocation (offset 1:
-    not 16-byte aligned, which sends the kernels down their scalar load / store paths)."""
-    n = int(np.prod(shape))
-    buf = torch.full((n + offset + 4,), fill, device="cuda")
-    return buf[offset:offset + n].view(*shape)
 
 
 # ------------------------------------------------------------------------------------------
@@ -503,14 +486,6 @@ def test_grad_reduce_bit_identical_to_sequential_fp32(n, splits):
 # ------------------------------------------------------------------------------------------
 # (d) rb200_adam_soft_update, rb200_soft_update, FusedAdam against torch on the CPU
 # ------------------------------------------------------------------------------------------
-LR, BETAS, EPS, GRAD_SCALE, TAU = 0.1, (0.5, 0.9), 1e-3, 0.5, 0.3
-
-
-def _seq_sum(parts):
-    s = parts[0].clone()
-    for k in range(1, parts.shape[0]):
-        s = s + parts[k]
-    return s
 
 
 def _adam_inputs(opt, ref_p):

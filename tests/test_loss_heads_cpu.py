@@ -9,8 +9,8 @@ import torch
 from oracle import heads_fp64 as H
 from oracle import td_oracle as O
 from tests import golden_util as G
-from tests.test_oracle_golden import (C51_CASES, DQN_CPE_CASES, PDQN_CASES, QRDQN_CASES,
-                                      _c51_kwargs, _dqn_kwargs)
+from tests.golden_cases import (C51_CASES, DQN_CPE_CASES, PDQN_CASES, QRDQN_CASES, _c51_kwargs,
+                                _dqn_kwargs)
 
 TOL = 1e-5
 f64 = torch.float64

@@ -27,7 +27,7 @@ import torch
 from oracle import heads_fp64 as H
 from reagent_b200 import _lib
 from tests import golden_util as G
-from tests.test_loss_reduction_gpu import _call, _set_ws, _ws
+from tests.kernel_util import _call, _set_ws, _ws
 
 pytestmark = pytest.mark.gpu
 

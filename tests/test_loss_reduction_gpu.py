@@ -9,15 +9,14 @@ reduces them in one of two fixed orders (rb200_common.cuh, DESIGN.md section 3):
             qr_head_kernel, bc_xent_head_kernel).
 Each test runs one kernel once, reads back the partials it wrote, and requires the loss bits to
 equal a float32 restatement of that kernel's order and final arithmetic."""
-import ctypes as C
 
 import numpy as np
 import pytest
 import torch
 
 from reagent_b200 import _lib
-from tests.test_actor_critic_gpu import _pbatch
-from tests.test_dqn_gpu import _assert_k2, _build_trainer, _rlt_batch, _select_k2
+from tests.builders import _assert_k2, _build_trainer, _pbatch, _rlt_batch, _select_k2
+from tests.kernel_util import _call, _set_ws, _ws
 
 pytestmark = pytest.mark.gpu
 f32 = np.float32
@@ -80,22 +79,6 @@ def _capture(monkeypatch, name, arg_index, fields):
 
     monkeypatch.setattr(lib, name, wrapped)
     return seen
-
-
-def _call(fn, a):
-    _lib.check(getattr(_lib.lib(), fn)(C.byref(a), _lib.cur_stream()), fn)
-    torch.cuda.synchronize()
-
-
-def _ws(n_partials, n_loss=1):
-    return dict(partials=torch.full((n_partials,), float("nan"), device="cuda"),
-                loss=torch.zeros(n_loss, device="cuda"),
-                counter=torch.zeros(1, dtype=torch.int32, device="cuda"))
-
-
-def _set_ws(a, ws):
-    a.loss_partials, a.loss, a.tile_counter = (ws["partials"].data_ptr(), ws["loss"].data_ptr(),
-                                               ws["counter"].data_ptr())
 
 
 def _onehot(B, A, gen):

@@ -5,24 +5,9 @@ import torch
 
 from oracle import td_oracle as O
 from tests import golden_util as G
-
-DQN_CASES = ["dqn_huber_double", "dqn_mse_single_masked", "dqn_sarsa", "dqn_multistep_boost",
-             "dqn_timediff_odd_dims", "dqn_dueling_double", "dqn_dueling_mse_masked",
-             "dqn_cartpole_config0"]
-
-
-def _dqn_kwargs(meta, batch):
-    kw = dict(double_q=meta["double_q"], maxq=meta["maxq"], loss=meta["loss"])
-    if meta["multi_steps"] is not None:
-        kw["discount_src"] = batch["step"]
-    elif meta["time_diff"]:
-        kw["discount_src"] = batch["time_diff"]
-    if meta["boost"]:
-        rb = torch.zeros(1, meta["A"])
-        for k, v in meta["boost"].items():
-            rb[0, int(k)] = v
-        kw["reward_boost"] = rb
-    return kw
+from tests.golden_cases import (C51_CASES, DQN_CASES, DQN_CPE_CASES, PDQN_CASES, QRDQN_CASES,
+                                SAC_CASES, TD3_CASES, _c51_kwargs, _dqn_kwargs)
+from tests.golden_util import _cmp_losses, _cmp_net
 
 
 @pytest.mark.parametrize("name", DQN_CASES)
@@ -90,24 +75,6 @@ def test_replay_oracle_matches_reference(name):
 # ---------------------------------------------------------------------------
 # SAC / TD3 restatements vs the reference trainers
 # ---------------------------------------------------------------------------
-SAC_CASES = ["sac_twin_alpha", "sac_single_fixed_alpha", "sac_twin_odd_dims"]
-TD3_CASES = ["td3_twin", "td3_single"]
-
-
-def _cmp_net(net, arrays, prefix, tol):
-    for i in range(len(net["W"])):
-        assert G.rel_err(net["W"][i], arrays[f"{prefix}.W{i}"]) < tol, f"{prefix}.W{i}"
-        assert G.rel_err(net["b"][i], arrays[f"{prefix}.b{i}"]) < tol, f"{prefix}.b{i}"
-
-
-def _cmp_losses(got, want, tol):
-    import numpy as np
-
-    for g, w in zip(got, want):
-        if g is None:
-            assert np.isnan(w)
-        else:
-            assert abs(g - w) <= tol * max(1.0, abs(w)), (got, want)
 
 
 @pytest.mark.parametrize("name", SAC_CASES)
@@ -165,7 +132,6 @@ def test_td3_oracle_matches_reference(name):
         _cmp_net(st.q2t, arrays, "q2t_N", 1e-5)
 
 
-QRDQN_CASES = ["qrdqn_double", "qrdqn_single_masked", "qrdqn_sarsa_multistep", "qrdqn_dueling"]
 # oracle-only for now: the dueling quantile head has no CUDA path yet (SURVEY M6 / config 3 note)
 QRDQN_ORACLE_ONLY = []
 
@@ -266,9 +232,6 @@ def test_replay_oracle_plus_inputmaker_formulas_match_reference(name):
             assert np.array_equal(eye[ob["next_action"]] * (~term)[:, None], arrays[pre + "next_action"])
 
 
-DQN_CPE_CASES = ["dqn_cpe_huber", "dqn_cpe_mse_sarsa_multistep"]
-
-
 @pytest.mark.parametrize("name", DQN_CPE_CASES)
 def test_dqn_cpe_oracle_matches_reference(name):
     """CPE heads (dqn_trainer_base.py:332-452): the oracle's reward / CPE q-value losses,
@@ -306,10 +269,6 @@ def test_dqn_cpe_oracle_matches_reference(name):
             assert G.rel_err(ps[2 * i + 1], b) < 1e-6, (prefix, i)
 
 
-PDQN_CASES = ["pdqn_double_mse", "pdqn_sarsa_huber_reward", "pdqn_single_multistep"]
-C51_CASES = ["c51_double", "c51_single_masked_boost", "c51_sarsa_multistep"]
-
-
 @pytest.mark.parametrize("name", PDQN_CASES)
 def test_pdqn_oracle_matches_reference(name):
     arrays, meta = G.load(name)
@@ -335,19 +294,6 @@ def test_pdqn_oracle_matches_reference(name):
         ps = O.net_params(net)
         for i, (w, b) in enumerate(G.net_pairs(arrays, prefix)):
             assert G.rel_err(ps[2 * i], w) < 1e-6 and G.rel_err(ps[2 * i + 1], b) < 1e-6, (prefix, i)
-
-
-def _c51_kwargs(meta, batch):
-    kw = dict(num_atoms=meta["N"], qmin=meta["qmin"], qmax=meta["qmax"], double_q=meta["double_q"],
-              maxq=meta["maxq"])
-    if meta["multi_steps"] is not None:
-        kw["discount_src"] = batch["step"]
-    if meta["boost"]:
-        rb = torch.zeros(1, meta["A"])
-        for k, v in meta["boost"].items():
-            rb[0, int(k)] = v
-        kw["reward_boost"] = rb
-    return kw
 
 
 @pytest.mark.parametrize("name", C51_CASES)

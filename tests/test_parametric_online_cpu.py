@@ -5,6 +5,7 @@ import ctypes as C
 
 import pytest
 import torch
+from tests.golden_cases import CARTPOLE_CASES, INPUTMAKER_CASES, cartpole_batch
 
 
 def test_parametric_dqn_manager_fields():
@@ -83,9 +84,6 @@ def test_tiled_forward_argument_checks():
 # the oracle restatements pinned against the reference's goldens
 # (oracle/make_parametric_golden.py)
 # ---------------------------------------------------------------------------
-INPUTMAKER_CASES = ["inputmaker_parametric_uniform_terminal", "inputmaker_parametric_h3_wrap",
-                    "inputmaker_parametric_masks_logprob", "inputmaker_parametric_per"]
-CARTPOLE_CASES = ["pdqn_adamw_amsgrad_cartpole", "pdqn_sarsa_adam_cartpole"]
 
 
 @pytest.mark.parametrize("name", INPUTMAKER_CASES)
@@ -132,13 +130,6 @@ def test_replay_oracle_plus_parametric_inputmaker_match_reference(name):
         lp = torch.from_numpy(np.asarray(ob["log_prob"], dtype=np.float32))
         assert np.array_equal(lp.exp().numpy().reshape(-1),
                               arrays[pre + "action_probability"].reshape(-1))
-
-
-def cartpole_batch(arrays, it, device="cpu"):
-    """The batch of update `it` of a make_parametric_golden.py CartPole case."""
-    pre = f"batch{it}."
-    return {k[len(pre):]: torch.from_numpy(v.copy()).to(device)
-            for k, v in arrays.items() if k.startswith(pre)}
 
 
 @pytest.mark.parametrize("name", CARTPOLE_CASES)

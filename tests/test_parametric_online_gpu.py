@@ -12,7 +12,8 @@ import pytest
 import torch
 
 from tests import golden_util as G
-from tests.test_oracle_golden import PDQN_CASES
+from tests.online_step import drawn_indices, online_steps
+from tests.golden_cases import CARTPOLE_CASES, INPUTMAKER_CASES, PDQN_CASES, cartpole_batch
 
 pytestmark = pytest.mark.gpu
 
@@ -556,19 +557,9 @@ def test_online_device_step_equals_eager_and_host_replica():
         random.seed(5)
         fused = FusedDqnStep(t, rb, B_ON, rng="device", online=True)
         losses, idx = [], []
-        for i in range(30):
-            tr = {k: v[i] for k, v in extra.items()}
-            if captured:
-                lh = fused.step(tr)
-                torch.cuda.current_stream().synchronize()
-                losses.append(float(lh[0]))
-            else:
-                fused.dr.stage(0, 0, **tr)
-                fused.dr.launch_add(1, slot=0)
-                losses.append(float(fused._one_update(None)))
-            idx.append(fused._idx_buf[0].cpu().numpy().copy())
-        torch.cuda.synchronize()
-        fused.dr.raise_if_failed()
+        for loss in online_steps(fused, extra, 30, captured):
+            losses.append(loss)
+            idx.append(drawn_indices(fused))
         runs.append((losses, idx, _trainer_state(t)))
     (l0, i0, p0), (l1, i1, p1) = runs
     assert l0 == l1 and all(np.isfinite(l0))
@@ -601,7 +592,6 @@ def test_online_step_refuses_per_and_shards():
 # ---------------------------------------------------------------------------
 # against the reference's goldens (oracle/make_parametric_golden.py)
 # ---------------------------------------------------------------------------
-from tests.test_parametric_online_cpu import CARTPOLE_CASES, INPUTMAKER_CASES, cartpole_batch  # noqa: E402
 
 
 def _golden_buffer(arrays, meta, bulk):

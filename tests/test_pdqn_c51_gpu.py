@@ -5,7 +5,7 @@ import pytest
 import torch
 
 from tests import golden_util as G
-from tests.test_oracle_golden import C51_CASES, PDQN_CASES
+from tests.golden_cases import C51_CASES, PDQN_CASES
 
 pytestmark = pytest.mark.gpu
 TOL = 1e-5

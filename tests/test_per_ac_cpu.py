@@ -10,7 +10,8 @@ import torch
 from oracle import per_ac_oracle as PA
 from oracle import td_oracle as O
 from tests import golden_util as G
-from tests.test_oracle_golden import SAC_CASES, TD3_CASES, _cmp_losses, _cmp_net
+from tests.golden_cases import SAC_CASES, TD3_CASES
+from tests.golden_util import _cmp_losses, _cmp_net
 
 
 @pytest.mark.parametrize("name", SAC_CASES)

@@ -11,10 +11,12 @@ import torch
 from oracle import per_ac_oracle as PA
 from oracle import td_oracle as O
 from tests import golden_util as G
-from tests.test_actor_critic_gpu import (_adam_close, _build_sac, _build_td3, _inject,
-                                         _net_arrays, _pbatch, _rand_net)
-from tests.test_oracle_golden import SAC_CASES, TD3_CASES
-from tests.test_per_gpu import _filled_heap, _ulps
+from tests.online_step import (assert_captured_equals_eager, assert_matches_host_replica,
+                               assert_nan_reward_raises, bench_setup, filled_heap, host_add,
+                               rows_update, transition_stream, tree, ulps)
+from tests.builders import _build_sac, _build_td3, _inject, _net_arrays, _pbatch, _rand_net
+from tests.golden_cases import SAC_CASES, TD3_CASES
+from tests.golden_util import _adam_close
 
 pytestmark = pytest.mark.gpu
 TOL = 1e-5
@@ -203,15 +205,6 @@ def test_weighted_update_at_config_shapes(algo):
             _adam_close(seq[0].weight, st.actor_t["W"][i], meta)
 
 
-def _rows_update(heap_d, depth, idx, row, per, p, dm, st):
-    from reagent_b200 import _lib
-
-    _lib.check(_lib.lib().rb200_per_priority_update_rows(
-        heap_d.data_ptr(), depth, idx.data_ptr(), row.data_ptr(), idx.numel(), 1.0, per.alpha,
-        per.eps, p.data_ptr(), dm.data_ptr(), st.data_ptr(), _lib.cur_stream()))
-    torch.cuda.synchronize()
-
-
 @pytest.mark.parametrize("name", SAC_CASES + TD3_CASES + ["sac_config4", "td3_config5"])
 def test_td_error_and_priorities(name):
     """td_error_out is torch's max(|q1 - y|, |q2 - y|) on the kernel's own outputs, bit for bit,
@@ -238,16 +231,16 @@ def test_td_error_and_priorities(name):
     n = meta["B"]
     rng = np.random.RandomState(n)
     cap = 1 << 12
-    heap, depth, _ = _filled_heap(cap, rng)
+    heap, depth, _ = filled_heap(cap, rng)
     heap_d = torch.from_numpy(heap).cuda()
     idx = torch.from_numpy(rng.randint(0, cap, n).astype(np.int64)).cuda()
     p = torch.empty(n, dtype=torch.float64, device="cuda")
     st = torch.zeros(2, dtype=torch.int32, device="cuda")
     dm = torch.tensor([0.0], dtype=torch.float64, device="cuda")
-    _rows_update(heap_d, depth, idx, ws["td_error"], per, p, dm, st)
+    rows_update(heap_d, depth, idx, ws["td_error"], 1.0, per, p, dm, st)
     pw = PA.twin_td_priorities(q1.cpu().numpy(), ws["q2_value"].cpu().numpy() if meta["twin"]
                                else None, y.cpu().numpy(), per.alpha, per.eps)
-    assert int(st[0]) == 0 and _ulps(p.cpu().numpy(), pw).max() <= 4
+    assert int(st[0]) == 0 and ulps(p.cpu().numpy(), pw).max() <= 4
 
 
 # ---------------------------------------------------------------------------
@@ -259,29 +252,8 @@ def _cfg(algo):
     return dict(bench.CONFIGS[4 if algo == "sac" else 5], cap=4096, B=256)
 
 
-def _stream(n, cfg, seed):
-    import bench
-
-    return bench.synth_stream(n, seed, cfg)
-
-
-def _setup(algo, base, seed=3):
-    import bench
-    from reagent_b200.replay_memory import PrioritizedReplayBuffer
-
-    cfg = _cfg(algo)
-    rb = PrioritizedReplayBuffer(stack_size=1, replay_capacity=cfg["cap"], batch_size=cfg["B"])
-    rb.add_batch(**base)
-    return rb, bench.build_trainer(cfg, torch.device("cuda"), seed=seed)
-
-
 def _bounds(cfg):
     return -np.ones(cfg["A"], np.float32), np.ones(cfg["A"], np.float32)
-
-
-def _host_add(rb, tr):
-    rb.add(**{k: (v.item() if np.ndim(v) == 0 and hasattr(v, "item") else v)
-              for k, v in tr.items()})
 
 
 class _Noise:
@@ -307,42 +279,21 @@ def test_online_per_loop_equals_host_replica(algo):
     cfg = _cfg(algo)
     B = cfg["B"]
     low, high = _bounds(cfg)
-    base = _stream(3000, cfg, 3)
-    extra = _stream(40, cfg, 4)
+    base = transition_stream(3000, 3, cfg=cfg)
     per = PrioritizedUpdate(alpha=0.6, beta0=0.4, beta_updates=20, eps=1e-6)
-    rb_d, t_d = _setup(algo, base)
-    rb_h, _ = _setup(algo, base)
-    random.seed(77)
-    saved = random.getstate()
-    fused = FusedPolicyStep(t_d, rb_d, B, low, high, online=True, per=per)
-    random.setstate(saved)
+    rb_d, t_d = bench_setup(cfg, base)
+    rb_h, _ = bench_setup(cfg, base)
 
-    def replica_update():
-        torch.cuda.synchronize()
-        idx_d = fused._idx_buf[0].cpu().numpy().copy()
-        idx_h = rb_h.sample_policy_network_batch(B, low, high).indices.cpu().numpy().reshape(-1)
-        assert np.array_equal(idx_h, idx_d)
-        pr = fused.priorities.cpu().numpy()
-        ws = t_d._ws
-        want = PA.twin_td_priorities(ws["q1_value"].cpu().numpy(), ws["q2_value"].cpu().numpy(),
+    def twin_critic_priorities(t):
+        ws = t._ws
+        return PA.twin_td_priorities(ws["q1_value"].cpu().numpy(), ws["q2_value"].cpu().numpy(),
                                      ws["td_target"].cpu().numpy(), per.alpha, per.eps)
-        assert _ulps(pr, want).max() <= 4
-        rb_h.set_priority(idx_h.astype(np.int32), pr)
 
-    replica_update()  # the constructor's warm-up update
-    for i in range(30):
-        tr = {k: v[i] for k, v in extra.items()}
-        if i % 3 == 1:
-            del tr["priority"]
-        fused.step(tr)
-        host_tr = dict(tr)
-        host_tr.setdefault("priority", rb_h.sum_tree.max_recorded_priority)
-        _host_add(rb_h, host_tr)
-        replica_update()
+    assert_matches_host_replica(
+        lambda: FusedPolicyStep(t_d, rb_d, B, low, high, online=True, per=per), rb_h,
+        transition_stream(40, 4, cfg=cfg), lambda rb: rb.sample_policy_network_batch(B, low, high),
+        twin_critic_priorities)
     assert t_d.all_batches_processed == 31
-    fused.dr.sync_to_host()
-    assert np.array_equal(rb_d.sum_tree.heap, rb_h.sum_tree.heap)
-    assert rb_d.sum_tree.max_recorded_priority == rb_h.sum_tree.max_recorded_priority
 
 
 @pytest.mark.parametrize("with_per", [False, True])
@@ -356,39 +307,20 @@ def test_online_captured_equals_eager(algo, with_per):
 
     cfg = _cfg(algo)
     low, high = _bounds(cfg)
-    base = _stream(3000, cfg, 7)
-    extra = _stream(7, cfg, 8)
+    base = transition_stream(3000, 7, cfg=cfg)
     per = PrioritizedUpdate(alpha=0.6, beta0=0.4, beta_updates=10, eps=1e-6) if with_per else None
-    runs = []
-    for captured in (True, False):
-        rb, t = _setup(algo, base)
+
+    def setup():
+        rb, t = bench_setup(cfg, base)
         noise = _Noise(t, cfg["B"], cfg["A"], 11)
         random.seed(5)
-        fused = FusedPolicyStep(t, rb, cfg["B"], low, high, online=True, per=per)
-        losses = []
-        for i in range(7):
-            noise.refill()
-            tr = {k: v[i] for k, v in extra.items()}
-            if with_per and i % 2:
-                del tr["priority"]
-            if captured:
-                out = fused.step(tr)
-                torch.cuda.current_stream().synchronize()
-                losses.append(out.clone())
-            else:
-                fused.dr.stage(0, 0, priority_from_max=with_per, **tr)
-                fused.dr.launch_add(1, slot=0, priority_from_max=with_per)
-                losses.append(fused._one_update(None).cpu())
-        torch.cuda.synchronize()
-        fused.dr.raise_if_failed()
-        runs.append((losses, _state(t), fused.dr.tree.clone(), float(fused.dr.max_priority),
-                     t.all_batches_processed))
-    (l0, s0, h0, m0, n0), (l1, s1, h1, m1, n1) = runs
-    assert all(torch.equal(a, b) for a, b in zip(l0, l1)) and all(
-        bool(torch.isfinite(a).all()) for a in l0)
-    assert all(torch.equal(a, b) for a, b in zip(s0, s1))
-    assert torch.equal(h0, h1) and m0 == m1
-    assert n0 == n1 == 8
+        return FusedPolicyStep(t, rb, cfg["B"], low, high, online=True, per=per), noise.refill
+
+    snap = assert_captured_equals_eager(
+        setup, transition_stream(7, 8, cfg=cfg), 7,
+        lambda f: [_state(f.trainer), tree(f), f.trainer.all_batches_processed],
+        drop_priority=(lambda i: i % 2) if with_per else None, scalar_loss=False)
+    assert snap[-1] == 8
 
 
 @pytest.mark.parametrize("algo", ["sac", "td3"])
@@ -400,10 +332,10 @@ def test_online_step_equals_train_batch_on_the_drawn_indices(algo):
     cfg = _cfg(algo)
     B = cfg["B"]
     low, high = _bounds(cfg)
-    base = _stream(3000, cfg, 12)
-    extra = _stream(3, cfg, 13)
-    rb1, t1 = _setup(algo, base)
-    rb2, t2 = _setup(algo, base)
+    base = transition_stream(3000, 12, cfg=cfg)
+    extra = transition_stream(3, 13, cfg=cfg)
+    rb1, t1 = bench_setup(cfg, base)
+    rb2, t2 = bench_setup(cfg, base)
     n1, n2 = _Noise(t1, B, cfg["A"], 21), _Noise(t2, B, cfg["A"], 21)
     random.seed(9)
     fused = FusedPolicyStep(t1, rb1, B, low, high, online=True)
@@ -416,7 +348,7 @@ def test_online_step_equals_train_batch_on_the_drawn_indices(algo):
         tr = {k: v[i] for k, v in extra.items()}
         out = fused.step(tr)
         torch.cuda.current_stream().synchronize()
-        _host_add(rb2, tr)
+        host_add(rb2, tr)
         idx = fused._idx_buf[0].clone()
         closs, _ = t2.train_batch(rb2.sample_policy_network_batch(B, low, high, indices=idx), i + 1)
         assert torch.equal(out, closs.cpu())
@@ -430,15 +362,7 @@ def test_online_per_nan_reward_raises(algo):
 
     cfg = _cfg(algo)
     low, high = _bounds(cfg)
-    rb, t = _setup(algo, _stream(3000, cfg, 5))
+    rb, t = bench_setup(cfg, transition_stream(3000, 5, cfg=cfg))
     random.seed(1)
     fused = FusedPolicyStep(t, rb, cfg["B"], low, high, online=True, per=PrioritizedUpdate())
-    extra = _stream(10, cfg, 6)
-    bad = {k: v[0] for k, v in extra.items()}
-    bad["reward"] = np.float32("nan")
-    bad["priority"] = 1e9  # drawn by the next update
-    with pytest.raises(FloatingPointError):
-        fused.step(bad)
-        for i in range(1, 10):
-            fused.step({k: v[i] for k, v in extra.items()})
-    torch.cuda.synchronize()
+    assert_nan_reward_raises(fused, transition_stream(10, 6, cfg=cfg))

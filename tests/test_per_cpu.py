@@ -9,8 +9,7 @@ import torch
 from oracle import per_oracle as P
 from oracle import td_oracle as O
 from tests import golden_util as G
-from tests.test_bcq_cpu import BCQ_DQN_CASES
-from tests.test_oracle_golden import DQN_CASES, _dqn_kwargs
+from tests.golden_cases import BCQ_DQN_CASES, DQN_CASES, _dqn_kwargs
 
 
 @pytest.mark.parametrize("name", DQN_CASES)

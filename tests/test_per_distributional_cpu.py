@@ -11,7 +11,7 @@ import torch
 from oracle import per_distributional_oracle as PD
 from oracle import td_oracle as O
 from tests import golden_util as G
-from tests.test_oracle_golden import C51_CASES, QRDQN_CASES, _c51_kwargs
+from tests.golden_cases import C51_CASES, QRDQN_CASES, _c51_kwargs
 
 
 def _qrdqn_kwargs(meta, batch):

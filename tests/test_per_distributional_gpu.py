@@ -11,10 +11,11 @@ import torch
 from oracle import per_distributional_oracle as PD
 from oracle import td_oracle as O
 from tests import golden_util as G
-from tests.test_oracle_golden import C51_CASES, QRDQN_CASES, _c51_kwargs
-from tests.test_per_gpu import _filled_heap, _stream, _ulps
-from tests.test_qrdqn_gpu import _batch
-from tests.test_qrdqn_gpu import _build as _build_qr
+from tests.online_step import (assert_captured_equals_eager, assert_matches_host_replica,
+                               assert_nan_reward_raises, bench_setup, filled_heap, params,
+                               prioritized_buffer, rows_update, transition_stream, tree, ulps)
+from tests.builders import _batch, _build_qr
+from tests.golden_cases import C51_CASES, QRDQN_CASES, _c51_kwargs
 
 pytestmark = pytest.mark.gpu
 TOL = 1e-5
@@ -159,15 +160,6 @@ def test_importance_weights_are_validated():
 # ---------------------------------------------------------------------------
 # row-loss priorities
 # ---------------------------------------------------------------------------
-def _rows_update(heap_d, depth, idx, row_loss, D, per, p, dm, st):
-    from reagent_b200 import _lib
-
-    _lib.check(_lib.lib().rb200_per_priority_update_rows(
-        heap_d.data_ptr(), depth, idx.data_ptr(), row_loss.data_ptr(), idx.numel(), float(D),
-        per.alpha, per.eps, p.data_ptr(), dm.data_ptr(), st.data_ptr(), _lib.cur_stream()))
-    torch.cuda.synchronize()
-
-
 @pytest.mark.parametrize("name", ["qrdqn_double", "qrdqn_sarsa_multistep", "c51_double",
                                   "c51_single_masked_boost", "config3_like"])
 def test_row_priorities_match_numpy_and_host_tree(name):
@@ -189,7 +181,7 @@ def test_row_priorities_match_numpy_and_host_tree(name):
     n = row_loss.numel()
     rng = np.random.RandomState(n)
     cap = 1 << 14
-    heap, depth, _ = _filled_heap(cap, rng)
+    heap, depth, _ = filled_heap(cap, rng)
     heap_d = torch.from_numpy(heap).cuda()
     ii = rng.randint(0, cap, n).astype(np.int64)
     ii[::7] = ii[0]  # repeated leaves
@@ -197,10 +189,10 @@ def test_row_priorities_match_numpy_and_host_tree(name):
     p = torch.empty(n, dtype=torch.float64, device="cuda")
     st = torch.zeros(2, dtype=torch.int32, device="cuda")
     dm = torch.tensor([0.0], dtype=torch.float64, device="cuda")
-    _rows_update(heap_d, depth, idx, row_loss, D, per, p, dm, st)
+    rows_update(heap_d, depth, idx, row_loss, D, per, p, dm, st)
     want = PD.row_loss_priorities(row_loss.cpu().numpy(), D, per.alpha, per.eps)
     got = p.cpu().numpy()
-    assert int(st[0]) == 0 and _ulps(got, want).max() <= 4
+    assert int(st[0]) == 0 and ulps(got, want).max() <= 4
     h, hm = heap.copy(), np.array([0.0])
     _lib.lib().rb200_sumtree_set_host(h.ctypes.data, depth, ii.ctypes.data, got.ctypes.data, n,
                                       hm.ctypes.data)
@@ -208,7 +200,7 @@ def test_row_priorities_match_numpy_and_host_tree(name):
     bad = row_loss.clone()
     bad[n // 2] = float("nan")
     before, mbefore = heap_d.clone(), dm.clone()
-    _rows_update(heap_d, depth, idx, bad, D, per, p, dm, st)
+    rows_update(heap_d, depth, idx, bad, D, per, p, dm, st)
     assert int(st[0]) == 3 and torch.equal(heap_d, before) and torch.equal(dm, mbefore)
 
 
@@ -226,14 +218,12 @@ def _setup(kind, base, seed=3):
     from reagent_b200.core.parameters import RLParameters
     from reagent_b200.models import CategoricalDQN, FullyConnectedDQN
     from reagent_b200.optimizer import Optimizer__Union
-    from reagent_b200.replay_memory import PrioritizedReplayBuffer
     from reagent_b200.training import C51Trainer
 
     cfg = _cfg(kind)
-    rb = PrioritizedReplayBuffer(stack_size=1, replay_capacity=cfg["cap"], batch_size=cfg["B"])
-    rb.add_batch(**base)
     if kind == "qrdqn":
-        return rb, bench.build_trainer(cfg, torch.device("cuda"), seed=seed)
+        return bench_setup(cfg, base, seed)
+    rb = prioritized_buffer(cfg, base)
     torch.manual_seed(seed)
     S, A, N = cfg["S"], cfg["A"], cfg["N"]
     q = CategoricalDQN(FullyConnectedDQN(S, A, cfg["sizes"], bench.ACTS, num_atoms=N),
@@ -248,48 +238,23 @@ def _setup(kind, base, seed=3):
 
 @pytest.mark.parametrize("kind", ["qrdqn", "c51"])
 def test_online_per_loop_equals_host_replica(kind):
+    """The online loop against a host replica; each update's priorities are its rows' own
+    losses."""
     from reagent_b200.replay_memory import PrioritizedUpdate
     from reagent_b200.training.fused_step import FusedDqnStep
 
     cfg = _cfg(kind)
     S, A, B = cfg["S"], cfg["A"], cfg["B"]
-    base = _stream(3000, S, A, 3)
-    extra = _stream(40, S, A, 4)
+    base = transition_stream(3000, 3, S, A)
     per = PrioritizedUpdate(alpha=0.6, beta0=0.4, beta_updates=20, eps=1e-6)
     rb_d, t_d = _setup(kind, base)
     rb_h, _ = _setup(kind, base)
-    random.seed(77)
-    saved = random.getstate()
-    fused = FusedDqnStep(t_d, rb_d, B, rng="device", online=True, per=per)
-    random.setstate(saved)
     D = cfg["N"] ** 2 if kind == "qrdqn" else 1
-
-    def replica_update():
-        torch.cuda.synchronize()
-        idx_d = fused._idx_buf[0].cpu().numpy().copy()
-        idx_h = rb_h.sample_discrete_dqn_batch(B, A).indices.cpu().numpy().reshape(-1)
-        assert np.array_equal(idx_h, idx_d)
-        pr = fused.priorities.cpu().numpy()
-        # the priorities are the rows' own losses of this update
-        want = PD.row_loss_priorities(t_d._ws["loss_partials"].cpu().numpy(), D, per.alpha,
-                                      per.eps)
-        assert _ulps(pr, want).max() <= 4
-        rb_h.set_priority(idx_h.astype(np.int32), pr)
-
-    replica_update()  # the constructor's warm-up update
-    for i in range(30):
-        tr = {k: v[i] for k, v in extra.items()}
-        if i % 3 == 1:
-            del tr["priority"]
-        fused.step(tr)
-        host_tr = dict(tr)
-        host_tr.setdefault("priority", rb_h.sum_tree.max_recorded_priority)
-        rb_h.add(**{k: (v.item() if np.ndim(v) == 0 and hasattr(v, "item") else v)
-                    for k, v in host_tr.items()})
-        replica_update()
-    fused.dr.sync_to_host()
-    assert np.array_equal(rb_d.sum_tree.heap, rb_h.sum_tree.heap)
-    assert rb_d.sum_tree.max_recorded_priority == rb_h.sum_tree.max_recorded_priority
+    assert_matches_host_replica(
+        lambda: FusedDqnStep(t_d, rb_d, B, rng="device", online=True, per=per), rb_h,
+        transition_stream(40, 4, S, A), lambda rb: rb.sample_discrete_dqn_batch(B, A),
+        lambda t: PD.row_loss_priorities(t._ws["loss_partials"].cpu().numpy(), D, per.alpha,
+                                         per.eps))
 
 
 @pytest.mark.parametrize("with_per", [False, True])
@@ -302,37 +267,18 @@ def test_online_captured_equals_eager(kind, with_per):
     from reagent_b200.training.fused_step import FusedDqnStep
 
     cfg = _cfg(kind)
-    base = _stream(3000, cfg["S"], cfg["A"], 7)
-    extra = _stream(12, cfg["S"], cfg["A"], 8)
+    base = transition_stream(3000, 7, cfg["S"], cfg["A"])
     per = PrioritizedUpdate(alpha=0.6, beta0=0.4, beta_updates=10, eps=1e-6) if with_per else None
-    runs = []
-    for captured in (True, False):
+
+    def setup():
         rb, t = _setup(kind, base)
         random.seed(5)
-        fused = FusedDqnStep(t, rb, cfg["B"], rng="device", online=True, per=per)
-        losses = []
-        for i in range(12):
-            tr = {k: v[i] for k, v in extra.items()}
-            if with_per and i % 2:
-                del tr["priority"]
-            if captured:
-                losses.append(fused.step(tr))
-                torch.cuda.current_stream().synchronize()
-                losses[-1] = float(losses[-1][0])
-            else:
-                fused.dr.stage(0, 0, priority_from_max=with_per, **tr)
-                fused.dr.launch_add(1, slot=0, priority_from_max=with_per)
-                losses.append(float(fused._one_update(None)))
-        torch.cuda.synchronize()
-        fused.dr.raise_if_failed()
-        runs.append((losses, [p.detach().clone() for p in t.q_network.parameters()],
-                     [p.detach().clone() for p in t.q_network_target.parameters()],
-                     fused.dr.tree.clone(), float(fused.dr.max_priority)))
-    (l0, p0, t0, h0, m0), (l1, p1, t1, h1, m1) = runs
-    assert l0 == l1 and all(np.isfinite(l0))
-    assert all(torch.equal(a, b) for a, b in zip(p0, p1))
-    assert all(torch.equal(a, b) for a, b in zip(t0, t1))
-    assert torch.equal(h0, h1) and m0 == m1
+        return FusedDqnStep(t, rb, cfg["B"], rng="device", online=True, per=per), None
+
+    assert_captured_equals_eager(
+        setup, transition_stream(12, 8, cfg["S"], cfg["A"]), 12,
+        lambda f: [params(f.trainer.q_network), params(f.trainer.q_network_target), tree(f)],
+        drop_priority=(lambda i: i % 2) if with_per else None)
 
 
 def test_online_per_qrdqn_nan_reward_raises():
@@ -350,18 +296,10 @@ def _online_per_nan_reward_raises(kind):
     from reagent_b200.training.fused_step import FusedDqnStep
 
     cfg = _cfg(kind)
-    rb, t = _setup(kind, _stream(3000, cfg["S"], cfg["A"], 5))
+    rb, t = _setup(kind, transition_stream(3000, 5, cfg["S"], cfg["A"]))
     random.seed(1)
     fused = FusedDqnStep(t, rb, cfg["B"], rng="device", online=True, per=PrioritizedUpdate())
-    extra = _stream(10, cfg["S"], cfg["A"], 6)
-    bad = {k: v[0] for k, v in extra.items()}
-    bad["reward"] = np.float32("nan")
-    bad["priority"] = 1e9  # drawn by the next update
-    with pytest.raises(FloatingPointError):
-        fused.step(bad)
-        for i in range(1, 10):
-            fused.step({k: v[i] for k, v in extra.items()})
-    torch.cuda.synchronize()
+    assert_nan_reward_raises(fused, transition_stream(10, 6, cfg["S"], cfg["A"]))
 
 
 def test_online_qrdqn_step_after_load_state_dict():
@@ -370,10 +308,10 @@ def test_online_qrdqn_step_after_load_state_dict():
     from reagent_b200.training.fused_step import FusedDqnStep
 
     cfg = _cfg("qrdqn")
-    rb, t = _setup("qrdqn", _stream(3000, cfg["S"], cfg["A"], 9))
+    rb, t = _setup("qrdqn", transition_stream(3000, 9, cfg["S"], cfg["A"]))
     random.seed(2)
     fused = FusedDqnStep(t, rb, cfg["B"], rng="device", online=True)
-    extra = _stream(3, cfg["S"], cfg["A"], 10)
+    extra = transition_stream(3, 10, cfg["S"], cfg["A"])
     fused.step({k: v[0] for k, v in extra.items()})
     torch.cuda.synchronize()
     sd = {k: v.clone() for k, v in t.q_network.state_dict().items()}

@@ -11,13 +11,14 @@ from oracle import bcq_oracle as BO
 from oracle import per_oracle as P
 from oracle import td_oracle as O
 from tests import golden_util as G
-from tests.test_bcq_cpu import BCQ_DQN_CASES
-from tests.test_bcq_gpu import _build as _build_bcq
-from tests.test_bcq_gpu import _golden_batch
-from tests.test_dqn_gpu import (CONFIG2_DZ_TOL, CONFIG2_MAX_ADAM_OUTLIER_FRAC,
-                                CONFIG2_MAX_FLIPPED_ROWS, CPE_CASES, TOL, _assert_k2,
-                                _build_cpe_trainer, _build_trainer, _rlt_batch, _select_k2)
-from tests.test_oracle_golden import _dqn_kwargs
+from tests.online_step import (assert_captured_equals_eager, assert_matches_host_replica,
+                               assert_nan_reward_raises, bench_setup, filled_heap, params,
+                               transition_stream, tree, ulps)
+from tests.builders import (CONFIG2_DZ_TOL, CONFIG2_MAX_ADAM_OUTLIER_FRAC, CONFIG2_MAX_FLIPPED_ROWS,
+                            _assert_k2, _build_bcq, _build_cpe_trainer, _build_trainer,
+                            _golden_batch, _rlt_batch, _select_k2)
+from tests.golden_cases import BCQ_DQN_CASES, DQN_CPE_CASES, _dqn_kwargs
+from tests.golden_util import TOL
 
 pytestmark = pytest.mark.gpu
 K2_PATHS = ["tcgen05", "rows"]
@@ -45,7 +46,7 @@ def test_unit_weights_are_bit_identical_to_unweighted(path, monkeypatch):
 
 
 WEIGHTED_CASES = (["dqn_huber_double", "dqn_mse_single_masked", "dqn_multistep_boost",
-                   "dqn_timediff_odd_dims"] + BCQ_DQN_CASES + CPE_CASES)
+                   "dqn_timediff_odd_dims"] + BCQ_DQN_CASES + DQN_CPE_CASES)
 
 
 @pytest.mark.parametrize("path", K2_PATHS)
@@ -195,23 +196,6 @@ def test_weighted_config2_matches_oracle(path, monkeypatch):
 # ---------------------------------------------------------------------------
 # ordered batched SumTree.set
 # ---------------------------------------------------------------------------
-def _depth(cap):
-    return int(np.ceil(np.log2(cap))) if cap > 1 else 0
-
-
-def _filled_heap(cap, rng):
-    from reagent_b200 import _lib
-
-    depth = _depth(cap)
-    heap = np.zeros((1 << (depth + 1)) - 1)
-    idx = np.arange(cap, dtype=np.int64)
-    val = rng.uniform(0.0, 10.0, cap)
-    mx = np.array([1.0])
-    assert _lib.lib().rb200_sumtree_set_host(heap.ctypes.data, depth, idx.ctypes.data,
-                                             val.ctypes.data, cap, mx.ctypes.data) == 0
-    return heap, depth, mx
-
-
 def _both(heap, depth, mx, idx, val):
     """(host heap, host max, host rc), (device heap, device max, device status)"""
     from reagent_b200 import _lib
@@ -236,7 +220,7 @@ def _both(heap, depth, mx, idx, val):
 @pytest.mark.parametrize("n", [1, 2, 31, 32, 33, 4096, 20000])
 def test_batched_tree_update_is_bit_equal_to_sequential(n, cap):
     rng = np.random.RandomState(n * 7 + cap)
-    heap, depth, mx = _filled_heap(cap, rng)
+    heap, depth, mx = filled_heap(cap, rng)
     idx = rng.randint(0, cap, n)
     idx[::5] = idx[0]  # repeated leaves: the order of their sets matters
     val = rng.uniform(0.0, 50.0, n)
@@ -250,7 +234,7 @@ def test_batched_tree_update_is_bit_equal_to_sequential(n, cap):
 def test_batched_tree_update_edge_cases(case):
     rng = np.random.RandomState(11)
     cap, n = 1 << 14, 6000
-    heap, depth, mx = _filled_heap(cap, rng)
+    heap, depth, mx = filled_heap(cap, rng)
     idx = rng.randint(0, 3, n) * 977
     val = rng.uniform(0.0, 1e3, n)
     if case == "all_one_leaf":
@@ -269,11 +253,6 @@ def test_batched_tree_update_edge_cases(case):
 # ---------------------------------------------------------------------------
 # priority and weight kernels
 # ---------------------------------------------------------------------------
-def _ulps(a, b):
-    a, b = np.asarray(a, np.float64), np.asarray(b, np.float64)
-    return np.abs(a - b) / np.spacing(np.maximum(np.abs(a), np.abs(b)))
-
-
 @pytest.mark.parametrize("t_frac", [0.0, 0.5, 1.0, 3.0])
 def test_priority_and_weight_kernels_match_numpy(t_frac):
     from reagent_b200 import _lib
@@ -282,7 +261,7 @@ def test_priority_and_weight_kernels_match_numpy(t_frac):
     per = PrioritizedUpdate(alpha=0.6, beta0=0.4, beta_updates=1000, eps=1e-6)
     rng = np.random.RandomState(3)
     cap, B = 1 << 12, 4096
-    heap, depth, mx = _filled_heap(cap, rng)
+    heap, depth, mx = filled_heap(cap, rng)
     heap_d = torch.from_numpy(heap).cuda()
     idx = torch.from_numpy(rng.randint(0, cap, B).astype(np.int64)).cuda()
     zero_leaf = int(idx[7])
@@ -299,7 +278,7 @@ def test_priority_and_weight_kernels_match_numpy(t_frac):
     want = P.importance_weights(leaves, b)
     got = w64.cpu().numpy()
     assert np.all(got[leaves == 0.0] == 0.0) and (leaves == 0.0).any()
-    assert _ulps(got, want).max() <= 4
+    assert ulps(got, want).max() <= 4
     assert np.array_equal(w.cpu().numpy(), got.astype(np.float32))
     # priorities from the device's own TD errors
     td = torch.randn(B, device="cuda")
@@ -312,7 +291,7 @@ def test_priority_and_weight_kernels_match_numpy(t_frac):
                                              qs.data_ptr(), B, per.alpha, per.eps, p.data_ptr(),
                                              dm.data_ptr(), st.data_ptr(), _lib.cur_stream()))
     want_p = P.priorities(qs.cpu().numpy(), td.cpu().numpy(), per.alpha, per.eps)
-    assert int(st[0]) == 0 and _ulps(p.cpu().numpy(), want_p).max() <= 4
+    assert int(st[0]) == 0 and ulps(p.cpu().numpy(), want_p).max() <= 4
     # and the write-back is SumTree.set with exactly those values
     hm = np.array([0.0])
     ii = idx.cpu().numpy()
@@ -331,130 +310,65 @@ def test_priority_and_weight_kernels_match_numpy(t_frac):
 # ---------------------------------------------------------------------------
 # the online loop against a host replica
 # ---------------------------------------------------------------------------
-def _stream(n, S, A, seed):
-    rng = np.random.RandomState(seed)
-    return dict(observation=rng.randn(n, S).astype(np.float32),
-                action=rng.randint(0, A, n).astype(np.int64),
-                reward=rng.randn(n).astype(np.float32), terminal=rng.rand(n) < 0.05,
-                priority=rng.uniform(0.1, 10.0, n))
-
-
-def _setup(cfg, base):
+def _cfg():
     import bench
-    from reagent_b200.replay_memory import PrioritizedReplayBuffer
 
-    rb = PrioritizedReplayBuffer(stack_size=1, replay_capacity=cfg["cap"], batch_size=cfg["B"])
-    rb.add_batch(**base)
-    return rb, bench.build_trainer(cfg, torch.device("cuda"), seed=3)
+    return dict(bench.CONFIGS[2], cap=4096, B=256)
 
 
 def test_online_per_loop_equals_host_replica():
-    import bench
     from reagent_b200.replay_memory import PrioritizedUpdate
     from reagent_b200.training.fused_step import FusedDqnStep
 
-    cfg = dict(bench.CONFIGS[2], cap=4096, B=256)
+    cfg = _cfg()
     S, A, B = cfg["S"], cfg["A"], cfg["B"]
-    base = _stream(3000, S, A, 3)
-    extra = _stream(40, S, A, 4)
+    base = transition_stream(3000, 3, S, A)
     per = PrioritizedUpdate(alpha=0.6, beta0=0.4, beta_updates=20, eps=1e-6)
-    rb_d, t_d = _setup(cfg, base)
-    rb_h, _ = _setup(cfg, base)
-    random.seed(77)
-    saved = random.getstate()
-    fused = FusedDqnStep(t_d, rb_d, B, rng="device", online=True, per=per)
-    random.setstate(saved)
-
-    def replica_update():
-        torch.cuda.synchronize()
-        idx_d = fused._idx_buf[0].cpu().numpy().copy()
-        idx_h = rb_h.sample_discrete_dqn_batch(B, A).indices.cpu().numpy().reshape(-1)
-        assert np.array_equal(idx_h, idx_d)
-        rb_h.set_priority(idx_h.astype(np.int32), fused.priorities.cpu().numpy())
-
-    replica_update()  # the constructor's warm-up update
-    for i in range(30):
-        tr = {k: v[i] for k, v in extra.items()}
-        if i % 3 == 1:
-            del tr["priority"]
-        fused.step(tr)
-        host_tr = dict(tr)
-        host_tr.setdefault("priority", rb_h.sum_tree.max_recorded_priority)
-        rb_h.add(**{k: (v.item() if np.ndim(v) == 0 and hasattr(v, "item") else v)
-                    for k, v in host_tr.items()})
-        replica_update()
-    fused.dr.sync_to_host()
-    assert np.array_equal(rb_d.sum_tree.heap, rb_h.sum_tree.heap)
-    assert rb_d.sum_tree.max_recorded_priority == rb_h.sum_tree.max_recorded_priority
+    rb_d, t_d = bench_setup(cfg, base)
+    rb_h, _ = bench_setup(cfg, base)
+    assert_matches_host_replica(
+        lambda: FusedDqnStep(t_d, rb_d, B, rng="device", online=True, per=per), rb_h,
+        transition_stream(40, 4, S, A), lambda rb: rb.sample_discrete_dqn_batch(B, A))
 
 
 def test_online_per_captured_equals_eager():
     """The same online steps through graph replay and through eager launches of the same
     update from identical starting states: losses, parameters, tree and max priority agree bit
     for bit."""
-    import bench
     from reagent_b200.replay_memory import PrioritizedUpdate
     from reagent_b200.training.fused_step import FusedDqnStep
 
-    cfg = dict(bench.CONFIGS[2], cap=4096, B=256)
-    base = _stream(3000, cfg["S"], cfg["A"], 7)
-    extra = _stream(12, cfg["S"], cfg["A"], 8)
+    cfg = _cfg()
+    base = transition_stream(3000, 7, cfg["S"], cfg["A"])
     per = PrioritizedUpdate(alpha=0.6, beta0=0.4, beta_updates=10, eps=1e-6)
-    runs = []
-    for captured in (True, False):
-        rb, t = _setup(cfg, base)
+
+    def setup():
+        rb, t = bench_setup(cfg, base)
         random.seed(5)
-        fused = FusedDqnStep(t, rb, cfg["B"], rng="device", online=True, per=per)
-        losses = []
-        for i in range(12):
-            tr = {k: v[i] for k, v in extra.items()}
-            if i % 2:
-                del tr["priority"]
-            if captured:
-                losses.append(fused.step(tr))
-                torch.cuda.current_stream().synchronize()
-                losses[-1] = float(losses[-1][0])
-            else:
-                fused.dr.stage(0, 0, priority_from_max=True, **tr)
-                fused.dr.launch_add(1, slot=0, priority_from_max=True)
-                losses.append(float(fused._one_update(None)))
-        torch.cuda.synchronize()
-        fused.dr.raise_if_failed()
-        runs.append((losses, [p.detach().clone() for p in t.q_network.parameters()],
-                     fused.dr.tree.clone(), float(fused.dr.max_priority)))
-    (l0, p0, h0, m0), (l1, p1, h1, m1) = runs
-    assert l0 == l1
-    assert all(torch.equal(a, b) for a, b in zip(p0, p1))
-    assert torch.equal(h0, h1) and m0 == m1
+        return FusedDqnStep(t, rb, cfg["B"], rng="device", online=True, per=per), None
+
+    assert_captured_equals_eager(setup, transition_stream(12, 8, cfg["S"], cfg["A"]), 12,
+                                 lambda f: [params(f.trainer.q_network), tree(f)],
+                                 drop_priority=lambda i: i % 2)
 
 
 def test_online_per_nan_reward_raises():
-    import bench
     from reagent_b200.replay_memory import PrioritizedUpdate
     from reagent_b200.training.fused_step import FusedDqnStep
 
-    cfg = dict(bench.CONFIGS[2], cap=4096, B=256)
-    rb, t = _setup(cfg, _stream(3000, cfg["S"], cfg["A"], 5))
+    cfg = _cfg()
+    rb, t = bench_setup(cfg, transition_stream(3000, 5, cfg["S"], cfg["A"]))
     random.seed(1)
     fused = FusedDqnStep(t, rb, cfg["B"], rng="device", online=True, per=PrioritizedUpdate())
-    extra = _stream(10, cfg["S"], cfg["A"], 6)
-    bad = {k: v[0] for k, v in extra.items()}
-    bad["reward"] = np.float32("nan")
-    bad["priority"] = 1e9  # drawn by the next update
-    with pytest.raises(FloatingPointError):
-        fused.step(bad)
-        for i in range(1, 10):
-            fused.step({k: v[i] for k, v in extra.items()})
-    torch.cuda.synchronize()
+    assert_nan_reward_raises(fused, transition_stream(10, 6, cfg["S"], cfg["A"]))
 
 
 def test_per_rejects_other_trainers():
-    import bench
     from reagent_b200.replay_memory import PrioritizedUpdate
     from reagent_b200.training.fused_step import FusedDqnStep
 
-    cfg = dict(bench.CONFIGS[2], cap=4096, B=256)
-    rb, t = _setup(cfg, _stream(3000, cfg["S"], cfg["A"], 5))
+    cfg = _cfg()
+    rb, t = bench_setup(cfg, transition_stream(3000, 5, cfg["S"], cfg["A"]))
 
     class NotDqn:
         num_actions = cfg["A"]

@@ -6,46 +6,11 @@ import torch
 
 from oracle import td_oracle as O
 from tests import golden_util as G
-from tests.test_oracle_golden import QRDQN_CASES
+from tests.builders import _batch, _build_qr
+from tests.golden_cases import QRDQN_CASES
 
 pytestmark = pytest.mark.gpu
 TOL = 1e-5
-
-
-def _build(meta, arrays):
-    from reagent_b200.core.parameters import EvaluationParameters, RLParameters
-    from reagent_b200.models import DuelingQNetwork, FullyConnectedDQN
-    from reagent_b200.optimizer import Optimizer__Union
-    from reagent_b200.training import QRDQNTrainer
-
-    if meta.get("dueling"):
-        q = DuelingQNetwork.make_fully_connected(meta["S"], meta["A"], meta["sizes"], meta["acts"],
-                                                 num_atoms=meta["N"])
-    else:
-        q = FullyConnectedDQN(meta["S"], meta["A"], meta["sizes"], meta["acts"], num_atoms=meta["N"])
-    qt = q.get_target_network()
-    G.load_into_module(arrays, "q0", q)
-    G.load_into_module(arrays, "qt0", qt)
-    rl = RLParameters(gamma=meta["gamma"], target_update_rate=meta["tau"],
-                      maxq_learning=meta["maxq"], multi_steps=meta["multi_steps"])
-    t = QRDQNTrainer(q, qt, actions=[str(i) for i in range(meta["A"])], rl=rl,
-                     double_q_learning=meta["double_q"], num_atoms=meta["N"],
-                     minibatch_size=meta["B"], optimizer=Optimizer__Union.default(lr=meta["lr"]),
-                     evaluation=EvaluationParameters(calc_cpe_in_training=False))
-    return t.cuda()
-
-
-def _batch(b, meta):
-    from reagent_b200.core import types as rlt
-
-    return rlt.DiscreteDqnInput(
-        state=rlt.FeatureData(b["state"]), next_state=rlt.FeatureData(b["next_state"]),
-        reward=b["reward"], time_diff=b["time_diff"],
-        step=b["step"] if meta["multi_steps"] is not None else None,
-        not_terminal=b["not_terminal"], action=b["action"], next_action=b["next_action"],
-        possible_actions_mask=b["possible_actions_mask"],
-        possible_next_actions_mask=b["possible_next_actions_mask"],
-        extras=rlt.ExtraData())
 
 
 @pytest.mark.parametrize("name", QRDQN_CASES)
@@ -54,7 +19,7 @@ def test_qrdqn_matches_reference(name, fast):
     from reagent_b200.training import run_update
 
     arrays, meta = G.load(name)
-    t = _build(meta, arrays)
+    t = _build_qr(meta, arrays)
     batch = _batch(G.batch_tensors(arrays, "cuda"), meta)
     for it in range(meta["n_updates"]):
         ref = arrays["losses"][it]
@@ -89,7 +54,7 @@ def test_dueling_quantile_forward_matches_reference():
     from reagent_b200.net_builder import DuelingQuantile
 
     arrays, meta = G.load("qrdqn_dueling")
-    t = _build(meta, arrays)
+    t = _build_qr(meta, arrays)
     x = rlt.FeatureData(torch.from_numpy(arrays["batch.state"]).cuda())
     out = t.q_network(x)
     B, A, N = meta["B"], meta["A"], meta["N"]
@@ -146,7 +111,7 @@ def test_qrdqn_config3_full_batch_matches_chunked_oracle():
              not_terminal=nt, action=torch.nn.functional.one_hot(act, A).float(),
              next_action=torch.nn.functional.one_hot(act, A).float() * nt,
              possible_actions_mask=torch.ones(B, A), possible_next_actions_mask=torch.ones(B, A))
-    t = _build(meta, arrays)
+    t = _build_qr(meta, arrays)
     qo = O.clone_net(q, requires_grad=True)
     lo, grads, next_action, all_q = _qrdqn_oracle_chunked(qo, qt, b, gamma=0.99, num_atoms=N)
     gb = _batch({k: (v.cuda() if v is not None else None) for k, v in b.items()}, meta)
@@ -183,7 +148,7 @@ def test_qrdqn_config3_shape_matches_oracle():
              not_terminal=nt, action=torch.nn.functional.one_hot(act, A).float(),
              next_action=torch.nn.functional.one_hot(act, A).float() * nt,
              possible_actions_mask=torch.ones(B, A), possible_next_actions_mask=torch.ones(B, A))
-    t = _build(meta, arrays)
+    t = _build_qr(meta, arrays)
     qo = O.clone_net(q, requires_grad=True)
     qt_before = O.clone_net(qt)
     adam = O.AdamState(O.net_params(qo), lr=1e-3)

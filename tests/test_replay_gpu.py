@@ -8,44 +8,12 @@ import pytest
 import torch
 
 from tests import golden_util as G
+from tests.builders import _build_replay
 
 pytestmark = pytest.mark.gpu
 
 CASES = ["replay_uniform_h1", "replay_uniform_h3_wrap", "replay_uniform_h5_cont",
          "replay_uniform_stack3", "replay_per_h1", "replay_per_h3_wrap_zero", "replay_per_big"]
-
-
-def _build(arrays, meta, bulk=False):
-    from reagent_b200.replay_memory import PrioritizedReplayBuffer, ReplayBuffer
-
-    if meta["prioritized"]:
-        rb = PrioritizedReplayBuffer(stack_size=meta["stack"], replay_capacity=meta["cap"],
-                                     batch_size=meta["B"], update_horizon=meta["horizon"],
-                                     gamma=meta["gamma"])
-    else:
-        rb = ReplayBuffer(stack_size=meta["stack"], replay_capacity=meta["cap"],
-                          batch_size=meta["B"], update_horizon=meta["horizon"],
-                          gamma=meta["gamma"])
-    keys = meta["keys"]
-    st = {k: arrays[f"stream.{k}"] for k in keys}
-    if bulk:
-        rb.add_batch(**st)
-        return rb
-    for t in range(meta["n_add"]):
-        kw = {}
-        for k in keys:
-            v = st[k][t]
-            if k == "terminal":
-                v = bool(v)
-            elif k == "priority":
-                v = float(v)
-            elif k == "action" and not meta["continuous"]:
-                v = int(v)
-            elif np.ndim(v) == 0:
-                v = float(v)
-            kw[k] = v
-        rb.add(**kw)
-    return rb
 
 
 def _cmp(name, got, want, terminal=None):
@@ -70,7 +38,7 @@ def test_replay_matches_reference(name, bulk):
     arrays, meta = G.load(name)
     if bulk and meta["stack"] != 1:
         pytest.skip("bulk loader is stack_size == 1 only")
-    rb = _build(arrays, meta, bulk)
+    rb = _build_replay(arrays, meta, bulk)
     assert np.array_equal(rb._is_index_valid.numpy(), arrays["valid"])
     assert rb.size == int(arrays["valid"].sum())
     random.seed(meta["seed"] + 100)
@@ -173,7 +141,7 @@ def test_checkpoint_load_rebuilds_device_mirrors(name, tmp_path):
     buffer whose device store, priority mirror and pinned staging block hold OTHER data must
     leave it sampling exactly like the buffer that was saved."""
     arrays, meta = G.load(name)
-    src = _build(arrays, meta, bulk=True)
+    src = _build_replay(arrays, meta, bulk=True)
     src.save(str(tmp_path), 3)
 
     # same add history (validity bookkeeping is private state and, as in the reference, not
@@ -188,7 +156,7 @@ def test_checkpoint_load_rebuilds_device_mirrors(name, tmp_path):
             other[f"stream.{k}"] = rng.uniform(0.5, 2.0, v.shape)
         elif np.issubdtype(v.dtype, np.floating):
             other[f"stream.{k}"] = rng.standard_normal(v.shape).astype(v.dtype)
-    dst = _build(other, meta, bulk=True)
+    dst = _build_replay(other, meta, bulk=True)
     B = meta["B"]
     random.seed(3); np.random.seed(3); torch.manual_seed(3)
     dst.sample_transition_batch(batch_size=B)  # device mirrors of the OLD contents now exist

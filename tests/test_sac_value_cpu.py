@@ -6,10 +6,7 @@ import torch
 
 from oracle import sac_value_oracle as V
 from tests import golden_util as G
-
-SAC_VALUE_CASES = ["sac_value_twin_alpha", "sac_value_single_prior", "sac_value_fixed_alpha_odd",
-                   "sac_crr_exponent", "sac_crr_indicator", "sac_pendulum_manager",
-                   "sac_crr_pendulum_manager"]
+from tests.golden_cases import SAC_VALUE_CASES, opt_names
 
 
 def oracle_state(arrays, meta):
@@ -22,12 +19,6 @@ def oracle_state(arrays, meta):
                            entropy_temperature=meta["entropy_temperature"],
                            learn_alpha=meta["learn_alpha"], target_entropy=meta["target_entropy"],
                            logged_action_uniform_prior=meta["uniform_prior"], crr=meta["crr"])
-
-
-def opt_names(meta):
-    """Optimizer order of the reference (sac_trainer.py:148-193)."""
-    return (["q1"] + (["q2"] if meta["twin"] else []) + ["actor"]
-            + (["alpha"] if meta["learn_alpha"] else []) + ["value"])
 
 
 def _cmp_net(net, arrays, prefix, tol):

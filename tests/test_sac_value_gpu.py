@@ -12,8 +12,10 @@ import torch
 
 from oracle import sac_value_oracle as V
 from tests import golden_util as G
-from tests.test_actor_critic_gpu import _adam_close, _cmp_module, _net_arrays, _pbatch, _rand_net
-from tests.test_sac_value_cpu import SAC_VALUE_CASES, opt_names
+from tests.online_step import assert_captured_equals_eager, tree
+from tests.builders import _net_arrays, _pbatch, _rand_net
+from tests.golden_cases import SAC_VALUE_CASES, opt_names
+from tests.golden_util import _adam_close, _cmp_module
 
 pytestmark = pytest.mark.gpu
 TOL = 1e-5
@@ -301,44 +303,33 @@ def test_online_captured_equals_eager(crr, with_per):
     cfg = dict(bench.CONFIGS[4], cap=4096, B=256)
     low, high = -np.ones(cfg["A"], np.float32), np.ones(cfg["A"], np.float32)
     base = bench.synth_stream(3000, 7, cfg)
-    extra = bench.synth_stream(5, 8, cfg)
     per = PrioritizedUpdate(alpha=0.6, beta0=0.4, beta_updates=10, eps=1e-6) if with_per else None
-    runs = []
-    for captured in (True, False):
+    draws = []  # the noise each run asked its hook for
+
+    def setup():
         rb, t = _online_setup(base, cfg, crr)
         gen = torch.Generator().manual_seed(11)
         buf = torch.empty(cfg["B"], cfg["A"], device="cuda")
-        draws = []
+        draws.append([])
 
         def hook(name, shape, device):
-            draws.append(name)
+            draws[-1].append(name)
             return buf
         t.noise_hook = hook
-        buf.copy_(torch.randn(buf.shape, generator=gen))
-        random.seed(5)
-        fused = FusedPolicyStep(t, rb, cfg["B"], low, high, online=True, per=per)
-        losses = []
-        for i in range(5):
+
+        def refill():
             torch.cuda.synchronize()
             buf.copy_(torch.randn(buf.shape, generator=gen))
-            tr = {k: v[i] for k, v in extra.items()}
-            if captured:
-                out = fused.step(tr)
-                torch.cuda.current_stream().synchronize()
-                losses.append(out.clone())
-            else:
-                fused.dr.stage(0, 0, priority_from_max=with_per, **tr)
-                fused.dr.launch_add(1, slot=0, priority_from_max=with_per)
-                losses.append(fused._one_update(None).cpu())
-        torch.cuda.synchronize()
-        fused.dr.raise_if_failed()
-        assert set(draws) == {"cur"}
-        runs.append((losses, _state(t), fused.dr.tree.clone(), t.all_batches_processed))
-    (l0, s0, h0, n0), (l1, s1, h1, n1) = runs
-    assert all(torch.equal(a, b) for a, b in zip(l0, l1))
-    assert all(bool(torch.isfinite(a).all()) for a in l0)
-    assert all(torch.equal(a, b) for a, b in zip(s0, s1))
-    assert torch.equal(h0, h1) and n0 == n1 == 6
+        refill()
+        random.seed(5)
+        return FusedPolicyStep(t, rb, cfg["B"], low, high, online=True, per=per), refill
+
+    snap = assert_captured_equals_eager(
+        setup, bench.synth_stream(5, 8, cfg), 5,
+        lambda f: [_state(f.trainer), tree(f), f.trainer.all_batches_processed],
+        scalar_loss=False)
+    assert [set(d) for d in draws] == [{"cur"}, {"cur"}]
+    assert snap[-1] == 6
 
 
 def test_online_per_write_back_is_twin_critic_priority():
