@@ -4,31 +4,32 @@ One process; records the card's name, power limit and maximum SM clock read in t
   a. K3 alone for Adam, AdamW and AdamW + AMSGrad on the q-network arena of bench.py's config 2
      (DQN 128-256-128-16) and config 3 (QR-DQN 128-256-128-6400), with the Polyak update of the
      target arena and 16 split-K gradient slabs (B 4096 / 256 rows per slab).  Timed with CUDA
-     events around one replay of a graph of --launches back-to-back K3 launches, so the window
-     holds no host enqueue.  AMSGrad reads and writes max_exp_avg_sq: 8 more bytes per
-     parameter per step.
+     events around one replay, after an untimed one, of a graph of --launches back-to-back K3
+     launches captured after 5 warm-up launches on a side stream, so the window holds no host
+     enqueue.  AMSGrad reads and writes max_exp_avg_sq: 8 more bytes per parameter per step.
   b. The captured QR-DQN online step at config 3 (FusedDqnStep(rng="device", online=True): add
      one transition, draw, update, all in one graph replay) with Adam against AdamW + AMSGrad,
-     --steps steps per run, CUDA events around the loop.
+     3 warm-up steps and then --steps steps per run, host-clocked from a synchronise to the
+     synchronise after the last step.
 
-Every variant is repeated --reps times in alternating order and the median is reported.
+Every variant is repeated --reps times, in the given order on even repetitions and reversed on
+odd ones, and the median is reported.
 
     python profiles/time_adamw.py --out DIR [--reps 11] [--launches 200] [--steps 100]
 
-Writes DIR/time_adamw.json and prints the same JSON.
+Writes DIR/time_adamw_<card>_<limit>w.json and prints the same JSON.
 """
 import argparse
-import json
 import os
 import random
-import statistics
 import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 if ROOT not in sys.path:
     sys.path.insert(0, ROOT)
 
-from profiles.time_k2 import card_info  # noqa: E402
+from profiles.timing import (alternate, capture, card_info, cuda_device,  # noqa: E402
+                             host_steps, replay_us, transitions, write_result)
 
 OPTIMIZERS = {"adam": ("Adam", {}), "adamw": ("AdamW", {}),
               "adamw_amsgrad": ("AdamW", {"amsgrad": True})}
@@ -52,27 +53,8 @@ def k3_graph(cfg, name, launches):
     opt = _union(name, bench.LR).make_optimizer_scheduler(t.q_network.parameters())["optimizer"]
     src, tgt = t.q_network.arena, t.q_network_target.arena
     grad = torch.randn(SPLITS, src.n, device="cuda") * 1e-3
-    opt.fused_step(target=tgt, tau=bench.TAU, grad=grad)  # warm-up: module load
-    torch.cuda.synchronize()
-    s = torch.cuda.Stream()
-    s.wait_stream(torch.cuda.current_stream())
-    g = torch.cuda.CUDAGraph()
-    with torch.cuda.stream(s), torch.cuda.graph(g, stream=s):
-        for _ in range(launches):
-            opt.fused_step(target=tgt, tau=bench.TAU, grad=grad)
-    torch.cuda.synchronize()
+    g = capture(lambda: opt.fused_step(target=tgt, tau=bench.TAU, grad=grad), launches)
     return g, src.n, (t, opt, grad)
-
-
-def time_graph(g):
-    import torch
-
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    g.replay()
-    e1.record()
-    e1.synchronize()
-    return e0.elapsed_time(e1) * 1e3  # us
 
 
 def online_step(cfg, name):
@@ -92,69 +74,48 @@ def online_step(cfg, name):
     return fused
 
 
-def time_online(fused, extra, steps):
-    import torch
-
-    for i in range(3):
-        fused.step({k: v[i] for k, v in extra.items()})
-    torch.cuda.synchronize()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for i in range(steps):
-        fused.step({k: v[3 + i] for k, v in extra.items()})
-    e1.record()
-    e1.synchronize()
+def time_online(fused, trs, steps):
+    host_steps(lambda i: fused.step(trs[i]), 3)
+    us, _ = host_steps(lambda i: fused.step(trs[i]), steps, 3)
     fused.dr.raise_if_failed()
-    return e0.elapsed_time(e1) * 1e3 / steps  # us per step
+    return us
 
 
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--out", required=True, help="directory for time_adamw.json")
+    ap.add_argument("--out", required=True, help="directory for the result file")
     ap.add_argument("--reps", type=int, default=11)
     ap.add_argument("--launches", type=int, default=200)
     ap.add_argument("--steps", type=int, default=100)
     args = ap.parse_args()
+
+    cuda_device(__file__)
     import torch
 
     import bench
 
-    if not torch.cuda.is_available():
-        raise SystemExit("time_adamw.py measures on the GPU; no CUDA device found")
-    torch.cuda.set_device(0)
     res = {"card": card_info(), "reps": args.reps, "launches_per_graph": args.launches,
            "split_k_slabs": SPLITS, "k3_alone_us": {}, "online_step_us": {}}
 
     for c in (2, 3):
         cfg = dict(bench.CONFIGS[c])
         graphs = {n: k3_graph(cfg, n, args.launches) for n in OPTIMIZERS}
-        times = {n: [] for n in OPTIMIZERS}
-        for _ in range(args.reps):
-            for n, (g, _, _) in graphs.items():
-                times[n].append(time_graph(g) / args.launches)
-        n_params = graphs["adam"][1]
+        times = alternate(graphs, args.reps,
+                          lambda n, rep: replay_us(graphs[n][0], args.launches))
         res["k3_alone_us"][f"config{c}"] = {
-            "params": n_params,
-            **{n: {"median": statistics.median(v), "min": min(v), "max": max(v)}
-               for n, v in times.items()}}
+            "params": graphs["adam"][1],
+            **{n: {s: v[s] for s in ("median", "min", "max")} for n, v in times.items()}}
         del graphs
         torch.cuda.empty_cache()
 
     cfg = dict(bench.CONFIGS[3], cap=1 << 20)
-    extra = bench.synth_stream(args.steps + 3, 77, cfg)
+    trs = transitions(cfg, args.steps + 3, seed=77)
     steps = {n: online_step(cfg, n) for n in ("adam", "adamw_amsgrad")}
-    times = {n: [] for n in steps}
-    for _ in range(args.reps):
-        for n, fused in steps.items():
-            times[n].append(time_online(fused, extra, args.steps))
+    times = alternate(steps, args.reps, lambda n, rep: time_online(steps[n], trs, args.steps))
     res["online_step_us"]["config3_qrdqn"] = {
         "steps_per_run": args.steps,
-        **{n: {"median": statistics.median(v), "min": min(v), "max": max(v)}
-           for n, v in times.items()}}
-    os.makedirs(args.out, exist_ok=True)
-    with open(os.path.join(args.out, "time_adamw.json"), "w") as f:
-        json.dump(res, f, indent=1)
-    print(json.dumps(res))
+        **{n: {s: v[s] for s in ("median", "min", "max")} for n, v in times.items()}}
+    write_result(args.out, __file__, res)
 
 
 if __name__ == "__main__":

@@ -12,20 +12,19 @@ clock are read in the same run.
 
     python profiles/time_bc.py --out DIR [--reps 11] [--steps 200]
 
-Writes DIR/time_bc.json and prints the same JSON.
+Writes DIR/time_bc_<card>_<limit>w.json and prints the same JSON.
 """
 import argparse
-import json
 import os
 import statistics
 import sys
-import time
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 if ROOT not in sys.path:
     sys.path.insert(0, ROOT)
 
-from profiles.time_bcq import card_info, time_launches  # noqa: E402
+from profiles.timing import (alternate, card_info, cuda_device, host_steps,  # noqa: E402
+                             launch_us, write_result)
 
 B, S, A, SIZES, LR = 4096, 128, 16, [256, 128], 1e-3
 
@@ -71,23 +70,19 @@ def build(dev):
 
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--out", required=True, help="directory for time_bc.json")
+    ap.add_argument("--out", required=True, help="directory for the result file")
     ap.add_argument("--reps", type=int, default=11)
     ap.add_argument("--steps", type=int, default=200)
     ap.add_argument("--warmup", type=int, default=20)
     ap.add_argument("--launches", type=int, default=500)
     args = ap.parse_args()
 
-    import torch
+    dev = cuda_device(__file__)
     import torch.nn.functional as F
 
     from reagent_b200 import _lib
     from reagent_b200.core import types as rlt
 
-    if not torch.cuda.is_available():
-        raise SystemExit("time_bc.py measures on the GPU; no CUDA device is visible")
-    dev = torch.device("cuda", 0)
-    torch.cuda.set_device(dev)
     info = card_info()
     data = make_data(dev)
     batches = [rlt.BehavioralCloningModelInput(rlt.FeatureData(d["state"]), d["action"],
@@ -110,60 +105,43 @@ def main():
     # same weights, same first batch: the first losses agree
     first = {k: float(fn(0)) for k, fn in variants.items()}
 
-    def run(fn, steps):
-        torch.cuda.synchronize()
-        t0 = time.perf_counter()
-        for i in range(steps):
-            loss = fn(i)
-        torch.cuda.synchronize()
-        return (time.perf_counter() - t0) / steps, float(loss)
-
     for fn in variants.values():
-        run(fn, args.warmup)
-    per_update = {k: [] for k in variants}
+        host_steps(fn, args.warmup)
     last_loss = {}
-    for rep in range(args.reps):
-        order = list(variants) if rep % 2 == 0 else list(variants)[::-1]
-        for k in order:
-            dt, last_loss[k] = run(variants[k], args.steps)
-            per_update[k].append(dt * 1e6)
+
+    def run(k, rep):
+        us, last_loss[k] = host_steps(variants[k], args.steps)
+        return us
+
+    per_update = alternate(variants, args.reps, run)
 
     # the loss head alone, on the fused trainer's workspace
-    ws = fused._ws
     d = data[0]
-    a = _lib.BcXentArgsT()
-    a.batch, a.num_actions = B, A
-    a.logits, a.labels = ws["scores"].data_ptr(), d["action"].data_ptr()
-    a.mask, a.dz = d["possible_actions_mask"].data_ptr(), ws["net"].dz[-1].data_ptr()
-    a.loss_partials, a.loss = ws["loss_partials"].data_ptr(), ws["loss"].data_ptr()
-    a.tile_counter = ws["counter"].data_ptr()
+    a = fused._xent_args(fused._ws, d["action"], d["possible_actions_mask"])
     lib, st = _lib.lib(), _lib.cur_stream()
 
     def head():
         _lib.check(lib.rb200_bc_xent_head(a, st), "rb200_bc_xent_head")
 
-    head_us = [time_launches(head, args.launches) for _ in range(3)]
+    head_us = [launch_us(head, args.launches) for _ in range(3)]
 
-    med = {k: statistics.median(v) for k, v in per_update.items()}
+    med = {k: v["median"] for k, v in per_update.items()}
     res = {
         "what": "BehavioralCloningTrainer.train_batch vs the same update in eager torch, per update",
         "card": info,
         "config": dict(B=B, S=S, A=A, sizes=SIZES, acts="relu", lr=LR, mask_keep=0.7),
         "method": (f"{args.reps} alternating repetitions of {args.steps} host-timed steps "
                    f"(synchronised) per variant after {args.warmup} warm-up steps, cycling over "
-                   f"{len(data)} batches; head: CUDA events over {args.launches} back-to-back "
-                   f"launches, 3 repetitions"),
-        "per_update_us": {k: dict(median=med[k], min=min(v), max=max(v), all=v)
-                          for k, v in per_update.items()},
+                   f"{len(data)} batches; head, with the arguments "
+                   f"BehavioralCloningTrainer._step builds: CUDA events over {args.launches} "
+                   f"back-to-back launches after 10 warm-up launches, 3 repetitions"),
+        "per_update_us": per_update,
         "speedup_median": med["eager"] / med["fused"],
         "bc_xent_head_us": dict(median=statistics.median(head_us), all=head_us),
         "first_loss": first,
         "last_loss": last_loss,
     }
-    os.makedirs(args.out, exist_ok=True)
-    with open(os.path.join(args.out, "time_bc.json"), "w") as f:
-        json.dump(res, f, indent=1)
-    print(json.dumps(res))
+    write_result(args.out, __file__, res)
 
 
 if __name__ == "__main__":

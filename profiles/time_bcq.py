@@ -11,34 +11,21 @@ and records the card's name, power limit and maximum SM clock read in the same r
 
     python profiles/time_bcq.py --out DIR [--reps 11] [--steps 200]
 
-Writes DIR/time_bcq.json and prints the same JSON.
+Writes DIR/time_bcq_<card>_<limit>w.json and prints the same JSON.
 """
 import argparse
-import json
 import os
-import statistics
-import subprocess
 import sys
-import time
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 if ROOT not in sys.path:
     sys.path.insert(0, ROOT)
 
+from profiles.timing import (alternate, card_info, cuda_device, host_steps,  # noqa: E402
+                             launch_us, write_result)
+
 THRESHOLD = 0.3
 CAPACITY = 1 << 18  # replay capacity; per-update time depends on it only through the tree depth
-
-
-def card_info():
-    q = "name,power.limit,clocks.max.sm"
-    try:
-        out = subprocess.run(["nvidia-smi", f"--query-gpu={q}", "--format=csv,noheader"],
-                             capture_output=True, text=True, timeout=60).stdout.strip()
-    except (OSError, subprocess.SubprocessError) as e:
-        out = f"nvidia-smi unavailable: {e}"
-    import torch
-
-    return {"torch_device_name": torch.cuda.get_device_name(0), "nvidia_smi": {q: out}}
 
 
 def make_imitator(cfg, dev):
@@ -79,50 +66,21 @@ def build(cfg, dev, bcq, rng):
     return t, FusedDqnStep(t, rb, cfg["B"], rng=rng)
 
 
-def time_steps(fused, steps):
-    import torch
-
-    torch.cuda.synchronize()
-    t0 = time.perf_counter()
-    for _ in range(steps):
-        lh = fused.step()
-    torch.cuda.synchronize()
-    dt = (time.perf_counter() - t0) / steps
-    return dt, float(lh[0])
-
-
-def time_launches(fn, n):
-    import torch
-
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    for _ in range(10):
-        fn()
-    e0.record()
-    for _ in range(n):
-        fn()
-    e1.record()
-    e1.synchronize()
-    return e0.elapsed_time(e1) * 1e3 / n  # microseconds per launch
-
-
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--out", required=True, help="directory for time_bcq.json")
+    ap.add_argument("--out", required=True, help="directory for the result file")
     ap.add_argument("--reps", type=int, default=11)
     ap.add_argument("--steps", type=int, default=200)
     ap.add_argument("--warmup", type=int, default=20)
     ap.add_argument("--launches", type=int, default=500)
     args = ap.parse_args()
 
+    dev = cuda_device(__file__)
     import torch
 
     import bench
     from reagent_b200 import _lib
 
-    if not torch.cuda.is_available():
-        raise SystemExit("time_bcq.py measures on the GPU; no CUDA device is visible")
-    dev = torch.device("cuda", 0)
-    torch.cuda.set_device(dev)
     cfg = dict(bench.CONFIGS[2])
     info = card_info()
     # rng="host": Python's random stream drawn on the host every step (the default);
@@ -130,14 +88,14 @@ def main():
     variants = {f"{k}/rng={rng}": build(cfg, dev, k == "bcq", rng)
                 for rng in ("host", "device") for k in ("plain", "bcq")}
     for _, fused in variants.values():
-        time_steps(fused, args.warmup)
-    per_update = {k: [] for k in variants}
+        host_steps(lambda i: fused.step(), args.warmup)
     last_loss = {}
-    for rep in range(args.reps):
-        order = list(variants) if rep % 2 == 0 else list(variants)[::-1]
-        for k in order:
-            dt, last_loss[k] = time_steps(variants[k][1], args.steps)
-            per_update[k].append(dt * 1e6)
+
+    def run(k, rep):
+        us, last_loss[k] = host_steps(lambda i: variants[k][1].step(), args.steps)
+        return us
+
+    per_update = alternate(variants, args.reps, run)
 
     # the two BCQ launches alone, eager, on one sampled batch's next_state
     t = variants["bcq/rng=host"][0]
@@ -156,13 +114,11 @@ def main():
         _lib.check(lib.rb200_bcq_filter(logits.data_ptr(), B, A, THRESHOLD, None,
                                         mask.data_ptr(), None, None, st), "rb200_bcq_filter")
 
-    kern = {}
-    for rep in range(3):
-        for name, fn in (("imitator_forward", imitator_forward), ("bcq_filter", bcq_filter)):
-            kern.setdefault(name, []).append(time_launches(fn, args.launches))
+    kernels = {"imitator_forward": imitator_forward, "bcq_filter": bcq_filter}
+    kern = alternate(kernels, 3, lambda k, rep: launch_us(kernels[k], args.launches))
     dropped = float((mask == 0).float().mean())
 
-    med = {k: statistics.median(v) for k, v in per_update.items()}
+    med = {k: v["median"] for k, v in per_update.items()}
     res = {
         "what": ("FusedDqnStep.step() per update, config-2 shapes, with and without BCQ, host "
                  "and device random streams"),
@@ -172,21 +128,18 @@ def main():
                        drop_threshold=THRESHOLD),
         "method": (f"{args.reps} alternating repetitions of {args.steps} host-timed steps "
                    f"(synchronised) per variant after {args.warmup} warm-up steps; kernels: "
-                   f"CUDA events over {args.launches} back-to-back launches, 3 repetitions"),
-        "per_update_us": {k: dict(median=med[k], min=min(v), max=max(v), all=v)
-                          for k, v in per_update.items()},
+                   f"CUDA events over {args.launches} back-to-back launches after 10 warm-up "
+                   f"launches, 3 alternating repetitions"),
+        "per_update_us": per_update,
         "bcq_overhead_us_median": {rng: med[f"bcq/rng={rng}"] - med[f"plain/rng={rng}"]
                                    for rng in ("host", "device")},
         "bcq_overhead_frac_median": {rng: med[f"bcq/rng={rng}"] / med[f"plain/rng={rng}"] - 1
                                      for rng in ("host", "device")},
-        "kernel_us": {k: dict(median=statistics.median(v), all=v) for k, v in kern.items()},
+        "kernel_us": {k: dict(median=v["median"], all=v["all"]) for k, v in kern.items()},
         "dropped_fraction_random_states": dropped,
         "last_loss": last_loss,
     }
-    os.makedirs(args.out, exist_ok=True)
-    with open(os.path.join(args.out, "time_bcq.json"), "w") as f:
-        json.dump(res, f, indent=1)
-    print(json.dumps(res))
+    write_result(args.out, __file__, res)
 
 
 if __name__ == "__main__":

@@ -11,7 +11,8 @@ FullyConnected critics, exploration_variance 1e-7) and config-2 shapes (S 128, A
     initial weights on the same data.
 Each is captured into a CUDA graph of `--calls` consecutive updates after warm-up; a run is one
 replay between two CUDA events, the variants alternate, and the median of `--reps` runs is
-reported per update.  The heads are timed the same way on the fused trainer's workspace.  The
+reported per update.  The heads are timed the same way on the fused trainer's workspace, with
+the arguments DiscreteCRRTrainer's critic and actor steps build, exploration noise included.  The
 online step is FusedDqnStep(rng="device", online=True).step(transition), host-timed over
 `--steps` steps that end in a synchronise.  The card's name, power limit and maximum SM clock are
 read (queried, never set) in the same run and name the output file.
@@ -21,18 +22,16 @@ read (queried, never set) in the same run and name the output file.
 Writes DIR/time_crr_<card>_<limit>w.json and prints the same JSON.  Fails without a GPU.
 """
 import argparse
-import json
 import os
-import re
 import statistics
 import sys
-import time
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 if ROOT not in sys.path:
     sys.path.insert(0, ROOT)
 
-from profiles.time_bcq import card_info  # noqa: E402
+from profiles.timing import (alternate, capture, card_info, cuda_device,  # noqa: E402
+                             host_steps, replay_us, write_result)
 
 SHAPES = {
     "cartpole": dict(S=4, A=2, B=256, sizes=[1024, 1024], noise=1e-7, gamma=0.99, tau=0.2),
@@ -173,76 +172,17 @@ def make_batch(cfg, dev):
     return d, batch
 
 
-def capture(fn, calls, warmup=5):
-    """A CUDA graph of `calls` consecutive calls of fn, captured after `warmup` eager calls."""
-    import torch
-
-    s = torch.cuda.Stream()
-    s.wait_stream(torch.cuda.current_stream())
-    with torch.cuda.stream(s):
-        for _ in range(warmup):
-            fn()
-    torch.cuda.current_stream().wait_stream(s)
-    torch.cuda.synchronize()
-    g = torch.cuda.CUDAGraph()
-    with torch.cuda.graph(g):
-        for _ in range(calls):
-            fn()
-    return g
-
-
-def replay_us(g, calls):
-    import torch
-
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    g.replay()
-    e1.record()
-    e1.synchronize()
-    return e0.elapsed_time(e1) * 1e3 / calls
-
-
-def alternate(graphs, calls, reps):
-    for g in graphs.values():  # one untimed replay each
-        replay_us(g, calls)
-    runs = {k: [] for k in graphs}
-    for rep in range(reps):
-        order = list(graphs) if rep % 2 == 0 else list(graphs)[::-1]
-        for k in order:
-            runs[k].append(replay_us(graphs[k], calls))
-    return {k: dict(median=statistics.median(v), min=min(v), max=max(v), all=v)
-            for k, v in runs.items()}
-
-
 def head_calls(trainer, batch):
-    """Closures launching each head alone on the trainer's workspace (left by one update)."""
+    """Closures launching each head alone on the trainer's workspace (left by one update), with
+    the arguments the trainer's critic and actor steps build, and the Pins that keep the tensors
+    those arguments point to alive."""
     from reagent_b200 import _lib
+    from reagent_b200.training.workspace import Pins
 
-    ws, lib, B, A = trainer._ws, _lib.lib(), batch.action.shape[0], trainer.num_actions
-    keep = [batch.reward.reshape(-1).contiguous(), batch.not_terminal.reshape(-1).contiguous(),
-            batch.extras.action_probability.reshape(-1).contiguous()]
-    c = _lib.CrrCriticArgsT()
-    c.batch, c.num_actions = B, A
-    c.actor_next, c.q1_target_next = ws["actor_next"].data_ptr(), ws["q1t_next"].data_ptr()
-    c.q2_target_next, c.q1, c.q2 = (ws["q2t_next"].data_ptr(), ws["q1_out"].data_ptr(),
-                                    ws["q2_out"].data_ptr())
-    c.action, c.reward, c.not_terminal = batch.action.data_ptr(), keep[0].data_ptr(), keep[1].data_ptr()
-    c.gamma = float(trainer.gamma)
-    c.td_target, c.q1_selected, c.q2_selected = (ws["td_target"].data_ptr(), ws["q1_sel"].data_ptr(),
-                                                 ws["q2_sel"].data_ptr())
-    c.dz_q1, c.dz_q2 = ws["q1"].dz[-1].data_ptr(), ws["q2"].dz[-1].data_ptr()
-    c.loss_partials, c.loss = ws["critic_partials"].data_ptr(), ws["critic_loss"].data_ptr()
-    c.tile_counter = ws["counter"][0:1].data_ptr()
-    a = _lib.CrrActorArgsT()
-    a.batch, a.num_actions = B, A
-    a.actor_out, a.q1, a.action = (ws["actor_out"].data_ptr(), ws["q1_out"].data_ptr(),
-                                   batch.action.data_ptr())
-    a.action_probability = keep[2].data_ptr()
-    a.inv_beta, a.max_weight, a.entropy_coeff, a.clip_limit = 1.0, 20.0, 0.0, 10.0
-    a.action_activation = _lib.ACT["tanh"]
-    a.weight, a.dz = ws["weight"].data_ptr(), ws["actor"].dz[-1].data_ptr()
-    a.loss_partials, a.loss = ws["actor_partials"].data_ptr(), ws["actor_loss"].data_ptr()
-    a.tile_counter = ws["counter"][1:2].data_ptr()
+    ws, lib = trainer._ws, _lib.lib()
+    pins = Pins(ws["dev"])
+    c = trainer._critic_args(batch, ws, pins)
+    a = trainer._actor_args(batch, ws, pins)
 
     def critic():
         _lib.check(lib.rb200_crr_critic_head(c, _lib.cur_stream()), "rb200_crr_critic_head")
@@ -250,12 +190,11 @@ def head_calls(trainer, batch):
     def actor():
         _lib.check(lib.rb200_crr_actor_head(a, _lib.cur_stream()), "rb200_crr_actor_head")
 
-    return {"critic_head": critic, "actor_head": actor}, keep
+    return {"critic_head": critic, "actor_head": actor}, pins
 
 
 def time_online(cfg, dev, steps):
     import numpy as np
-    import torch
 
     from reagent_b200.replay_memory import PrioritizedReplayBuffer
     from reagent_b200.training.fused_step import FusedDqnStep
@@ -271,16 +210,8 @@ def time_online(cfg, dev, steps):
     fused = FusedDqnStep(build_fused(cfg, dev), rb, B, rng="device", online=True)
     tr = dict(observation=rng.standard_normal(S).astype(np.float32), action=1, reward=0.5,
               terminal=False, priority=1.0)
-    for _ in range(20):
-        fused.step(tr)
-    out = []
-    for _ in range(3):
-        torch.cuda.synchronize()
-        t0 = time.perf_counter()
-        for _ in range(steps):
-            fused.step(tr)
-        torch.cuda.synchronize()
-        out.append((time.perf_counter() - t0) / steps * 1e6)
+    host_steps(lambda i: fused.step(tr), 20)
+    out = [host_steps(lambda i: fused.step(tr), steps)[0] for _ in range(3)]
     fused.dr.raise_if_failed()
     return dict(median=statistics.median(out), all=out)
 
@@ -293,12 +224,7 @@ def main():
     ap.add_argument("--steps", type=int, default=300)
     args = ap.parse_args()
 
-    import torch
-
-    if not torch.cuda.is_available():
-        raise SystemExit("time_crr.py measures on the GPU; no CUDA device is visible")
-    dev = torch.device("cuda", 0)
-    torch.cuda.set_device(dev)
+    dev = cuda_device(__file__)
     info = card_info()
     results = {}
     for name, cfg in SHAPES.items():
@@ -308,37 +234,31 @@ def main():
         first = dict(fused=float(fused.train_batch(batch, 0)[0][0]), eager=float(eager.step(d)))
         graphs = {"fused": capture(lambda: fused.train_batch(batch, 0), args.calls),
                   "eager": capture(lambda: eager.step(d), args.calls)}
-        per_update = alternate(graphs, args.calls, args.reps)
+        per_update = alternate(graphs, args.reps, lambda k, rep: replay_us(graphs[k], args.calls))
         calls, keep = head_calls(fused, batch)
-        heads = alternate({k: capture(fn, args.calls) for k, fn in calls.items()}, args.calls,
-                          args.reps)
+        head_graphs = {k: capture(fn, args.calls) for k, fn in calls.items()}
+        heads = alternate(head_graphs, args.reps,
+                          lambda k, rep: replay_us(head_graphs[k], args.calls))
         results[name] = dict(
             config=dict(cfg, lr=LR, acts="relu", twin=True), first_q1_loss=first,
             per_update_us=per_update,
             eager_over_fused=per_update["eager"]["median"] / per_update["fused"]["median"],
             head_us=heads, head_algorithmic_bytes=algorithmic_bytes(cfg),
             online_step_us=time_online(cfg, dev, args.steps))
-        del graphs, keep
+        del graphs, head_graphs, keep
     res = {
         "what": "DiscreteCRRTrainer.train_batch vs the same update in eager torch, the CRR loss "
                 "heads alone, and the captured online FusedDqnStep step",
         "card": info,
         "method": (f"CUDA events around one replay of a CUDA graph of {args.calls} consecutive "
-                   f"calls, captured after warm-up; medians of {args.reps} runs, variants "
-                   f"alternating; online step: host clock over {args.steps} steps ending in a "
-                   "synchronise, 3 repetitions"),
+                   f"calls, captured after 5 warm-up calls on a side stream, each timed replay "
+                   f"after an untimed one; medians of {args.reps} runs, variants alternating; "
+                   f"heads with the arguments the trainer builds, exploration noise included; "
+                   f"online step: host clock over {args.steps} steps ending in a synchronise, "
+                   "3 repetitions"),
         "results": results,
     }
-    smi = list(info["nvidia_smi"].values())[0].split(",")
-    model = re.search(r"\b([a-z]+\d+)\b", smi[0].lower()) if len(smi) == 3 else None  # "h100"
-    card = model.group(1) if model else "gpu"
-    limit = re.sub(r"[^0-9.]", "", smi[1]).split(".")[0] if len(smi) == 3 else "unknown"
-    os.makedirs(args.out, exist_ok=True)
-    path = os.path.join(args.out, f"time_crr_{card}_{limit}w.json")
-    with open(path, "w") as f:
-        json.dump(res, f, indent=1)
-    print(json.dumps(res))
-    print("wrote", path)
+    write_result(args.out, __file__, res)
 
 
 if __name__ == "__main__":

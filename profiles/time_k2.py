@@ -15,18 +15,18 @@ power limit and maximum SM clock read in the same run.
   c. The whole captured step per update in both of those arrangements, alternating.
 
 K2 alone is timed with CUDA events around one replay of a graph of --launches back-to-back
-launches (no host enqueue in the window); every variant is repeated --reps times in alternating
-order and the median is reported.
+launches (no host enqueue in the window), captured after 5 warm-up launches on a side stream;
+every variant is repeated --reps times in alternating order, each timed replay after an untimed
+one, and the median is reported.
 
     python profiles/time_k2.py --out DIR [--reps 11] [--launches 200] [--steps 100]
 
-Writes DIR/time_k2.json and prints the same JSON.
+Writes DIR/time_k2_<card>_<limit>w.json and prints the same JSON.
 """
 import argparse
 import json
 import os
 import statistics
-import subprocess
 import sys
 import tempfile
 
@@ -34,28 +34,17 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 if ROOT not in sys.path:
     sys.path.insert(0, ROOT)
 
+from profiles.timing import (alternate, capture, card_info, cuda_device,  # noqa: E402
+                             replay_us, write_result)
+
 CTAS = (1, 8, 32, 64, 128)
 ARRANGEMENTS = {"k1_on_side_stream": True, "one_stream": False}  # capture_device_only overlap
-
-
-def card_info():
-    q = "name,power.limit,clocks.max.sm"
-    try:
-        out = subprocess.run(["nvidia-smi", f"--query-gpu={q}", "--format=csv,noheader"],
-                             capture_output=True, text=True, timeout=60).stdout.strip()
-    except (OSError, subprocess.SubprocessError) as e:
-        out = f"nvidia-smi unavailable: {e}"
-    import torch
-
-    return {"torch_device_name": torch.cuda.get_device_name(0), "nvidia_smi": {q: out}}
 
 
 def k2_graph(trainer, rb, rows, A, launches):
     """One eager update at `rows` rows (sizes the trainer's TD workspace and writes the weight
     images), then a graph of `launches` K2 launches on those inputs with the weights prepacked.
     Returns (graph, what must stay alive with it)."""
-    import torch
-
     from reagent_b200 import _lib
 
     batch = rb.sample_discrete_dqn_batch(rows, A)
@@ -69,25 +58,7 @@ def k2_graph(trainer, rb, rows, A, launches):
         _lib.check(lib.rb200_dqn_td_step_tc(qd, qtd, a, wsc, pack.data_ptr(), pack.numel(), 1,
                                             _lib.cur_stream()), "rb200_dqn_td_step_tc")
 
-    launch()  # eager first: the shared-memory opt-in happens outside the capture
-    torch.cuda.synchronize()
-    g = torch.cuda.CUDAGraph()
-    with torch.cuda.graph(g):
-        for _ in range(launches):
-            launch()
-    return g, alive
-
-
-def time_graph(g, n):
-    import torch
-
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    g.replay()
-    e0.record()
-    g.replay()
-    e1.record()
-    e1.synchronize()
-    return e0.elapsed_time(e1) * 1e3 / n  # microseconds per launch / per update
+    return capture(launch, launches), alive
 
 
 def draw(rb, n, B, dev):
@@ -153,22 +124,19 @@ def breakdown(g, steps, tmp, tag):
 
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--out", required=True, help="directory for time_k2.json")
+    ap.add_argument("--out", required=True, help="directory for the result file")
     ap.add_argument("--reps", type=int, default=11)
     ap.add_argument("--launches", type=int, default=200)
     ap.add_argument("--steps", type=int, default=100)
     args = ap.parse_args()
 
+    dev = cuda_device(__file__)
     import torch
 
     import bench
     from reagent_b200.replay_memory import PrioritizedReplayBuffer
     from reagent_b200.training.fused_step import capture_device_only
 
-    if not torch.cuda.is_available():
-        raise SystemExit("time_k2.py measures on the GPU; no CUDA device is visible")
-    dev = torch.device("cuda", 0)
-    torch.cuda.set_device(dev)
     cfg = dict(bench.CONFIGS[2])
     B, A = cfg["B"], cfg["A"]
     info = card_info()
@@ -181,13 +149,9 @@ def main():
     for n in CTAS:
         graphs[n], keep = k2_graph(trainer, rb, 32 * n, A, args.launches)
         alive.append(keep)
-    k2 = {n: [] for n in CTAS}
-    for rep in range(args.reps):
-        for n in (CTAS if rep % 2 == 0 else CTAS[::-1]):
-            k2[n].append(time_graph(graphs[n], args.launches))
+    k2 = alternate(CTAS, args.reps, lambda n, rep: replay_us(graphs[n], args.launches))
     del graphs
-    sweep = {str(n): dict(median=statistics.median(v), min=min(v), max=max(v))
-             for n, v in k2.items()}
+    sweep = {str(n): {s: v[s] for s in ("median", "min", "max")} for n, v in k2.items()}
 
     # ---- b + c: the captured step, K1 next to the update or in line with it ----
     for _ in range(3):  # eager updates first: workspaces and weight images outside the capture
@@ -195,10 +159,7 @@ def main():
     torch.cuda.synchronize()
     steps = {k: capture_device_only(trainer, rb, B, args.steps, draw(rb, args.steps, B, dev),
                                     overlap_sampling=ov) for k, ov in ARRANGEMENTS.items()}
-    per_update = {k: [] for k in steps}
-    for rep in range(args.reps):
-        for k in (list(steps) if rep % 2 == 0 else list(steps)[::-1]):
-            per_update[k].append(time_graph(steps[k], args.steps))
+    per_update = alternate(steps, args.reps, lambda k, rep: replay_us(steps[k], args.steps))
     with tempfile.TemporaryDirectory() as tmp:
         traced = {k: breakdown(g, args.steps, tmp, k) for k, g in steps.items()}
 
@@ -211,20 +172,18 @@ def main():
         "card": info,
         "config": dict(B=B, S=cfg["S"], A=A, sizes=cfg["sizes"], double_q=True, loss="huber"),
         "method": (f"K2: CUDA events around one replay of a graph of {args.launches} launches "
-                   f"(weights prepacked), {args.reps} alternating repetitions, medians; step: "
-                   f"CUDA events around one replay of a {args.steps}-update capture_device_only "
-                   f"graph, {args.reps} alternating repetitions; breakdown: torch.profiler "
-                   f"(CUDA activities) over one replay of the same graphs, in a separate pass"),
+                   f"(weights prepacked), captured after 5 warm-up launches on a side stream, "
+                   f"{args.reps} alternating repetitions, medians; step: CUDA events around one "
+                   f"replay of a {args.steps}-update capture_device_only graph, {args.reps} "
+                   f"alternating repetitions; every timed replay after an untimed one; "
+                   f"breakdown: torch.profiler (CUDA activities) over one replay of the same "
+                   f"graphs, in a separate pass"),
         "k2_alone_us_by_ctas": sweep,
         "k2_128_over_1_cta": full / one,
-        "step_per_update_us": {k: dict(median=statistics.median(v), min=min(v), max=max(v),
-                                       all=v) for k, v in per_update.items()},
+        "step_per_update_us": per_update,
         "step_breakdown": traced,
     }
-    os.makedirs(args.out, exist_ok=True)
-    with open(os.path.join(args.out, "time_k2.json"), "w") as f:
-        json.dump(res, f, indent=1)
-    print(json.dumps(res))
+    write_result(args.out, __file__, res)
 
 
 if __name__ == "__main__":

@@ -8,28 +8,28 @@ Two variants of the same double-Q, max-Q `train_batch` (with the reward network)
   materialised  the path it replaced, rebuilt here: next_state.repeat_interleave(M) + torch.cat
                 with the possible next actions, then one rb200_mlp_forward per network.
 Both give bit-identical results.  For each variant a CUDA graph of --iters back-to-back
-`train_batch` calls is captured and one replay is timed with CUDA events; the next-state
-forward alone (the part that differs) is timed the same way.  The variants run alternately,
---reps times each, and the median is reported.
+`train_batch` calls is captured after 5 warm-up calls on a side stream, and one replay, after an
+untimed one, is timed with CUDA events; the next-state forward alone (the part that differs) is
+timed the same way.  The variants run alternately, --reps times each, and the median is
+reported.
 
 Shapes: the CartPole configuration (S 4, A 2, [128, 64] leaky_relu, B 1024) and
 S 128 / A 16 / B 4096 / [256, 128] relu, one-hot actions with the identity tiling.
 
     python profiles/time_pdqn.py --out DIR [--reps 11] [--iters 50]
 
-Writes DIR/time_pdqn.json and prints the same JSON.
+Writes DIR/time_pdqn_<card>_<limit>w.json and prints the same JSON.
 """
 import argparse
-import json
 import os
-import statistics
 import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 if ROOT not in sys.path:
     sys.path.insert(0, ROOT)
 
-from profiles.time_k2 import card_info  # noqa: E402
+from profiles.timing import (alternate, capture, card_info, cuda_device,  # noqa: E402
+                             replay_us, write_result)
 
 SHAPES = {
     "cartpole": dict(S=4, A=2, B=1024, sizes=[128, 64], act="leaky_relu"),
@@ -82,32 +82,6 @@ def build(shape):
     return t, batch
 
 
-def capture(fn, iters):
-    import torch
-
-    fn()  # warm-up: lazy allocations, module load, optimizer state
-    torch.cuda.synchronize()
-    s = torch.cuda.Stream()
-    s.wait_stream(torch.cuda.current_stream())
-    g = torch.cuda.CUDAGraph()
-    with torch.cuda.stream(s), torch.cuda.graph(g, stream=s):
-        for _ in range(iters):
-            fn()
-    torch.cuda.synchronize()
-    return g
-
-
-def time_graph(g, iters):
-    import torch
-
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    g.replay()
-    e1.record()
-    e1.synchronize()
-    return e0.elapsed_time(e1) * 1e3 / iters  # us per call
-
-
 def variants(shape, iters):
     """{(variant, what): graph} for one shape; every graph keeps its own trainer alive."""
     import torch
@@ -136,36 +110,31 @@ def variants(shape, iters):
 
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--out", required=True, help="directory for time_pdqn.json")
+    ap.add_argument("--out", required=True, help="directory for the result file")
     ap.add_argument("--reps", type=int, default=11)
     ap.add_argument("--iters", type=int, default=50)
     args = ap.parse_args()
+
+    cuda_device(__file__)
     import torch
 
-    torch.cuda.set_device(0)
     result = {"card": card_info(), "reps": args.reps, "iters_per_graph": args.iters,
               "unit": "us per call, median [min, max] over reps", "shapes": {}}
     for sname, shape in SHAPES.items():
         graphs, keep = variants(shape, args.iters)
-        times = {k: [] for k in graphs}
-        for r in range(args.reps):
-            order = sorted(graphs) if r % 2 == 0 else sorted(graphs, reverse=True)
-            for k in order:
-                times[k].append(time_graph(graphs[k], args.iters))
+        times = alternate(sorted(graphs), args.reps,
+                          lambda k, rep: replay_us(graphs[k], args.iters))
         res = {"shape": shape}
-        for (variant, what), v in times.items():
-            res.setdefault(what, {})[variant] = {"median": statistics.median(v), "min": min(v),
-                                                 "max": max(v)}
+        for variant, what in graphs:
+            v = times[(variant, what)]
+            res.setdefault(what, {})[variant] = {s: v[s] for s in ("median", "min", "max")}
         for what in ("train_batch", "next_q_forward"):
             r = res[what]
             r["materialised_over_fused"] = r["materialised"]["median"] / r["fused"]["median"]
         result["shapes"][sname] = res
         del graphs, keep
         torch.cuda.synchronize()
-    os.makedirs(args.out, exist_ok=True)
-    with open(os.path.join(args.out, "time_pdqn.json"), "w") as f:
-        json.dump(result, f, indent=1)
-    print(json.dumps(result, indent=1))
+    write_result(args.out, __file__, result)
 
 
 if __name__ == "__main__":

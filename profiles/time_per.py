@@ -12,21 +12,21 @@ and records the card's name, power limit and maximum SM clock read in the same r
 
     python profiles/time_per.py --out DIR [--reps 11] [--steps 200]
 
-Writes DIR/time_per.json and prints the same JSON.
+Writes DIR/time_per_<card>_<limit>w.json and prints the same JSON.
 """
 import argparse
 import ctypes
-import json
 import os
-import statistics
 import subprocess
 import sys
 import tempfile
-import time
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 if ROOT not in sys.path:
     sys.path.insert(0, ROOT)
+
+from profiles.timing import (alternate, card_info, cuda_device, host_steps,  # noqa: E402
+                             launch_us, transitions, write_result)
 
 CAPACITY = 1 << 20
 
@@ -67,18 +67,6 @@ extern "C" int old_sumtree_set(double* tree, int depth, const int64_t* idx, cons
 """
 
 
-def card_info():
-    q = "name,power.limit,clocks.max.sm"
-    try:
-        out = subprocess.run(["nvidia-smi", f"--query-gpu={q}", "--format=csv,noheader"],
-                             capture_output=True, text=True, timeout=60).stdout.strip()
-    except (OSError, subprocess.SubprocessError) as e:
-        out = f"nvidia-smi unavailable: {e}"
-    import torch
-
-    return {"torch_device_name": torch.cuda.get_device_name(0), "nvidia_smi": {q: out}}
-
-
 def build(cfg, dev, per):
     import bench
     from reagent_b200.replay_memory import PrioritizedReplayBuffer
@@ -89,38 +77,6 @@ def build(cfg, dev, per):
     rb.add_batch(**bench.synth_stream(CAPACITY, 0, cfg))
     t = bench.build_trainer(cfg, dev, seed=0)
     return FusedDqnStep(t, rb, cfg["B"], rng="device", online=True, per=per)
-
-
-def transitions(cfg, n):
-    import bench
-
-    st = bench.synth_stream(n, 1, cfg)
-    return [{k: v[i] for k, v in st.items()} for i in range(n)]
-
-
-def time_steps(fused, trs, steps, k0):
-    import torch
-
-    torch.cuda.synchronize()
-    t0 = time.perf_counter()
-    for i in range(steps):
-        lh = fused.step(trs[(k0 + i) % len(trs)])
-    torch.cuda.synchronize()
-    return (time.perf_counter() - t0) / steps, float(lh[0])
-
-
-def time_launches(fn, n):
-    import torch
-
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    for _ in range(5):
-        fn()
-    e0.record()
-    for _ in range(n):
-        fn()
-    e1.record()
-    e1.synchronize()
-    return e0.elapsed_time(e1) * 1e3 / n  # microseconds per launch
 
 
 def old_kernel_lib(tmp):
@@ -139,13 +95,14 @@ def old_kernel_lib(tmp):
 
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--out", required=True, help="directory for time_per.json")
+    ap.add_argument("--out", required=True, help="directory for the result file")
     ap.add_argument("--reps", type=int, default=11)
     ap.add_argument("--steps", type=int, default=200)
     ap.add_argument("--warmup", type=int, default=20)
     ap.add_argument("--launches", type=int, default=200)
     args = ap.parse_args()
 
+    dev = cuda_device(__file__)
     import numpy as np
     import torch
 
@@ -153,24 +110,21 @@ def main():
     from reagent_b200 import _lib
     from reagent_b200.replay_memory import PrioritizedUpdate
 
-    if not torch.cuda.is_available():
-        raise SystemExit("time_per.py measures on the GPU; no CUDA device is visible")
-    dev = torch.device("cuda", 0)
-    torch.cuda.set_device(dev)
     cfg = dict(bench.CONFIGS[2])
     info = card_info()
     per = PrioritizedUpdate(alpha=0.6, beta0=0.4, beta_updates=100_000, eps=1e-6)
     variants = {"plain": build(cfg, dev, None), "per": build(cfg, dev, per)}
     trs = transitions(cfg, 1000)
     for fused in variants.values():
-        time_steps(fused, trs, args.warmup, 0)
-    per_update = {k: [] for k in variants}
+        host_steps(lambda i: fused.step(trs[i % len(trs)]), args.warmup)
     last_loss = {}
-    for rep in range(args.reps):
-        order = list(variants) if rep % 2 == 0 else list(variants)[::-1]
-        for k in order:
-            dt, last_loss[k] = time_steps(variants[k], trs, args.steps, rep * args.steps)
-            per_update[k].append(dt * 1e6)
+
+    def run(k, rep):
+        us, last_loss[k] = host_steps(lambda i: variants[k].step(trs[i % len(trs)]), args.steps,
+                                      rep * args.steps)
+        return us
+
+    per_update = alternate(variants, args.reps, run)
     for fused in variants.values():
         fused.dr.raise_if_failed()
 
@@ -196,10 +150,8 @@ def main():
             assert old.old_sumtree_set(tree.data_ptr(), depth, idx.data_ptr(), val.data_ptr(), B,
                                        mx.data_ptr(), st.data_ptr(), stream) == 0
 
-        kern = {}
-        for rep in range(3):
-            for name, fn in (("batched_sumtree_set", new_update), ("one_warp_sumtree_set", old_update)):
-                kern.setdefault(name, []).append(time_launches(fn, args.launches))
+        updates = {"batched_sumtree_set": new_update, "one_warp_sumtree_set": old_update}
+        kern = alternate(updates, 3, lambda k, rep: launch_us(updates[k], args.launches))
         # both give the same tree from the same start
         tree.zero_(); mx.zero_()
         new_update()
@@ -208,8 +160,8 @@ def main():
         old_update()
         same = bool(torch.equal(a, tree))
 
-    med = {k: statistics.median(v) for k, v in per_update.items()}
-    kmed = {k: statistics.median(v) for k, v in kern.items()}
+    med = {k: v["median"] for k, v in per_update.items()}
+    kmed = {k: v["median"] for k, v in kern.items()}
     res = {
         "what": ("FusedDqnStep(rng='device', online=True).step() per update, config-2 shapes, "
                  "with and without per; the batched SumTree.set against the one-warp kernel"),
@@ -220,21 +172,18 @@ def main():
                                                           eps=per.eps)),
         "method": (f"{args.reps} alternating repetitions of {args.steps} host-timed steps "
                    f"(synchronised) per variant after {args.warmup} warm-up steps; tree "
-                   f"updates: CUDA events over {args.launches} back-to-back launches, 3 "
-                   f"repetitions, n = {B} sets on a 2^{depth}-leaf tree"),
-        "per_update_us": {k: dict(median=med[k], min=min(v), max=max(v), all=v)
-                          for k, v in per_update.items()},
+                   f"updates: CUDA events over {args.launches} back-to-back launches after 10 "
+                   f"warm-up launches, 3 alternating repetitions, n = {B} sets on a "
+                   f"2^{depth}-leaf tree"),
+        "per_update_us": per_update,
         "per_overhead_us_median": med["per"] - med["plain"],
         "per_overhead_frac_median": med["per"] / med["plain"] - 1,
-        "tree_update_us": {k: dict(median=kmed[k], all=v) for k, v in kern.items()},
+        "tree_update_us": {k: dict(median=v["median"], all=v["all"]) for k, v in kern.items()},
         "tree_update_speedup_median": kmed["one_warp_sumtree_set"] / kmed["batched_sumtree_set"],
         "tree_update_results_identical": same,
         "last_loss": last_loss,
     }
-    os.makedirs(args.out, exist_ok=True)
-    with open(os.path.join(args.out, "time_per.json"), "w") as f:
-        json.dump(res, f, indent=1)
-    print(json.dumps(res))
+    write_result(args.out, __file__, res)
 
 
 if __name__ == "__main__":

@@ -17,24 +17,23 @@ and records the card's name, power limit and maximum SM clock read in the same r
 
     python profiles/time_per_ac.py --out DIR [--reps 11] [--steps 200]
 
-Writes DIR/time_per_ac.json and prints the same JSON.
+Writes DIR/time_per_ac_<card>_<limit>w.json and prints the same JSON.
 """
 import argparse
-import json
 import os
 import statistics
 import sys
 import time
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-HERE = os.path.dirname(os.path.abspath(__file__))
-for p in (ROOT, HERE):
-    if p not in sys.path:
-        sys.path.insert(0, p)
+if ROOT not in sys.path:
+    sys.path.insert(0, ROOT)
 
-from time_per import CAPACITY, card_info, time_launches, time_steps, transitions  # noqa: E402
+from profiles.timing import (alternate, card_info, cuda_device, host_steps,  # noqa: E402
+                             launch_us, transitions, write_result)
 
 B = 2048
+CAPACITY = 1 << 20
 
 
 class EagerLoop:
@@ -78,13 +77,14 @@ def build(cfg, dev, stream, variant, per):
 
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--out", required=True, help="directory for time_per_ac.json")
+    ap.add_argument("--out", required=True, help="directory for the result file")
     ap.add_argument("--reps", type=int, default=11)
     ap.add_argument("--steps", type=int, default=200)
     ap.add_argument("--warmup", type=int, default=20)
     ap.add_argument("--launches", type=int, default=200)
     args = ap.parse_args()
 
+    dev = cuda_device(__file__)
     import random
 
     import numpy as np
@@ -94,10 +94,6 @@ def main():
     from reagent_b200 import _lib
     from reagent_b200.replay_memory import PrioritizedUpdate
 
-    if not torch.cuda.is_available():
-        raise SystemExit("time_per_ac.py measures on the GPU; no CUDA device is visible")
-    dev = torch.device("cuda", 0)
-    torch.cuda.set_device(dev)
     random.seed(1234)
     cfgs = {"sac": dict(bench.CONFIGS[4], B=B), "td3": dict(bench.CONFIGS[5], B=B)}
     info = card_info()
@@ -110,14 +106,14 @@ def main():
         del stream
         trs = transitions(cfg, 1000)
         for v in variants.values():
-            time_steps(v, trs, args.warmup, 0)
-        for k in variants:
-            per_update[k] = []
-        for rep in range(args.reps):
-            order = list(variants) if rep % 2 == 0 else list(variants)[::-1]
-            for k in order:
-                dt, last_loss[k] = time_steps(variants[k], trs, args.steps, rep * args.steps)
-                per_update[k].append(dt * 1e6)
+            host_steps(lambda i: v.step(trs[i % len(trs)]), args.warmup)
+
+        def run(k, rep):
+            us, last_loss[k] = host_steps(lambda i: variants[k].step(trs[i % len(trs)]),
+                                          args.steps, rep * args.steps)
+            return us
+
+        per_update.update(alternate(variants, args.reps, run))
         for k, v in variants.items():
             if hasattr(v, "dr"):
                 v.dr.raise_if_failed()
@@ -141,11 +137,11 @@ def main():
             tree.data_ptr(), depth, idx.data_ptr(), td.data_ptr(), B, 1.0, per.alpha, per.eps,
             p.data_ptr(), mx.data_ptr(), st.data_ptr(), cs))
 
-    wb = [time_launches(write_back, args.launches) for _ in range(3)]
+    wb = [launch_us(write_back, args.launches) for _ in range(3)]
     torch.cuda.synchronize()
     assert int(st[0]) == 0
 
-    med = {k: statistics.median(v) for k, v in per_update.items()}
+    med = {k: v["median"] for k, v in per_update.items()}
     res = {
         "what": ("per update: the eager host-RNG loop, FusedPolicyStep(rng='device', "
                  "online=True).step() without and with per, for SACTrainer (config-4 per-GPU "
@@ -158,10 +154,9 @@ def main():
         "method": (f"{args.reps} alternating repetitions of {args.steps} host-timed steps "
                    f"(synchronised) per variant after {args.warmup} warm-up steps; the eager "
                    f"loop adds no transition, the captured steps add one each; write-back: CUDA "
-                   f"events over {args.launches} back-to-back launches, 3 repetitions, n = {B} "
-                   f"sets on a 2^{depth}-leaf tree"),
-        "per_update_us": {k: dict(median=med[k], min=min(v), max=max(v), all=v)
-                          for k, v in per_update.items()},
+                   f"events over {args.launches} back-to-back launches after 10 warm-up "
+                   f"launches, 3 repetitions, n = {B} sets on a 2^{depth}-leaf tree"),
+        "per_update_us": per_update,
         "captured_vs_eager_frac_median": {a: med[f"{a}_captured"] / med[f"{a}_eager"] - 1
                                           for a in cfgs},
         "per_overhead_us_median": {a: med[f"{a}_captured_per"] - med[f"{a}_captured"]
@@ -170,10 +165,7 @@ def main():
         "last_loss": last_loss,
         "timestamp": time.strftime("%Y-%m-%dT%H:%M:%SZ", time.gmtime()),
     }
-    os.makedirs(args.out, exist_ok=True)
-    with open(os.path.join(args.out, "time_per_ac.json"), "w") as f:
-        json.dump(res, f, indent=1)
-    print(json.dumps(res))
+    write_result(args.out, __file__, res)
 
 
 if __name__ == "__main__":

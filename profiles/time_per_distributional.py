@@ -15,22 +15,20 @@ and records the card's name, power limit and maximum SM clock read in the same r
 
     python profiles/time_per_distributional.py --out DIR [--reps 11] [--steps 200]
 
-Writes DIR/time_per_distributional.json and prints the same JSON.
+Writes DIR/time_per_distributional_<card>_<limit>w.json and prints the same JSON.
 """
 import argparse
-import json
 import os
-import statistics
 import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-HERE = os.path.dirname(os.path.abspath(__file__))
-for p in (ROOT, HERE):
-    if p not in sys.path:
-        sys.path.insert(0, p)
+if ROOT not in sys.path:
+    sys.path.insert(0, ROOT)
 
-from time_per import CAPACITY, card_info, time_launches, time_steps, transitions  # noqa: E402
+from profiles.timing import (alternate, card_info, cuda_device, host_steps,  # noqa: E402
+                             launch_us, transitions, write_result)
 
+CAPACITY = 1 << 20
 C51_N, C51_QMIN, C51_QMAX = 51, -10.0, 10.0
 
 
@@ -69,13 +67,14 @@ def build(kind, cfg, dev, per):
 
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--out", required=True, help="directory for time_per_distributional.json")
+    ap.add_argument("--out", required=True, help="directory for the result file")
     ap.add_argument("--reps", type=int, default=11)
     ap.add_argument("--steps", type=int, default=200)
     ap.add_argument("--warmup", type=int, default=20)
     ap.add_argument("--launches", type=int, default=200)
     args = ap.parse_args()
 
+    dev = cuda_device(__file__)
     import numpy as np
     import torch
 
@@ -83,10 +82,6 @@ def main():
     from reagent_b200 import _lib
     from reagent_b200.replay_memory import PrioritizedUpdate
 
-    if not torch.cuda.is_available():
-        raise SystemExit("time_per_distributional.py measures on the GPU; no CUDA device is visible")
-    dev = torch.device("cuda", 0)
-    torch.cuda.set_device(dev)
     cfgs = {"qrdqn": dict(bench.CONFIGS[3]), "c51": dict(bench.CONFIGS[3], N=C51_N)}
     info = card_info()
     per = PrioritizedUpdate(alpha=0.6, beta0=0.4, beta_updates=100_000, eps=1e-6)
@@ -96,14 +91,15 @@ def main():
         variants[f"{kind}_per"] = build(kind, cfg, dev, per)
     trs = transitions(cfgs["qrdqn"], 1000)
     for fused in variants.values():
-        time_steps(fused, trs, args.warmup, 0)
-    per_update = {k: [] for k in variants}
+        host_steps(lambda i: fused.step(trs[i % len(trs)]), args.warmup)
     last_loss = {}
-    for rep in range(args.reps):
-        order = list(variants) if rep % 2 == 0 else list(variants)[::-1]
-        for k in order:
-            dt, last_loss[k] = time_steps(variants[k], trs, args.steps, rep * args.steps)
-            per_update[k].append(dt * 1e6)
+
+    def run(k, rep):
+        us, last_loss[k] = host_steps(lambda i: variants[k].step(trs[i % len(trs)]), args.steps,
+                                      rep * args.steps)
+        return us
+
+    per_update = alternate(variants, args.reps, run)
     for fused in variants.values():
         fused.dr.raise_if_failed()
 
@@ -131,16 +127,12 @@ def main():
             tree.data_ptr(), depth, idx.data_ptr(), rows.data_ptr(), B, 200.0 * 200.0, per.alpha,
             per.eps, p.data_ptr(), mx.data_ptr(), st.data_ptr(), stream))
 
-    kern = {}
-    for rep in range(3):
-        for name, fn in (("td_error_priority_update", td_update),
-                         ("row_loss_priority_update", rows_update)):
-            kern.setdefault(name, []).append(time_launches(fn, args.launches))
+    updates = {"td_error_priority_update": td_update, "row_loss_priority_update": rows_update}
+    kern = alternate(updates, 3, lambda k, rep: launch_us(updates[k], args.launches))
     torch.cuda.synchronize()
     assert int(st[0]) == 0
 
-    med = {k: statistics.median(v) for k, v in per_update.items()}
-    kmed = {k: statistics.median(v) for k, v in kern.items()}
+    med = {k: v["median"] for k, v in per_update.items()}
     res = {
         "what": ("FusedDqnStep(rng='device', online=True).step() per update for QRDQNTrainer "
                  "(config 3) and C51Trainer (config-3 trunk, A and B; N 51), with and without "
@@ -151,19 +143,16 @@ def main():
         "per": dict(alpha=per.alpha, beta0=per.beta0, beta_updates=per.beta_updates, eps=per.eps),
         "method": (f"{args.reps} alternating repetitions of {args.steps} host-timed steps "
                    f"(synchronised) per variant after {args.warmup} warm-up steps; write-backs: "
-                   f"CUDA events over {args.launches} back-to-back launches, 3 repetitions, "
-                   f"n = {B} sets on a 2^{depth}-leaf tree"),
-        "per_update_us": {k: dict(median=med[k], min=min(v), max=max(v), all=v)
-                          for k, v in per_update.items()},
+                   f"CUDA events over {args.launches} back-to-back launches after 10 warm-up "
+                   f"launches, 3 alternating repetitions, n = {B} sets on a 2^{depth}-leaf tree"),
+        "per_update_us": per_update,
         "per_overhead_us_median": {k: med[f"{k}_per"] - med[f"{k}_plain"] for k in cfgs},
         "per_overhead_frac_median": {k: med[f"{k}_per"] / med[f"{k}_plain"] - 1 for k in cfgs},
-        "priority_update_us": {k: dict(median=kmed[k], all=v) for k, v in kern.items()},
+        "priority_update_us": {k: dict(median=v["median"], all=v["all"])
+                               for k, v in kern.items()},
         "last_loss": last_loss,
     }
-    os.makedirs(args.out, exist_ok=True)
-    with open(os.path.join(args.out, "time_per_distributional.json"), "w") as f:
-        json.dump(res, f, indent=1)
-    print(json.dumps(res))
+    write_result(args.out, __file__, res)
 
 
 if __name__ == "__main__":

@@ -13,22 +13,20 @@ and records the card's name, power limit and maximum SM clock read in the same r
 
     python profiles/time_sac_value.py --out DIR [--reps 11] [--steps 100]
 
-Writes DIR/time_sac_value.json and prints the same JSON.
+Writes DIR/time_sac_value_<card>_<limit>w.json and prints the same JSON.
 """
 import argparse
-import json
 import os
 import statistics
 import sys
 import time
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-HERE = os.path.dirname(os.path.abspath(__file__))
-for p in (ROOT, HERE):
-    if p not in sys.path:
-        sys.path.insert(0, p)
+if ROOT not in sys.path:
+    sys.path.insert(0, ROOT)
 
-from time_per import card_info, time_launches, time_steps, transitions  # noqa: E402
+from profiles.timing import (alternate, card_info, cuda_device, host_steps,  # noqa: E402
+                             launch_us, transitions, write_result)
 
 SHAPES = {
     "pendulum": dict(S=3, A=1, B=256, sizes=[64, 64], acts=["leaky_relu", "leaky_relu"]),
@@ -86,13 +84,14 @@ class TrainLoop:
 
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--out", required=True, help="directory for time_sac_value.json")
+    ap.add_argument("--out", required=True, help="directory for the result file")
     ap.add_argument("--reps", type=int, default=11)
     ap.add_argument("--steps", type=int, default=100)
     ap.add_argument("--warmup", type=int, default=20)
     ap.add_argument("--launches", type=int, default=200)
     args = ap.parse_args()
 
+    dev = cuda_device(__file__)
     import random
 
     import numpy as np
@@ -104,10 +103,6 @@ def main():
     from reagent_b200.training.fused_step import FusedPolicyStep
     from reagent_b200.training.workspace import Pins
 
-    if not torch.cuda.is_available():
-        raise SystemExit("time_sac_value.py measures on the GPU; no CUDA device is visible")
-    dev = torch.device("cuda", 0)
-    torch.cuda.set_device(dev)
     random.seed(1234)
     info = card_info()
     per_update, kernel_us, last_loss = {}, {}, {}
@@ -127,36 +122,31 @@ def main():
         else:
             trs = [None]
         for v in loops.values():
-            time_steps(v, trs, args.warmup, 0)
-        for k in loops:
-            per_update[k] = []
-        for rep in range(args.reps):
-            order = list(loops) if rep % 2 == 0 else list(loops)[::-1]
-            for k in order:
-                dt, last_loss[k] = time_steps(loops[k], trs, args.steps, rep * args.steps)
-                per_update[k].append(dt * 1e6)
+            host_steps(lambda i: v.step(trs[i % len(trs)]), args.warmup)
+
+        def run(k, rep):
+            us, last_loss[k] = host_steps(lambda i: loops[k].step(trs[i % len(trs)]),
+                                          args.steps, rep * args.steps)
+            return us
+
+        per_update.update(alternate(loops, args.reps, run))
 
         # ac_value_rows_kernel alone, on the workspace of the "value" trainer
         t = loops[f"{sname}_train_batch_value"].t
         pins = Pins(dev)
-        a, _ = t._base_args(b, t._ws, pins)
-        a.loss = t._ws["value_loss"].data_ptr()
-        a.min_q_out = t._ws["min_q"].data_ptr()
-        a.log_prob_out = t._ws["log_prob"].data_ptr()
-        a.alpha = t._alpha_dev.data_ptr()
-        a.logged_action_uniform_prior = 1
+        a, _ = t._value_args(b, t._ws, pins)
         desc, lib, cs = t.value_network.arena.desc(), _lib.lib(), _lib.cur_stream()
         ws = t._ws["value"].c
 
         def value_step():
             _lib.check(lib.rb200_ac_value_step(desc, a, ws, cs), "rb200_ac_value_step")
 
-        kernel_us[sname] = [time_launches(value_step, args.launches) for _ in range(3)]
+        kernel_us[sname] = [launch_us(value_step, args.launches) for _ in range(3)]
         del loops
         torch.cuda.synchronize()
         torch.cuda.empty_cache()
 
-    med = {k: statistics.median(v) for k, v in per_update.items()}
+    med = {k: v["median"] for k, v in per_update.items()}
     res = {
         "what": ("per update: SACTrainer.train_batch without a value network, with one, and with "
                  "one plus CRR; the captured FusedPolicyStep step with a value network; "
@@ -165,10 +155,11 @@ def main():
         "shapes": SHAPES,
         "method": (f"{args.reps} alternating repetitions of {args.steps} host-timed synchronised "
                    f"updates per variant after {args.warmup} warm-up updates; the captured step "
-                   f"adds one transition to a 2^16 prioritized buffer each; the value kernel: "
-                   f"CUDA events over {args.launches} back-to-back launches, 3 repetitions"),
-        "per_update_us": {k: dict(median=med[k], min=min(v), max=max(v), all=v)
-                          for k, v in per_update.items()},
+                   f"adds one transition to a 2^16 prioritized buffer each; the value kernel "
+                   f"with the arguments SACTrainer._value_step builds: CUDA events over "
+                   f"{args.launches} back-to-back launches after 10 warm-up launches, 3 "
+                   f"repetitions"),
+        "per_update_us": per_update,
         "value_vs_no_value_frac_median": {
             s: med[f"{s}_train_batch_value"] / med[f"{s}_train_batch_no_value"] - 1
             for s in SHAPES},
@@ -179,10 +170,7 @@ def main():
         "last_loss": last_loss,
         "timestamp": time.strftime("%Y-%m-%dT%H:%M:%SZ", time.gmtime()),
     }
-    os.makedirs(args.out, exist_ok=True)
-    with open(os.path.join(args.out, "time_sac_value.json"), "w") as f:
-        json.dump(res, f, indent=1)
-    print(json.dumps(res))
+    write_result(args.out, __file__, res)
 
 
 if __name__ == "__main__":

@@ -70,17 +70,23 @@ class BehavioralCloningTrainer(ReAgentLightningModule):
         ws = self._workspace(B, pins.device)
         net = ws["net"]
         ar.forward(state, ws["scores"], save=net if do_backward else None)
-        a = _lib.BcXentArgsT()
-        a.batch, a.num_actions = B, A
-        a.logits, a.labels, a.mask = ws["scores"].data_ptr(), labels.data_ptr(), mask.data_ptr()
-        a.dz = net.dz[-1].data_ptr() if do_backward else None
-        a.loss_partials = ws["loss_partials"].data_ptr()
-        a.loss = ws["loss"].data_ptr()
-        a.tile_counter = ws["counter"].data_ptr()
+        a = self._xent_args(ws, labels, mask, do_backward)
         _lib.check(_lib.lib().rb200_bc_xent_head(a, _lib.cur_stream()), "rb200_bc_xent_head")
         if do_backward:
             backward_wgrad(ar, net, state, B)
         return ws["loss"].reshape(())
+
+    def _xent_args(self, ws, labels: torch.Tensor, mask: torch.Tensor, do_backward: bool = True):
+        """The loss head's arguments on workspace `ws`, for the fp32 [B, A] device tensors
+        `labels` (one-hot) and `mask`."""
+        a = _lib.BcXentArgsT()
+        a.batch, a.num_actions = ws["B"], self.bc_net.action_dim
+        a.logits, a.labels, a.mask = ws["scores"].data_ptr(), labels.data_ptr(), mask.data_ptr()
+        a.dz = ws["net"].dz[-1].data_ptr() if do_backward else None
+        a.loss_partials = ws["loss_partials"].data_ptr()
+        a.loss = ws["loss"].data_ptr()
+        a.tile_counter = ws["counter"].data_ptr()
+        return a
 
     # ------------------------------------------------------------------
     def train_step_gen(self, training_batch: rlt.BehavioralCloningModelInput, batch_idx: int):

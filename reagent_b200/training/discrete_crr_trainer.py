@@ -210,6 +210,19 @@ class DiscreteCRRTrainer(DQNTrainerBaseLightning):
         if q2 is not None:
             self._forward(self.q2_network_target, next_state, ws["q2t_next"])
             self._forward(q2, state, ws["q2_out"], ws["q2"] if do_backward else None)
+        a = self._critic_args(batch, ws, pins)
+        _lib.check(_lib.lib().rb200_crr_critic_head(a, _lib.cur_stream()), "rb200_crr_critic_head")
+        if do_backward:
+            for net, w in ((self.q1_network, ws["q1"]), (q2, ws["q2"])):
+                if net is not None:
+                    backward_wgrad(net.arena, w, state, B)
+                    net.arena.finish_grads()  # dueling: folded-layer gradient -> true parameters
+        return ws["critic_loss"]
+
+    def _critic_args(self, batch: rlt.DiscreteDqnInput, ws, pins: Pins):
+        """The critic head's arguments on workspace `ws`, with the draw of the next-state
+        exploration noise; `pins` keeps the tensors they point to alive."""
+        B, q2 = ws["B"], self.q2_network
         a = _lib.CrrCriticArgsT()
         a.batch, a.num_actions = B, self.num_actions
         a.actor_next = ws["actor_next"].data_ptr()
@@ -228,13 +241,7 @@ class DiscreteCRRTrainer(DQNTrainerBaseLightning):
         a.loss_partials = ws["critic_partials"].data_ptr()
         a.loss = ws["critic_loss"].data_ptr()
         a.tile_counter = ws["counter"][0:1].data_ptr()
-        _lib.check(_lib.lib().rb200_crr_critic_head(a, _lib.cur_stream()), "rb200_crr_critic_head")
-        if do_backward:
-            for net, w in ((self.q1_network, ws["q1"]), (q2, ws["q2"])):
-                if net is not None:
-                    backward_wgrad(net.arena, w, state, B)
-                    net.arena.finish_grads()  # dueling: folded-layer gradient -> true parameters
-        return ws["critic_loss"]
+        return a
 
     def _actor_step(self, batch: rlt.DiscreteDqnInput, do_backward: bool = True) -> torch.Tensor:
         """Actor losses with the current q1 (and the actor's gradient partials).  Returns the [2]
@@ -246,6 +253,16 @@ class DiscreteCRRTrainer(DQNTrainerBaseLightning):
         actor = self.actor_network
         self._forward(self.q1_network, state, ws["q1_out"])
         self._forward(actor, state, ws["actor_out"], ws["actor"] if do_backward else None)
+        a = self._actor_args(batch, ws, pins, do_backward)
+        _lib.check(_lib.lib().rb200_crr_actor_head(a, _lib.cur_stream()), "rb200_crr_actor_head")
+        if do_backward:
+            backward_wgrad(actor.arena, ws["actor"], state, B)
+        return ws["actor_loss"]
+
+    def _actor_args(self, batch: rlt.DiscreteDqnInput, ws, pins: Pins, do_backward: bool = True):
+        """The actor head's arguments on workspace `ws`, with the draw of the current-state
+        exploration noise; `pins` keeps the tensors they point to alive."""
+        B = ws["B"]
         a = _lib.CrrActorArgsT()
         a.batch, a.num_actions = B, self.num_actions
         a.actor_out, a.q1 = ws["actor_out"].data_ptr(), ws["q1_out"].data_ptr()
@@ -261,16 +278,13 @@ class DiscreteCRRTrainer(DQNTrainerBaseLightning):
         a.inv_beta = 1 / self.beta
         a.max_weight, a.entropy_coeff = float(self.max_weight), float(self.entropy_coeff)
         a.clip_limit = float(self.clip_limit)
-        a.action_activation = actor.arena.acts[-1]
+        a.action_activation = self.actor_network.arena.acts[-1]
         a.weight = ws["weight"].data_ptr()
         a.dz = ws["actor"].dz[-1].data_ptr() if do_backward else None
         a.loss_partials = ws["actor_partials"].data_ptr()
         a.loss = ws["actor_loss"].data_ptr()
         a.tile_counter = ws["counter"][1:2].data_ptr()
-        _lib.check(_lib.lib().rb200_crr_actor_head(a, _lib.cur_stream()), "rb200_crr_actor_head")
-        if do_backward:
-            backward_wgrad(actor.arena, ws["actor"], state, B)
-        return ws["actor_loss"]
+        return a
 
     def _cpe_step(self, batch: rlt.DiscreteDqnInput) -> torch.Tensor:
         """:358-367: the next-state propensities come from q1_network_target(next_state) as the

@@ -216,17 +216,22 @@ class SACTrainer(ActorCriticBase):
         B = batch.state.float_features.shape[0]
         pins = Pins(batch_device(batch.state.float_features, type(self).__name__))
         ws = self._workspace(B, pins.device)
+        a, state = self._value_args(batch, ws, pins)
+        rc = _lib.lib().rb200_ac_value_step(self._desc(self.value_network), a, ws["value"].c,
+                                            _lib.cur_stream())
+        _lib.check(rc, "rb200_ac_value_step")
+        wgrad(self.value_network.arena, ws["value"], state, B)
+        return ws["value_loss"]
+
+    def _value_args(self, batch, ws, pins):
+        """(args, state) of rb200_ac_value_step on workspace `ws`, as _base_args."""
         a, state = self._base_args(batch, ws, pins)
         a.loss = ws["value_loss"].data_ptr()
         a.min_q_out = ws["min_q"].data_ptr()
         a.log_prob_out = ws["log_prob"].data_ptr()
         a.alpha = _lib.ptr(self._alpha_dev, ws["dev"])
         a.logged_action_uniform_prior = int(bool(self.logged_action_uniform_prior))
-        rc = _lib.lib().rb200_ac_value_step(self._desc(self.value_network), a, ws["value"].c,
-                                            _lib.cur_stream())
-        _lib.check(rc, "rb200_ac_value_step")
-        wgrad(self.value_network.arena, ws["value"], state, B)
-        return ws["value_loss"]
+        return a, state
 
     def _critic_targets(self):
         if self.value_network is not None:
