@@ -31,8 +31,6 @@ class SoftUpdate(torch.optim.Optimizer):
             if key not in seen:
                 seen[key] = True
                 self._pairs.append((ta, sa))
-        # set by a trainer when the Polyak update was already fused into the Adam launch
-        self.fused_ahead = False
 
     @classmethod
     def make_optimizer_scheduler(cls, target_params, source_params, tau):
@@ -45,19 +43,19 @@ class SoftUpdate(torch.optim.Optimizer):
         if closure is not None:
             with torch.enable_grad():
                 loss = closure()
-        if self.fused_ahead:
-            self.fused_ahead = False
-            return loss
-        tau = self.param_groups[0]["tau"]
         for ta, sa in self._pairs:
-            if ta is sa:
-                continue  # aliased target: soft_update.py:64-67
-            _lib.check(
-                _lib.lib().rb200_soft_update(ta.flat.data_ptr(), sa.flat.data_ptr(), ta.n,
-                                             float(tau), float(1.0 - tau), _lib.cur_stream()),
-                "rb200_soft_update")
-            ta.data_epoch = getattr(ta, "data_epoch", 0) + 1
+            if ta is not sa:  # aliased target: soft_update.py:64-67
+                self.update(ta, sa)
         return loss
+
+    def update(self, ta, sa):
+        """target arena `ta` <- tau * source arena `sa` + (1 - tau) * `ta`."""
+        tau = self.param_groups[0]["tau"]
+        _lib.check(
+            _lib.lib().rb200_soft_update(ta.flat.data_ptr(), sa.flat.data_ptr(), ta.n,
+                                         float(tau), float(1.0 - tau), _lib.cur_stream()),
+            "rb200_soft_update")
+        ta.data_epoch = getattr(ta, "data_epoch", 0) + 1
 
     def zero_grad(self, set_to_none: bool = True):
         pass

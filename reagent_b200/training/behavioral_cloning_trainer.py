@@ -103,11 +103,8 @@ class BehavioralCloningTrainer(ReAgentLightningModule):
         synchronisation and without the data checks of _check_input.  With `process_group`
         (data parallel, equal shards per rank) the gradient is averaged over the ranks before
         Adam, as in DQNTrainer.train_batch."""
-        from .data_parallel import dp_fused_step
-
-        opts = self.optimizers()
         self._step(training_batch)
-        dp_fused_step(opts[0], self.bc_net.arena, process_group)
+        self.adam_step(self.bc_net.arena, process_group)
         self.all_batches_processed += 1
         return self._ws["loss"]
 

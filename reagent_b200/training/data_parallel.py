@@ -114,7 +114,7 @@ def p2p_for(group):
     return _EXCHANGES.get(id(group) if group is not None else 0)
 
 
-def dp_fused_step(opt, arena, process_group, **kw):
+def dp_fused_step(opt, process_group, **kw):
     """One optimizer sub-step of a data-parallel update.  `process_group` None: single rank.
     With a P2P exchange enabled for the group: ONE launch (gradient exchange fused into the
     Adam kernel over NVLink peer memory).  Otherwise: rb200_grad_reduce + NCCL all-reduce +
@@ -126,6 +126,6 @@ def dp_fused_step(opt, arena, process_group, **kw):
         return opt.fused_step(dp=ex, **kw)
     from .workspace import reduced_grad
 
-    g = reduced_grad(arena)
+    g = reduced_grad(opt.arena)
     scale = allreduce_mean_(g, process_group)
     return opt.fused_step(grad=g, grad_scale=scale, **kw)

@@ -333,34 +333,20 @@ class DiscreteCRRTrainer(DQNTrainerBaseLightning):
         its network's Adam launch.  Returns (critic losses [2], actor losses [2] or None).  With
         `process_group` (data parallel, equal shards per rank) every gradient is averaged over
         the ranks before its Adam step."""
-        from .data_parallel import dp_fused_step
-
-        opts = self.optimizers()
-        tau = self.tau
         closs = self._critic_step(training_batch)
-        i = 0
-        dp_fused_step(opts[i], self.q1_network.arena, process_group,
-                      target=self.q1_network_target.arena, tau=tau)
-        i += 1
+        self.adam_step(self.q1_network.arena, process_group)
         if self.q2_network:
-            dp_fused_step(opts[i], self.q2_network.arena, process_group,
-                          target=self.q2_network_target.arena, tau=tau)
-            i += 1
+            self.adam_step(self.q2_network.arena, process_group)
         aloss = None
-        at, asrc = self.actor_network_target.arena, self.actor_network.arena
         if self._actor_batch(batch_idx):
             aloss = self._actor_step(training_batch)
-            dp_fused_step(opts[i], asrc, process_group, target=at, tau=tau)
+            self.adam_step(self.actor_network.arena, process_group)
         else:  # no Adam launch to fold it into: the actor target's soft update on its own
-            _lib.check(_lib.lib().rb200_soft_update(at.flat.data_ptr(), asrc.flat.data_ptr(), at.n,
-                                                    float(tau), float(1.0 - tau),
-                                                    _lib.cur_stream()), "rb200_soft_update")
-        i += 1
+            self.soft_update(self.actor_network.arena)
         if self.calc_cpe_in_training:
             self.cpe_losses = self._cpe_step(training_batch)
-            dp_fused_step(opts[i], self.reward_network.arena, process_group)
-            dp_fused_step(opts[i + 1], self.q_network_cpe.arena, process_group,
-                          target=self.q_network_cpe_target.arena, tau=tau)
+            self.adam_step(self.reward_network.arena, process_group)
+            self.adam_step(self.q_network_cpe.arena, process_group)
         self.all_batches_processed += 1
         return closs, aloss
 

@@ -74,12 +74,8 @@ class DistributionalStep:
         """`importance_weights` ([B] fp32 on the batch's device, prioritized replay): the loss
         becomes mean_b(w_b * loss_b) over the per-row losses and row b of the head gradient is
         scaled by w_b."""
-        from .data_parallel import dp_fused_step
-
-        opts = self.optimizers()
         self._step(training_batch, sample_weight=importance_weights)
-        dp_fused_step(opts[0], self.q_network.arena, process_group,
-                      target=self.q_network_target.arena, tau=self.tau)
+        self.adam_step(self.q_network.arena, process_group)
         self.all_batches_processed += 1
         return self._ws["loss"]
 

@@ -332,20 +332,14 @@ class DQNTrainer(DQNTrainerBaseLightning):
         gradient is summed over ranks and scaled by 1/world before Adam (every loss is a batch
         mean, SURVEY.md 8e) -- inside the Adam kernel over NVLink peer memory when
         data_parallel.enable_p2p(group) was called, else by ONE NCCL all-reduce."""
-        opts = self.optimizers()
         self._td_step(training_batch, sample_weight=importance_weights)
         tcp = self._tc_pack_in_adam() if self._last_td_call[-1] is not None else None
-        from .data_parallel import dp_fused_step
-
-        packed = dp_fused_step(opts[0], self.q_network.arena, process_group,
-                               target=self.q_network_target.arena, tau=self.tau, tc_pack=tcp)
-        if packed:
+        if self.adam_step(self.q_network.arena, process_group, tc_pack=tcp):
             self._tc_images_state = self._tc_state()
         if self.calc_cpe_in_training:
             cpe = self._calculate_cpes(training_batch, self._cpe_next_mask(training_batch))
-            dp_fused_step(opts[1], self.reward_network.arena, process_group)
-            dp_fused_step(opts[2], self.q_network_cpe.arena, process_group,
-                          target=self.q_network_cpe_target.arena, tau=self.tau)
+            self.adam_step(self.reward_network.arena, process_group)
+            self.adam_step(self.q_network_cpe.arena, process_group)
             self.cpe_losses = cpe
         self.all_batches_processed += 1
         return self._ws["loss"]

@@ -61,6 +61,7 @@ def _query_keyword(rb) -> str:
 class FusedDqnStep:
     _per_trainers = (DQNTrainer, QRDQNTrainer, C51Trainer)  # exact types `per` covers
     _index_buffers = 2  # of a device draw: the prefetch path alternates two
+    _beta_net = "q_network"  # the network whose Adam step count anneals per's beta
 
     def __init__(self, trainer, replay_buffer, batch_size: int, process_group=None,
                  slots: int = 2, prefetch: bool = False, shard=None, rng: str = "host",
@@ -242,7 +243,7 @@ class FusedDqnStep:
     def _per_train(self, batch):
         """Importance weights of the drawn rows -> weighted update -> priority write-back."""
         idx = self._idx_buf[0]
-        opt = self.trainer.optimizers()[0]  # its Adam step count anneals beta
+        opt = self.trainer.optimizer_of(getattr(self.trainer, self._beta_net).arena)
         opt._ensure_state()
         self.dr.importance_weights(idx, opt.step_t, self.per, self.weights)
         loss = self._train_batch(batch, importance_weights=self.weights)
@@ -420,6 +421,7 @@ class FusedPolicyStep(FusedDqnStep):
     _loss_width = 2
     _per_trainers = (SACTrainer, TD3Trainer)  # the exact types it covers, with or without per
     _index_buffers = 1
+    _beta_net = "q1_network"
 
     def __init__(self, trainer, replay_buffer, batch_size: int, action_low, action_high,
                  online: bool = True, per: Optional[PrioritizedUpdate] = None,

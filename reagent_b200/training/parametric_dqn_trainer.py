@@ -166,15 +166,11 @@ class ParametricDQNTrainer(RLTrainerMixin, ReAgentLightningModule):
 
     def train_batch(self, training_batch: rlt.ParametricDqnInput, batch_idx: int = 0,
                     process_group=None):
-        from .data_parallel import dp_fused_step
-
-        opts = self.optimizers()
         self._td_step(training_batch)
-        dp_fused_step(opts[0], self.q_network.arena, process_group,
-                      target=self.q_network_target.arena, tau=self.tau)
+        self.adam_step(self.q_network.arena, process_group)
         if self.reward_network is not None:
             self._reward_step(training_batch)
-            dp_fused_step(opts[1], self.reward_network.arena, process_group)
+            self.adam_step(self.reward_network.arena, process_group)
         self.all_batches_processed += 1
         return self._ws["loss"]
 

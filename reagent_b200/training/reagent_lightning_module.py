@@ -12,6 +12,9 @@ import logging
 
 import torch
 
+from ..optimizer import FusedAdam, SoftUpdate
+from .data_parallel import dp_fused_step
+
 logger = logging.getLogger(__name__)
 
 
@@ -126,8 +129,40 @@ class ReAgentLightningModule(torch.nn.Module):
 
     def optimizers(self, use_pl_optimizer: bool = True):
         if self._optimizers_cache is None:
-            self._optimizers_cache = [o["optimizer"] for o in self.configure_optimizers()]
+            opts = [o["optimizer"] for o in self.configure_optimizers()]
+            # which optimizer trains each network arena, and which target its SoftUpdate moves
+            # with it: the fast path's Adam and Polyak launches follow configure_optimizers()
+            self._adam_of = {o.arena: o for o in opts if isinstance(o, FusedAdam)}
+            self._polyak_of = {sa: (ta, o) for o in opts if isinstance(o, SoftUpdate)
+                               for ta, sa in o._pairs}
+            self._optimizers_cache = opts
         return self._optimizers_cache
+
+    def optimizer_of(self, arena):
+        """The FusedAdam / FusedAdamW of configure_optimizers() that trains `arena`."""
+        self.optimizers()
+        opt = self._adam_of.get(arena)
+        if opt is None:
+            raise KeyError(f"no optimizer of {type(self).__name__}.configure_optimizers() trains "
+                           "this network (was it moved after optimizers() was first called?)")
+        return opt
+
+    def adam_step(self, arena, process_group=None, polyak: bool = True, **kw):
+        """The Adam step of `arena` (data_parallel.dp_fused_step), with the Polyak update of the
+        target that configure_optimizers()' SoftUpdate pairs with it folded into the same launch
+        when `polyak` is set and there is one.  Returns what FusedAdam.fused_step returns."""
+        opt = self.optimizer_of(arena)
+        pair = self._polyak_of.get(arena) if polyak else None
+        if pair is not None:
+            kw.update(target=pair[0], tau=pair[1].param_groups[0]["tau"])
+        return dp_fused_step(opt, process_group, **kw)
+
+    def soft_update(self, arena):
+        """The Polyak update of the target paired with `arena`, as a launch of its own (a
+        batch that moves the target without an Adam step of `arena`)."""
+        self.optimizers()
+        target, su = self._polyak_of[arena]
+        su.update(target, arena)
 
     def training_step(self, batch, batch_idx: int, optimizer_idx: int = 0):
         assert (optimizer_idx == 0) or (self._num_optimizing_steps > 1)

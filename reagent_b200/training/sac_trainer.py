@@ -282,36 +282,21 @@ class SACTrainer(ActorCriticBase):
         `importance_weights` ([B] fp32 on the batch's device, prioritized replay): each critic
         loss becomes mean_b(w_b * (q_b - y_b)^2); the actor, alpha and value losses stay
         unweighted."""
-        opts = self.optimizers()
-        i = 0
-        q1t, q2t = self._critic_targets()
-        closs = self._critic_step(training_batch, self.actor_network, q1t, q2t,
+        closs = self._critic_step(training_batch, self.actor_network, *self._critic_targets(),
                                   self._fill_critic, sample_weight=importance_weights)
-        self._dp_step(opts[i], self.q1_network.arena, None if q1t is None else q1t.arena,
-                      process_group)
-        i += 1
+        self.adam_step(self.q1_network.arena, process_group)
         if self.q2_network:
-            self._dp_step(opts[i], self.q2_network.arena, None if q2t is None else q2t.arena,
-                          process_group)
-            i += 1
+            self.adam_step(self.q2_network.arena, process_group)
         aloss = self._actor_step(training_batch, self._fill_actor)
-        self._dp_step(opts[i], self.actor_network.arena, None, process_group)
-        i += 1
+        self.adam_step(self.actor_network.arena, process_group)
         if self.alpha_optimizer is not None:
             arena = self._alpha_arena()
             arena.gpart = self._ws["alpha_grad"]
             arena.grad_ready = True
-            self._dp_step(opts[i], arena, None, process_group, exp_out=self._alpha_dev)
+            self.adam_step(arena, process_group, exp_out=self._alpha_dev)
             self.entropy_temperature = self._alpha_dev
-            i += 1
         if self.value_network is not None:
             self._value_step(training_batch)
-            self._dp_step(opts[i], self.value_network.arena, self.value_network_target.arena,
-                          process_group)
+            self.adam_step(self.value_network.arena, process_group)
         self.all_batches_processed += 1
         return closs, aloss
-
-    def _dp_step(self, opt, arena, target, process_group, exp_out=None):
-        from .data_parallel import dp_fused_step
-
-        dp_fused_step(opt, arena, process_group, target=target, tau=self.tau, exp_out=exp_out)

@@ -106,28 +106,16 @@ class TD3Trainer(ActorCriticBase):
         """Fast path; Polyak updates fused into the Adam launches on policy-update batches.
         `importance_weights` ([B] fp32 on the batch's device, prioritized replay): each critic
         loss becomes mean_b(w_b * (q_b - y_b)^2); the actor loss stays unweighted."""
-        opts = self.optimizers()
         upd = batch_idx % self.delayed_policy_update == 0
         closs = self._critic_step(training_batch, self.actor_network_target,
                                   self.q1_network_target, self.q2_network_target, self._fill,
                                   sample_weight=importance_weights)
-        i = 0
-        self._dp_step(opts[i], self.q1_network.arena,
-                      self.q1_network_target.arena if upd else None, process_group)
-        i += 1
+        self.adam_step(self.q1_network.arena, process_group, polyak=upd)
         if self.q2_network:
-            self._dp_step(opts[i], self.q2_network.arena,
-                          self.q2_network_target.arena if upd else None, process_group)
-            i += 1
+            self.adam_step(self.q2_network.arena, process_group, polyak=upd)
         aloss = None
         if upd:
             aloss = self._actor_step(training_batch, self._fill)
-            self._dp_step(opts[i], self.actor_network.arena, self.actor_network_target.arena,
-                          process_group)
+            self.adam_step(self.actor_network.arena, process_group)
         self.all_batches_processed += 1
         return closs, aloss
-
-    def _dp_step(self, opt, arena, target, process_group):
-        from .data_parallel import dp_fused_step
-
-        dp_fused_step(opt, arena, process_group, target=target, tau=self.tau)
