@@ -398,6 +398,83 @@ typedef struct rb200_crr_actor_args {
 } rb200_crr_actor_args_t;
 int rb200_crr_actor_head(const rb200_crr_actor_args_t* args, void* stream);
 
+/* Policy gradient (rb200_pg.cu): ReinforceTrainer and PPOTrainer,                     */
+/* reagent/training/reinforce_trainer.py and ppo_trainer.py.  A batch is packed: the    */
+/* rows of n_traj trajectories one after another, trajectory t at rows                  */
+/* [offsets[t], offsets[t + 1]).                                                        */
+/* rb200_pg_returns, per trajectory (utils.py discounted_returns and whiten):           */
+/*   r = min(reward, reward_clip)    (upper bound only)                                 */
+/*   gamma != 0: running = r_t + gamma * running from the last row back, each op        */
+/*               rounded to fp32 in the reference's order (bit-identical returns)       */
+/*   norm: WHITEN (x - mean) / (std + EPS), WHITEN_NO_MEAN x / (std + EPS),              */
+/*         SUBTRACT_MEAN x - mean; std is the population std, mean/var in double        */
+/*   offset_clamp_min: max(x, 0)                                                        */
+/* One warp per trajectory, any length.  Allocates nothing (graph-capturable).          */
+#define RB200_PG_NORM_NONE 0
+#define RB200_PG_NORM_WHITEN 1
+#define RB200_PG_NORM_WHITEN_NO_MEAN 2
+#define RB200_PG_NORM_SUBTRACT_MEAN 3
+#define RB200_PG_WHITEN_EPS 2.220446049250313e-16 /* np.finfo(float).eps */
+typedef struct rb200_pg_returns_args {
+  int32_t n_traj;
+  const int32_t* offsets;          /* [n_traj + 1] */
+  const float* reward;             /* [R] */
+  float reward_clip, gamma;
+  int32_t norm;                    /* RB200_PG_NORM_* */
+  int32_t offset_clamp_min;
+  float* returns;                  /* [R] */
+} rb200_pg_returns_args_t;
+int rb200_pg_returns(const rb200_pg_returns_args_t* args, void* stream);
+
+/* rb200_pg_head, one warp per row, 1 <= num_actions <= 1024:                           */
+/*   x = (scores + (-1e10) * (1 - mask)) / temperature,  a = first arg max of action     */
+/*   log_pi = log_softmax(x)[a]                                                          */
+/*   advantage: RETURNS   adv = returns                                                  */
+/*              BASELINE  adv = returns - value,              value target y = returns    */
+/*              TD        y = min(reward, reward_clip) + gamma * nt * V',  adv = y - value, */
+/*                        then max(adv, 0) with offset_clamp_min.  V' = next_value, or    */
+/*                        without it the next row's value (0 after a trajectory's last    */
+/*                        row); nt = not_terminal, or without it 0 on a last row, else 1  */
+/*   REINFORCE: loss[0] = -sum adv * elig, elig = log_pi, or with logged_log_prob         */
+/*              exp(min(log_pi - logged, log_clip_param)) (gradient 0 where it clamps)    */
+/*   PPO:       loss[0] = -sum min(adv * rho, adv * clamp(rho, ppo_clip_lo, ppo_clip_hi)) */
+/*              - entropy_weight * sum_rows H(softmax(x)),  rho = exp(log_pi - logged)    */
+/*   loss[1] = value_scale * sum (value - y)^2,  dz_value = 2 * value_scale * (value - y) */
+/*   dz = d loss[0] / d scores (the 1/temperature included; the mask adds nothing)       */
+/* Sums in a fixed order (deterministic); allocates nothing.                             */
+#define RB200_PG_ROWS_PER_BLOCK 8
+#define RB200_PG_LOSS_REINFORCE 0
+#define RB200_PG_LOSS_PPO 1
+#define RB200_PG_ADV_RETURNS 0
+#define RB200_PG_ADV_BASELINE 1
+#define RB200_PG_ADV_TD 2
+typedef struct rb200_pg_head_args {
+  int32_t rows, num_actions, n_traj;
+  const int32_t* offsets;          /* [n_traj + 1] */
+  const float* scores;             /* [R,A] policy net output, before the mask */
+  const float* mask;               /* [R,A] possible_actions_mask or NULL */
+  const float* action;             /* [R,A] one-hot logged action */
+  const float* logged_log_prob;    /* [R]: PPO; off-policy REINFORCE; else NULL */
+  const float* returns;            /* [R] rb200_pg_returns output (RETURNS, BASELINE) */
+  const float* value;              /* [R] V(state) (BASELINE, TD) or NULL */
+  const float* next_value;         /* [R] V(next_state) or NULL (TD) */
+  const float* reward;             /* [R] (TD) */
+  const float* not_terminal;       /* [R] or NULL (TD) */
+  float temperature, gamma, reward_clip, log_clip_param, entropy_weight;
+  float ppo_clip_lo, ppo_clip_hi;  /* float(1 - eps), float(1 + eps), rounded from double */
+  float value_scale;               /* 1/T: MSELoss(mean) of one trajectory; 1: MSELoss(sum) */
+  int32_t loss_kind;               /* RB200_PG_LOSS_* */
+  int32_t advantage_kind;          /* RB200_PG_ADV_* */
+  int32_t offset_clamp_min;        /* TD advantage only */
+  float* advantage_out;            /* [R] or NULL */
+  float* dz;                       /* [R,A] or NULL */
+  float* dz_value;                 /* [R] or NULL */
+  float* loss_partials;            /* 2 * ceil(R / RB200_PG_ROWS_PER_BLOCK) */
+  float* loss;                     /* [2]: policy loss, value loss */
+  uint32_t* tile_counter;          /* [1] zero-initialised, self-resetting */
+} rb200_pg_head_args_t;
+int rb200_pg_head(const rb200_pg_head_args_t* args, void* stream);
+
 /* ------------------------------------------------------------------------- */
 /* QR-DQN (reagent/training/qrdqn_trainer.py:108-194).  The [hidden -> A*N] head  */
 /* is too wide for a row tile, so it runs as 2-D tiled launches:                   */

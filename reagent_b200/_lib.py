@@ -214,6 +214,32 @@ class CrrActorArgsT(C.Structure):
                 ("dz", _vp), ("loss_partials", _vp), ("loss", _vp), ("tile_counter", _vp)]
 
 
+PG_ROWS_PER_BLOCK = 8  # rb200_pg_head: loss_partials holds 2 * ceil(rows / 8) floats
+PG_NORM_NONE, PG_NORM_WHITEN, PG_NORM_WHITEN_NO_MEAN, PG_NORM_SUBTRACT_MEAN = 0, 1, 2, 3
+PG_LOSS_REINFORCE, PG_LOSS_PPO = 0, 1
+PG_ADV_RETURNS, PG_ADV_BASELINE, PG_ADV_TD = 0, 1, 2
+
+
+class PgReturnsArgsT(C.Structure):
+    _fields_ = [("n_traj", C.c_int32), ("offsets", _vp), ("reward", _vp),
+                ("reward_clip", C.c_float), ("gamma", C.c_float), ("norm", C.c_int32),
+                ("offset_clamp_min", C.c_int32), ("returns", _vp)]
+
+
+class PgHeadArgsT(C.Structure):
+    _fields_ = [("rows", C.c_int32), ("num_actions", C.c_int32), ("n_traj", C.c_int32),
+                ("offsets", _vp), ("scores", _vp), ("mask", _vp), ("action", _vp),
+                ("logged_log_prob", _vp), ("returns", _vp), ("value", _vp),
+                ("next_value", _vp), ("reward", _vp), ("not_terminal", _vp),
+                ("temperature", C.c_float), ("gamma", C.c_float), ("reward_clip", C.c_float),
+                ("log_clip_param", C.c_float), ("entropy_weight", C.c_float),
+                ("ppo_clip_lo", C.c_float), ("ppo_clip_hi", C.c_float), ("value_scale", C.c_float),
+                ("loss_kind", C.c_int32), ("advantage_kind", C.c_int32),
+                ("offset_clamp_min", C.c_int32), ("advantage_out", _vp), ("dz", _vp),
+                ("dz_value", _vp), ("loss_partials", _vp), ("loss", _vp),
+                ("tile_counter", _vp)]
+
+
 class CpeArgsT(C.Structure):
     _fields_ = [("batch", C.c_int32), ("num_actions", C.c_int32), ("num_metrics", C.c_int32),
                 ("next_scores", _vp), ("mask", _vp), ("temperature", C.c_float), ("action", _vp),
@@ -336,6 +362,8 @@ def _declare(lib):
     lib.rb200_bc_xent_head.argtypes = [C.POINTER(BcXentArgsT), _vp]
     lib.rb200_crr_critic_head.argtypes = [C.POINTER(CrrCriticArgsT), _vp]
     lib.rb200_crr_actor_head.argtypes = [C.POINTER(CrrActorArgsT), _vp]
+    lib.rb200_pg_returns.argtypes = [C.POINTER(PgReturnsArgsT), _vp]
+    lib.rb200_pg_head.argtypes = [C.POINTER(PgHeadArgsT), _vp]
     lib.rb200_replay_add_device.argtypes = [C.POINTER(AddArgsT), _vp]
     lib.rb200_sumtree_set_device.argtypes = [_vp, C.c_int32, _vp, _vp, C.c_int32, _vp, _vp, _vp]
     lib.rb200_per_draw_indices.argtypes = [C.POINTER(PerDrawArgsT), _vp]

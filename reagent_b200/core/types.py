@@ -200,3 +200,50 @@ class BehavioralCloningModelInput(TensorDataClass):
     def batch_size(self):
         assert self.state.float_features.ndim == 2
         return self.state.float_features.size()[0]
+
+
+@dataclass
+class PolicyGradientInput(TensorDataClass):
+    """core/types.py:919-966: ONE trajectory -- its states, the logged one-hot actions [T, A],
+    rewards [T] and log-probabilities [T] of the logged actions, and optionally the possible
+    actions, the next states and a per-step not_terminal [T] (None: a complete episode that
+    ends in a terminal state)."""
+    state: FeatureData
+    action: torch.Tensor
+    reward: torch.Tensor
+    log_prob: torch.Tensor
+    possible_actions_mask: Optional[torch.Tensor] = None
+    next_state: Optional[FeatureData] = None
+    not_terminal: Optional[torch.Tensor] = None
+
+    @classmethod
+    def input_prototype(cls, action_dim=2, batch_size=10, state_dim=3):
+        return cls(
+            state=FeatureData(float_features=torch.randn(batch_size, state_dim)),
+            action=torch.nn.functional.one_hot(
+                torch.randint(high=action_dim, size=(batch_size,)), num_classes=action_dim),
+            reward=torch.rand(batch_size),
+            log_prob=torch.log(torch.rand(batch_size)),
+            possible_actions_mask=torch.ones(batch_size, action_dim),
+        )
+
+    @classmethod
+    def from_dict(cls, d):
+        next_observation = d.get("next_observation", None)
+        return cls(
+            state=FeatureData(float_features=d["observation"]),
+            action=d["action"],
+            reward=d["reward"],
+            log_prob=d["log_prob"],
+            possible_actions_mask=d.get("possible_actions_mask", None),
+            next_state=(FeatureData(float_features=next_observation)
+                        if next_observation is not None else None),
+            not_terminal=d.get("not_terminal", None),
+        )
+
+    def __len__(self):
+        assert self.action.ndim == 2
+        return len(self.action)
+
+    def batch_size(self):
+        return len(self)

@@ -2,7 +2,8 @@
 the reference's flow (reagent/model_managers/model_manager.py:84-96 and
 discrete/discrete_dqn.py:63-116, discrete/discrete_qrdqn.py:73-121,
 discrete/discrete_c51dqn.py:43-88, parametric/parametric_dqn.py:45-81,
-actor_critic/sac.py:80-113, actor_critic/td3.py:70-102, discrete/discrete_crr.py:104-179): build the networks from the net
+actor_critic/sac.py:80-113, actor_critic/td3.py:70-102, discrete/discrete_crr.py:104-179,
+policy_gradient/reinforce.py, policy_gradient/ppo.py): build the networks from the net
 builders, copy the target, hand everything to the trainer; `create_policy` gives the online
 act-time policy.  Serving modules, data modules and reporters are out of scope (SURVEY.md
 section 2 rows 8, 12, 15, 16)."""
@@ -16,7 +17,8 @@ from ..net_builder import (ActorFullyConnected, Categorical, DiscreteActorFullyC
                            Quantile, ValueFullyConnected)
 from ..optimizer import Optimizer__Union
 from ..training import (C51Trainer, CRRWeightFn, DiscreteCRRTrainer, DQNTrainer,
-                        ParametricDQNTrainer, QRDQNTrainer, SACTrainer, TD3Trainer)
+                        ParametricDQNTrainer, PPOTrainer, QRDQNTrainer, ReinforceTrainer,
+                        SACTrainer, TD3Trainer)
 
 
 def _device(use_gpu: bool):
@@ -331,3 +333,100 @@ class TD3(_ActorPolicyMixin):
             actor_network_optimizer=self.actor_network_optimizer,
             minibatch_size=self.minibatch_size, noise_variance=self.noise_variance,
             noise_clip=self.noise_clip, delayed_policy_update=self.delayed_policy_update).to(dev)
+
+
+class _PolicyGradientManager:
+    """What Reinforce and PPO share (reagent/model_managers/policy_gradient/reinforce.py and
+    ppo.py): the policy network from `policy_net_builder` (a discrete-DQN builder, because it
+    takes possible_actions_mask), an optional value network, and ONE cached Policy of that
+    network and a SoftmaxActionSampler, which the trainer holds and create_policy returns."""
+    _name = ""
+    _trainer_fields = ()
+
+    def __post_init__(self):
+        self._policy = None
+        assert len(self.actions) > 1, (
+            f"{self._name} needs at least 2 actions. Got {self.actions}.")
+
+    @property
+    def action_names(self) -> List[str]:
+        return self.actions
+
+    def _create_policy(self, policy_network):
+        from ..gym.policies import Policy, SoftmaxActionSampler
+
+        if self._policy is None:
+            sampler = SoftmaxActionSampler(temperature=self.sampler_temperature)
+            self._policy = Policy(scorer=policy_network, sampler=sampler)
+        return self._policy
+
+    def create_policy(self, trainer_module, serving: bool = False, normalization_data_map=None):
+        if serving:
+            raise NotImplementedError("serving modules are out of scope of reagent_b200")
+        return self._create_policy(trainer_module.scorer)
+
+    def build_trainer(self, normalization_data_map: Dict[str, NormalizationData], use_gpu: bool,
+                      reward_options=None):
+        dev = _device(use_gpu)
+        s_norm = normalization_data_map[NormalizationKey.STATE]
+        policy_network = self.policy_net_builder.build_q_network(
+            None, s_norm, len(self.actions)).to(dev)
+        value_net = None
+        if self.value_net_builder is not None:
+            value_net = self.value_net_builder.build_value_network(s_norm).to(dev)
+        kw = {k: getattr(self, k) for k in self._trainer_fields}
+        return self._trainer(policy=self._create_policy(policy_network), value_net=value_net,
+                             actions=self.actions, **kw).to(dev)
+
+
+@dataclass
+class Reinforce(_PolicyGradientManager):
+    """reagent/model_managers/policy_gradient/reinforce.py with its `trainer_param`
+    (ReinforceTrainerParameters) flattened into the manager, as DiscreteCRR does."""
+    actions: List[str] = field(default_factory=list)
+    gamma: float = 0.0
+    optimizer: Optimizer__Union = field(default_factory=Optimizer__Union.default)
+    optimizer_value_net: Optimizer__Union = field(default_factory=Optimizer__Union.default)
+    off_policy: bool = False
+    reward_clip: float = 1e6
+    clip_param: float = 1e6
+    normalize: bool = True
+    subtract_mean: bool = True
+    offset_clamp_min: bool = False
+    policy_net_builder: Union[Dueling, FullyConnected] = field(default_factory=Dueling)
+    value_net_builder: Optional[ValueFullyConnected] = None
+    sampler_temperature: float = 1.0
+
+    _name = "REINFORCE"
+    _trainer = ReinforceTrainer
+    _trainer_fields = ("gamma", "optimizer", "optimizer_value_net", "off_policy", "reward_clip",
+                       "clip_param", "normalize", "subtract_mean", "offset_clamp_min")
+
+
+@dataclass
+class PPO(_PolicyGradientManager):
+    """reagent/model_managers/policy_gradient/ppo.py with its `trainer_param`
+    (PPOTrainerParameters) flattened into the manager."""
+    actions: List[str] = field(default_factory=list)
+    gamma: float = 0.9
+    optimizer: Optimizer__Union = field(default_factory=Optimizer__Union.default)
+    optimizer_value_net: Optimizer__Union = field(default_factory=Optimizer__Union.default)
+    reward_clip: float = 1e6
+    normalize: bool = True
+    subtract_mean: bool = True
+    offset_clamp_min: bool = False
+    update_freq: int = 1
+    update_epochs: int = 1
+    ppo_batch_size: int = 1
+    ppo_epsilon: float = 0.2
+    entropy_weight: float = 0.0
+    td_error_advantage: bool = False
+    policy_net_builder: Union[Dueling, FullyConnected] = field(default_factory=Dueling)
+    value_net_builder: Optional[ValueFullyConnected] = None
+    sampler_temperature: float = 1.0
+
+    _name = "PPO"
+    _trainer = PPOTrainer
+    _trainer_fields = ("gamma", "optimizer", "optimizer_value_net", "reward_clip", "normalize",
+                       "subtract_mean", "offset_clamp_min", "update_freq", "update_epochs",
+                       "ppo_batch_size", "ppo_epsilon", "entropy_weight", "td_error_advantage")

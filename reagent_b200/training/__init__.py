@@ -4,7 +4,9 @@ from .discrete_crr_trainer import DiscreteCRRTrainer  # noqa: F401
 from .dqn_trainer import BCQConfig, DQNTrainer  # noqa: F401
 from .loop import run_update  # noqa: F401
 from .parametric_dqn_trainer import ParametricDQNTrainer  # noqa: F401
+from .ppo_trainer import PPOTrainer  # noqa: F401
 from .qrdqn_trainer import QRDQNTrainer  # noqa: F401
 from .reagent_lightning_module import ReAgentLightningModule  # noqa: F401
+from .reinforce_trainer import ReinforceTrainer  # noqa: F401
 from .sac_trainer import CRRWeightFn, SACTrainer  # noqa: F401
 from .td3_trainer import TD3Trainer  # noqa: F401
