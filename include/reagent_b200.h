@@ -860,6 +860,69 @@ int rb200_per_priority_update_rows(double* tree, int32_t depth, const int64_t* i
                                    int32_t* status, void* stream);
 
 /* ------------------------------------------------------------------------- */
+/* MDN-RNN (reagent/models/mdn_rnn.py, reagent/training/world_model/mdnrnn_trainer.py):  */
+/* an nn.LSTM over cat(action, state) and a mixture-density head gmm_linear on every     */
+/* step's top hidden state.  Three launches per update, then Adam:                      */
+/*   rb200_mdnrnn_forward   per row tile, every step and layer (h / c in shared memory), */
+/*                          the head, the outputs, and (with targets) the three losses   */
+/*                          and dL/d(gmm_outs); with `acts` the gate activations too.    */
+/*   rb200_mdnrnn_backward  BPTT per row tile: dGates[l, t] into `dgates`.               */
+/*   rb200_mdnrnn_wgrad     split-K weight gradients of every LSTM layer and of the head */
+/*                          into `gpart` ([splits, n_params], the arena's layout).        */
+/* Layouts (dense fp32, time-major): state/next_state [T,B,S], action [T,B,A],           */
+/* reward/not_terminal [T,B], out [T,B,NG] with NG = (2S+1)G + 2 = mus (G*S) | sigmas     */
+/* (G*S, exp applied) | logpi (G) | reward | not_terminal; hs / cs [L, T+1, B, H] with    */
+/* slot 0 = the zero initial state (written by the forward); xin [T,B,A+S];              */
+/* acts / dgates [L,T,B,4H] (i, f, g, o); dy [T,B,NG].                                    */
+/* Limits: H <= 128, L <= 4, G <= 32, A + S <= 256, NG <= 1024; anything past them is     */
+/* refused with RB200_E_INVALID before a launch.                                          */
+/* ------------------------------------------------------------------------- */
+#define RB200_MDNRNN_MAX_HIDDEN 128
+#define RB200_MDNRNN_MAX_LAYERS 4
+#define RB200_MDNRNN_MAX_GAUSSIANS 32
+#define RB200_MDNRNN_MAX_INPUT 256
+#define RB200_MDNRNN_MAX_OUT 1024
+#define RB200_MDNRNN_ROWS_PER_BLOCK 16 /* loss_partials holds 3 * ceil(B / 16) floats */
+typedef struct rb200_mdnrnn_args {
+  int32_t seq_len, batch, state_dim, action_dim, hidden, layers, gaussians;
+  const float* params;                           /* the arena */
+  int64_t n_params;
+  int64_t w_ih_off[RB200_MDNRNN_MAX_LAYERS], w_hh_off[RB200_MDNRNN_MAX_LAYERS];
+  int64_t b_ih_off[RB200_MDNRNN_MAX_LAYERS], b_hh_off[RB200_MDNRNN_MAX_LAYERS];
+  int64_t w_gmm_off, b_gmm_off;
+  const float* state;
+  const float* action;
+  /* targets: all three or none (no loss) */
+  const float* next_state;
+  const float* reward;
+  const float* not_terminal;
+  float next_state_weight, not_terminal_weight, reward_weight;
+  float gmm_divisor;                             /* loss = gmm / gmm_divisor + bce + mse */
+  int32_t fit_only_one_next_step;                /* loss on the last step only           */
+  float* out;                                    /* or NULL                              */
+  float* hs;
+  float* cs;
+  /* training: all or none */
+  float* xin;
+  float* acts;
+  float* dgates;
+  float* dy;
+  /* loss (with targets) */
+  float* loss_partials;
+  uint32_t* tile_counter;
+  float* loss;                                   /* [4]: gmm, bce, mse, loss */
+  /* weight gradients */
+  float* gpart;
+  int32_t splits;
+} rb200_mdnrnn_args_t;
+/* 0 if the shape is within the limits above, else RB200_E_INVALID (text via last_error) */
+int rb200_mdnrnn_check_shape(int32_t state_dim, int32_t action_dim, int32_t hidden,
+                             int32_t layers, int32_t gaussians);
+int rb200_mdnrnn_forward(const rb200_mdnrnn_args_t* args, void* stream);
+int rb200_mdnrnn_backward(const rb200_mdnrnn_args_t* args, void* stream);
+int rb200_mdnrnn_wgrad(const rb200_mdnrnn_args_t* args, void* stream);
+
+/* ------------------------------------------------------------------------- */
 /* Peer-memory plumbing of the fused data-parallel step (one process per GPU).  The    */
 /* reference has no collective on this path (docs/distributed.rst:12-22 states the     */
 /* intent: synchronous data parallelism with a gradient all-reduce).                   */

@@ -281,6 +281,28 @@ class QrdqnArgsT(C.Structure):
     ]
 
 
+MDNRNN_MAX_LAYERS = 4
+MDNRNN_ROWS_PER_BLOCK = 16  # rb200_mdnrnn_forward: loss_partials holds 3 * ceil(batch / 16) floats
+
+
+class MdnrnnArgsT(C.Structure):
+    _fields_ = [
+        ("seq_len", C.c_int32), ("batch", C.c_int32), ("state_dim", C.c_int32),
+        ("action_dim", C.c_int32), ("hidden", C.c_int32), ("layers", C.c_int32),
+        ("gaussians", C.c_int32), ("params", _vp), ("n_params", C.c_int64),
+        ("w_ih_off", C.c_int64 * MDNRNN_MAX_LAYERS), ("w_hh_off", C.c_int64 * MDNRNN_MAX_LAYERS),
+        ("b_ih_off", C.c_int64 * MDNRNN_MAX_LAYERS), ("b_hh_off", C.c_int64 * MDNRNN_MAX_LAYERS),
+        ("w_gmm_off", C.c_int64), ("b_gmm_off", C.c_int64),
+        ("state", _vp), ("action", _vp), ("next_state", _vp), ("reward", _vp),
+        ("not_terminal", _vp), ("next_state_weight", C.c_float),
+        ("not_terminal_weight", C.c_float), ("reward_weight", C.c_float),
+        ("gmm_divisor", C.c_float), ("fit_only_one_next_step", C.c_int32),
+        ("out", _vp), ("hs", _vp), ("cs", _vp), ("xin", _vp), ("acts", _vp), ("dgates", _vp),
+        ("dy", _vp), ("loss_partials", _vp), ("tile_counter", _vp), ("loss", _vp),
+        ("gpart", _vp), ("splits", C.c_int32),
+    ]
+
+
 class Rb200Error(RuntimeError):
     pass
 
@@ -373,6 +395,9 @@ def _declare(lib):
                                               C.c_double, _vp, _vp, _vp, _vp]
     lib.rb200_per_priority_update_rows.argtypes = [_vp, C.c_int32, _vp, _vp, C.c_int32, C.c_double,
                                                    C.c_double, C.c_double, _vp, _vp, _vp, _vp]
+    lib.rb200_mdnrnn_check_shape.argtypes = [C.c_int32] * 5
+    for f in ("rb200_mdnrnn_forward", "rb200_mdnrnn_backward", "rb200_mdnrnn_wgrad"):
+        getattr(lib, f).argtypes = [C.POINTER(MdnrnnArgsT), _vp]
     lib.rb200_adam_blocks.argtypes = [C.c_int64]
     lib.rb200_dp_alloc.argtypes = [C.c_int64, C.POINTER(_vp)]
     lib.rb200_dp_free.argtypes = [_vp]

@@ -56,6 +56,22 @@ class NormalizationData:
     dense_normalization_parameters: Dict[int, NormalizationParameters] = field(default_factory=dict)
 
 
+@dataclass(frozen=True)
+class MDNRNNTrainerParameters:
+    hidden_size: int = 64
+    num_hidden_layers: int = 2
+    learning_rate: float = 0.001
+    num_gaussians: int = 5
+    # weight in calculating world-model loss
+    reward_loss_weight: float = 1.0
+    next_state_loss_weight: float = 1.0
+    not_terminal_loss_weight: float = 1.0
+    fit_only_one_next_step: bool = False
+    action_dim: int = 2
+    action_names: Optional[List[str]] = None
+    multi_steps: int = 1
+
+
 class NormalizationKey:
     STATE = "state"
     ACTION = "action"

@@ -49,8 +49,10 @@ class FeatureData(TensorDataClass):
     float_features: torch.Tensor
 
     def __post_init__(self):
-        if self.float_features.ndim != 2:
-            raise ValueError(f"float_features should be 2D; got {tuple(self.float_features.shape)}")
+        # (batch_size, feature_dim), or (seq_len, batch_size, feature_dim) for sequences
+        if self.float_features.ndim not in (2, 3):
+            raise ValueError("float_features should be 2D (or 3D for a sequence); got "
+                             f"{tuple(self.float_features.shape)}")
 
 
 @dataclass
@@ -247,3 +249,45 @@ class PolicyGradientInput(TensorDataClass):
 
     def batch_size(self):
         return len(self)
+
+
+@dataclass
+class MemoryNetworkInput(BaseInput):
+    """A time-major batch of sequences (reagent/core/types.py MemoryNetworkInput): state,
+    next_state and action are [T, B, dim]; reward and not_terminal are [T, B]."""
+    action: FeatureData = None
+    valid_step: Optional[torch.Tensor] = None
+    extras: ExtraData = field(default_factory=ExtraData)
+
+    @classmethod
+    def from_dict(cls, d):
+        return cls(
+            state=FeatureData(float_features=d["state"]),
+            next_state=FeatureData(float_features=d["next_state"]),
+            action=FeatureData(float_features=d["action"]),
+            reward=d["reward"],
+            time_diff=d["time_diff"],
+            not_terminal=d["not_terminal"],
+            step=d["step"],
+            extras=ExtraData(**{f.name: d.get(f.name) for f in dataclasses.fields(ExtraData)}),
+        )
+
+    def __len__(self):
+        if len(self.state.float_features.size()) == 2:
+            return self.state.float_features.size()[0]
+        elif len(self.state.float_features.size()) == 3:
+            return self.state.float_features.size()[1]
+        else:
+            raise NotImplementedError()
+
+
+@dataclass
+class MemoryNetworkOutput(TensorDataClass):
+    mus: torch.Tensor
+    sigmas: torch.Tensor
+    logpi: torch.Tensor
+    reward: torch.Tensor
+    not_terminal: torch.Tensor
+    last_step_lstm_hidden: torch.Tensor
+    last_step_lstm_cell: torch.Tensor
+    all_steps_lstm_hidden: torch.Tensor

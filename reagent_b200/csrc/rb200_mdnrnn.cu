@@ -1,0 +1,413 @@
+// reagent_b200 -- MDN-RNN: a multi-layer LSTM with a mixture-density head
+// (reagent/models/mdn_rnn.py MDNRNN.forward and gmm_loss, reagent/training/world_model/
+// mdnrnn_trainer.py get_loss).
+//
+// Rows of an LSTM are independent across the batch, so one CTA carries a tile of R = 16 rows
+// through every step and every layer with no grid-wide synchronisation: h and c of every layer
+// stay in shared memory, weights stream from L2 through the row-tile primitives of
+// rb200_tile.cuh (3xTF32 mma.sync).  Gates follow ATen's CPU LSTM cell:
+//   gates = (h . W_hh^T + b_hh) + (x . W_ih^T + b_ih),   i, f, g, o = chunk(gates, 4)
+//   c' = f * c + i * g  (each product rounded),   h' = o * tanh(c')
+// The backward walks time in reverse per row tile and writes dGates[l, t]; the weight gradients
+// are one launch of the shared split-K kernel (rb200_wgrad.cuh) over the T * B rows.
+#include <math.h>
+
+#include "rb200_tile.cuh"
+#include "rb200_wgrad.cuh"
+
+namespace rb200 {
+
+constexpr int kMdnNT = 256, kMdnTM = 4, kMdnKC = 32;
+constexpr int kMdnR = (kMdnNT / 64) * kMdnTM;  // 16 rows per CTA
+static_assert(kMdnR == RB200_MDNRNN_ROWS_PER_BLOCK, "rows per block");
+constexpr float kLogSqrt2Pi = 0.91893853320467274f;  // math.log(math.sqrt(2 * math.pi))
+
+struct MdnDims {
+  int T, B, S, A, H, L, G, NG, DX;  // DX = A + S
+  int ld_x, ld_h, ld_s;             // smem strides: input tile, h / c tiles, scratch
+};
+
+__host__ __device__ inline MdnDims mdn_dims(const rb200_mdnrnn_args_t& a) {
+  MdnDims d;
+  d.T = a.seq_len; d.B = a.batch; d.S = a.state_dim; d.A = a.action_dim; d.H = a.hidden;
+  d.L = a.layers; d.G = a.gaussians;
+  d.NG = (2 * d.S + 1) * d.G + 2;
+  d.DX = d.A + d.S;
+  d.ld_x = round_up4(d.DX) + 4;
+  d.ld_h = round_up4(d.H) + 4;
+  const int ld_g = round_up4(4 * d.H) + 4, ld_y = round_up4(d.NG) + 4;
+  d.ld_s = 2 * ld_g > ld_y ? 2 * ld_g : ld_y;
+  return d;
+}
+
+inline size_t mdn_fwd_smem(const MdnDims& d) {
+  return sizeof(float) * (2 * (size_t)wstage_floats<kMdnKC>() +
+                          (size_t)kMdnR * (d.ld_x + 2 * d.L * d.ld_h + d.ld_s) + 3 * kMdnR);
+}
+inline size_t mdn_bwd_smem(const MdnDims& d) {
+  return sizeof(float) * (2 * (size_t)wstage_floats<kMdnKC>() +
+                          (size_t)kMdnR * ((2 * d.L + 1) * d.ld_h + d.ld_s));
+}
+
+__device__ __forceinline__ float sigmoidf_(float x) { return 1.f / (1.f + expf(-x)); }
+
+// hs / cs slot s (0 = initial state) of layer l, row b
+__device__ __forceinline__ size_t hc_idx(const MdnDims& d, int l, int s, int b) {
+  return (((size_t)l * (d.T + 1) + s) * d.B + b) * d.H;
+}
+__device__ __forceinline__ size_t gate_idx(const MdnDims& d, int l, int t, int b) {
+  return (((size_t)l * d.T + t) * d.B + b) * (size_t)(4 * d.H);
+}
+
+// ---------------------------------------------------------------------------
+// Forward (+ loss and dL/d(gmm_outs) with targets)
+// ---------------------------------------------------------------------------
+__global__ void __launch_bounds__(kMdnNT, 1) mdnrnn_fwd_kernel(const rb200_mdnrnn_args_t a) {
+  constexpr int NT = kMdnNT, R = kMdnR;
+  const MdnDims d = mdn_dims(a);
+  extern __shared__ __align__(16) float smem[];
+  tile_smem_zero_all<NT>(smem);
+  float* Wst = smem;
+  float* xs = Wst + 2 * wstage_floats<kMdnKC>();
+  float* hsm = xs + R * d.ld_x;             // [L][R][ld_h]
+  float* csm = hsm + d.L * R * d.ld_h;      // [L][R][ld_h]
+  float* scr = csm + d.L * R * d.ld_h;      // [R][ld_s]: G1 | G2, then the head output
+  float* s_row = scr + R * d.ld_s;          // [3][R] per-row nll, bce, squared error
+  const int ld_g = round_up4(4 * d.H) + 4;
+  const int row0 = blockIdx.x * R;
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const bool has_loss = a.next_state != nullptr;
+  const bool train = a.dy != nullptr;
+  const float* P = a.params;
+  const int H = d.H, H4 = 4 * d.H, GS = d.G * d.S;
+  const float n_rows = a.fit_only_one_next_step ? (float)d.B : (float)d.T * (float)d.B;
+  float acc[3] = {0.f, 0.f, 0.f};  // thread 0: this block's sums, rows and steps in order
+
+  // slot 0 of hs / cs: the zero initial state read by the backward and the weight gradients
+  for (int i = tid; i < d.L * R * H; i += NT) {
+    const int l = i / (R * H), r = (i / H) % R, j = i % H;
+    if (row0 + r < d.B) {
+      a.hs[hc_idx(d, l, 0, row0 + r) + j] = 0.f;
+      a.cs[hc_idx(d, l, 0, row0 + r) + j] = 0.f;
+    }
+  }
+
+  for (int t = 0; t < d.T; ++t) {
+    // x = cat(action, state), action first (MDNRNN.forward)
+    const size_t tb = (size_t)t * d.B;
+    for (int i = tid; i < R * d.DX; i += NT) {
+      const int r = i / d.DX, c = i - r * d.DX, b = row0 + r;
+      float v = 0.f;
+      if (b < d.B)
+        v = c < d.A ? a.action[(tb + b) * d.A + c] : a.state[(tb + b) * d.S + (c - d.A)];
+      xs[r * d.ld_x + c] = v;
+      if (train && b < d.B) a.xin[(tb + b) * d.DX + c] = v;
+    }
+    __syncthreads();
+    for (int l = 0; l < d.L; ++l) {
+      float* h = hsm + l * R * d.ld_h;
+      float* c = csm + l * R * d.ld_h;
+      const float* in = l == 0 ? xs : hsm + (l - 1) * R * d.ld_h;
+      const int K = l == 0 ? d.DX : H, ld_in = l == 0 ? d.ld_x : d.ld_h;
+      tile_linear_fwd<NT, kMdnTM, kMdnKC>(in, ld_in, K, P + a.w_ih_off[l], K, P + a.b_ih_off[l],
+                                          H4, RB200_ACT_LINEAR, scr, d.ld_s, Wst);
+      tile_linear_fwd<NT, kMdnTM, kMdnKC>(h, d.ld_h, H, P + a.w_hh_off[l], H, P + a.b_hh_off[l],
+                                          H4, RB200_ACT_LINEAR, scr + ld_g, d.ld_s, Wst);
+      for (int i = tid; i < R * H; i += NT) {
+        const int r = i / H, j = i - r * H, b = row0 + r;
+        const float* g1 = scr + r * d.ld_s;
+        const float* g2 = g1 + ld_g;
+        const float gi = sigmoidf_(__fadd_rn(g2[j], g1[j]));
+        const float gf = sigmoidf_(__fadd_rn(g2[H + j], g1[H + j]));
+        const float gg = tanhf(__fadd_rn(g2[2 * H + j], g1[2 * H + j]));
+        const float go = sigmoidf_(__fadd_rn(g2[3 * H + j], g1[3 * H + j]));
+        const float cn = __fadd_rn(__fmul_rn(gf, c[r * d.ld_h + j]), __fmul_rn(gi, gg));
+        const float hn = __fmul_rn(go, tanhf(cn));
+        c[r * d.ld_h + j] = b < d.B ? cn : 0.f;
+        h[r * d.ld_h + j] = b < d.B ? hn : 0.f;
+        if (b < d.B) {
+          a.hs[hc_idx(d, l, t + 1, b) + j] = hn;
+          a.cs[hc_idx(d, l, t + 1, b) + j] = cn;
+          if (train) {
+            float* ga = a.acts + gate_idx(d, l, t, b);
+            ga[j] = gi; ga[H + j] = gf; ga[2 * H + j] = gg; ga[3 * H + j] = go;
+          }
+        }
+      }
+      __syncthreads();
+    }
+    // gmm_linear on the top layer's h_t
+    tile_linear_fwd<NT, kMdnTM, kMdnKC>(hsm + (d.L - 1) * R * d.ld_h, d.ld_h, H,
+                                        P + a.w_gmm_off, H, P + a.b_gmm_off, d.NG,
+                                        RB200_ACT_LINEAR, scr, d.ld_s, Wst);
+    const bool in_loss = has_loss && (!a.fit_only_one_next_step || t == d.T - 1);
+    // one warp per row; lane k < G carries gaussian k
+    for (int r = warp; r < R; r += NT / 32) {
+      const int b = row0 + r;
+      if (b >= d.B) {
+        if (lane == 0) { s_row[r] = 0.f; s_row[R + r] = 0.f; s_row[2 * R + r] = 0.f; }
+        continue;
+      }
+      const float* y = scr + r * d.ld_s;
+      const bool gl = lane < d.G;
+      // logpi = log_softmax(y[2GS .. 2GS+G))
+      const float rp = gl ? y[2 * GS + lane] : -INFINITY;
+      const float pm = warp_max(rp);
+      const float pe = warp_sum(gl ? expf(__fsub_rn(rp, pm)) : 0.f);
+      const float logpi = gl ? __fsub_rn(__fsub_rn(rp, pm), logf(pe)) : -INFINITY;
+      float* o = a.out ? a.out + (tb + b) * d.NG : nullptr;
+      const float* x = in_loss ? a.next_state + (tb + b) * d.S : nullptr;
+      float lp = 0.f;
+      if (gl) {
+        for (int s = 0; s < d.S; ++s) {
+          const float mu = y[lane * d.S + s];
+          const float sg = expf(y[GS + lane * d.S + s]);
+          if (o) { o[lane * d.S + s] = mu; o[GS + lane * d.S + s] = sg; }
+          if (x) {
+            // Normal.log_prob: -(x - mu)^2 / (2 var) - log(sigma) - log(sqrt(2 pi))
+            const float df = __fsub_rn(x[s], mu);
+            const float q = __fdiv_rn(-__fmul_rn(df, df), __fmul_rn(2.f, __fmul_rn(sg, sg)));
+            lp = __fadd_rn(lp, __fsub_rn(__fsub_rn(q, logf(sg)), kLogSqrt2Pi));
+          }
+        }
+        if (o) o[2 * GS + lane] = logpi;
+      }
+      if (o && lane == 0) { o[d.NG - 2] = y[d.NG - 2]; o[d.NG - 1] = y[d.NG - 1]; }
+      if (!has_loss) continue;
+      float* dy = train ? a.dy + (tb + b) * d.NG : nullptr;
+      if (!in_loss) {
+        if (dy)
+          for (int c = lane; c < d.NG; c += 32) dy[c] = 0.f;
+        if (lane == 0) { s_row[r] = 0.f; s_row[R + r] = 0.f; s_row[2 * R + r] = 0.f; }
+        continue;
+      }
+      // log-sum-exp over gaussians, shifted by the max
+      const float z = gl ? __fadd_rn(logpi, lp) : -INFINITY;
+      const float zm = warp_max(z);
+      const float ez = gl ? expf(__fsub_rn(z, zm)) : 0.f;
+      const float zs = warp_sum(ez);
+      const float log_prob = __fadd_rn(zm, logf(zs));
+      const float rh = y[d.NG - 2], nt = y[d.NG - 1];
+      const float rt = a.reward[tb + b], yt = a.not_terminal[tb + b];
+      if (lane == 0) {
+        // binary_cross_entropy_with_logits: (1 - y) x - log_sigmoid(x)
+        const float ls = __fsub_rn(fminf(nt, 0.f), log1pf(expf(-fabsf(nt))));
+        const float dr = __fsub_rn(rh, rt);
+        s_row[r] = -log_prob;
+        s_row[R + r] = __fsub_rn(__fmul_rn(__fsub_rn(1.f, yt), nt), ls);
+        s_row[2 * R + r] = __fmul_rn(dr, dr);
+      }
+      if (!dy) continue;
+      // d loss / d log_prob of this row = -(w_ns / N) / gmm_divisor
+      const float cg = -__fdiv_rn(__fdiv_rn(a.next_state_weight, n_rows), a.gmm_divisor);
+      const float dz = gl ? __fmul_rn(cg, __fdiv_rn(ez, zs)) : 0.f;  // d/dz_k
+      if (gl) {
+        for (int s = 0; s < d.S; ++s) {
+          const float mu = y[lane * d.S + s];
+          const float sg = expf(y[GS + lane * d.S + s]);
+          const float var = __fmul_rn(sg, sg);
+          const float df = __fsub_rn(x[s], mu);
+          dy[lane * d.S + s] = __fmul_rn(dz, __fdiv_rn(df, var));
+          dy[GS + lane * d.S + s] = __fmul_rn(dz, __fsub_rn(__fdiv_rn(__fmul_rn(df, df), var), 1.f));
+        }
+      }
+      // log_softmax backward: d raw_j = dz_j - softmax_j * sum_k dz_k
+      const float dzs = warp_sum(dz);
+      if (gl) dy[2 * GS + lane] = __fsub_rn(dz, __fmul_rn(expf(logpi), dzs));
+      if (lane == 0) {
+        dy[d.NG - 2] = __fmul_rn(__fdiv_rn(a.reward_weight, n_rows), __fmul_rn(2.f, __fsub_rn(rh, rt)));
+        dy[d.NG - 1] = __fmul_rn(__fdiv_rn(a.not_terminal_weight, n_rows), __fsub_rn(sigmoidf_(nt), yt));
+      }
+    }
+    __syncthreads();
+    if (has_loss && tid == 0 && in_loss) {
+      for (int r = 0; r < R; ++r) {
+        acc[0] += s_row[r];
+        acc[1] += s_row[R + r];
+        acc[2] += s_row[2 * R + r];
+      }
+    }
+  }
+  if (has_loss && tid == 0) {
+    float* loss = a.loss;
+    const float w0 = a.next_state_weight, w1 = a.not_terminal_weight, w2 = a.reward_weight;
+    const float div = a.gmm_divisor;
+    finish_serial<3>(a.loss_partials, a.tile_counter, acc, [=](const float (&s)[3]) {
+      const float gmm = __fmul_rn(__fdiv_rn(s[0], n_rows), w0);
+      const float bce = __fmul_rn(__fdiv_rn(s[1], n_rows), w1);
+      const float mse = __fmul_rn(__fdiv_rn(s[2], n_rows), w2);
+      loss[0] = gmm;
+      loss[1] = bce;
+      loss[2] = mse;
+      loss[3] = __fadd_rn(__fadd_rn(__fdiv_rn(gmm, div), bce), mse);
+    });
+  }
+}
+
+// ---------------------------------------------------------------------------
+// Backward through time: dGates[l, t] for every layer and step
+// ---------------------------------------------------------------------------
+__global__ void __launch_bounds__(kMdnNT, 1) mdnrnn_bwd_kernel(const rb200_mdnrnn_args_t a) {
+  constexpr int NT = kMdnNT, R = kMdnR;
+  const MdnDims d = mdn_dims(a);
+  extern __shared__ __align__(16) float smem[];
+  tile_smem_zero_all<NT>(smem);
+  float* Wst = smem;
+  float* dhr = Wst + 2 * wstage_floats<kMdnKC>();  // [L][R][ld_h] dL/dh_{t-1} through W_hh
+  float* dcs = dhr + d.L * R * d.ld_h;             // [L][R][ld_h] dL/dc_{t-1} through f
+  float* dx = dcs + d.L * R * d.ld_h;              // [R][ld_h] dL/dh_t from above
+  float* scr = dx + R * d.ld_h;                    // [R][ld_s]: dY of the step, then dGates
+  const int row0 = blockIdx.x * R;
+  const int tid = threadIdx.x;
+  const float* P = a.params;
+  const int H = d.H, H4 = 4 * d.H;
+  for (int t = d.T - 1; t >= 0; --t) {
+    tile_load_rows<NT, R>(scr, d.ld_s, a.dy + (size_t)t * d.B * d.NG, d.NG, d.NG, row0, d.B);
+    __syncthreads();
+    // dh_top = dY . W_gmm
+    tile_linear_bwd<NT, kMdnTM, kMdnKC>(scr, d.ld_s, d.NG, P + a.w_gmm_off, H, H, nullptr, 0, 0,
+                                        dx, d.ld_h, Wst);
+    for (int l = d.L - 1; l >= 0; --l) {
+      float* dh_rec = dhr + l * R * d.ld_h;
+      float* dc = dcs + l * R * d.ld_h;
+      for (int i = tid; i < R * H; i += NT) {
+        const int r = i / H, j = i - r * H, b = row0 + r;
+        float* dg = scr + r * d.ld_s;
+        if (b >= d.B) {
+          dg[j] = dg[H + j] = dg[2 * H + j] = dg[3 * H + j] = 0.f;
+          continue;
+        }
+        const float* ga = a.acts + gate_idx(d, l, t, b);
+        const float gi = ga[j], gf = ga[H + j], gg = ga[2 * H + j], go = ga[3 * H + j];
+        const float cn = a.cs[hc_idx(d, l, t + 1, b) + j];
+        const float cp = a.cs[hc_idx(d, l, t, b) + j];
+        const float tc = tanhf(cn);
+        const float dh = __fadd_rn(dx[r * d.ld_h + j], dh_rec[r * d.ld_h + j]);
+        const float dct = __fadd_rn(dc[r * d.ld_h + j],
+                                    __fmul_rn(__fmul_rn(dh, go), __fsub_rn(1.f, __fmul_rn(tc, tc))));
+        const float di = __fmul_rn(__fmul_rn(dct, gg), __fmul_rn(__fsub_rn(1.f, gi), gi));
+        const float df = __fmul_rn(__fmul_rn(dct, cp), __fmul_rn(__fsub_rn(1.f, gf), gf));
+        const float dgg = __fmul_rn(__fmul_rn(dct, gi), __fsub_rn(1.f, __fmul_rn(gg, gg)));
+        const float dgo = __fmul_rn(__fmul_rn(dh, tc), __fmul_rn(__fsub_rn(1.f, go), go));
+        dc[r * d.ld_h + j] = __fmul_rn(dct, gf);
+        dg[j] = di; dg[H + j] = df; dg[2 * H + j] = dgg; dg[3 * H + j] = dgo;
+        float* out = a.dgates + gate_idx(d, l, t, b);
+        out[j] = di; out[H + j] = df; out[2 * H + j] = dgg; out[3 * H + j] = dgo;
+      }
+      __syncthreads();
+      // dL/dh_{t-1} of this layer, and dL/dh_t of the layer below
+      tile_linear_bwd<NT, kMdnTM, kMdnKC>(scr, d.ld_s, H4, P + a.w_hh_off[l], H, H, nullptr, 0, 0,
+                                          dh_rec, d.ld_h, Wst);
+      if (l > 0)
+        tile_linear_bwd<NT, kMdnTM, kMdnKC>(scr, d.ld_s, H4, P + a.w_ih_off[l], H, H, nullptr, 0,
+                                            0, dx, d.ld_h, Wst);
+    }
+  }
+}
+
+static int mdn_validate(const rb200_mdnrnn_args_t* a, const char* who) {
+  if (!a) { set_last_error("%s: args is null", who); return RB200_E_INVALID; }
+  if (int rc = rb200_mdnrnn_check_shape(a->state_dim, a->action_dim, a->hidden, a->layers,
+                                        a->gaussians))
+    return rc;
+  if (a->seq_len <= 0 || a->batch <= 0) {
+    set_last_error("%s: seq_len %d and batch %d must be positive", who, a->seq_len, a->batch);
+    return RB200_E_INVALID;
+  }
+  if ((long long)a->seq_len * a->batch > INT32_MAX / 4) {
+    set_last_error("%s: seq_len * batch = %lld is too large", who,
+                   (long long)a->seq_len * a->batch);
+    return RB200_E_INVALID;
+  }
+  if (!a->params || !a->hs || !a->cs) {
+    set_last_error("%s: params, hs and cs are required", who);
+    return RB200_E_INVALID;
+  }
+  return RB200_OK;
+}
+
+}  // namespace rb200
+
+using namespace rb200;
+
+extern "C" int rb200_mdnrnn_check_shape(int32_t S, int32_t A, int32_t H, int32_t L, int32_t G) {
+  if (S < 1 || A < 1 || H < 1 || L < 1 || G < 1) {
+    set_last_error("rb200_mdnrnn: state_dim %d, action_dim %d, hidden %d, layers %d and "
+                   "gaussians %d must be positive", S, A, H, L, G);
+    return RB200_E_INVALID;
+  }
+  const long long ng = (2LL * S + 1) * G + 2;
+  if (H > RB200_MDNRNN_MAX_HIDDEN || L > RB200_MDNRNN_MAX_LAYERS ||
+      G > RB200_MDNRNN_MAX_GAUSSIANS || S + A > RB200_MDNRNN_MAX_INPUT ||
+      ng > RB200_MDNRNN_MAX_OUT) {
+    set_last_error("rb200_mdnrnn: unsupported shape (hidden %d <= %d, layers %d <= %d, "
+                   "gaussians %d <= %d, state_dim + action_dim %d <= %d, (2 state_dim + 1) "
+                   "gaussians + 2 = %lld <= %d)", H, RB200_MDNRNN_MAX_HIDDEN, L,
+                   RB200_MDNRNN_MAX_LAYERS, G, RB200_MDNRNN_MAX_GAUSSIANS, S + A,
+                   RB200_MDNRNN_MAX_INPUT, ng, RB200_MDNRNN_MAX_OUT);
+    return RB200_E_INVALID;
+  }
+  return RB200_OK;
+}
+
+extern "C" int rb200_mdnrnn_forward(const rb200_mdnrnn_args_t* a, void* stream) {
+  if (int rc = mdn_validate(a, "rb200_mdnrnn_forward")) return rc;
+  if (!a->state || !a->action) {
+    set_last_error("rb200_mdnrnn_forward: state and action are required");
+    return RB200_E_INVALID;
+  }
+  const int n_tgt = !!a->next_state + !!a->reward + !!a->not_terminal;
+  const int n_train = !!a->xin + !!a->acts + !!a->dy;
+  if ((n_tgt != 0 && n_tgt != 3) || (n_train != 0 && n_train != 3) || (n_train && !n_tgt) ||
+      (n_tgt && (!a->loss_partials || !a->tile_counter || !a->loss)) ||
+      (n_tgt && !(a->gmm_divisor > 0.f))) {
+    set_last_error("rb200_mdnrnn_forward: targets (next_state, reward, not_terminal) need loss "
+                   "buffers and gmm_divisor > 0; training (xin, acts, dy) needs the targets");
+    return RB200_E_INVALID;
+  }
+  const MdnDims d = mdn_dims(*a);
+  return launch<mdnrnn_fwd_kernel>(ceil_div(d.B, kMdnR), kMdnNT, mdn_fwd_smem(d),
+                                   (cudaStream_t)stream, "mdnrnn_fwd_kernel launch", *a);
+}
+
+extern "C" int rb200_mdnrnn_backward(const rb200_mdnrnn_args_t* a, void* stream) {
+  if (int rc = mdn_validate(a, "rb200_mdnrnn_backward")) return rc;
+  if (!a->acts || !a->dy || !a->dgates) {
+    set_last_error("rb200_mdnrnn_backward: acts, dy and dgates are required");
+    return RB200_E_INVALID;
+  }
+  const MdnDims d = mdn_dims(*a);
+  return launch<mdnrnn_bwd_kernel>(ceil_div(d.B, kMdnR), kMdnNT, mdn_bwd_smem(d),
+                                   (cudaStream_t)stream, "mdnrnn_bwd_kernel launch", *a);
+}
+
+extern "C" int rb200_mdnrnn_wgrad(const rb200_mdnrnn_args_t* a, void* stream) {
+  if (int rc = mdn_validate(a, "rb200_mdnrnn_wgrad")) return rc;
+  if (!a->xin || !a->dgates || !a->dy || !a->gpart || a->splits <= 0) {
+    set_last_error("rb200_mdnrnn_wgrad: xin, dgates, dy, gpart and splits > 0 are required");
+    return RB200_E_INVALID;
+  }
+  const MdnDims d = mdn_dims(*a);
+  const size_t TB = (size_t)d.T * d.B, slot = (size_t)(d.T + 1) * d.B * d.H;
+  WgradLayer jobs[kWgradMaxJobs] = {};
+  int n = 0;
+  for (int l = 0; l < d.L; ++l) {
+    const float* dz = a->dgates + (size_t)l * TB * 4 * d.H;
+    // dW_ih = dGates^T . x (x: the network input, or h_t of the layer below); db_ih = sum dGates
+    WgradLayer& ih = jobs[n++];
+    ih.A = l == 0 ? a->xin : a->hs + (size_t)(l - 1) * slot + (size_t)d.B * d.H;
+    ih.dZ = dz; ih.K = l == 0 ? d.DX : d.H; ih.N = 4 * d.H;
+    ih.w_off = a->w_ih_off[l]; ih.b_off = a->b_ih_off[l];
+    // dW_hh = dGates^T . h_{t-1} (slots 0 .. T-1, slot 0 the zero state); db_hh = sum dGates
+    WgradLayer& hh = jobs[n++];
+    hh.A = a->hs + (size_t)l * slot;
+    hh.dZ = dz; hh.K = d.H; hh.N = 4 * d.H;
+    hh.w_off = a->w_hh_off[l]; hh.b_off = a->b_hh_off[l];
+  }
+  WgradLayer& head = jobs[n++];
+  head.A = a->hs + (size_t)(d.L - 1) * slot + (size_t)d.B * d.H;
+  head.dZ = a->dy; head.K = d.H; head.N = d.NG;
+  head.w_off = a->w_gmm_off; head.b_off = a->b_gmm_off;
+  return wgrad_jobs_launch(jobs, n, (int)TB, a->splits, a->gpart, a->n_params,
+                           (cudaStream_t)stream, "rb200_mdnrnn_wgrad");
+}

@@ -4,6 +4,7 @@
 #include <stdlib.h>
 
 #include "rb200_dqn_tc_layout.cuh"
+#include "rb200_wgrad.cuh"
 
 namespace rb200 {
 
@@ -19,20 +20,16 @@ constexpr int kWgTile = 64;
 constexpr int kWgRows = 32;  // batch rows staged per step
 constexpr int kWgLd = kWgTile + 8;
 
-struct WgradLayer {
-  const float* A;   // [B, K] input activations of this layer
-  const float* dZ;  // [B, N] pre-activation gradients of this layer
-  int K, N;
-  long long w_off, b_off;
-  int tiles_n, tiles_k, tile_start;
-};
-struct WgradParams {
+// (WgradLayer: rb200_wgrad.cuh)  kJobs is the capacity of the job list passed by value.
+template <int kJobs>
+struct WgradParamsN {
   int n_layers;
-  WgradLayer L[kMaxLayers];
+  WgradLayer L[kJobs];
   int B, splits, rows_per_split;
   float* gpart;
   long long P;
 };
+using WgradParams = WgradParamsN<kMaxLayers>;
 
 __device__ __forceinline__ void wg_split(float x, uint32_t& hi, uint32_t& lo) {
   hi = (__float_as_uint(x) + 0x1000u) & 0xffffe000u;
@@ -46,7 +43,8 @@ __device__ __forceinline__ void wg_mma(float (&c)[4], const uint32_t (&a)[4], co
       : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b[0]), "r"(b[1]));
 }
 
-__global__ void __launch_bounds__(kThreads) wgrad_kernel(const WgradParams p) {
+template <int kJobs>
+__global__ void __launch_bounds__(kThreads) wgrad_kernel(const WgradParamsN<kJobs> p) {
   __shared__ __align__(16) float zs[2][kWgRows][kWgLd];
   __shared__ __align__(16) float as[2][kWgRows][kWgLd];
   int li = 0;
@@ -176,6 +174,32 @@ __global__ void __launch_bounds__(kThreads) wgrad_kernel(const WgradParams p) {
         if (n < N && k < K) gp[Ly.w_off + (size_t)n * K + k] = acc[i][j][e];
       }
   if (tk == 0 && tid < kWgTile && n0 + tid < N) gp[Ly.b_off + n0 + tid] = bsum;
+}
+
+int wgrad_jobs_launch(WgradLayer* jobs, int n_jobs, int rows, int splits, float* gpart,
+                      long long P, cudaStream_t st, const char* what) {
+  if (n_jobs < 1 || n_jobs > kWgradMaxJobs || rows <= 0 || splits <= 0) {
+    set_last_error("%s: bad job count %d, rows %d or splits %d", what, n_jobs, rows, splits);
+    return RB200_E_INVALID;
+  }
+  WgradParamsN<kWgradMaxJobs> p = {};
+  p.n_layers = n_jobs;
+  p.B = rows;
+  p.splits = splits;
+  p.rows_per_split = ceil_div(ceil_div(rows, splits), kWgRows) * kWgRows;
+  p.gpart = gpart;
+  p.P = P;
+  int tiles = 0;
+  for (int j = 0; j < n_jobs; ++j) {
+    WgradLayer& L = jobs[j];
+    L.tiles_n = ceil_div(L.N, kWgTile);
+    L.tiles_k = ceil_div(L.K, kWgTile);
+    L.tile_start = tiles;
+    tiles += L.tiles_n * L.tiles_k;
+    p.L[j] = L;
+  }
+  for (int j = n_jobs; j < kWgradMaxJobs; ++j) p.L[j].tile_start = 1 << 30;
+  return launch<wgrad_kernel<kWgradMaxJobs>>(dim3(tiles, splits), kThreads, 0, st, what, p);
 }
 
 // g[i] = sum_s gpart[s*P + i]

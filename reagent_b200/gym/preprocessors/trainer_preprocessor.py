@@ -4,6 +4,7 @@ namedtuple that is already on the GPU (a few elementwise torch ops on (B, A) ten
 hot path uses ReplayBuffer.sample_discrete_dqn_batch / sample_policy_network_batch, which
 produce the same batches inside the fused sample kernel."""
 import inspect
+from typing import Optional
 
 import numpy as np
 import torch
@@ -94,9 +95,67 @@ class PolicyNetworkInputMaker:
             extras=rlt.ExtraData(action_probability=None if log_prob is None else log_prob.exp()))
 
 
+class MemoryNetworkInputMaker:
+    """trainer_preprocessor.py:281-354: a ReplayBuffer(stack_size=T,
+    return_everything_as_stack=True) batch -> a time-major MemoryNetworkInput.  Layout only:
+    one-hot discrete actions, [B, dim, T] -> [T, B, dim], [B, T] -> [T, B], and
+    not_terminal = 1 before the last step of the stack."""
+
+    def __init__(self, num_actions: Optional[int] = None):
+        self.num_actions = num_actions
+
+    @classmethod
+    def create_for_env(cls, env):
+        n = getattr(env.action_space, "n", None)
+        if n is not None:
+            return cls(int(n))
+        if getattr(env.action_space, "low", None) is not None:
+            return cls()
+        raise NotImplementedError()
+
+    def __call__(self, batch):
+        action = batch.action
+        if self.num_actions is not None:
+            assert action.dim() == 2, f"{tuple(action.shape)}"
+            # [B, T] indices -> [B, A, T]
+            action = F.one_hot(action, self.num_actions).float().transpose(1, 2)
+
+        def vector(name, t):  # [B, dim] (T == 1) or [B, dim, T] -> [T, B, dim]
+            if t.dim() == 2:
+                t = t.unsqueeze(2)
+            assert t.dim() == 3, f"{name} has shape {tuple(t.shape)}"
+            return t.permute(2, 0, 1)
+
+        def scalar(name, t):  # [B] or [B, T] -> [T, B]
+            if t.dim() == 1:
+                t = t.unsqueeze(1)
+            assert t.dim() == 2, f"{name} has shape {tuple(t.shape)}"
+            return t.transpose(0, 1)
+
+        reward = scalar("reward", batch.reward)
+        not_terminal = scalar("not_terminal", 1.0 - batch.terminal.float())
+        if reward.shape[0] > 1:
+            # the replay buffer returns the terminal flag of the last step only: the earlier
+            # steps of a stack cannot have been terminal
+            assert not_terminal.shape == (1, reward.shape[1]), f"{tuple(not_terminal.shape)}"
+            stacked = torch.ones_like(reward)
+            stacked[-1] = not_terminal
+            not_terminal = stacked
+        return rlt.MemoryNetworkInput.from_dict({
+            "state": vector("state", batch.state),
+            "next_state": vector("next_state", batch.next_state),
+            "action": vector("action", action),
+            "reward": reward,
+            "not_terminal": not_terminal,
+            "step": None,
+            "time_diff": None,
+        })
+
+
 REPLAY_BUFFER_MAKER_MAP = {
     rlt.DiscreteDqnInput: DiscreteDqnInputMaker,
     rlt.PolicyNetworkInput: PolicyNetworkInputMaker,
+    rlt.MemoryNetworkInput: MemoryNetworkInputMaker,
 }
 
 

@@ -3,21 +3,21 @@ the reference's flow (reagent/model_managers/model_manager.py:84-96 and
 discrete/discrete_dqn.py:63-116, discrete/discrete_qrdqn.py:73-121,
 discrete/discrete_c51dqn.py:43-88, parametric/parametric_dqn.py:45-81,
 actor_critic/sac.py:80-113, actor_critic/td3.py:70-102, discrete/discrete_crr.py:104-179,
-policy_gradient/reinforce.py, policy_gradient/ppo.py): build the networks from the net
+policy_gradient/reinforce.py, policy_gradient/ppo.py, model_based/world_model.py): build the networks from the net
 builders, copy the target, hand everything to the trainer; `create_policy` gives the online
 act-time policy.  Serving modules, data modules and reporters are out of scope (SURVEY.md
 section 2 rows 8, 12, 15, 16)."""
 from dataclasses import dataclass, field
 from typing import Union, Dict, List, Optional
 
-from ..core.parameters import (EvaluationParameters, NormalizationData, NormalizationKey,
-                               RLParameters)
+from ..core.parameters import (EvaluationParameters, MDNRNNTrainerParameters,
+                               NormalizationData, NormalizationKey, RLParameters)
 from ..net_builder import (ActorFullyConnected, Categorical, DiscreteActorFullyConnected,
                            Dueling, DuelingQuantile, FullyConnected, GaussianFullyConnected, ParametricFullyConnected,
                            Quantile, ValueFullyConnected)
 from ..optimizer import Optimizer__Union
 from ..training import (C51Trainer, CRRWeightFn, DiscreteCRRTrainer, DQNTrainer,
-                        ParametricDQNTrainer, PPOTrainer, QRDQNTrainer, ReinforceTrainer,
+                        MDNRNNTrainer, ParametricDQNTrainer, PPOTrainer, QRDQNTrainer, ReinforceTrainer,
                         SACTrainer, TD3Trainer)
 
 
@@ -430,3 +430,25 @@ class PPO(_PolicyGradientManager):
     _trainer_fields = ("gamma", "optimizer", "optimizer_value_net", "reward_clip", "normalize",
                        "subtract_mean", "offset_clamp_min", "update_freq", "update_epochs",
                        "ppo_batch_size", "ppo_epsilon", "entropy_weight", "td_error_advantage")
+
+
+@dataclass
+class WorldModel:
+    """reagent/model_managers/model_based/world_model.py: a MemoryNetwork trained by
+    MDNRNNTrainer.  `reward_boost` is WorldModelBase's field (unused by this trainer)."""
+    trainer_param: MDNRNNTrainerParameters = field(default_factory=MDNRNNTrainerParameters)
+    reward_boost: Optional[Dict[str, float]] = None
+
+    def build_trainer(self, normalization_data_map: Dict[str, NormalizationData], use_gpu: bool,
+                      reward_options=None) -> MDNRNNTrainer:
+        from ..models.world_model import MemoryNetwork
+        from ..preprocessing.normalization import get_num_output_features
+
+        dev = _device(use_gpu)
+        p = self.trainer_param
+        memory_network = MemoryNetwork(
+            state_dim=get_num_output_features(
+                normalization_data_map[NormalizationKey.STATE].dense_normalization_parameters),
+            action_dim=p.action_dim, num_hiddens=p.hidden_size,
+            num_hidden_layers=p.num_hidden_layers, num_gaussians=p.num_gaussians).to(dev)
+        return MDNRNNTrainer(memory_network=memory_network, params=p)

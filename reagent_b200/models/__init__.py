@@ -10,3 +10,4 @@ from .fully_connected_network import (  # noqa: F401
     FloatFeatureFullyConnected,
     FullyConnectedNetwork,
 )
+from .world_model import MDNRNN, LstmArena, MemoryNetwork  # noqa: F401

@@ -3,6 +3,7 @@ from .c51_trainer import C51Trainer  # noqa: F401
 from .discrete_crr_trainer import DiscreteCRRTrainer  # noqa: F401
 from .dqn_trainer import BCQConfig, DQNTrainer  # noqa: F401
 from .loop import run_update  # noqa: F401
+from .mdnrnn_trainer import MDNRNNTrainer  # noqa: F401
 from .parametric_dqn_trainer import ParametricDQNTrainer  # noqa: F401
 from .ppo_trainer import PPOTrainer  # noqa: F401
 from .qrdqn_trainer import QRDQNTrainer  # noqa: F401

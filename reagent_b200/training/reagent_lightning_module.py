@@ -129,7 +129,9 @@ class ReAgentLightningModule(torch.nn.Module):
 
     def optimizers(self, use_pl_optimizer: bool = True):
         if self._optimizers_cache is None:
-            opts = [o["optimizer"] for o in self.configure_optimizers()]
+            # configure_optimizers() returns {"optimizer": ...} dicts or bare optimizers
+            opts = [o["optimizer"] if isinstance(o, dict) else o
+                    for o in self.configure_optimizers()]
             # which optimizer trains each network arena, and which target its SoftUpdate moves
             # with it: the fast path's Adam and Polyak launches follow configure_optimizers()
             self._adam_of = {o.arena: o for o in opts if isinstance(o, FusedAdam)}
