@@ -923,6 +923,64 @@ int rb200_mdnrnn_backward(const rb200_mdnrnn_args_t* args, void* stream);
 int rb200_mdnrnn_wgrad(const rb200_mdnrnn_args_t* args, void* stream);
 
 /* ------------------------------------------------------------------------- */
+/* Cross-entropy-method planner (reagent/models/cem_planner.py): one launch of          */
+/* rb200_cem_rollout per CEM iteration.  CTA (j, m) of the grid [ceil(P / 16), K] takes  */
+/* the j-th group of 16 trajectories that drew world model m (model_idx), carries them   */
+/* through all `horizon` steps -- each a T = 1 MDN-RNN forward from h = c = 0, so W_hh   */
+/* drops out and c' = i * g -- samples mixture / next state / terminal from the noise,   */
+/* and writes each trajectory's fp64 value.  The last CTA to finish reduces:             */
+/*   continuous: elites (the num_elites largest values, ties to the larger index),       */
+/*     mean / var update in fp64, `done` = 1 once max(var) <= epsilon;                   */
+/*   discrete: first-action tally, nanargmax into action_out / one_hot.                  */
+/* A launch that finds `done` set returns at once, so a plan needs no host sync.         */
+/* Noise (dense, per plan): model_idx int32 [iters, P]; action_idx int32 [P, horizon]    */
+/* (discrete); truncnorm fp64 [iters, P, horizon * A] (continuous); step_noise fp32      */
+/* [iters, P, horizon, S + 2] = mixture uniform | S standard normals | Bernoulli uniform. */
+/* `net` carries the shape and arena offsets (identical for every model); its params,    */
+/* seq_len and batch are not read.                                                        */
+/* Limits: the MDN-RNN limits, P <= 1024, K <= 8, horizon * A <= 4096,                    */
+/* 1 <= num_elites <= P, horizon >= 1.                                                    */
+/* ------------------------------------------------------------------------- */
+#define RB200_CEM_MAX_MODELS 8
+#define RB200_CEM_MAX_POPULATION 1024
+#define RB200_CEM_MAX_PLAN 4096 /* horizon * action_dim */
+#define RB200_CEM_ROWS_PER_BLOCK 16
+typedef struct rb200_cem_args {
+  rb200_mdnrnn_args_t net;
+  int32_t num_models;
+  const float* params[RB200_CEM_MAX_MODELS]; /* arena of each world model */
+  int32_t population, horizon, iters, num_elites;
+  int32_t discrete, terminal_effective;
+  int32_t iter;                              /* the iteration this launch runs */
+  double alpha, epsilon;
+  const float* state;                        /* [S] */
+  const float* discount;                     /* [horizon] fp32(gamma ** j) */
+  const double* lower;                       /* [horizon * A] tiled bounds (continuous) */
+  const double* upper;
+  const int32_t* model_idx;
+  const int32_t* action_idx;
+  const double* truncnorm;
+  const float* step_noise;
+  double* mean;                              /* [horizon * A], read and updated */
+  double* var;
+  double* values;                            /* [iters, P] */
+  int32_t* elites;                           /* [iters, num_elites], ascending value */
+  double* mean_hist;                         /* [iters, horizon * A] after each update */
+  double* var_hist;
+  int32_t* done;
+  int32_t* n_iters;
+  int64_t* action_out;                       /* discrete: [1] */
+  float* one_hot;                            /* discrete: [A] */
+  uint32_t* counter;                         /* 0 between launches */
+  float* dump;                               /* or NULL: iteration 0's per-step input and */
+                                             /* head outputs, [P, horizon, A + S + NG]    */
+} rb200_cem_args_t;
+int rb200_cem_check_shape(int32_t state_dim, int32_t action_dim, int32_t hidden, int32_t layers,
+                          int32_t gaussians, int32_t population, int32_t num_models,
+                          int32_t horizon, int32_t num_elites);
+int rb200_cem_rollout(const rb200_cem_args_t* args, void* stream);
+
+/* ------------------------------------------------------------------------- */
 /* Peer-memory plumbing of the fused data-parallel step (one process per GPU).  The    */
 /* reference has no collective on this path (docs/distributed.rst:12-22 states the     */
 /* intent: synchronous data parallelism with a gradient all-reduce).                   */

@@ -303,6 +303,24 @@ class MdnrnnArgsT(C.Structure):
     ]
 
 
+CEM_MAX_MODELS = 8
+CEM_ROWS_PER_BLOCK = 16
+
+
+class CemArgsT(C.Structure):
+    _fields_ = [
+        ("net", MdnrnnArgsT), ("num_models", C.c_int32), ("params", _vp * CEM_MAX_MODELS),
+        ("population", C.c_int32), ("horizon", C.c_int32), ("iters", C.c_int32),
+        ("num_elites", C.c_int32), ("discrete", C.c_int32), ("terminal_effective", C.c_int32),
+        ("iter", C.c_int32), ("alpha", C.c_double), ("epsilon", C.c_double),
+        ("state", _vp), ("discount", _vp), ("lower", _vp), ("upper", _vp),
+        ("model_idx", _vp), ("action_idx", _vp), ("truncnorm", _vp), ("step_noise", _vp),
+        ("mean", _vp), ("var", _vp), ("values", _vp), ("elites", _vp), ("mean_hist", _vp),
+        ("var_hist", _vp), ("done", _vp), ("n_iters", _vp), ("action_out", _vp),
+        ("one_hot", _vp), ("counter", _vp), ("dump", _vp),
+    ]
+
+
 class Rb200Error(RuntimeError):
     pass
 
@@ -398,6 +416,8 @@ def _declare(lib):
     lib.rb200_mdnrnn_check_shape.argtypes = [C.c_int32] * 5
     for f in ("rb200_mdnrnn_forward", "rb200_mdnrnn_backward", "rb200_mdnrnn_wgrad"):
         getattr(lib, f).argtypes = [C.POINTER(MdnrnnArgsT), _vp]
+    lib.rb200_cem_check_shape.argtypes = [C.c_int32] * 9
+    lib.rb200_cem_rollout.argtypes = [C.POINTER(CemArgsT), _vp]
     lib.rb200_adam_blocks.argtypes = [C.c_int64]
     lib.rb200_dp_alloc.argtypes = [C.c_int64, C.POINTER(_vp)]
     lib.rb200_dp_free.argtypes = [_vp]

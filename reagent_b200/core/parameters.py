@@ -72,6 +72,20 @@ class MDNRNNTrainerParameters:
     multi_steps: int = 1
 
 
+@dataclass(frozen=True)
+class CEMTrainerParameters:
+    plan_horizon_length: int = 0
+    num_world_models: int = 0
+    cem_population_size: int = 0
+    cem_num_iterations: int = 0
+    ensemble_population_size: int = 0
+    num_elites: int = 0
+    mdnrnn: MDNRNNTrainerParameters = field(default_factory=MDNRNNTrainerParameters)
+    rl: RLParameters = field(default_factory=RLParameters)
+    alpha: float = 0.25
+    epsilon: float = 0.001
+
+
 class NormalizationKey:
     STATE = "state"
     ACTION = "action"

@@ -3,20 +3,23 @@ the reference's flow (reagent/model_managers/model_manager.py:84-96 and
 discrete/discrete_dqn.py:63-116, discrete/discrete_qrdqn.py:73-121,
 discrete/discrete_c51dqn.py:43-88, parametric/parametric_dqn.py:45-81,
 actor_critic/sac.py:80-113, actor_critic/td3.py:70-102, discrete/discrete_crr.py:104-179,
-policy_gradient/reinforce.py, policy_gradient/ppo.py, model_based/world_model.py): build the networks from the net
+policy_gradient/reinforce.py, policy_gradient/ppo.py, model_based/world_model.py,
+model_based/cross_entropy_method.py): build the networks from the net
 builders, copy the target, hand everything to the trainer; `create_policy` gives the online
 act-time policy.  Serving modules, data modules and reporters are out of scope (SURVEY.md
 section 2 rows 8, 12, 15, 16)."""
 from dataclasses import dataclass, field
 from typing import Union, Dict, List, Optional
 
-from ..core.parameters import (EvaluationParameters, MDNRNNTrainerParameters,
-                               NormalizationData, NormalizationKey, RLParameters)
+from ..core import types as rlt
+from ..core.parameters import (CEMTrainerParameters, EvaluationParameters,
+                               MDNRNNTrainerParameters, NormalizationData, NormalizationKey,
+                               RLParameters)
 from ..net_builder import (ActorFullyConnected, Categorical, DiscreteActorFullyConnected,
                            Dueling, DuelingQuantile, FullyConnected, GaussianFullyConnected, ParametricFullyConnected,
                            Quantile, ValueFullyConnected)
 from ..optimizer import Optimizer__Union
-from ..training import (C51Trainer, CRRWeightFn, DiscreteCRRTrainer, DQNTrainer,
+from ..training import (C51Trainer, CEMTrainer, CRRWeightFn, DiscreteCRRTrainer, DQNTrainer,
                         MDNRNNTrainer, ParametricDQNTrainer, PPOTrainer, QRDQNTrainer, ReinforceTrainer,
                         SACTrainer, TD3Trainer)
 
@@ -452,3 +455,82 @@ class WorldModel:
             action_dim=p.action_dim, num_hiddens=p.hidden_size,
             num_hidden_layers=p.num_hidden_layers, num_gaussians=p.num_gaussians).to(dev)
         return MDNRNNTrainer(memory_network=memory_network, params=p)
+
+
+class CEMPolicy:
+    """reagent/model_managers/model_based/cross_entropy_method.py CEMPolicy: the planner's
+    action, returned on the CPU as a [1, A] tensor with log_prob 0."""
+
+    def __init__(self, cem_planner_network, discrete_action: bool):
+        self.cem_planner_network = cem_planner_network
+        self.discrete_action = discrete_action
+
+    def act(self, obs: rlt.FeatureData, possible_actions_mask=None) -> rlt.ActorOutput:
+        import torch
+
+        greedy = self.cem_planner_network(obs)
+        if self.discrete_action:
+            _, onehot = greedy
+            return rlt.ActorOutput(action=onehot.unsqueeze(0), log_prob=torch.tensor(0.0))
+        return rlt.ActorOutput(action=greedy.unsqueeze(0), log_prob=torch.tensor(0.0))
+
+
+@dataclass
+class CrossEntropyMethod:
+    """reagent/model_managers/model_based/cross_entropy_method.py: num_world_models
+    MemoryNetworks, each with its MDNRNNTrainer, and the CEMPlannerNetwork over them.
+    `reward_boost` is WorldModelBase's field (unused by this trainer)."""
+    trainer_param: CEMTrainerParameters = field(default_factory=CEMTrainerParameters)
+    reward_boost: Optional[Dict[str, float]] = None
+
+    def create_policy(self, trainer_module, serving: bool = False, normalization_data_map=None):
+        if serving:
+            raise NotImplementedError("serving modules are out of scope of reagent_b200")
+        assert isinstance(trainer_module, CEMTrainer)
+        return CEMPolicy(trainer_module.cem_planner_network, self.discrete_action)
+
+    def build_trainer(self, normalization_data_map: Dict[str, NormalizationData], use_gpu: bool,
+                      reward_options=None) -> CEMTrainer:
+        """As the reference builds it: one WorldModel trainer built and discarded (it draws its
+        initial weights from torch's generator, so the models after it start from the
+        reference's weights under torch.manual_seed), then num_world_models trainers, and the
+        planner over their networks.  The action type and bounds come from the ACTION
+        normalization: discrete unless its features are CONTINUOUS_ACTION, bounds from
+        max_value / min_value."""
+        import numpy as np
+
+        from ..models.cem_planner import CEMPlannerNetwork
+        from ..preprocessing.identify_types import CONTINUOUS_ACTION
+        from ..preprocessing.normalization import get_num_output_features
+
+        p = self.trainer_param
+        world_model_manager = WorldModel(trainer_param=p.mdnrnn)
+        world_model_manager.build_trainer(normalization_data_map, use_gpu=use_gpu,
+                                          reward_options=reward_options)
+        world_model_trainers = [
+            world_model_manager.build_trainer(normalization_data_map, use_gpu=use_gpu,
+                                              reward_options=reward_options)
+            for _ in range(p.num_world_models)]
+        world_model_nets = [t.memory_network for t in world_model_trainers]
+        terminal_effective = p.mdnrnn.not_terminal_loss_weight > 0
+        action_norm = normalization_data_map[NormalizationKey.ACTION].dense_normalization_parameters
+        sorted_action_norm_vals = list(action_norm.values())
+        discrete_action = sorted_action_norm_vals[0].feature_type != CONTINUOUS_ACTION
+        upper = lower = None
+        if not discrete_action:
+            upper = np.array([v.max_value for v in sorted_action_norm_vals])
+            lower = np.array([v.min_value for v in sorted_action_norm_vals])
+        planner = CEMPlannerNetwork(
+            mem_net_list=world_model_nets, cem_num_iterations=p.cem_num_iterations,
+            cem_population_size=p.cem_population_size,
+            ensemble_population_size=p.ensemble_population_size, num_elites=p.num_elites,
+            plan_horizon_length=p.plan_horizon_length,
+            state_dim=get_num_output_features(
+                normalization_data_map[NormalizationKey.STATE].dense_normalization_parameters),
+            action_dim=get_num_output_features(action_norm), discrete_action=discrete_action,
+            terminal_effective=terminal_effective, gamma=p.rl.gamma, alpha=p.alpha,
+            epsilon=p.epsilon, action_upper_bounds=upper, action_lower_bounds=lower)
+        # kept for create_policy
+        self.discrete_action = discrete_action
+        return CEMTrainer(cem_planner_network=planner, world_model_trainers=world_model_trainers,
+                          parameters=p)

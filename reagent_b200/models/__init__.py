@@ -3,6 +3,7 @@ from .actor import FullyConnectedActor, GaussianFullyConnectedActor  # noqa: F40
 from .base import ModelBase  # noqa: F401
 from .bcq import BatchConstrainedDQN  # noqa: F401
 from .categorical_dqn import CategoricalDQN  # noqa: F401
+from .cem_planner import CEMNoise, CEMPlan, CEMPlannerNetwork  # noqa: F401
 from .critic import FullyConnectedCritic  # noqa: F401
 from .dqn import FullyConnectedDQN  # noqa: F401
 from .dueling_q_network import DuelingQNetwork  # noqa: F401

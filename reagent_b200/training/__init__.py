@@ -1,5 +1,6 @@
 from .behavioral_cloning_trainer import BehavioralCloningTrainer  # noqa: F401
 from .c51_trainer import C51Trainer  # noqa: F401
+from .cem_trainer import CEMTrainer  # noqa: F401
 from .discrete_crr_trainer import DiscreteCRRTrainer  # noqa: F401
 from .dqn_trainer import BCQConfig, DQNTrainer  # noqa: F401
 from .loop import run_update  # noqa: F401
