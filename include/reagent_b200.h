@@ -3,10 +3,14 @@
  * The reference (facebookresearch/ReAgent) has no FFI for this path: it is plain
  * Python over torch (SURVEY.md section 8b).  This header is the boundary one level
  * beneath the Python surface: every entry point replaces a chain of eager aten ops
- * in the reference file:line it cites.  All pointers are DEVICE pointers unless the
- * parameter name ends in `_host`; every function takes the CUDA stream to launch on
- * (as void*), owns no memory, starts no threads and returns 0 on success or a
- * negative RB200_E_* code (text via rb200_last_error()).
+ * in the reference file:line it cites.  All pointers are DEVICE pointers except:
+ *   - a pointer to an rb200_*_t struct, parameter or field: a HOST descriptor
+ *     (rb200_mlp_t, rb200_net_ws_t, the *_args_t, ...) read during the call.  The one
+ *     exception is rb200_feature_col_t, whose pointers are device arrays;
+ *   - a parameter whose name ends in `_host`.
+ * Every function takes the CUDA stream to launch on (as void*), owns no memory, starts
+ * no threads and returns 0 on success or a negative RB200_E_* code (text via
+ * rb200_last_error()).
  */
 #ifndef REAGENT_B200_H_
 #define REAGENT_B200_H_
@@ -318,14 +322,16 @@ int rb200_c51_head(const rb200_c51_args_t* args, void* stream);
 /*   y = first arg max of the label row  (each row's own logged action)              */
 /*   loss = mean_b -log_softmax(z)[y],   dz = (softmax(z) - onehot(y)) / B            */
 /* 1 <= num_actions <= 1024.  dz NULL: loss only.  Deterministic (fixed-order mean),  */
-/* no allocation (graph-capturable).                                                  */
+/* no allocation (graph-capturable); loss_partials holds                              */
+/* ceil(B / RB200_BC_ROWS_PER_BLOCK) floats.                                          */
+#define RB200_BC_ROWS_PER_BLOCK 8
 typedef struct rb200_bc_xent_args {
   int32_t batch, num_actions;
   const float* logits;             /* [B,A] bc_net scores, unmasked */
   const float* labels;             /* [B,A] one-hot logged action */
   const float* mask;               /* [B,A] possible_actions_mask (1 = possible) */
   float* dz;                       /* [B,A] d loss / d logits, or NULL */
-  float* loss_partials;            /* [ceil(B/8)] */
+  float* loss_partials;
   float* loss;                     /* [1] */
   uint32_t* tile_counter;          /* [1] zero-initialised, self-resetting */
 } rb200_bc_xent_args_t;

@@ -236,7 +236,7 @@ __global__ void __launch_bounds__(256) c51_head_kernel(const C51Dev d) {
 // ---------------------------------------------------------------------------
 // Behavioral cloning: one warp per row, lanes striding over the actions
 // ---------------------------------------------------------------------------
-constexpr int kBcRowsPerBlock = 8;
+constexpr int kBcRowsPerBlock = RB200_BC_ROWS_PER_BLOCK;
 
 __global__ void __launch_bounds__(32 * kBcRowsPerBlock) bc_xent_head_kernel(const rb200_bc_xent_args_t a) {
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;

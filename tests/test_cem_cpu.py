@@ -1,6 +1,5 @@
 """The cross-entropy-method planner on the host: the fp64 oracle against the reference's
-goldens, the parameters, the refusals, the limits and the ABI."""
-import ctypes
+goldens, the parameters, the refusals and the limits."""
 import dataclasses
 import os
 import sys
@@ -132,7 +131,3 @@ def test_shape_past_limit_refused(shape):
     with pytest.raises(_lib.Rb200Error, match="unsupported shape"):
         _planner(nets, cem_population_size=P, plan_horizon_length=hor, num_elites=E,
                  state_dim=S, action_dim=A)
-
-
-def test_abi_sizeof():
-    assert _lib.lib().rb200_abi_sizeof(b"rb200_cem_args_t") == ctypes.sizeof(_lib.CemArgsT)

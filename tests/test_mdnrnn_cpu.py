@@ -1,6 +1,5 @@
 """MDN-RNN on the host: the fp64 oracle against the reference's goldens, the API surface
-(parameters, state_dict, seeded initial weights, optimizers), the refusals and the ABI."""
-import ctypes
+(parameters, state_dict, seeded initial weights, optimizers) and the refusals."""
 import os
 import sys
 
@@ -202,10 +201,6 @@ def test_shape_past_limit_refused(shape):
         # refused before the device check: the batch is on the CPU
         with pytest.raises(_lib.Rb200Error, match="unsupported shape"):
             net(rlt.FeatureData(torch.zeros(T, B, shape[0])), rlt.FeatureData(torch.zeros(T, B, shape[1])))
-
-
-def test_abi_sizeof():
-    assert _lib.lib().rb200_abi_sizeof(b"rb200_mdnrnn_args_t") == ctypes.sizeof(_lib.MdnrnnArgsT)
 
 
 @pytest.mark.parametrize("kind,num_actions", [("discrete", 3), ("continuous", None)])

@@ -1,7 +1,6 @@
 """Prioritized replay for SACTrainer and TD3Trainer without a GPU: the weighted oracles against
-the reference's SAC and TD3 goldens, the twin-critic priorities, the grown C struct, and the
-argument checks of FusedPolicyStep and of `importance_weights`."""
-import ctypes as C
+the reference's SAC and TD3 goldens, the twin-critic priorities, and the argument checks of
+FusedPolicyStep and of `importance_weights`."""
 
 import numpy as np
 import pytest
@@ -111,17 +110,6 @@ def test_twin_td_priorities_known_values():
     p = PA.twin_td_priorities([2.0], None, [0.5], 1.0, 1e-6)
     assert p[0] == 1.5 + 1e-6
     assert np.isnan(PA.twin_td_priorities([np.nan], [0.0], [0.0], 0.6, 1e-6)[0])
-
-
-def test_ac_args_struct_grows_by_the_per_fields():
-    from reagent_b200 import _lib
-
-    lib = _lib.lib()
-    assert lib.rb200_abi_sizeof(b"rb200_ac_args_t") == C.sizeof(_lib.AcArgsT)
-    names = [f[0] for f in _lib.AcArgsT._fields_]
-    assert names[-2:] == ["sample_weight", "td_error_out"]
-    assert _lib.AcArgsT.td_error_out.offset == C.sizeof(_lib.AcArgsT) - 8
-    assert _lib.AcArgsT.sample_weight.offset == C.sizeof(_lib.AcArgsT) - 16
 
 
 def _cpu_trainers(delay=2):

@@ -138,13 +138,3 @@ def test_per_c_abi_null_and_size_checks():
     a.n, a.rb.capacity, a.rb.update_horizon = 1, 4, 1
     assert lib.rb200_replay_add_device(a, None) == -1
     assert b"priority_from_max" in lib.rb200_last_error()
-
-
-def test_grown_structs_match_their_mirrors():
-    from reagent_b200 import _lib
-
-    lib = _lib.lib()
-    for name, mirror in (("rb200_dqn_args_t", _lib.DqnArgsT), ("rb200_add_args_t", _lib.AddArgsT)):
-        assert lib.rb200_abi_sizeof(name.encode()) == C.sizeof(mirror), name
-    assert _lib.DqnArgsT.sample_weight.offset == C.sizeof(_lib.DqnArgsT) - 8
-    assert _lib.AddArgsT.priority_from_max.offset > _lib.AddArgsT.rows.offset

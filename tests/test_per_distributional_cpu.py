@@ -1,6 +1,6 @@
 """Prioritized replay for QRDQNTrainer and C51Trainer without a GPU: the weighted oracles against
 the reference's QR-DQN and C51 goldens, the row-loss priorities, the C ABI of
-rb200_per_priority_update_rows and the grown head structs, and FusedDqnStep's argument checks."""
+rb200_per_priority_update_rows, and FusedDqnStep's argument checks."""
 import ctypes as C
 import math
 
@@ -127,16 +127,6 @@ def test_rows_priority_c_abi_rejects_bad_arguments():
         assert lib.rb200_per_priority_update_rows(*args) == -1, (pos, val)
         err = lib.rb200_last_error()
         assert b"rb200_per_priority_update_rows" in err and what in err, (pos, val, err)
-
-
-def test_head_structs_grow_by_sample_weight():
-    from reagent_b200 import _lib
-
-    lib = _lib.lib()
-    for name, mirror in (("rb200_qrdqn_args_t", _lib.QrdqnArgsT), ("rb200_c51_args_t", _lib.C51ArgsT)):
-        assert lib.rb200_abi_sizeof(name.encode()) == C.sizeof(mirror), name
-        assert mirror._fields_[-1][0] == "sample_weight", name
-        assert mirror.sample_weight.offset == C.sizeof(mirror) - 8, name
 
 
 def _cpu_trainers():

@@ -1,7 +1,6 @@
 """REINFORCE and PPO without a GPU: the plain-torch restatement (oracle/pg_oracle.py) against
 every golden of the unmodified reference, regeneration from the reference, constructor and
-manager defaults, the yield counts and optimizer order, the refusals, and the C ABI mirrors."""
-import ctypes as C
+manager defaults, the yield counts and optimizer order, and the refusals."""
 import glob
 import inspect
 import os
@@ -259,15 +258,6 @@ def test_manager_defaults_and_cartpole_configs():
         assert pol.sampler.temperature == 1.0
     with pytest.raises(RuntimeError, match="CUDA only"):
         r.build_trainer({"state": nd}, use_gpu=False)
-
-
-def test_abi_sizes():
-    from reagent_b200 import _lib
-
-    lib = _lib.lib()
-    for name, cls in (("rb200_pg_returns_args_t", _lib.PgReturnsArgsT),
-                      ("rb200_pg_head_args_t", _lib.PgHeadArgsT)):
-        assert lib.rb200_abi_sizeof(name.encode()) == C.sizeof(cls), name
 
 
 def test_policy_gradient_input_from_dict():
