@@ -987,6 +987,118 @@ int rb200_cem_check_shape(int32_t state_dim, int32_t action_dim, int32_t hidden,
 int rb200_cem_rollout(const rb200_cem_args_t* args, void* stream);
 
 /* ------------------------------------------------------------------------- */
+/* Seq2Reward (reagent/models/seq2reward_model.py, reagent/training/world_model/         */
+/* seq2reward_trainer.py, compress_model_trainer.py): an nn.LSTM over the one-hot action  */
+/* sequence whose initial h of every layer is map_linear(state[0]) (c = 0), and a width-1 */
+/* head lstm_linear on the top h of step valid_step - 1.  Per update:                     */
+/*   rb200_seq2reward_forward   per 16-row tile: h0, every step and layer (h / c in       */
+/*                              shared memory), acc_reward; with `reward` the target       */
+/*                              cumsum(reward * discount)[valid - 1] (fp64 sum, rounded    */
+/*                              once), the MSE (`loss`) and dy; with `step_labels` the     */
+/*                              one-hot [B, multi_steps] of valid - 1.                     */
+/*   rb200_seq2reward_backward  BPTT per row tile: dGates into `dgates`, and dh0 = the sum  */
+/*                              over layers of dL/dh_{-1} (the map_linear output gradient). */
+/*   rb200_seq2reward_wgrad     split-K weight gradients of every layer and lstm_linear     */
+/*                              over T*B rows, then map_linear over B rows, into `gpart`.   */
+/* valid_step (int64 [B], or NULL = T) is clamped to [1, T] by the kernels; callers check  */
+/* its range.  No k-chunk rotation (see tile_linear_fwd): a row's outputs are the same in  */
+/* whichever CTA computes it, which makes the plan bit-identical to the forward.           */
+/* Layouts (dense fp32): state [B, S] (the sequence's first state), action [T, B, A],     */
+/* reward [T, B], discount [T] = fp32(gamma ** t), acc_reward / target [B],               */
+/* dy [T, B] = dL/dacc_reward on step valid - 1, else 0; hs / cs [L, T+1, B, H] with slot  */
+/* 0 = the initial state; acts / dgates [L, T, B, 4H] (i, f, g, o); dh0 [B, H].            */
+/* Limits: H <= 128, L <= 4 (the MDN-RNN limits), 1 <= S <= 256, 1 <= A <= 16,             */
+/* 1 <= multi_steps <= 16, A ** multi_steps <= 65536, and the forward's tile within the    */
+/* 227 KiB of shared memory of one CTA: 4 * (2 * 9216 + 16 * (round_up4(max(S, A)) + 4 +   */
+/* (2L + 1)(round_up4(H) + 4) + 2 (round_up4(4H) + 4) + 1)) + 64 bytes, so L 4 with        */
+/* H 128 takes S <= 252 (every other H, L takes S 256).  Anything else is refused before   */
+/* any launch.                                                                              */
+/* ------------------------------------------------------------------------- */
+#define RB200_SEQ2REWARD_MAX_STATE 256
+#define RB200_SEQ2REWARD_MAX_ACTIONS 16
+#define RB200_SEQ2REWARD_MAX_STEPS 16
+#define RB200_SEQ2REWARD_MAX_PERMUTATIONS 65536 /* num_action ** multi_steps */
+#define RB200_SEQ2REWARD_PLAN_BUDGET_BYTES 268435456 /* plan workspace cap (256 MiB) */
+#define RB200_SEQ2REWARD_ROWS_PER_BLOCK 16 /* loss_partials holds ceil(B / 16) floats */
+typedef struct rb200_seq2reward_args {
+  int32_t seq_len, batch, state_dim, action_dim, hidden, layers;
+  const float* params;                           /* the arena */
+  int64_t n_params;
+  int64_t w_ih_off[RB200_MDNRNN_MAX_LAYERS], w_hh_off[RB200_MDNRNN_MAX_LAYERS];
+  int64_t b_ih_off[RB200_MDNRNN_MAX_LAYERS], b_hh_off[RB200_MDNRNN_MAX_LAYERS];
+  int64_t w_lin_off, b_lin_off;                  /* lstm_linear [1, H], [1] */
+  int64_t w_map_off, b_map_off;                  /* map_linear [H, S], [H] */
+  const float* state;
+  const float* action;
+  const int64_t* valid_step;                     /* or NULL */
+  float* acc_reward;
+  /* target and loss: reward, discount, target, loss_partials, tile_counter, loss, or none */
+  const float* reward;
+  const float* discount;
+  float* target;
+  float* loss_partials;
+  uint32_t* tile_counter;
+  float* loss;                                   /* [1] */
+  float* step_labels;                            /* [B, multi_steps] or NULL */
+  int32_t multi_steps;
+  /* training (needs the target): hs, cs, acts, dy; the backward adds dgates and dh0 */
+  float* hs;
+  float* cs;
+  float* acts;
+  float* dy;
+  float* dgates;
+  float* dh0;
+  /* weight gradients */
+  float* gpart;
+  int32_t splits;
+} rb200_seq2reward_args_t;
+/* rb200_seq2reward_plan: get_Q over the prefix tree of the action sequences.  q[b, a] is   */
+/* the max of lstm_linear(h_top) over the A ** (k-1) sequences of length k that start with */
+/* a; q_all[b, j-1, a] the same max over the sequences of length j, for j = 1..k.  Level j */
+/* (one launch per level and state chunk) carries its B * A ** j nodes one LSTM step from  */
+/* their parents: node i's children are i * A + a, the input is the one-hot of a.  Level j */
+/* < k stores node i's h / c ([L, 2, H] per node) at row i * A ** (k-1-j) of `workspace`;  */
+/* child 0 takes its parent's row, so a CTA holds every child of its parents (16 / A       */
+/* parents, 16 / A * A rows).  Level k stores nothing.  Peak workspace = Bc * A ** (k-1) * */
+/* L * 2 * H * 4 bytes for a chunk of Bc states: the call chunks the batch to what         */
+/* `workspace_bytes` holds (rb200_seq2reward_plan_workspace_bytes gives the size for a     */
+/* batch, at most RB200_SEQ2REWARD_PLAN_BUDGET_BYTES).  The maxima are taken by atomicMax  */
+/* on order-preserving integer images in `qbits` [B, k, A] (order-free, so deterministic). */
+typedef struct rb200_seq2reward_plan_args {
+  rb200_seq2reward_args_t net;                   /* shape and arena; its seq_len, batch,   */
+                                                 /* state, action and buffers are not read */
+  int32_t batch, multi_steps;                    /* num_action is net.action_dim           */
+  const float* state;                            /* [B, S] */
+  float* q;                                      /* [B, A] */
+  float* q_all;                                  /* [B, k, A] or NULL */
+  uint32_t* qbits;                               /* [B, k, A] */
+  float* workspace;
+  int64_t workspace_bytes;
+} rb200_seq2reward_plan_args_t;
+/* CompressModelTrainer's head: loss = mean((out - q) ** 2) over B * A, dout = dL/dout (or */
+/* NULL), accuracy = mean(argmax q == argmax out), first maximum on ties.  out / q [B, A]; */
+/* loss_partials holds 2 * ceil(B / 256) floats; out_loss [2] = loss, accuracy.           */
+typedef struct rb200_seq2reward_compress_args {
+  int32_t batch, num_action;
+  const float* out;
+  const float* q;
+  float* dout;
+  float* loss_partials;
+  uint32_t* tile_counter;
+  float* out_loss;
+} rb200_seq2reward_compress_args_t;
+/* 0 if the shape is within the limits above, else RB200_E_INVALID (text via last_error) */
+int rb200_seq2reward_check_shape(int32_t state_dim, int32_t action_dim, int32_t hidden,
+                                 int32_t layers, int32_t multi_steps);
+int rb200_seq2reward_forward(const rb200_seq2reward_args_t* args, void* stream);
+int rb200_seq2reward_backward(const rb200_seq2reward_args_t* args, void* stream);
+int rb200_seq2reward_wgrad(const rb200_seq2reward_args_t* args, void* stream);
+int64_t rb200_seq2reward_plan_workspace_bytes(int32_t batch, int32_t action_dim,
+                                              int32_t multi_steps, int32_t hidden, int32_t layers);
+int rb200_seq2reward_plan(const rb200_seq2reward_plan_args_t* args, void* stream);
+int rb200_seq2reward_compress_head(const rb200_seq2reward_compress_args_t* args, void* stream);
+
+/* ------------------------------------------------------------------------- */
 /* Peer-memory plumbing of the fused data-parallel step (one process per GPU).  The    */
 /* reference has no collective on this path (docs/distributed.rst:12-22 states the     */
 /* intent: synchronous data parallelism with a gradient all-reduce).                   */

@@ -73,6 +73,18 @@ class MDNRNNTrainerParameters:
 
 
 @dataclass(frozen=True)
+class Seq2RewardTrainerParameters:
+    learning_rate: float = 0.001
+    multi_steps: int = 1
+    action_names: List[str] = field(default_factory=lambda: [])
+    compress_model_learning_rate: float = 0.001
+    gamma: float = 1.0
+    view_q_value: bool = False
+    step_predict_net_size: int = 64
+    reward_boost: Optional[Dict[str, float]] = None
+
+
+@dataclass(frozen=True)
 class CEMTrainerParameters:
     plan_horizon_length: int = 0
     num_world_models: int = 0

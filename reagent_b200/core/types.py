@@ -282,6 +282,11 @@ class MemoryNetworkInput(BaseInput):
 
 
 @dataclass
+class Seq2RewardOutput(TensorDataClass):
+    acc_reward: torch.Tensor
+
+
+@dataclass
 class MemoryNetworkOutput(TensorDataClass):
     mus: torch.Tensor
     sigmas: torch.Tensor

@@ -3,22 +3,19 @@
 // mdnrnn_trainer.py get_loss).
 //
 // Rows of an LSTM are independent across the batch, so one CTA carries a tile of R = 16 rows
-// through every step and every layer with no grid-wide synchronisation: h and c of every layer
-// stay in shared memory, weights stream from L2 through the row-tile primitives of
-// rb200_tile.cuh (3xTF32 mma.sync).  Gates follow ATen's CPU LSTM cell:
-//   gates = (h . W_hh^T + b_hh) + (x . W_ih^T + b_ih),   i, f, g, o = chunk(gates, 4)
-//   c' = f * c + i * g  (each product rounded),   h' = o * tanh(c')
-// The backward walks time in reverse per row tile and writes dGates[l, t]; the weight gradients
-// are one launch of the shared split-K kernel (rb200_wgrad.cuh) over the T * B rows.
+// through every step and every layer with no grid-wide synchronisation, on the row-tile LSTM step
+// of rb200_lstm.cuh.  The backward walks time in reverse per row tile and writes dGates[l, t];
+// the weight gradients are one launch of the shared split-K kernel (rb200_wgrad.cuh) over the
+// T * B rows.
 #include <math.h>
 
-#include "rb200_tile.cuh"
+#include "rb200_lstm.cuh"
 #include "rb200_wgrad.cuh"
 
 namespace rb200 {
 
-constexpr int kMdnNT = 256, kMdnTM = 4, kMdnKC = 32;
-constexpr int kMdnR = (kMdnNT / 64) * kMdnTM;  // 16 rows per CTA
+constexpr int kMdnNT = kLstmNT, kMdnTM = kLstmTM, kMdnKC = kLstmKC;
+constexpr int kMdnR = kLstmR;  // 16 rows per CTA
 static_assert(kMdnR == RB200_MDNRNN_ROWS_PER_BLOCK, "rows per block");
 constexpr float kLogSqrt2Pi = 0.91893853320467274f;  // math.log(math.sqrt(2 * math.pi))
 
@@ -49,14 +46,8 @@ inline size_t mdn_bwd_smem(const MdnDims& d) {
                           (size_t)kMdnR * ((2 * d.L + 1) * d.ld_h + d.ld_s));
 }
 
-__device__ __forceinline__ float sigmoidf_(float x) { return 1.f / (1.f + expf(-x)); }
-
-// hs / cs slot s (0 = initial state) of layer l, row b
 __device__ __forceinline__ size_t hc_idx(const MdnDims& d, int l, int s, int b) {
-  return (((size_t)l * (d.T + 1) + s) * d.B + b) * d.H;
-}
-__device__ __forceinline__ size_t gate_idx(const MdnDims& d, int l, int t, int b) {
-  return (((size_t)l * d.T + t) * d.B + b) * (size_t)(4 * d.H);
+  return lstm_hc_idx(d.T, d.B, d.H, l, s, b);
 }
 
 // ---------------------------------------------------------------------------
@@ -79,7 +70,7 @@ __global__ void __launch_bounds__(kMdnNT, 1) mdnrnn_fwd_kernel(const rb200_mdnrn
   const bool has_loss = a.next_state != nullptr;
   const bool train = a.dy != nullptr;
   const float* P = a.params;
-  const int H = d.H, H4 = 4 * d.H, GS = d.G * d.S;
+  const int H = d.H, GS = d.G * d.S;
   const float n_rows = a.fit_only_one_next_step ? (float)d.B : (float)d.T * (float)d.B;
   float acc[3] = {0.f, 0.f, 0.f};  // thread 0: this block's sums, rows and steps in order
 
@@ -104,38 +95,17 @@ __global__ void __launch_bounds__(kMdnNT, 1) mdnrnn_fwd_kernel(const rb200_mdnrn
       if (train && b < d.B) a.xin[(tb + b) * d.DX + c] = v;
     }
     __syncthreads();
-    for (int l = 0; l < d.L; ++l) {
-      float* h = hsm + l * R * d.ld_h;
-      float* c = csm + l * R * d.ld_h;
-      const float* in = l == 0 ? xs : hsm + (l - 1) * R * d.ld_h;
-      const int K = l == 0 ? d.DX : H, ld_in = l == 0 ? d.ld_x : d.ld_h;
-      tile_linear_fwd<NT, kMdnTM, kMdnKC>(in, ld_in, K, P + a.w_ih_off[l], K, P + a.b_ih_off[l],
-                                          H4, RB200_ACT_LINEAR, scr, d.ld_s, Wst);
-      tile_linear_fwd<NT, kMdnTM, kMdnKC>(h, d.ld_h, H, P + a.w_hh_off[l], H, P + a.b_hh_off[l],
-                                          H4, RB200_ACT_LINEAR, scr + ld_g, d.ld_s, Wst);
-      for (int i = tid; i < R * H; i += NT) {
-        const int r = i / H, j = i - r * H, b = row0 + r;
-        const float* g1 = scr + r * d.ld_s;
-        const float* g2 = g1 + ld_g;
-        const float gi = sigmoidf_(__fadd_rn(g2[j], g1[j]));
-        const float gf = sigmoidf_(__fadd_rn(g2[H + j], g1[H + j]));
-        const float gg = tanhf(__fadd_rn(g2[2 * H + j], g1[2 * H + j]));
-        const float go = sigmoidf_(__fadd_rn(g2[3 * H + j], g1[3 * H + j]));
-        const float cn = __fadd_rn(__fmul_rn(gf, c[r * d.ld_h + j]), __fmul_rn(gi, gg));
-        const float hn = __fmul_rn(go, tanhf(cn));
-        c[r * d.ld_h + j] = b < d.B ? cn : 0.f;
-        h[r * d.ld_h + j] = b < d.B ? hn : 0.f;
-        if (b < d.B) {
-          a.hs[hc_idx(d, l, t + 1, b) + j] = hn;
-          a.cs[hc_idx(d, l, t + 1, b) + j] = cn;
-          if (train) {
-            float* ga = a.acts + gate_idx(d, l, t, b);
-            ga[j] = gi; ga[H + j] = gf; ga[2 * H + j] = gg; ga[3 * H + j] = go;
-          }
-        }
-      }
-      __syncthreads();
-    }
+    lstm_tile_step<true>(a, d.L, H, d.B, row0, xs, d.ld_x, d.DX, hsm, csm, d.ld_h, scr, d.ld_s,
+                         ld_g, Wst,
+                         [&](int l, int r, int b, int j, float gi, float gf, float gg, float go,
+                             float cn, float hn) {
+                           a.hs[hc_idx(d, l, t + 1, b) + j] = hn;
+                           a.cs[hc_idx(d, l, t + 1, b) + j] = cn;
+                           if (train) {
+                             float* ga = a.acts + lstm_gate_idx(d.T, d.B, H, l, t, b);
+                             ga[j] = gi; ga[H + j] = gf; ga[2 * H + j] = gg; ga[3 * H + j] = go;
+                           }
+                         });
     // gmm_linear on the top layer's h_t
     tile_linear_fwd<NT, kMdnTM, kMdnKC>(hsm + (d.L - 1) * R * d.ld_h, d.ld_h, H,
                                         P + a.w_gmm_off, H, P + a.b_gmm_off, d.NG,
@@ -216,7 +186,7 @@ __global__ void __launch_bounds__(kMdnNT, 1) mdnrnn_fwd_kernel(const rb200_mdnrn
       if (gl) dy[2 * GS + lane] = __fsub_rn(dz, __fmul_rn(expf(logpi), dzs));
       if (lane == 0) {
         dy[d.NG - 2] = __fmul_rn(__fdiv_rn(a.reward_weight, n_rows), __fmul_rn(2.f, __fsub_rn(rh, rt)));
-        dy[d.NG - 1] = __fmul_rn(__fdiv_rn(a.not_terminal_weight, n_rows), __fsub_rn(sigmoidf_(nt), yt));
+        dy[d.NG - 1] = __fmul_rn(__fdiv_rn(a.not_terminal_weight, n_rows), __fsub_rn(lstm_sigmoid(nt), yt));
       }
     }
     __syncthreads();
@@ -258,50 +228,15 @@ __global__ void __launch_bounds__(kMdnNT, 1) mdnrnn_bwd_kernel(const rb200_mdnrn
   float* dx = dcs + d.L * R * d.ld_h;              // [R][ld_h] dL/dh_t from above
   float* scr = dx + R * d.ld_h;                    // [R][ld_s]: dY of the step, then dGates
   const int row0 = blockIdx.x * R;
-  const int tid = threadIdx.x;
   const float* P = a.params;
-  const int H = d.H, H4 = 4 * d.H;
+  const int H = d.H;
   for (int t = d.T - 1; t >= 0; --t) {
     tile_load_rows<NT, R>(scr, d.ld_s, a.dy + (size_t)t * d.B * d.NG, d.NG, d.NG, row0, d.B);
     __syncthreads();
     // dh_top = dY . W_gmm
     tile_linear_bwd<NT, kMdnTM, kMdnKC>(scr, d.ld_s, d.NG, P + a.w_gmm_off, H, H, nullptr, 0, 0,
                                         dx, d.ld_h, Wst);
-    for (int l = d.L - 1; l >= 0; --l) {
-      float* dh_rec = dhr + l * R * d.ld_h;
-      float* dc = dcs + l * R * d.ld_h;
-      for (int i = tid; i < R * H; i += NT) {
-        const int r = i / H, j = i - r * H, b = row0 + r;
-        float* dg = scr + r * d.ld_s;
-        if (b >= d.B) {
-          dg[j] = dg[H + j] = dg[2 * H + j] = dg[3 * H + j] = 0.f;
-          continue;
-        }
-        const float* ga = a.acts + gate_idx(d, l, t, b);
-        const float gi = ga[j], gf = ga[H + j], gg = ga[2 * H + j], go = ga[3 * H + j];
-        const float cn = a.cs[hc_idx(d, l, t + 1, b) + j];
-        const float cp = a.cs[hc_idx(d, l, t, b) + j];
-        const float tc = tanhf(cn);
-        const float dh = __fadd_rn(dx[r * d.ld_h + j], dh_rec[r * d.ld_h + j]);
-        const float dct = __fadd_rn(dc[r * d.ld_h + j],
-                                    __fmul_rn(__fmul_rn(dh, go), __fsub_rn(1.f, __fmul_rn(tc, tc))));
-        const float di = __fmul_rn(__fmul_rn(dct, gg), __fmul_rn(__fsub_rn(1.f, gi), gi));
-        const float df = __fmul_rn(__fmul_rn(dct, cp), __fmul_rn(__fsub_rn(1.f, gf), gf));
-        const float dgg = __fmul_rn(__fmul_rn(dct, gi), __fsub_rn(1.f, __fmul_rn(gg, gg)));
-        const float dgo = __fmul_rn(__fmul_rn(dh, tc), __fmul_rn(__fsub_rn(1.f, go), go));
-        dc[r * d.ld_h + j] = __fmul_rn(dct, gf);
-        dg[j] = di; dg[H + j] = df; dg[2 * H + j] = dgg; dg[3 * H + j] = dgo;
-        float* out = a.dgates + gate_idx(d, l, t, b);
-        out[j] = di; out[H + j] = df; out[2 * H + j] = dgg; out[3 * H + j] = dgo;
-      }
-      __syncthreads();
-      // dL/dh_{t-1} of this layer, and dL/dh_t of the layer below
-      tile_linear_bwd<NT, kMdnTM, kMdnKC>(scr, d.ld_s, H4, P + a.w_hh_off[l], H, H, nullptr, 0, 0,
-                                          dh_rec, d.ld_h, Wst);
-      if (l > 0)
-        tile_linear_bwd<NT, kMdnTM, kMdnKC>(scr, d.ld_s, H4, P + a.w_ih_off[l], H, H, nullptr, 0,
-                                            0, dx, d.ld_h, Wst);
-    }
+    lstm_tile_bwd_step(a, d.T, d.B, d.H, d.L, t, row0, dhr, dcs, dx, d.ld_h, scr, d.ld_s, Wst);
   }
 }
 

@@ -73,7 +73,7 @@ constexpr int kLWB = kNC + 8;  // bwd staging row stride (== 8 mod 32)
 //        Ws[256][KC+4] (K contiguous), k >= K zero filled
 // All NT threads must call (contains __syncthreads).
 // ---------------------------------------------------------------------------
-template <int NT, int TM, int KC>
+template <int NT, int TM, int KC, bool kRotate = true>
 __device__ __noinline__ void tile_linear_fwd(const float* __restrict__ As, int lda, int K,
                                              const float* __restrict__ Wg, int ldw,
                                              const float* __restrict__ bg, int N, int act,
@@ -92,8 +92,9 @@ __device__ __noinline__ void tile_linear_fwd(const float* __restrict__ As, int l
   const int nk = ceil_div(K, KC), nn = ceil_div(N, kNC), total = nk * nn;
   const bool vec = ((ldw & 3) == 0) && ((reinterpret_cast<uintptr_t>(Wg) & 15) == 0);
   // every CTA walks the k-chunks in a different rotation: all CTAs stream the SAME weights,
-  // and in lock-step they would hammer the same L2 lines at the same time
-  const int rot = blockIdx.x % nk;
+  // and in lock-step they would hammer the same L2 lines at the same time.  Without kRotate a
+  // row's result does not depend on the CTA that computes it.
+  const int rot = kRotate ? blockIdx.x % nk : 0;
 
   // staging map: thread -> (quad lq of the k-chunk, rows lr0, lr0+RPI, ...): fixed per thread
   constexpr int RPI = NT / QPR;

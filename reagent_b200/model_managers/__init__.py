@@ -14,14 +14,14 @@ from typing import Union, Dict, List, Optional
 from ..core import types as rlt
 from ..core.parameters import (CEMTrainerParameters, EvaluationParameters,
                                MDNRNNTrainerParameters, NormalizationData, NormalizationKey,
-                               RLParameters)
+                               RLParameters, Seq2RewardTrainerParameters)
 from ..net_builder import (ActorFullyConnected, Categorical, DiscreteActorFullyConnected,
                            Dueling, DuelingQuantile, FullyConnected, GaussianFullyConnected, ParametricFullyConnected,
-                           Quantile, ValueFullyConnected)
+                           Quantile, Seq2RewardNetBuilder, ValueFullyConnected)
 from ..optimizer import Optimizer__Union
 from ..training import (C51Trainer, CEMTrainer, CRRWeightFn, DiscreteCRRTrainer, DQNTrainer,
                         MDNRNNTrainer, ParametricDQNTrainer, PPOTrainer, QRDQNTrainer, ReinforceTrainer,
-                        SACTrainer, TD3Trainer)
+                        SACTrainer, Seq2RewardTrainer, TD3Trainer)
 
 
 def _device(use_gpu: bool):
@@ -534,3 +534,25 @@ class CrossEntropyMethod:
         self.discrete_action = discrete_action
         return CEMTrainer(cem_planner_network=planner, world_model_trainers=world_model_trainers,
                           parameters=p)
+
+
+@dataclass
+class Seq2RewardModel:
+    """reagent/model_managers/model_based/seq2reward_model.py: a Seq2RewardNetwork trained by
+    Seq2RewardTrainer; `compress_net_builder` builds the policy network that
+    CompressModelTrainer fits to its plan.  `reward_boost` is WorldModelBase's field (unused by
+    this trainer)."""
+    net_builder: Seq2RewardNetBuilder = field(default_factory=Seq2RewardNetBuilder)
+    compress_net_builder: ValueFullyConnected = field(default_factory=ValueFullyConnected)
+    trainer_param: Seq2RewardTrainerParameters = field(
+        default_factory=Seq2RewardTrainerParameters)
+    reward_boost: Optional[Dict[str, float]] = None
+
+    def build_trainer(self, normalization_data_map: Dict[str, NormalizationData], use_gpu: bool,
+                      reward_options=None) -> Seq2RewardTrainer:
+        dev = _device(use_gpu)
+        seq2reward_network = self.net_builder.build_value_network(
+            normalization_data_map[NormalizationKey.STATE])
+        trainer = Seq2RewardTrainer(seq2reward_network=seq2reward_network,
+                                    params=self.trainer_param)
+        return trainer.to(dev)

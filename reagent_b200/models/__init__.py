@@ -11,4 +11,5 @@ from .fully_connected_network import (  # noqa: F401
     FloatFeatureFullyConnected,
     FullyConnectedNetwork,
 )
+from .seq2reward_model import Seq2RewardNetwork  # noqa: F401
 from .world_model import MDNRNN, LstmArena, MemoryNetwork  # noqa: F401

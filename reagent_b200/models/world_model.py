@@ -19,17 +19,18 @@ from .base import ModelBase
 
 
 class LstmArena(ParamArena):
-    """Flat layout of an MDNRNN: per layer weight_ih, weight_hh, bias_ih, bias_hh, then
-    gmm_linear.weight and .bias, each on a 16-byte boundary."""
+    """Flat layout of an LSTM network: per layer weight_ih, weight_hh, bias_ih, bias_hh, then
+    the head's weight and bias (MDNRNN.gmm_linear, Seq2RewardNetwork.lstm_linear), then any
+    `extra` shapes (Seq2RewardNetwork.map_linear), each on a 16-byte boundary."""
 
-    def __init__(self, input_dim: int, hidden: int, layers: int, out_dim: int):
+    def __init__(self, input_dim: int, hidden: int, layers: int, out_dim: int, extra=()):
         self.dims, self.acts, self.w_off, self.b_off = [], [], [], []
         self.input_dim, self.hidden, self.layers, self.out_dim = input_dim, hidden, layers, out_dim
         self.shapes = []
         for l in range(layers):
             k = input_dim if l == 0 else hidden
             self.shapes += [(4 * hidden, k), (4 * hidden, hidden), (4 * hidden,), (4 * hidden,)]
-        self.shapes += [(out_dim, hidden), (out_dim,)]
+        self.shapes += [(out_dim, hidden), (out_dim,)] + [tuple(e) for e in extra]
         self.offsets = []
         off = 0
         for s in self.shapes:
@@ -61,13 +62,17 @@ class LstmArena(ParamArena):
         self.grad_ready = False
         return flat
 
-    def fill(self, a: "_lib.MdnrnnArgsT"):
-        """The arena fields of the kernels' arguments."""
+    def fill_lstm(self, a):
+        """The arena pointer and LSTM layer offsets of the kernels' arguments."""
         a.params = self.flat.data_ptr()
         a.n_params = self.n
         for l in range(self.layers):
             a.w_ih_off[l], a.w_hh_off[l], a.b_ih_off[l], a.b_hh_off[l] = self.offsets[4 * l: 4 * l + 4]
-        a.w_gmm_off, a.b_gmm_off = self.offsets[-2:]
+
+    def fill(self, a: "_lib.MdnrnnArgsT"):
+        """The arena fields of the MDN-RNN kernels' arguments."""
+        self.fill_lstm(a)
+        a.w_gmm_off, a.b_gmm_off = self.offsets[4 * self.layers: 4 * self.layers + 2]
 
 
 def check_shape(state_dim, action_dim, num_hiddens, num_hidden_layers, num_gaussians):
@@ -77,26 +82,9 @@ def check_shape(state_dim, action_dim, num_hiddens, num_hidden_layers, num_gauss
     _lib.check(rc, "MDNRNN")
 
 
-class MDNRNN(nn.Module):
-    """Mixture Density Network - Recurrent Neural Network"""
-
-    def __init__(self, state_dim, action_dim, num_hiddens, num_hidden_layers, num_gaussians):
-        super().__init__()
-        self.state_dim = state_dim
-        self.action_dim = action_dim
-        self.num_hiddens = num_hiddens
-        self.num_hidden_layers = num_hidden_layers
-        self.rnn = nn.LSTM(input_size=state_dim + action_dim, hidden_size=num_hiddens,
-                           num_layers=num_hidden_layers)
-        self.num_gaussians = num_gaussians
-        # outputs: mu, sigma and pi of every gaussian, then reward and the non-terminal logit
-        self.gmm_linear = nn.Linear(num_hiddens, (2 * state_dim + 1) * num_gaussians + 2)
-        self._arena = self._new_arena()
-        self._arena.flatten(self.parameters())
-
-    def _new_arena(self):
-        return LstmArena(self.state_dim + self.action_dim, self.num_hiddens,
-                         self.num_hidden_layers, self.gmm_linear.out_features)
+class LstmArenaModule(nn.Module):
+    """A module whose parameters live in the LstmArena of `_new_arena()`, kept there across
+    `.to()` / `.cuda()` and deep copies."""
 
     @property
     def arena(self) -> LstmArena:
@@ -118,6 +106,28 @@ class MDNRNN(nn.Module):
         new._arena = new._new_arena()
         new._arena.flatten(new.parameters())
         return new
+
+
+class MDNRNN(LstmArenaModule):
+    """Mixture Density Network - Recurrent Neural Network"""
+
+    def __init__(self, state_dim, action_dim, num_hiddens, num_hidden_layers, num_gaussians):
+        super().__init__()
+        self.state_dim = state_dim
+        self.action_dim = action_dim
+        self.num_hiddens = num_hiddens
+        self.num_hidden_layers = num_hidden_layers
+        self.rnn = nn.LSTM(input_size=state_dim + action_dim, hidden_size=num_hiddens,
+                           num_layers=num_hidden_layers)
+        self.num_gaussians = num_gaussians
+        # outputs: mu, sigma and pi of every gaussian, then reward and the non-terminal logit
+        self.gmm_linear = nn.Linear(num_hiddens, (2 * state_dim + 1) * num_gaussians + 2)
+        self._arena = self._new_arena()
+        self._arena.flatten(self.parameters())
+
+    def _new_arena(self):
+        return LstmArena(self.state_dim + self.action_dim, self.num_hiddens,
+                         self.num_hidden_layers, self.gmm_linear.out_features)
 
     def args(self, T: int, B: int) -> "_lib.MdnrnnArgsT":
         """The shape and arena fields of the kernels' arguments for a [T, B] batch."""

@@ -192,3 +192,18 @@ class ValueFullyConnected:
         return FloatFeatureFullyConnected(
             state_dim=_dim(state_normalization_data), output_dim=output_dim, sizes=self.sizes,
             activations=self.activations, use_layer_norm=self.use_layer_norm)
+
+
+@dataclass
+class Seq2RewardNetBuilder:
+    """reagent/net_builder/value/seq2reward_rnn.py"""
+    action_dim: int = 2
+    num_hiddens: int = 64
+    num_hidden_layers: int = 2
+
+    def build_value_network(self, state_normalization_data: NormalizationData):
+        from ..models.seq2reward_model import Seq2RewardNetwork
+
+        return Seq2RewardNetwork(state_dim=_dim(state_normalization_data),
+                                 action_dim=self.action_dim, num_hiddens=self.num_hiddens,
+                                 num_hidden_layers=self.num_hidden_layers)
