@@ -1099,6 +1099,62 @@ int rb200_seq2reward_plan(const rb200_seq2reward_plan_args_t* args, void* stream
 int rb200_seq2reward_compress_head(const rb200_seq2reward_compress_args_t* args, void* stream);
 
 /* ------------------------------------------------------------------------- */
+/* Counterfactual policy evaluation (rb200_ope.cu), reagent/evaluation/*.py.  Every input is */
+/* a dense row-major device array of the page's N rows; episodes are runs of equal mdp_id */
+/* in a page sorted by (mdp_id, sequence_number, row).  ep_off[E+1] are their row offsets. */
+/*   rb200_ope_page          per-row fields of EvaluationDataPage.create_from_tensors_dqn  */
+/*   rb200_ope_episode_marks episode starts + validate()'s sequence / run checks           */
+/*   rb200_ope_logged_values compute_values_for_mdps, column 0 of [N, C]                     */
+/*   rb200_ope_sdr           SequentialDoublyRobustEstimator's per-episode value and return */
+/*   rb200_ope_dr_rows       DoublyRobustEstimator's DM, IPS and DR rows                     */
+/*   rb200_ope_boot_means    bootstrap sample means, from given int32 indices or in-kernel  */
+/*                           Philox draws (idx == NULL)                                     */
+/*   rb200_ope_wsdr_rows     WSDR per-row cumulative importance weights, V(s), Q(s, a_log)  */
+/*   rb200_ope_seg_sum       fixed-order sums of segments (perm: row order, or NULL)        */
+/*   rb200_ope_wsdr_returns  normalised weights -> every j-step return per trajectory      */
+/*   rb200_ope_cov           np.cov of [J, T] rows, ddof 1                                   */
+/* fp64 = 1 selects float64 weights (the padded trajectories of the reference), 0 float32.  */
+/* ------------------------------------------------------------------------- */
+#define RB200_OPE_MAX_J 32
+int rb200_ope_page(int32_t n, int32_t num_actions, int32_t num_metrics, const float* q,
+                   const float* reward_out, const float* qcpe_out, const float* mask,
+                   const float* action, const float* reward, const float* reward_boost,
+                   float temperature, float* boosted_reward, float* propensities,
+                   int64_t* eval_action_idx, float* model_reward_logged,
+                   float* model_metrics_logged, float* model_metrics_values_logged, void* stream);
+int rb200_ope_episode_marks(int32_t n, const int64_t* mdp_id, const int64_t* seq,
+                            uint8_t* is_start, int32_t* flags, void* stream);
+/* step_discount[r] = (float)pow(gamma, seq[r+1] - seq[r]), computed by the host's libm pow */
+int rb200_ope_logged_values(int32_t num_episodes, const int32_t* ep_off,
+                            const float* step_discount, int32_t cols, const float* x, float* out,
+                            void* stream);
+int rb200_ope_sdr(int32_t num_episodes, const int32_t* ep_off, int32_t num_actions,
+                  const float* propensities, const float* model_values, const float* action_mask,
+                  const float* logged_reward, const float* logged_propensity, float gamma,
+                  float* episode_dr, float* episode_value, void* stream);
+int rb200_ope_dr_rows(int32_t n, int32_t num_actions, const float* propensities,
+                      const float* model_rewards, const float* action_mask,
+                      const float* logged_reward, const float* model_reward_logged,
+                      const float* logged_propensity, float* dm, float* ips, float* dr,
+                      void* stream);
+int rb200_ope_boot_means(const float* data, int32_t n, const int32_t* idx, int32_t samples,
+                         int32_t sample_size, int64_t seed, int64_t offset, double* means,
+                         void* stream);
+int rb200_ope_wsdr_rows(int32_t num_episodes, const int32_t* ep_off, int32_t num_actions,
+                        int32_t fp64, const float* propensities, const float* model_values,
+                        const float* action_mask, const float* logged_propensity, void* weight,
+                        void* state_value, void* q_logged, void* stream);
+int rb200_ope_seg_sum(int32_t fp64, const void* x, const int64_t* perm, const int64_t* seg_off,
+                      int32_t num_segments, void* out, void* stream);
+int rb200_ope_wsdr_returns(int32_t num_episodes, const int32_t* ep_off, int32_t fp64,
+                           const void* weight, const void* state_value, const void* q_logged,
+                           const float* logged_reward, const double* discounts, int32_t max_len,
+                           const void* col_sum, int32_t num_j, const int32_t* j_steps,
+                           int32_t num_subsets, const int32_t* subset_off, const void* subset_col_sum,
+                           double* ret, double* subset_ret, double* episode_value, void* stream);
+int rb200_ope_cov(const double* x, int32_t rows, int32_t cols, double* cov, void* stream);
+
+/* ------------------------------------------------------------------------- */
 /* Peer-memory plumbing of the fused data-parallel step (one process per GPU).  The    */
 /* reference has no collective on this path (docs/distributed.rst:12-22 states the     */
 /* intent: synchronous data parallelism with a gradient all-reduce).                   */

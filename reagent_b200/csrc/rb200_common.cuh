@@ -117,6 +117,28 @@ __device__ __forceinline__ void warp_row_max_sumexp(const Row& x, int n, float& 
   sum = warp_sum(s);
 }
 
+// masked_softmax(x, mask, temperature) of one row held by one thread (reagent/core/torch_utils.py:
+// 62-73): logit(c) = x/t - (1 - m)*1e20, mx its max, den = sum_c exp(logit - mx)*m in column order,
+// p(c) = exp(logit - mx)*m / den with NaN (a fully masked row) -> 0.  The CPE heads of the training
+// step and the evaluation page share these, so both give the same propensity bits.
+__device__ __forceinline__ float masked_softmax_logit(float x, float m, float t) {
+  return __fsub_rn(__fdiv_rn(x, t), __fmul_rn(__fsub_rn(1.f, m), 1e20f));
+}
+__device__ __forceinline__ void masked_softmax_stats(const float* x, const float* mk, float t, int A,
+                                                     float& mx, float& den) {
+  mx = -INFINITY;
+  for (int c = 0; c < A; ++c) mx = fmaxf(mx, masked_softmax_logit(x[c], mk ? mk[c] : 1.f, t));
+  den = 0.f;
+  for (int c = 0; c < A; ++c) {
+    const float m = mk ? mk[c] : 1.f;
+    den += __fmul_rn(expf(__fsub_rn(masked_softmax_logit(x[c], m, t), mx)), m);
+  }
+}
+__device__ __forceinline__ float masked_softmax_p(float x, float m, float t, float mx, float den) {
+  const float p = __fdiv_rn(__fmul_rn(expf(__fsub_rn(masked_softmax_logit(x, m, t), mx)), m), den);
+  return p != p ? 0.f : p;
+}
+
 // ----------------------------------------------------------------------------
 // deterministic loss means
 // ----------------------------------------------------------------------------

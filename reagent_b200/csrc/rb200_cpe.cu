@@ -28,18 +28,8 @@ __global__ void __launch_bounds__(256) cpe_heads_kernel(const CpeDev d) {
     // ---- model propensities on the next state: masked_softmax(q(s'), mask, temperature) ----
     const float* x = a.next_scores + (size_t)b * A;
     const float* mk = a.mask ? a.mask + (size_t)b * A : nullptr;
-    float mx = -INFINITY;
-    for (int c = 0; c < A; ++c) {
-      const float m = mk ? mk[c] : 1.f;
-      const float v = __fsub_rn(__fdiv_rn(x[c], a.temperature), __fmul_rn(__fsub_rn(1.f, m), 1e20f));
-      mx = fmaxf(mx, v);
-    }
-    float den = 0.f;
-    for (int c = 0; c < A; ++c) {
-      const float m = mk ? mk[c] : 1.f;
-      const float v = __fsub_rn(__fdiv_rn(x[c], a.temperature), __fmul_rn(__fsub_rn(1.f, m), 1e20f));
-      den += __fmul_rn(expf(__fsub_rn(v, mx)), m);
-    }
+    float mx, den;
+    masked_softmax_stats(x, mk, a.temperature, A, mx, den);
     // logged action: torch.argmax(action, dim=1) -- first maximum
     const float* act = a.action + (size_t)b * A;
     int logged = 0;
@@ -59,10 +49,7 @@ __global__ void __launch_bounds__(256) cpe_heads_kernel(const CpeDev d) {
       a.dz_reward[row + logged] = 2.f * dr * inv;
       float nq = 0.f;
       for (int c = 0; c < A; ++c) {
-        const float m = mk ? mk[c] : 1.f;
-        const float v = __fsub_rn(__fdiv_rn(x[c], a.temperature), __fmul_rn(__fsub_rn(1.f, m), 1e20f));
-        float p = __fdiv_rn(__fmul_rn(expf(__fsub_rn(v, mx)), m), den);
-        if (p != p) p = 0.f;  // a fully masked row: NaN -> 0 (torch_utils.py:71-72)
+        const float p = masked_softmax_p(x[c], mk ? mk[c] : 1.f, a.temperature, mx, den);
         if (i == 0 && a.propensities_next) a.propensities_next[(size_t)b * A + c] = p;
         nq += a.qcpe_target_next[row + c] * p;
       }

@@ -349,6 +349,33 @@ class DQNTrainer(DQNTrainerBaseLightning):
         """validation_step's eval_td_loss (dqn_trainer.py:363-379): forward/loss, no grads."""
         return self._td_step(batch, do_backward=False).clone()
 
+    @torch.no_grad()
+    def _scores(self, net, state):
+        x = state.float_features if isinstance(state, rlt.FeatureData) else state
+        x = x.float().contiguous()
+        out = torch.empty(x.shape[0], self.num_actions, device=x.device)
+        net.arena.refresh()
+        net.arena.forward(x, out)
+        return out
+
+    def get_detached_model_outputs(self, state):
+        """(q_network(s), q_network_target(s)) on the fused MLP forward (dqn_trainer.py:158-164)."""
+        return self._scores(self.q_network, state), self._scores(self.q_network_target, state)
+
+    def page_model_outputs(self, state):
+        """q_network(s) alone: the page does not read the target's scores."""
+        return self._scores(self.q_network, state)
+
+    def validation_step(self, batch, batch_idx):
+        """Log eval_td_loss and return the batch's EvaluationDataPage (dqn_trainer.py:362-379,
+        dqn_trainer_base.py:488-496), kept on the batch's device."""
+        from ..evaluation.evaluation_data_page import EvaluationDataPage
+
+        if isinstance(batch, dict):
+            batch = rlt.DiscreteDqnInput.from_dict(batch)
+        self.log("eval_td_loss", self.compute_td_loss_only(batch), batch_size=batch.batch_size())
+        return EvaluationDataPage.create_from_training_batch(batch, self)
+
     def q_network_grads(self):
         """Per-parameter gradients of the last fused backward (inspection / tests)."""
         return param_grads(self.q_network.arena, list(self.q_network.parameters()))

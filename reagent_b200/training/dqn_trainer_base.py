@@ -1,9 +1,9 @@
 """DQNTrainerMixin / DQNTrainerBaseLightning: the parts of
 reagent/training/dqn_trainer_base.py:23-452 that are on the hot path, including the CPE
 heads (reward network, q_network_cpe, `_calculate_cpes`, :243-452): two extra MLPs evaluated
-by the generic forward / backward / weight-gradient kernels with rb200_cpe_heads in between.
-The offline evaluation machinery behind them (Evaluator, EvaluationDataPage, :454-509) is
-reporting, not training, and stays out of scope."""
+by the generic forward / backward / weight-gradient kernels with rb200_cpe_heads in between,
+and the counterfactual policy evaluation they feed (gather_eval_data / validation_epoch_end,
+:454-509): EvaluationDataPages reduced by the Evaluator of reagent_b200.evaluation."""
 from typing import List, Optional
 
 import torch
@@ -67,8 +67,9 @@ class DQNTrainerBaseLightning(DQNTrainerMixin, RLTrainerMixin, ReAgentLightningM
         self.strict_input_checks = False
 
     def _initialize_cpe(self, reward_network, q_network_cpe, q_network_cpe_target, optimizer):
-        """dqn_trainer_base.py:243-311: store the reward / CPE networks and the offsets of
-        every metric's block of `num_actions` outputs (no Evaluator: reporting is out of scope)."""
+        """dqn_trainer_base.py:243-311: store the reward / CPE networks, the offsets of every
+        metric's block of `num_actions` outputs, and the Evaluator that validation_epoch_end
+        runs on the pages of validation_step."""
         self._cpe_ws = None
         if not self.calc_cpe_in_training:
             self.reward_network = None
@@ -86,6 +87,35 @@ class DQNTrainerBaseLightning(DQNTrainerMixin, RLTrainerMixin, ReAgentLightningM
         num_output_nodes = len(self.metrics_to_score) * self.num_actions
         self.register_buffer("reward_idx_offsets",
                              torch.arange(0, num_output_nodes, self.num_actions, dtype=torch.long))
+        from ..evaluation.evaluator import Evaluator
+
+        reward_stripped = self.metrics_to_score[:-1] if len(self.metrics_to_score) > 1 else None
+        self.evaluator = Evaluator(self._actions, self.rl_parameters.gamma, self,
+                                   metrics_to_score=reward_stripped)
+
+    def page_model_outputs(self, state):
+        """The model outputs an EvaluationDataPage scores the policy with (the first element of
+        get_detached_model_outputs: q_network for DQN, the actor for CRR)."""
+        return self.get_detached_model_outputs(state)[0]
+
+    def gather_eval_data(self, validation_step_outputs):
+        """Concatenate the EvaluationDataPages of validation_step, then sort, compute_values and
+        validate when the pages carry mdp_id (:454-486).  The pages stay on their device."""
+        eval_data = None
+        for edp in validation_step_outputs:
+            eval_data = edp if eval_data is None else eval_data.append(edp)
+        if eval_data and eval_data.mdp_id is not None:
+            eval_data = eval_data.sort()
+            eval_data = eval_data.compute_values(self.gamma)
+            eval_data.validate()
+        return eval_data
+
+    def validation_epoch_end(self, valid_step_outputs):
+        """Run the Evaluator on the gathered pages and log its CpeDetails (:498-509)."""
+        eval_data = self.gather_eval_data(valid_step_outputs)
+        if eval_data and eval_data.mdp_id is not None:
+            cpe_details = self.evaluator.evaluate_post_training(eval_data)
+            self.reporter.log(cpe_details=cpe_details)
 
     def _configure_cpe_optimizers(self):
         """(target params, source params, [reward optimizer, cpe optimizer]) -- :313-330."""
