@@ -615,16 +615,13 @@ int rb200_ac_value_step(const rb200_mlp_t* value, const rb200_ac_args_t* args,
 
 /* ------------------------------------------------------------------------- */
 /* Weight gradients: dW_l = dZ_l^T . A_{l-1}, db_l = sum_b dZ_l, split over    */
-/* the batch; partial s lands at gpart + s*n_params (arena layout).            */
-/* Default: mma.sync 3xTF32 tiles (rb200_optim.cu).  RB200_WGRAD_TC=1 selects the  */
-/* wgmma kernel (rb200_wgrad_tc.cu: operands transposed into K-major planes while   */
-/* staging, accumulators in registers); same results to 1e-5.                        */
+/* the batch; partial s lands at gpart + s*n_params (arena layout), on mma.sync */
+/* 3xTF32 tiles (rb200_optim.cu).                                               */
 /* Replaces autograd's Linear backward (torch) reached from                    */
 /* loss.backward() in the Lightning loop (reagent_lightning_module.py:108-133).*/
 /* ------------------------------------------------------------------------- */
+/* batch splits for rb200_mlp_wgrad: one per 256 rows, between 1 and 64 */
 int rb200_wgrad_splits(int batch);
-/* slabs for this network (wgmma kernel: enough (tile, slab) jobs to fill the SMs twice) */
-int rb200_wgrad_splits_for(const rb200_mlp_t* net, int32_t batch);
 int rb200_mlp_wgrad(const rb200_mlp_t* net, const float* net_input, int32_t batch,
                     const rb200_net_ws_t* ws, float* gpart, int32_t splits, void* stream);
 /* g[i] = sum_s gpart[s*P + i]  (fixed order; feeds all-reduce / .grad views) */

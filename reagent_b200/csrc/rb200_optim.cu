@@ -1,8 +1,6 @@
 // reagent_b200 -- weight-gradient, gradient-reduce, fused Adam + soft-update kernels (K3).
 #include <math.h>
 
-#include <stdlib.h>
-
 #include "rb200_dqn_tc_layout.cuh"
 #include "rb200_wgrad.cuh"
 
@@ -408,40 +406,11 @@ using namespace rb200;
 
 extern "C" int rb200_wgrad_splits(int batch) {
   // enough batch splits that even a single 64x64 tile layer fills a good part of the
-  // SMs; rows per split stay a multiple of the 32-row staging step.
-  const char* e = getenv("RB200_WGRAD_ROWS");  // tuning knob (rows per split), default 256
-  int rows = e ? atoi(e) : 256;
-  if (rows < 32) rows = 32;
-  int s = batch / rows;
+  // SMs: 256 rows per split, a multiple of the 32-row staging step.
+  int s = batch / 256;
   if (s < 1) s = 1;
   if (s > 64) s = 64;
   return s;
-}
-
-int rb200_wgrad_tc_launch(const rb200_mlp_t* net, const float* net_input, int32_t batch,
-                          const rb200_net_ws_t* ws, float* gpart, int32_t splits, void* stream);
-
-// The wgmma weight-gradient kernel (rb200_wgrad_tc.cu) is opt-in (RB200_WGRAD_TC=1); the default
-// stays this file's mma.sync kernel: at 128-row slabs both are bound by their prologue /
-// epilogue rather than by the tensor pipe.
-static bool wgrad_use_tc() {
-  const char* d = getenv("RB200_DISABLE_WGMMA");
-  const char* w = getenv("RB200_WGRAD_TC");
-  return !(d && d[0] && d[0] != '0') && (w && w[0] == '1');
-}
-
-// Batch slabs for a network: enough (layer tile, slab) jobs to fill the SMs about twice,
-// slabs of at least 128 rows (the wgmma kernel stages 32-row chunks; fewer, longer slabs
-// keep the partials the Adam kernel has to read small for wide heads).
-extern "C" int rb200_wgrad_splits_for(const rb200_mlp_t* net, int32_t batch) {
-  if (!net || !wgrad_use_tc()) return rb200_wgrad_splits(batch);
-  int jobs = 0;
-  for (int l = 0; l < net->n_layers; ++l) jobs += ceil_div(net->dims[l + 1], 128) * ceil_div(net->dims[l], 256);
-  int s = ceil_div(2 * kNumSMs, jobs < 1 ? 1 : jobs);
-  const int smax = batch / 128 < 1 ? 1 : batch / 128;
-  if (s > smax) s = smax;
-  if (s > 64) s = 64;
-  return s < 1 ? 1 : s;
 }
 
 extern "C" int rb200_mlp_wgrad(const rb200_mlp_t* net, const float* net_input, int32_t batch,
@@ -450,7 +419,6 @@ extern "C" int rb200_mlp_wgrad(const rb200_mlp_t* net, const float* net_input, i
   if (!net || !ws || !gpart) { set_last_error("rb200_mlp_wgrad: null argument"); return RB200_E_INVALID; }
   if (int rc = validate_mlp(net, "net")) return rc;
   if (batch <= 0 || splits <= 0) { set_last_error("rb200_mlp_wgrad: bad batch/splits"); return RB200_E_INVALID; }
-  if (wgrad_use_tc()) return rb200_wgrad_tc_launch(net, net_input, batch, ws, gpart, splits, stream);
   WgradParams p = {};
   p.n_layers = net->n_layers;
   p.B = batch;

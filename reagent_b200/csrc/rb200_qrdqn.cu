@@ -1,118 +1,15 @@
-// reagent_b200 -- QR-DQN: wide-head layer kernels + fused quantile-regression head.
+// reagent_b200 -- QR-DQN: fused quantile-regression loss head.
 //
-// QRDQNTrainer.train_step_gen (reagent/training/qrdqn_trainer.py:108-194) on a network whose
-// last layer is [hidden -> A*N] (FullyConnectedDQN with num_atoms, reagent/models/
-// fully_connected_network.py:166-217).  The (B, A, N) head output does not fit a row tile's
-// shared memory, so the head layer runs as a 2-D tiled launch (row tiles x column blocks) built
-// from the same tile primitives, and the distributional loss is one CTA per batch row:
+// The loss of QRDQNTrainer.train_step_gen (reagent/training/qrdqn_trainer.py:108-194) on the
+// (B, A, N) output of a network whose last layer is [hidden -> A*N] (FullyConnectedDQN with
+// num_atoms, reagent/models/fully_connected_network.py:166-217), one CTA per batch row:
 //   qr_head_kernel   mean over atoms -> masked argmax -> target distribution -> pairwise
 //                    quantile-Huber loss and its gradient WITHOUT materialising the
 //                    (N, B, N) tensor (qrdqn_trainer.py:125-155, :210-218).
-#include "rb200_rows.cuh"
+// The network around it runs on the layer kernels of rb200_mlp.cu.
+#include "rb200_common.cuh"
 
 namespace rb200 {
-
-constexpr int kColBlock = 512;  // head columns per CTA
-
-// ---------------- wide single Linear layer forward: out = act(in . W^T + b) ----------------
-struct LinFwdDev {
-  const float* in; int K;
-  const float* W; const float* b; int N; int act;
-  float* out; int batch; int ld_in, ld_o;
-};
-
-template <int NT, int TM, int KC>
-__global__ void __launch_bounds__(NT, 1) linear_fwd_wide_kernel(const LinFwdDev p) {
-  constexpr int R = (NT / 64) * TM;
-  extern __shared__ __align__(16) float smem[];
-  tile_smem_zero_all<NT>(smem);
-  float* Wst = smem;
-  float* xin = Wst + 2 * wstage_floats<KC>();
-  float* xo = xin + R * p.ld_in;
-  const int row0 = blockIdx.x * R;
-  const int c0 = blockIdx.y * kColBlock;
-  const int nloc = min(kColBlock, p.N - c0);
-  tile_load_rows<NT, R>(xin, p.ld_in, p.in, p.K, p.K, row0, p.batch);
-  __syncthreads();
-  tile_linear_fwd<NT, TM, KC>(xin, p.ld_in, p.K, p.W + (size_t)c0 * p.K, p.K,
-                              p.b ? p.b + c0 : nullptr, nloc, p.act, xo, p.ld_o, Wst);
-  tile_store_rows<NT, R>(xo, p.ld_o, p.out + c0, p.N, nloc, row0, p.batch);
-}
-
-// -------- wide contraction backward: dz_prev = (dz . W) * act'(h_prev), N large --------
-struct LinBwdDev {
-  const float* dz; int N;       // [B, N]
-  const float* W; int K;        // [N, K]
-  const float* h_prev; int act_prev;  // [B, K] output of the previous layer (or nullptr)
-  float* out;                   // [B, K]
-  int batch, ld_z, ld_k;
-};
-
-template <int NT, int TM, int KC>
-__global__ void __launch_bounds__(NT, 1) linear_bwd_wide_kernel(const LinBwdDev p) {
-  constexpr int R = (NT / 64) * TM;
-  extern __shared__ __align__(16) float smem[];
-  tile_smem_zero_all<NT>(smem);
-  float* Wst = smem;
-  float* zs = Wst + 2 * wstage_floats<KC>();  // [R, ld_z] slab of dz
-  float* accb = zs + R * p.ld_z;              // [R, ld_k] running sum
-  float* tmp = accb + R * p.ld_k;             // [R, ld_k] per-slab result
-  const int row0 = blockIdx.x * R;
-  const int K4 = round_up4(p.K);
-  for (int idx = threadIdx.x; idx < R * p.ld_k; idx += NT) accb[idx] = 0.f;
-  for (int n0 = 0; n0 < p.N; n0 += kColBlock) {
-    const int nloc = min(kColBlock, p.N - n0);
-    // slab of dz columns [n0, n0+nloc)
-    tile_load_rows<NT, R>(zs, p.ld_z, p.dz + n0, p.N, nloc, row0, p.batch);
-    __syncthreads();
-    tile_linear_bwd<NT, TM, KC>(zs, p.ld_z, nloc, p.W + (size_t)n0 * p.K, p.K, p.K, nullptr, 0, 0,
-                                tmp, p.ld_k, Wst);
-    for (int idx = threadIdx.x; idx < R * K4; idx += NT) {
-      const int r = idx / K4, c = idx - r * K4;
-      accb[r * p.ld_k + c] += tmp[r * p.ld_k + c];
-    }
-    __syncthreads();
-  }
-  for (int idx = threadIdx.x; idx < R * K4; idx += NT) {
-    const int r = idx / K4, c = idx - r * K4;
-    const int row = row0 + r;
-    if (row < p.batch && c < p.K) {
-      float g = accb[r * p.ld_k + c];
-      if (p.h_prev) g *= act_bwd_from_out(p.h_prev[(size_t)row * p.K + c], p.act_prev);
-      p.out[(size_t)row * p.K + c] = g;
-    }
-  }
-}
-
-// ---------------- whole-MLP backward (dZ chain) from a given last-layer dz ----------------
-struct MlpBwdDev {
-  const float* dz_last;  // [B, dims[L]] pre-activation gradient of the last layer
-  rb200_net_ws_t ws;
-  int batch, ld_h, ld_o;
-};
-
-template <int NT, int TM, int KC>
-__global__ void __launch_bounds__(NT, 1) mlp_bwd_rows_kernel(const Mlp net, const MlpBwdDev p) {
-  constexpr int R = (NT / 64) * TM;
-  extern __shared__ __align__(16) float smem[];
-  tile_smem_zero_all<NT>(smem);
-  float* Wst = smem;
-  float* gA = Wst + 2 * wstage_floats<KC>();
-  float* gB = gA + R * p.ld_h;
-  float* hb = gB + R * p.ld_h;
-  float* zl = hb + R * p.ld_h;
-  const int row0 = blockIdx.x * R;
-  const int DL = net.dims[net.n_layers];
-  tile_load_rows<NT, R>(zl, p.ld_o, p.dz_last, DL, DL, row0, p.batch);
-  __syncthreads();
-  // dz of the last layer is already in global memory: do not store it again
-  rb200_net_ws_t ws = p.ws;
-  float* keep = ws.dz[net.n_layers - 1];
-  ws.dz[net.n_layers - 1] = nullptr;
-  tile_mlp_bwd<NT, TM, KC>(net, zl, p.ld_o, gA, gB, hb, p.ld_h, Wst, ws.hidden, ws.dz, row0,
-                           p.batch, nullptr, 0, 0, 0);
-  (void)keep;
-}
 
 // ---------------- fused distributional head: one CTA per batch row ----------------
 struct QrDev {
@@ -275,65 +172,6 @@ __global__ void __launch_bounds__(256) qr_head_kernel(const QrDev d) {
 }  // namespace rb200
 
 using namespace rb200;
-
-extern "C" int rb200_linear_forward_tc(const float* W, const float* b, int32_t act, int32_t K,
-                                       int32_t N, const float* in, int32_t batch, float* out,
-                                       void* stream);
-
-extern "C" int rb200_linear_forward(const float* W, const float* b, int32_t act, int32_t K,
-                                    int32_t N, const float* in, int32_t batch, float* out,
-                                    void* stream) {
-  if (!W || !in || !out || K <= 0 || N <= 0 || batch <= 0) { set_last_error("rb200_linear_forward: bad argument"); return RB200_E_INVALID; }
-  // GEMM-shaped problems (>= one full 128x128 tile) go to the wgmma kernel
-  static const bool no_tc = getenv("RB200_DISABLE_WGMMA") != nullptr;  // debugging aid
-  if (!no_tc && batch >= 128 && N >= 128) return rb200_linear_forward_tc(W, b, act, K, N, in, batch, out, stream);
-  LinFwdDev p{in, K, W, b, N, act, out, batch, 0, kColBlock + 4};
-  RowsCfg cfg = pick_rows_cfg(batch, K, 4, 1, 0, p.ld_o, 0);
-  if (cfg.tm == 0) { set_last_error("rb200_linear_forward: tile does not fit in shared memory"); return RB200_E_SMEM; }
-  p.ld_in = cfg.ld_in;
-  dim3 grid(ceil_div(batch, rows_per_tile(cfg)), ceil_div(N, kColBlock));
-  return dispatch_rows(cfg, [&](auto NT, auto KC) {
-    return launch<linear_fwd_wide_kernel<NT(), 4, KC()>>(grid, NT(), cfg.smem_bytes, (cudaStream_t)stream,
-                                                         "linear_fwd_wide_kernel launch", p);
-  });
-}
-
-extern "C" int rb200_linear_backward_dx(const float* W, int32_t K, int32_t N, const float* dz,
-                                        const float* h_prev, int32_t act_prev, int32_t batch,
-                                        float* out, void* stream) {
-  if (!W || !dz || !out || K <= 0 || N <= 0 || batch <= 0) { set_last_error("rb200_linear_backward_dx: bad argument"); return RB200_E_INVALID; }
-  LinBwdDev p{dz, N, W, K, h_prev, act_prev, out, batch, kColBlock + 4, round_up4(K) + 4};
-  RowsCfg cfg = pick_rows_cfg(batch, kColBlock, 4, 1, 0, 2 * p.ld_k, 0);
-  if (cfg.tm == 0) { set_last_error("rb200_linear_backward_dx: tile does not fit in shared memory"); return RB200_E_SMEM; }
-  p.ld_z = cfg.ld_in;
-  dim3 grid(ceil_div(batch, rows_per_tile(cfg)));
-  return dispatch_rows(cfg, [&](auto NT, auto KC) {
-    return launch<linear_bwd_wide_kernel<NT(), 4, KC()>>(grid, NT(), cfg.smem_bytes, (cudaStream_t)stream,
-                                                         "linear_bwd_wide_kernel launch", p);
-  });
-}
-
-extern "C" int rb200_mlp_backward(const rb200_mlp_t* net, const float* dz_last, int32_t batch,
-                                  const rb200_net_ws_t* ws, void* stream) {
-  if (!net || !dz_last || !ws || batch <= 0) { set_last_error("rb200_mlp_backward: bad argument"); return RB200_E_INVALID; }
-  if (int rc = validate_mlp(net, "net")) return rc;
-  if (net->n_layers < 2) return RB200_OK;  // nothing below the last layer
-  MlpBwdDev p;
-  p.dz_last = dz_last;
-  p.ws = *ws;
-  p.batch = batch;
-  const int DL = net->dims[net->n_layers];
-  p.ld_o = round_up4(DL) + 4;
-  RowsCfg cfg = pick_rows_cfg(batch, 4, mlp_max_hidden(net), 0, 3, p.ld_o, 0);
-  if (cfg.tm == 0) { set_last_error("rb200_mlp_backward: tile does not fit in shared memory"); return RB200_E_SMEM; }
-  p.ld_h = cfg.ld_h;
-  const Mlp m = make_mlp(net);
-  dim3 grid(ceil_div(batch, rows_per_tile(cfg)));
-  return dispatch_rows(cfg, [&](auto NT, auto KC) {
-    return launch<mlp_bwd_rows_kernel<NT(), 4, KC()>>(grid, NT(), cfg.smem_bytes, (cudaStream_t)stream,
-                                                      "mlp_bwd_rows_kernel launch", m, p);
-  });
-}
 
 extern "C" int rb200_qrdqn_head(const rb200_qrdqn_args_t* a, void* stream) {
   if (!a || a->batch <= 0 || a->num_actions <= 0 || a->num_atoms <= 0) { set_last_error("rb200_qrdqn_head: bad argument"); return RB200_E_INVALID; }

@@ -10,8 +10,7 @@ from typing import Optional
 import torch
 
 from ..core import types as rlt
-from .workspace import (NetWorkspace, Pins, batch_device, head_backward_dx, param_grads, wgrad,
-                        ws_fits)
+from .workspace import NetWorkspace, Pins, batch_device, param_grads, wgrad, ws_fits
 
 
 class DistributionalStep:
@@ -61,7 +60,7 @@ class DistributionalStep:
         qa.forward_wide(state, ws["cur"], net.hidden[L - 2] if L > 1 else None, save=net)
         self._launch_head(batch, ws, pins, sample_weight)
         if L > 1:
-            head_backward_dx(qa, net, B, ws)
+            qa.layer_backward_dx(L - 1, net, B, ws)
             if L > 2:
                 qa.backward(net, B, n_layers=L - 1)
         wgrad(qa, net, state, B)

@@ -165,12 +165,16 @@ class DQNTrainer(DQNTrainerBaseLightning):
     _tc_prepacked = False  # set by a caller that already ran rb200_dqn_tc_pack (fused_step.py)
 
     def _tc_pack(self, qd, a, device):
-        """Scratch for the wgmma path of K2 (packed weight images), or None when the
-        network does not fit it (or RB200_DISABLE_WGMMA is set): then the mma.sync row-tile
-        kernel runs.  Both are this library's CUDA kernels; there is no other fallback."""
+        """Scratch for the wgmma path of K2 (packed weight images), or None: see _tc_pack_for."""
         return self._tc_pack_for((int(a.double_q), int(a.do_backward)), qd, device)
 
     def _tc_pack_for(self, key, qd, device):
+        """Weight-image scratch of the wgmma K2 (dqn_td_tc_kernel) for `key` = (double_q,
+        do_backward), cached per key, or None when the network's shapes do not fit that kernel:
+        then K2 runs on the mma.sync row-tile kernel (dqn_td_rows_kernel).  Both are this
+        library's CUDA kernels; there is no other fallback.  Setting RB200_DISABLE_WGMMA before
+        a key's first step puts K2 on dqn_td_rows_kernel for every shape, so that kernel can be
+        checked on the shapes the wgmma kernel takes; nothing else reads it."""
         cache = self.__dict__.setdefault("_tc_pack_cache", {})
         pack = cache.get(key, False)
         if pack is False or (pack is not None and pack.device != device):
@@ -208,7 +212,7 @@ class DQNTrainer(DQNTrainerBaseLightning):
         from ..models.arena import ParamArena
 
         qa = self.q_network.arena
-        if type(qa) is not ParamArena or os.environ.get("RB200_ADAM_PACK", "1") != "1":
+        if type(qa) is not ParamArena:
             return None
         pack = self._tc_pack_for((int(bool(self.double_q_learning)), 1), qa.desc(), qa.flat.device)
         return None if pack is None else (pack, 1)

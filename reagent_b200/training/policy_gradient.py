@@ -168,7 +168,7 @@ class PolicyGradientStep:
     def _wgrad(self, arena, ws: NetWorkspace, x, rows: int):
         """rb200_mlp_wgrad into the leading `splits` rows of a grow-only partial slab."""
         lib = _lib.lib()
-        splits = lib.rb200_wgrad_splits_for(arena.desc(), rows)
+        splits = lib.rb200_wgrad_splits(rows)
         slab = self._slabs.get(id(arena))
         if slab is None or slab.shape[0] < splits or slab.device != arena.flat.device:
             # zeroed once: alignment padding is never written

@@ -112,7 +112,7 @@ def ensure_gpart(arena: ParamArena, splits: int):
 
 def wgrad(arena: ParamArena, ws: NetWorkspace, net_input, batch: int):
     """Launch the split-K weight-gradient kernel for one network."""
-    splits = _lib.lib().rb200_wgrad_splits_for(arena.desc(), batch)
+    splits = _lib.lib().rb200_wgrad_splits(batch)
     g = ensure_gpart(arena, splits)
     rc = _lib.lib().rb200_mlp_wgrad(arena.desc(), _lib.ptr(net_input), batch, ws.c,
                                     g.data_ptr(), splits, _lib.cur_stream())
@@ -125,13 +125,6 @@ def backward_wgrad(arena: ParamArena, ws: NetWorkspace, net_input, batch: int):
     weight gradients."""
     arena.backward(ws, batch)
     wgrad(arena, ws, net_input, batch)
-
-
-def head_backward_dx(arena: ParamArena, ws: NetWorkspace, batch: int, cache: dict):
-    """dZ of the layer below a wide head: dz[L-2] = (dz[L-1] . W_head) * act'(h[L-2])
-    (torch.nn.functional.linear's backward w.r.t. its input).  Wide heads (QR-DQN: A*N atoms,
-    C51: A*51) take the wgmma split-K path, which needs a scratch buffer kept in `cache`."""
-    arena.layer_backward_dx(len(arena.acts) - 1, ws, batch, cache)
 
 
 def reduced_grad(arena: ParamArena) -> torch.Tensor:

@@ -11,9 +11,9 @@ from tests import golden_util as G
 from tests.golden_util import TOL
 
 # K2 has two implementations in the library: the warpgroup-MMA kernel (rb200_dqn_tc.cu,
-# preferred when the shapes fit; path id "tcgen05" is its historical name) and the mma.sync
-# row-tile kernel (rb200_dqn.cu); every golden case runs on both.
-K2_PATHS = ["tcgen05", "rows"]
+# preferred when the shapes fit) and the mma.sync row-tile kernel (rb200_dqn.cu); every golden
+# case runs on both.
+K2_PATHS = ["wgmma", "rows"]
 
 
 def _select_k2(monkeypatch, path):
@@ -25,7 +25,7 @@ def _select_k2(monkeypatch, path):
 
 def _assert_k2(t, path):
     used_tc = t._last_td_call[-1] is not None
-    assert used_tc == (path == "tcgen05"), f"K2 ran on the wrong kernel (wanted {path})"
+    assert used_tc == (path == "wgmma"), f"K2 ran on the wrong kernel (wanted {path})"
 
 
 def _build_trainer(meta, arrays=None, dev="cuda"):
@@ -89,7 +89,7 @@ CONFIG2_MAX_ADAM_OUTLIER_FRAC = 1.2e-3
 
 # the mma.sync row-tile kernel (the library's second K2, taken when shapes do not fit the
 # wgmma kernel) accumulates its 3xTF32 products in a different order, so per-row dZ gets 2e-5
-CONFIG2_DZ_TOL = {"tcgen05": TOL, "rows": 2e-5}
+CONFIG2_DZ_TOL = {"wgmma": TOL, "rows": 2e-5}
 
 
 def _build_cpe_trainer(meta, arrays):

@@ -359,10 +359,9 @@ def test_sac_with_adamw_amsgrad_matches_reference():
 
 @pytest.mark.parametrize("amsgrad", [False, True])
 @pytest.mark.parametrize("S,sizes,A", [(128, [256, 128], 16), (36, [300, 130, 20], 9)])
-def test_adamw_writes_the_same_weight_images_as_the_pack_kernel(S, sizes, A, amsgrad, monkeypatch):
+def test_adamw_writes_the_same_weight_images_as_the_pack_kernel(S, sizes, A, amsgrad):
     from reagent_b200.optimizer import Optimizer__Union, FusedAdamW
 
-    monkeypatch.setenv("RB200_ADAM_PACK", "1")
     B = 64
     meta = dict(S=S, A=A, B=B, sizes=sizes, acts=["relu"] * len(sizes), gamma=0.9, tau=0.1,
                 loss="huber", maxq=True, multi_steps=None, time_diff=False, boost=None,

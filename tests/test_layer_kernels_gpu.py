@@ -4,7 +4,7 @@ and compared with plain references at the shapes where tiled kernels go wrong.
 * rb200_mlp_forward / rb200_mlp_backward / rb200_linear_backward_dx (row-tile path) against an
   fp64 chain computed from exactly the fp32 inputs the kernel received, in every row-tile
   configuration (RB200_FORCE_CFG) and at the 256-column chunk and k-chunk edges.
-* rb200_mlp_wgrad (mma.sync and wgmma kernels) slab by slab against fp64 dZ^T.A, with the
+* rb200_mlp_wgrad (the mma.sync kernel) slab by slab against fp64 dZ^T.A, with the
   gradient partials prefilled with NaN so an unwritten (empty) slab cannot pass.
 * rb200_grad_reduce bit for bit against a sequential fp32 sum in slab order.
 * rb200_adam_soft_update / FusedAdam against torch.optim.Adam(foreach=False) on the CPU, and
@@ -359,9 +359,9 @@ def test_linear_backward_dx_matches_fp64(monkeypatch, cfg, batch):
 
 
 # ------------------------------------------------------------------------------------------
-# (c) rb200_mlp_wgrad (both kernels) and rb200_grad_reduce
+# (c) rb200_mlp_wgrad and rb200_grad_reduce
 # ------------------------------------------------------------------------------------------
-# every layer sits on an edge of the 64x64 (mma.sync) or 128x256 (wgmma) tiles
+# every layer sits on an edge of the kernel's 64x64 tiles
 WGRAD_NETS = [
     [65, 63, 64, 129, 257, 127, 255, 128, 256],
     [1, 3, 1],
@@ -385,14 +385,9 @@ def _wgrad_inputs(net, batch, seed, offset=0):
     return acts, dZs, dev[:L], dev[L:]
 
 
-@pytest.mark.parametrize("tc", [False, True], ids=["mma_sync", "wgmma"])
+@pytest.mark.parametrize("kernel", ["mma_sync"])
 @pytest.mark.parametrize("batch", [1, 31, 100, 257, 4096])
-def test_mlp_wgrad_slabs_match_fp64(monkeypatch, tc, batch):
-    monkeypatch.delenv("RB200_DISABLE_WGMMA", raising=False)
-    if tc:
-        monkeypatch.setenv("RB200_WGRAD_TC", "1")
-    else:
-        monkeypatch.delenv("RB200_WGRAD_TC", raising=False)
+def test_mlp_wgrad_slabs_match_fp64(kernel, batch):
     lib = _lib_()
     worst = 0.0
     for ni, dims in enumerate(WGRAD_NETS):
@@ -401,8 +396,7 @@ def test_mlp_wgrad_slabs_match_fp64(monkeypatch, tc, batch):
         # layer l's input activation is hidden[l-1]: feed the random activations through ws
         ws = _ws(hidden=acts_d[1:], dz=dZs_d)
         d = net.desc()
-        split_set = sorted({1, 3, 8, lib.rb200_wgrad_splits(batch),
-                            lib.rb200_wgrad_splits_for(d, batch), 64})
+        split_set = sorted({1, 3, 8, lib.rb200_wgrad_splits(batch), 64})
         for splits in split_set:
             gpart = torch.full((splits, net.n), NAN, device="cuda")
             rc = lib.rb200_mlp_wgrad(d, acts_d[0].data_ptr(), batch, ws, gpart.data_ptr(), splits,
@@ -411,7 +405,7 @@ def test_mlp_wgrad_slabs_match_fp64(monkeypatch, tc, batch):
             torch.cuda.synchronize()
             worst = max(worst, _check_wgrad_layers(net, acts, dZs, batch, splits, gpart,
                                                    (dims, splits)))
-    _record("mlp_wgrad", kernel="wgmma" if tc else "mma_sync", batch=batch, max_rel_err=worst)
+    _record("mlp_wgrad", kernel=kernel, batch=batch, max_rel_err=worst)
 
 
 def _check_wgrad_layers(net, acts, dZs, batch, splits, gpart, what):
@@ -440,15 +434,10 @@ def _check_wgrad_layers(net, acts, dZs, batch, splits, gpart, what):
     return worst
 
 
-@pytest.mark.parametrize("tc", [False, True], ids=["mma_sync", "wgmma"])
-def test_mlp_wgrad_odd_offsets_and_unaligned_inputs(monkeypatch, tc):
-    """A hand-built descriptor whose weights start at odd arena offsets (the scalar epilogue of
-    wgrad_tc_kernel) over activations that are not 16-byte aligned (scalar staging)."""
-    monkeypatch.delenv("RB200_DISABLE_WGMMA", raising=False)
-    if tc:
-        monkeypatch.setenv("RB200_WGRAD_TC", "1")
-    else:
-        monkeypatch.delenv("RB200_WGRAD_TC", raising=False)
+@pytest.mark.parametrize("kernel", ["mma_sync"])
+def test_mlp_wgrad_odd_offsets_and_unaligned_inputs(kernel):
+    """A hand-built descriptor whose weights start at odd arena offsets over activations that
+    are not 16-byte aligned (scalar staging)."""
     lib = _lib_()
     worst = 0.0
     for batch in (100, 257):
@@ -464,7 +453,7 @@ def test_mlp_wgrad_odd_offsets_and_unaligned_inputs(monkeypatch, tc):
             torch.cuda.synchronize()
             worst = max(worst, _check_wgrad_layers(net, acts, dZs, batch, splits, gpart,
                                                    ("odd w_off", batch, splits)))
-    _record("mlp_wgrad_odd_offsets", kernel="wgmma" if tc else "mma_sync", max_rel_err=worst)
+    _record("mlp_wgrad_odd_offsets", kernel=kernel, max_rel_err=worst)
 
 
 @pytest.mark.parametrize("n", [1, 255, 257, NUM_SMS * 8 * 256 + 5])

@@ -90,7 +90,7 @@ def _rand(*shape, gen):
 
 
 # ---------------------------------------------------------------- serial tails
-@pytest.mark.parametrize("path", ["tcgen05", "rows"])
+@pytest.mark.parametrize("path", ["wgmma", "rows"])
 def test_dqn_td_serial_tail(path, monkeypatch):
     """K2 on both paths; B = 1000 leaves a ragged last tile (16 rows, 32 rows on wgmma)."""
     _select_k2(monkeypatch, path)
@@ -107,13 +107,13 @@ def test_dqn_td_serial_tail(path, monkeypatch):
              not_terminal=torch.ones(B, 1, device="cuda"), action=act, next_action=act,
              possible_actions_mask=torch.ones(B, A, device="cuda"),
              possible_next_actions_mask=torch.ones(B, A, device="cuda"))
-    rows = 32 if path == "tcgen05" else 16
+    rows = 32 if path == "wgmma" else 16
     fields = {"loss_partials": lambda B: -(-B // rows), "loss": lambda B: 1}
     seen_tc = _capture(monkeypatch, "rb200_dqn_td_step_tc", 2, fields)
     seen_rows = _capture(monkeypatch, "rb200_dqn_td_step", 2, fields)
     t.train_batch(_rlt_batch(b, meta), 0)
     _assert_k2(t, path)
-    (got,) = seen_tc if path == "tcgen05" else seen_rows
+    (got,) = seen_tc if path == "wgmma" else seen_rows
     (tot,) = _serial(got["loss_partials"], -(-B // rows))
     _same_bits(got["loss"][0], tot / f32(B))
 

@@ -15,13 +15,12 @@ from tests.online_step import (assert_captured_equals_eager, assert_matches_host
                                assert_nan_reward_raises, bench_setup, filled_heap, params,
                                transition_stream, tree, ulps)
 from tests.builders import (CONFIG2_DZ_TOL, CONFIG2_MAX_ADAM_OUTLIER_FRAC, CONFIG2_MAX_FLIPPED_ROWS,
-                            _assert_k2, _build_bcq, _build_cpe_trainer, _build_trainer,
+                            K2_PATHS, _assert_k2, _build_bcq, _build_cpe_trainer, _build_trainer,
                             _golden_batch, _rlt_batch, _select_k2)
 from tests.golden_cases import BCQ_DQN_CASES, DQN_CPE_CASES, _dqn_kwargs
 from tests.golden_util import TOL
 
 pytestmark = pytest.mark.gpu
-K2_PATHS = ["tcgen05", "rows"]
 
 
 @pytest.mark.parametrize("path", K2_PATHS)
