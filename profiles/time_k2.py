@@ -22,11 +22,17 @@ one, and the median is reported.
     python profiles/time_k2.py --out DIR [--reps 11] [--launches 200] [--steps 100]
 
 Writes DIR/time_k2_<card>_<limit>w.json and prints the same JSON.
+
+With --against LIB (another build of libreagent_b200.so, e.g. the parent commit's) the whole
+measurement above runs --runs times with each library, alternating, each run in a process of its
+own (RB200_LIB selects the library), and DIR/time_k2_against_<card>_<limit>w.json holds every
+run of both and the median over runs of each headline number.
 """
 import argparse
 import json
 import os
 import statistics
+import subprocess
 import sys
 import tempfile
 
@@ -122,13 +128,60 @@ def breakdown(g, steps, tmp, tag):
     }
 
 
+def headline(res):
+    """The numbers a comparison of two builds is about, from one run's result."""
+    k2 = res["k2_alone_us_by_ctas"]
+    return {"k2_alone_us_1_cta": k2["1"]["median"], f"k2_alone_us_{CTAS[-1]}_ctas": k2[str(CTAS[-1])]["median"],
+            **{f"step_us_{k}": v["median"] for k, v in res["step_per_update_us"].items()},
+            "k2_us_in_step_k1_on_side_stream": res["step_breakdown"]["k1_on_side_stream"]["median_us"]["K2"]}
+
+
+def against(args):
+    """--against: alternate whole runs of this script between the tree's library and args.against."""
+    libs = {"this_tree": None, "against": args.against}
+    runs = {k: [] for k in libs}
+    with tempfile.TemporaryDirectory() as tmp:
+        for r in range(args.runs):
+            for k in (list(libs) if r % 2 == 0 else list(libs)[::-1]):
+                env = dict(os.environ)
+                env.pop("RB200_LIB", None)
+                if libs[k]:
+                    env["RB200_LIB"] = os.path.abspath(libs[k])
+                out = os.path.join(tmp, f"{k}_{r}")
+                subprocess.run([sys.executable, os.path.abspath(__file__), "--out", out, "--reps", str(args.reps),
+                                "--launches", str(args.launches), "--steps", str(args.steps)],
+                               env=env, check=True, stdout=subprocess.DEVNULL)
+                (name,) = os.listdir(out)
+                with open(os.path.join(out, name)) as f:
+                    runs[k].append(json.load(f))
+    first = runs["this_tree"][0]
+    res = {
+        "what": first["what"] + f"; {args.runs} runs with each of two libraries, alternating",
+        "card": first["card"],
+        "cards_of_all_runs": sorted({json.dumps(x["card"]) for v in runs.values() for x in v}),
+        "libraries": {k: v or "the tree's reagent_b200/libreagent_b200.so" for k, v in libs.items()},
+        "config": first["config"],
+        "method": first["method"] + "; each run a separate process, the two libraries alternating",
+        "median_over_runs": {k: {h: statistics.median(headline(x)[h] for x in v) for h in headline(v[0])}
+                             for k, v in runs.items()},
+        "min_max_over_runs": {k: {h: [min(headline(x)[h] for x in v), max(headline(x)[h] for x in v)]
+                                  for h in headline(v[0])} for k, v in runs.items()},
+        "runs": {k: [headline(x) for x in v] for k, v in runs.items()},
+    }
+    write_result(args.out, "time_k2_against", res)
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--out", required=True, help="directory for the result file")
     ap.add_argument("--reps", type=int, default=11)
     ap.add_argument("--launches", type=int, default=200)
     ap.add_argument("--steps", type=int, default=100)
+    ap.add_argument("--against", metavar="LIB", help="another build of libreagent_b200.so to compare with")
+    ap.add_argument("--runs", type=int, default=5, help="runs per library with --against")
     args = ap.parse_args()
+    if args.against:
+        return against(args)
 
     dev = cuda_device(__file__)
     import torch

@@ -16,7 +16,8 @@
 //                images).  The two MMA warpgroups read their A fragments straight from the
 //                ring (conflict-free 4-byte loads), split them into TF32 hi / lo in registers
 //                and issue the MMAs with A FROM REGISTERS: every weight byte crosses shared
-//                memory once in and once out as raw fp32.
+//                memory once in and once out as raw fp32.  The MMAs of a 32-k chunk go out as
+//                one chain while the next chunk's fragments are read and split.
 //   activations  live in shared memory as hi/lo planes in the canonical K-major layout (rows =
 //                batch rows); the epilogue of layer l (registers -> bias -> activation -> split)
 //                writes them straight into the B operand of layer l+1 and, for the online
@@ -33,6 +34,8 @@
 // Reference semantics: reagent/training/dqn_trainer.py:157-239, dqn_trainer_base.py:33-77,
 // 216-241 (see rb200_dqn.cu for the line-by-line map; the loss code is the same).
 #include <string.h>
+
+#include <type_traits>
 
 #include "rb200_dqn_tc_layout.cuh"
 #include "rb200_wgmma.cuh"
@@ -143,6 +146,30 @@ __global__ void __launch_bounds__(256) dqn_tc_pack_kernel(const PackDev p) {
 // epilogues stay small enough for the instruction cache
 __device__ __noinline__ float act_fwd_slow(float x, int act) { return act_fwd(x, act); }
 __device__ __noinline__ float act_bwd_slow(float y, int act) { return act_bwd_from_out(y, act); }
+
+constexpr int kQCK = kQKC / 8;  // K = 8 MMA steps in a chunk
+
+// The MMAs of one chunk of NK k steps, issued as one chain: one fence, per k step
+// W_hi . [X_hi | X_lo] then W_lo . X_hi into the same accumulators, in k order, one commit.
+// b0 is the shared-memory address of the chunk's first k quad in the B operand.
+template <int NK>
+__device__ __forceinline__ void chunk_mma(float (&acc)[32], const uint32_t (&ah)[kQCK][4],
+                                          const uint32_t (&al)[kQCK][4], uint32_t b0) {
+  wgmma_fence();
+#pragma unroll
+  for (int kk = 0; kk < NK; ++kk) {
+    const uint64_t bd = wgmma_desc(b0 + (uint32_t)(2 * kk) * kQLboB, kQLboB, 128);
+    wgmma_rs_n64(acc, ah[kk], bd, 1u);  // W_hi . [X_hi | X_lo]
+    wgmma_rs_n32(acc, al[kk], bd, 1u);  // W_lo . X_hi
+  }
+  wgmma_commit();
+}
+// f(std::integral_constant<int, nk>()) for a run-time nk in [1, NK]
+template <int NK, typename F>
+__device__ __forceinline__ void with_ksteps(int nk, F&& f) {
+  if (nk == NK) f(std::integral_constant<int, NK>());
+  else if constexpr (NK > 1) with_ksteps<NK - 1>(nk, f);
+}
 
 // kWeighted: prioritized-replay importance weights (a.sample_weight), a separate instantiation so
 // that the unweighted kernel stays exactly as it is
@@ -314,58 +341,80 @@ dqn_td_tc_kernel(const Mlp q, const Mlp qt, const QDev p) {
         const bool ok0 = live && m0 < rows8, ok1 = live && m0 + 8 < rows8;
         float acc[32];
 #pragma unroll
-        for (int i = 0; i < 32; ++i) acc[i] = 0.f;
-        for (int c = 0; c < kch; c += kQSub) {
-          const int nsub = kch - c < kQSub ? kch - c : kQSub;
-          mbar_wait(full + ss, spar);
-          // A fragments of the stage: raw fp32 from the ring -> TF32 hi / lo in registers
-          uint32_t ah[kQSub * 4][4], al[kQSub * 4][4];
-          int ksteps[kQSub];
-#pragma unroll
-          for (int j = 0; j < kQSub; ++j) {
-            const int kl = st.K - kQKC * (c + j);
-            ksteps[j] = j < nsub ? round_up8(kl < kQKC ? kl : kQKC) / 8 : 0;
-            const unsigned char* src = ring + ss * kQStageBytes + (uint32_t)j * (kQKC / 4) * lbo + tq * 4;
-#pragma unroll
-            for (int ks = 0; ks < 4; ++ks) {
-              float v[4] = {0.f, 0.f, 0.f, 0.f};
-              if (ks < ksteps[j]) {
-                const unsigned char* s0 = src + (uint32_t)(2 * ks) * lbo;  // k = 8 ks + tq
-                const unsigned char* s1 = s0 + lbo;                        // k = 8 ks + 4 + tq
-                if (ok0) { v[0] = *reinterpret_cast<const float*>(s0 + m0 * 16); v[2] = *reinterpret_cast<const float*>(s1 + m0 * 16); }
-                if (ok1) { v[1] = *reinterpret_cast<const float*>(s0 + (m0 + 8) * 16); v[3] = *reinterpret_cast<const float*>(s1 + (m0 + 8) * 16); }
-              }
-#pragma unroll
-              for (int e = 0; e < 4; ++e) {
-                float h, lo_;
-                split1(v[e], h, lo_);
-                ah[4 * j + ks][e] = __float_as_uint(h);
-                al[4 * j + ks][e] = __float_as_uint(lo_);
-              }
-            }
-          }
-          // the stage's values are in registers: the ring stage can be refilled
-          __syncwarp();
-          if (lane == 0) mbar_arrive(sfree + ss);
-          if (++ss == kQStages) { ss = 0; spar ^= 1u; }
-          // (a warpgroup without features in this tile multiplies zeros: issuing unconditionally
-          // keeps the MMAs out of divergent code, which the compiler would serialise)
-          wgmma_fence();
-#pragma unroll
-          for (int j = 0; j < kQSub; ++j) {
-#pragma unroll
-            for (int ks = 0; ks < 4; ++ks) {
-              if (ks < ksteps[j]) {
-                const uint32_t kq = (uint32_t)(2 * (4 * (c + j) + ks));  // first k quad of this K = 8 step
-                const uint64_t bd = wgmma_desc(bbase + kq * kQLboB, kQLboB, 128);
-                wgmma_rs_n64(acc, ah[4 * j + ks], bd, 1u);  // W_hi . [X_hi | X_lo]
-                wgmma_rs_n32(acc, al[4 * j + ks], bd, 1u);  // W_lo . X_hi
-              }
-            }
-          }
-          wgmma_commit();
-          wgmma_wait<0>();
+        for (int i = 0; i < 32; ++i) {
+          acc[i] = 0.f;
+          wgmma_fence_operand(acc[i]);
         }
+        // The MMAs are issued a chunk (kQCK k steps, 8 MMAs) at a time, each chunk as one
+        // unbroken chain, and the next chunk's A fragments are read and split while that chain
+        // runs.  Chunk c is chunk c % 2 of its ring stage and uses fragment buffer c % 2; wait<1>
+        // before a read retires the chain that last used the buffer it overwrites.  Buffers of
+        // a whole stage (2 x 64 registers) do not fit: with 9 warps, 3 share an SM
+        // sub-partition's 64 KB register file, which caps the kernel at 168 registers per
+        // thread.  A short last chunk (K not a multiple of 32) is issued after the others have
+        // retired: inside the loop, its extra code paths make ptxas serialise all the MMAs of the
+        // kernel (notes C7512 / C7513).
+        static_assert(kQSub == 2, "one fragment buffer per chunk of a ring stage");
+        const int kfull = st.K / kQKC;                            // chunks of kQCK k steps
+        const int nk_last = round_up8(st.K - kQKC * kfull) / 8;  // k steps of a short last chunk
+        uint32_t ah[2][kQCK][4], al[2][kQCK][4];
+        // A fragments of chunk c: raw fp32 from the ring (k steps past nk and rows past the tile
+        // read as zeros), the ring stage released once both its chunks are in registers, then
+        // TF32 hi / lo, every register final before the chunk's MMAs are issued
+        auto fetch = [&](uint32_t (&fh)[kQCK][4], uint32_t (&fl)[kQCK][4], int c, int nk) {
+          if (c % 2 == 0) mbar_wait(full + ss, spar);
+          float v[kQCK][4];
+#pragma unroll
+          for (int kk = 0; kk < kQCK; ++kk) {
+            v[kk][0] = v[kk][1] = v[kk][2] = v[kk][3] = 0.f;
+            const unsigned char* s0 = ring + ss * kQStageBytes + (uint32_t)((c % 2) * (kQKC / 4) + 2 * kk) * lbo + tq * 4;  // k = 8 kk + tq
+            const unsigned char* s1 = s0 + lbo;                                                                         // k = 8 kk + 4 + tq
+            if (kk < nk && ok0) { v[kk][0] = *reinterpret_cast<const float*>(s0 + m0 * 16); v[kk][2] = *reinterpret_cast<const float*>(s1 + m0 * 16); }
+            if (kk < nk && ok1) { v[kk][1] = *reinterpret_cast<const float*>(s0 + (m0 + 8) * 16); v[kk][3] = *reinterpret_cast<const float*>(s1 + (m0 + 8) * 16); }
+          }
+          if (c % 2 == 1 || c + 1 == kch) {
+            // the stage's values are in registers: the ring stage can be refilled
+            __syncwarp();
+            if (lane == 0) mbar_arrive(sfree + ss);
+            if (++ss == kQStages) { ss = 0; spar ^= 1u; }
+          }
+#pragma unroll
+          for (int kk = 0; kk < kQCK; ++kk)
+#pragma unroll
+            for (int e = 0; e < 4; ++e) {
+              float h, lo_;
+              split1(v[kk][e], h, lo_);
+              fh[kk][e] = __float_as_uint(h);
+              fl[kk][e] = __float_as_uint(lo_);
+              wgmma_fence_operand(fh[kk][e]);
+              wgmma_fence_operand(fl[kk][e]);
+            }
+        };
+        auto b_of = [&](int c) { return bbase + (uint32_t)(2 * kQCK * c) * kQLboB; };
+        // (a warpgroup without features in this tile multiplies zeros: issuing unconditionally
+        // keeps the MMAs out of divergent code, which the compiler would serialise)
+        if (kfull > 0) fetch(ah[0], al[0], 0, kQCK);
+        for (int c = 0; c < kfull; c += 2) {
+          chunk_mma<kQCK>(acc, ah[0], al[0], b_of(c));
+          if (c + 1 == kfull) break;
+          wgmma_wait<1>();  // chunk c - 1 retired: buffer 1 is free
+          fetch(ah[1], al[1], c + 1, kQCK);
+          chunk_mma<kQCK>(acc, ah[1], al[1], b_of(c + 1));
+          if (c + 2 == kfull) break;
+          wgmma_wait<1>();  // chunk c retired: buffer 0 is free
+          fetch(ah[0], al[0], c + 2, kQCK);
+        }
+        if (kfull < kch) {
+          // the short last chunk: its k-step count is a template argument, so no branch either
+          wgmma_wait<0>();
+          fetch(ah[0], al[0], kfull, nk_last);
+          with_ksteps<kQCK>(nk_last, [&](auto nk_c) {
+            chunk_mma<decltype(nk_c)::value>(acc, ah[0], al[0], b_of(kfull));
+          });
+        }
+        wgmma_wait<0>();
+#pragma unroll
+        for (int i = 0; i < 32; ++i) wgmma_fence_operand(acc[i]);
         if (!live) continue;
 
         // ---- epilogue of this tile ----

@@ -33,6 +33,12 @@ template <int N>
 __device__ __forceinline__ void wgmma_wait() {
   asm volatile("wgmma.wait_group.sync.aligned %0;\n" ::"n"(N) : "memory");
 }
+// Pins a register operand of a wgmma at this point of the program: its definition cannot move
+// below the (empty) asm.  Applied to the fragments and accumulators before wgmma_fence(), it
+// keeps every register write out of the MMA chain that follows; otherwise ptxas injects a
+// warpgroup.arrive in front of each MMA (note C7519) and the MMAs run one at a time.
+__device__ __forceinline__ void wgmma_fence_operand(uint32_t& r) { asm volatile("" : "+r"(r)::"memory"); }
+__device__ __forceinline__ void wgmma_fence_operand(float& r) { asm volatile("" : "+f"(r)::"memory"); }
 
 __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
   asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;\n" ::"r"(smem_u32(bar)), "r"(count));
