@@ -925,6 +925,66 @@ int rb200_mdnrnn_forward(const rb200_mdnrnn_args_t* args, void* stream);
 int rb200_mdnrnn_backward(const rb200_mdnrnn_args_t* args, void* stream);
 int rb200_mdnrnn_wgrad(const rb200_mdnrnn_args_t* args, void* stream);
 
+/* World-model evaluation (reagent/evaluation/world_model_evaluator.py):                  */
+/*   rb200_mdnrnn_eval         the loss of num_variants perturbed copies of one batch in one  */
+/*                             launch, grid [ceil(B / 16), V].  Variant v replaces columns     */
+/*                             [col_begin[v], col_end[v]) of x = cat(action, state) by         */
+/*                             fill[fill_off[v] ...] at every step and row (an empty range     */
+/*                             keeps x); variant perm_variant (or -1) reads action row perm[b] */
+/*                             (int64 [B]) for row b.  Targets are never changed.  `net` gives */
+/*                             the shape, arena, inputs, targets, loss weights, gmm_divisor   */
+/*                             and fit_only_one_next_step; its outputs, workspace and loss     */
+/*                             buffers are not read.  Writes loss [V][4] (gmm, bce, mse, loss) */
+/*                             -- each variant's the bits rb200_mdnrnn_forward gives on the    */
+/*                             batch with its replacement made -- and, when mus is not NULL,   */
+/*                             the means mus [V][T][B][G*S].  loss_partials holds              */
+/*                             V * 3 * ceil(B / 16) floats, tile_counter V zeros.  A perm      */
+/*                             value outside [0, B) makes that variant's results NaN.          */
+/*   rb200_mdnrnn_fill_values  per feature group of x's columns (rows = T * B): a width-1     */
+/*                             group's column mean (fp64 sum, rounded once); a wider (enum)    */
+/*                             group's one-hot at the first column whose column sum equals the */
+/*                             lower median of the group's column sums.  Into fill[column].   */
+/*   rb200_mdnrnn_sensitivity  per group of state columns: the mean over (rows, G) of the sum  */
+/*                             over the group's columns of |mus1 - mus0| (mus [rows, G, S]).   */
+/* Groups: num_groups >= 1, group g is [group_begin[g], group_begin[g + 1]), boundaries       */
+/* strictly increasing inside [0, width].  Limits: the MDN-RNN limits, and                   */
+/* 1 <= num_variants <= 1 + action_dim + state_dim (<= 257).                                 */
+#define RB200_MDNRNN_EVAL_MAX_VARIANTS (RB200_MDNRNN_MAX_INPUT + 1)
+typedef struct rb200_mdnrnn_eval_args {
+  rb200_mdnrnn_args_t net;
+  int32_t num_variants;
+  int32_t col_begin[RB200_MDNRNN_EVAL_MAX_VARIANTS];
+  int32_t col_end[RB200_MDNRNN_EVAL_MAX_VARIANTS];
+  int32_t fill_off[RB200_MDNRNN_EVAL_MAX_VARIANTS];
+  const float* fill;
+  int32_t fill_len;                              /* floats in fill */
+  int32_t perm_variant;
+  const int64_t* perm;
+  float* mus;                                    /* or NULL */
+  float* loss_partials;
+  uint32_t* tile_counter;
+  float* loss;
+} rb200_mdnrnn_eval_args_t;
+typedef struct rb200_mdnrnn_fill_args {
+  int32_t rows, action_dim, state_dim;
+  const float* action;                           /* [rows, action_dim] */
+  const float* state;                            /* [rows, state_dim] */
+  int32_t num_groups;
+  int32_t group_begin[RB200_MDNRNN_MAX_INPUT + 1];  /* columns of x, width action_dim + state_dim */
+  float* fill;                                   /* [action_dim + state_dim] */
+} rb200_mdnrnn_fill_args_t;
+typedef struct rb200_mdnrnn_sensitivity_args {
+  int32_t rows, state_dim, gaussians;
+  const float* mus0;
+  const float* mus1;
+  int32_t num_groups;
+  int32_t group_begin[RB200_MDNRNN_MAX_INPUT + 1];  /* state columns, width state_dim */
+  float* out;                                    /* [num_groups] */
+} rb200_mdnrnn_sensitivity_args_t;
+int rb200_mdnrnn_eval(const rb200_mdnrnn_eval_args_t* args, void* stream);
+int rb200_mdnrnn_fill_values(const rb200_mdnrnn_fill_args_t* args, void* stream);
+int rb200_mdnrnn_sensitivity(const rb200_mdnrnn_sensitivity_args_t* args, void* stream);
+
 /* ------------------------------------------------------------------------- */
 /* Cross-entropy-method planner (reagent/models/cem_planner.py): one launch of          */
 /* rb200_cem_rollout per CEM iteration.  CTA (j, m) of the grid [ceil(P / 16), K] takes  */

@@ -76,6 +76,9 @@ extern "C" int64_t rb200_abi_sizeof(const char* type_name) {
   RB200_SZ(rb200_add_args_t);
   RB200_SZ(rb200_per_draw_args_t);
   RB200_SZ(rb200_mdnrnn_args_t);
+  RB200_SZ(rb200_mdnrnn_eval_args_t);
+  RB200_SZ(rb200_mdnrnn_fill_args_t);
+  RB200_SZ(rb200_mdnrnn_sensitivity_args_t);
   RB200_SZ(rb200_cem_args_t);
   RB200_SZ(rb200_seq2reward_args_t);
   RB200_SZ(rb200_seq2reward_plan_args_t);
