@@ -337,6 +337,57 @@ typedef struct rb200_bc_xent_args {
 } rb200_bc_xent_args_t;
 int rb200_bc_xent_head(const rb200_bc_xent_args_t* args, void* stream);
 
+/* Loss head of SlateQTrainer (rb200_slateq.cu), reagent/training/slate_q_trainer.py:       */
+/* 199-276, one warp per row.  Per row b it forms the next slate (next_action[b], or with  */
+/* maxq the first slate_size candidates of q_next * docs_value in (score desc, index asc)  */
+/* order), weights the target network's values of that slate by the docs value            */
+/* (softmax(value * mask) over the slate with single_selection, value * mask without),     */
+/* divides by min(sum(mask), slate_size) of the current or next candidate mask without     */
+/* single_selection, and writes target = reward + discount * (next_q * not_terminal) with  */
+/* discount = gamma ** (time_diff / time_scale) when time_diff is given, else gamma.  The  */
+/* loss is mse(q_cur, target) over the reward_mask entries (single_selection) or all B*K   */
+/* entries; dz = d loss / d q_cur.  A terminal row's next slate is candidate 0 everywhere, */
+/* and in SARSA those rows of next_action are zeroed in place, as the reference does.     */
+/* With single_selection a one-CTA pass first counts the reward_mask entries (an integer, */
+/* so the count and the gradient scale 1 / count do not depend on the order); an empty    */
+/* mask gives a NaN loss and dz = 0.  Indices follow torch's indexing: one in [-C, 0)     */
+/* means C + index; one outside [-C, C) (the reference's IndexError) is never read: the   */
+/* row uses candidate 0 instead and status[0] is set to 1 (sticky).                       */
+/* Limits: 1 <= C <= RB200_SLATEQ_MAX_CANDIDATES, 1 <= K, K_next <= RB200_SLATEQ_MAX_SLATE, */
+/* 1 <= slate_size <= min(C, RB200_SLATEQ_MAX_SLATE) (one slate entry per lane); beyond   */
+/* them RB200_E_INVALID.                                                                   */
+#define RB200_SLATEQ_MAX_CANDIDATES 1024
+#define RB200_SLATEQ_MAX_SLATE 32
+#define RB200_SLATEQ_ROWS_PER_BLOCK 8
+#define RB200_SLATEQ_NORM_CURRENT 0 /* NORM_BY_CURRENT_SLATE_SIZE */
+#define RB200_SLATEQ_NORM_NEXT 1    /* NORM_BY_NEXT_SLATE_SIZE */
+typedef struct rb200_slateq_args {
+  int32_t batch, num_candidates;   /* B, C */
+  int32_t slate_width;             /* K = action.shape[1] */
+  int32_t next_width;              /* K_next = next_action.shape[1] (SARSA); ignored with maxq */
+  int32_t slate_size, maxq, single_selection, norm_method;
+  const float* q_cur;              /* [B*K] q_network(state, docs[b, action]) */
+  const float* q_next;             /* [B*C] q_network_target(next_state, every next candidate) */
+  const float* next_value;         /* [B*C] next candidate_docs.value */
+  const float* next_mask;          /* [B*C] next candidate_docs.mask */
+  const float* cur_mask;           /* [B*C] current candidate_docs.mask (NORM_CURRENT) */
+  int64_t* next_action;            /* [B*K_next] (SARSA, terminal rows zeroed) or NULL (maxq) */
+  const int64_t* action;           /* [B*K] current slate, range-checked only; or NULL */
+  const float* reward;             /* [B*K] */
+  const float* reward_mask;        /* [B*K] (single_selection) */
+  const float* not_terminal;       /* [B] */
+  const float* time_diff;          /* [B] or NULL */
+  float gamma, time_scale;
+  float* dz;                       /* [B*K] d loss / d q_cur */
+  float* target;                   /* [B*K] or NULL */
+  int32_t* mask_count;             /* [1] scratch (single_selection) */
+  int32_t* status;                 /* [1] sticky: 1 = an index outside [0, C) */
+  float* loss_partials;            /* [ceil(B / RB200_SLATEQ_ROWS_PER_BLOCK)] */
+  float* loss;                     /* [1] */
+  uint32_t* tile_counter;          /* [1] zero-initialised, self-resetting */
+} rb200_slateq_args_t;
+int rb200_slateq_head(const rb200_slateq_args_t* args, void* stream);
+
 /* Loss heads of DiscreteCRRTrainer (rb200_crr.cu), reagent/training/                 */
 /* discrete_crr_trainer.py, one warp per row, 1 <= num_actions <= 1024.  The actor's    */
 /* logits are FullyConnectedActor.forward's output (reagent/models/actor.py:90-110):    */

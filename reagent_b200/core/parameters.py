@@ -2,6 +2,7 @@
 reference (reagent/core/parameters.py:46-67, :118-120, :138-152).  The reference's
 pydantic/registry config machinery is out of scope (SURVEY.md section 2 row 6); plain frozen
 dataclasses carry the same values."""
+import enum
 from dataclasses import dataclass, field
 from typing import Dict, List, Optional
 
@@ -96,6 +97,53 @@ class CEMTrainerParameters:
     rl: RLParameters = field(default_factory=RLParameters)
     alpha: float = 0.25
     epsilon: float = 0.001
+
+
+class SlateOptMethod(enum.Enum):
+    """reagent/core/parameters.py:33-36"""
+    GREEDY = "greedy"
+    TOP_K = "top_k"
+    EXACT = "exact"
+
+
+@dataclass(frozen=True)
+class SlateOptParameters:
+    method: SlateOptMethod = SlateOptMethod.TOP_K
+
+
+def _default_optimizer():
+    from ..optimizer import Optimizer__Union
+
+    return Optimizer__Union.default()
+
+
+def _norm_by_current_slate_size():
+    from ..training.slate_q_trainer import NextSlateValueNormMethod
+
+    return NextSlateValueNormMethod.NORM_BY_CURRENT_SLATE_SIZE
+
+
+@dataclass(frozen=True)
+class SlateQTrainerParameters:
+    """The arguments of SlateQTrainer after the networks and slate_size, with the reference's
+    defaults (the reference generates this class from the trainer's __init__).  The optimizer
+    is an Optimizer__Union and the norm method a NextSlateValueNormMethod
+    (reagent_b200.training.slate_q_trainer); both defaults are made on first use, since those
+    modules import this one."""
+    rl: RLParameters = field(default_factory=lambda: RLParameters(maxq_learning=False))
+    optimizer: object = field(default_factory=_default_optimizer)
+    slate_opt_parameters: Optional[SlateOptParameters] = None
+    discount_time_scale: Optional[float] = None
+    single_selection: bool = True
+    next_slate_value_norm_method: object = field(default_factory=_norm_by_current_slate_size)
+    minibatch_size: int = 1024
+    evaluation: EvaluationParameters = field(
+        default_factory=lambda: EvaluationParameters(calc_cpe_in_training=False))
+
+    def asdict(self):
+        import dataclasses
+
+        return {f.name: getattr(self, f.name) for f in dataclasses.fields(self)}
 
 
 class NormalizationKey:

@@ -44,9 +44,40 @@ class TensorDataClass:
 
 
 @dataclass
+class DocList(TensorDataClass):
+    """core/types.py:250-284: the candidate documents of each row.  float_features is
+    (batch_size, num_candidates, doc_dim); mask (present or not) and value (e.g. a selection
+    probability) are (batch_size, num_candidates), defaulting to all present and 1."""
+    float_features: torch.Tensor
+    mask: torch.Tensor = None
+    value: torch.Tensor = None
+
+    def __post_init__(self):
+        assert len(self.float_features.shape) == 3, f"Unexpected shape: {self.float_features.shape}"
+        if self.mask is None:
+            self.mask = self.float_features.new_ones(self.float_features.shape[:2], dtype=torch.bool)
+        if self.value is None:
+            self.value = self.float_features.new_ones(self.float_features.shape[:2])
+
+    @torch.no_grad()
+    def select_slate(self, action: torch.Tensor):
+        """The documents at `action` [batch_size, slate_size] (indices into the candidates)."""
+        row_idx = torch.repeat_interleave(
+            torch.arange(action.shape[0], device=action.device).unsqueeze(1), action.shape[1], dim=1)
+        return DocList(self.float_features[row_idx, action], self.mask[row_idx, action],
+                       self.value[row_idx, action])
+
+    def as_feature_data(self):
+        _batch_size, _slate_size, feature_dim = self.float_features.shape
+        return FeatureData(self.float_features.view(-1, feature_dim))
+
+
+@dataclass
 class FeatureData(TensorDataClass):
     # dense features, shape (batch_size, feature_dim)
     float_features: torch.Tensor
+    # the candidate documents of each row (SlateQ), core/types.py:329
+    candidate_docs: Optional[DocList] = None
 
     def __post_init__(self):
         # (batch_size, feature_dim), or (seq_len, batch_size, feature_dim) for sequences
@@ -180,6 +211,38 @@ class ParametricDqnInput(BaseInput):
             step=batch.get("step"),
             extras=batch.get("extras"),
             weight=batch.get("weight"),
+        )
+
+
+@dataclass
+class SlateQInput(BaseInput):
+    """core/types.py:820-863: `action` / `next_action` are (batch_size, slate_size) indices into
+    the candidate docs of state / next_state; `reward` and `reward_mask` are per slate position,
+    (batch_size, slate_size)."""
+    action: torch.Tensor = None
+    next_action: torch.Tensor = None
+    reward_mask: torch.Tensor = None
+    extras: Optional[ExtraData] = None
+
+    @classmethod
+    def from_dict(cls, d):
+        return cls(
+            state=FeatureData(
+                float_features=d["state_features"],
+                candidate_docs=DocList(float_features=d["candidate_features"],
+                                       mask=d["item_mask"], value=d["item_probability"])),
+            next_state=FeatureData(
+                float_features=d["next_state_features"],
+                candidate_docs=DocList(float_features=d["next_candidate_features"],
+                                       mask=d["next_item_mask"], value=d["next_item_probability"])),
+            action=d["action"],
+            next_action=d["next_action"],
+            reward=d["position_reward"],
+            reward_mask=d["reward_mask"],
+            time_diff=d["time_diff"],
+            not_terminal=d["not_terminal"],
+            step=None,
+            extras=ExtraData(**{f.name: d.get(f.name) for f in dataclasses.fields(ExtraData)}),
         )
 
 

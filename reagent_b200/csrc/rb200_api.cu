@@ -67,6 +67,7 @@ extern "C" int64_t rb200_abi_sizeof(const char* type_name) {
   RB200_SZ(rb200_replay_dev_t);
   RB200_SZ(rb200_cpe_args_t);
   RB200_SZ(rb200_pdqn_args_t);
+  RB200_SZ(rb200_slateq_args_t);
   RB200_SZ(rb200_c51_args_t);
   RB200_SZ(rb200_bc_xent_args_t);
   RB200_SZ(rb200_crr_critic_args_t);

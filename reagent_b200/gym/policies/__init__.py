@@ -3,6 +3,9 @@ then an action sampler -- the reference's Policy = scorer o sampler composition.
 
   discrete_dqn_scorer        reagent/gym/policies/scorers/discrete_scorer.py:16-48
   parametric_dqn_scorer      reagent/gym/policies/scorers/discrete_scorer.py:65-87
+  slate_q_scorer, TopKSampler
+                             reagent/gym/policies/scorers/slate_q_scorer.py:13-30,
+                             reagent/gym/policies/samplers/top_k_sampler.py
   Greedy / EpsilonGreedy / Softmax samplers
                              reagent/gym/policies/samplers/discrete_sampler.py:14-183
   Policy                     reagent/gym/policies/policy.py:13-43
@@ -81,6 +84,49 @@ def parametric_dqn_scorer(max_num_actions: int, q_network):
         return out.view(-1, max_num_actions)
 
     return score
+
+
+def slate_q_scorer(num_candidates: int, q_network):
+    """reagent/gym/policies/scorers/slate_q_scorer.py:13-30: softmax(candidate value) times
+    q_network(state, candidate) for every candidate of every row, (n, num_candidates).  The
+    repeated states are built per row tile inside one rb200_mlp_forward_tiled launch."""
+    from ...models.arena import run_mlp_tiled
+
+    @torch.no_grad()
+    def score(state: rlt.FeatureData) -> torch.Tensor:
+        docs = state.candidate_docs
+        assert docs is not None
+        arena = q_network.arena
+        dev = arena.flat.device
+        obs = state.float_features.to(dev, torch.float32).contiguous()
+        n = obs.shape[0]
+        cand = docs.float_features.to(dev, torch.float32).reshape(n * num_candidates, -1).contiguous()
+        q_network.eval()
+        out = torch.empty(n * num_candidates, arena.dims[-1], device=dev)
+        run_mlp_tiled([arena], obs, cand, num_candidates, [out])
+        q_network.train()
+        scores = out.view(-1, num_candidates)
+        select_prob = F.softmax(docs.value.to(dev), dim=1)
+        assert select_prob.shape == scores.shape
+        return select_prob * scores
+
+    return score
+
+
+class TopKSampler:
+    """reagent/gym/policies/samplers/top_k_sampler.py: the indices of the k best scores of each
+    row, log_prob 0."""
+
+    def __init__(self, k: int) -> None:
+        self.k = k
+
+    def sample_action(self, scores: torch.Tensor) -> rlt.ActorOutput:
+        _, item_idxs = torch.topk(scores, self.k, dim=1)
+        return rlt.ActorOutput(action=item_idxs,
+                               log_prob=torch.zeros(item_idxs.shape[0], 1, device=scores.device))
+
+    def log_prob(self, scores: torch.Tensor, action: torch.Tensor) -> torch.Tensor:
+        raise NotImplementedError
 
 
 class GreedyActionSampler:

@@ -152,10 +152,56 @@ class MemoryNetworkInputMaker:
         })
 
 
+class SlateQInputMaker:
+    """trainer_preprocessor.py:230-278: a replay batch with the extras doc,
+    augmentation_value, response_click and response_watch_time (and their next_ forms) -> a
+    SlateQInput.  A null slot is appended to every slate: index slate_size in action /
+    next_action, reward 0 in position_reward, and in reward_mask True exactly when nothing
+    was clicked.  Every candidate is present (item masks of ones)."""
+
+    def __init__(self):
+        self.metric = "watch_time"
+
+    @classmethod
+    def create_for_env(cls, env):
+        return cls()
+
+    def __call__(self, batch):
+        n = batch.state.shape[0]
+        dev = batch.state.device
+        item_mask = torch.ones(batch.doc.shape[:2], device=dev)
+        next_item_mask = torch.ones(batch.doc.shape[:2], device=dev)
+        null_action = torch.full((n, 1), batch.action.shape[1], dtype=torch.int64, device=dev)
+        action = torch.cat([batch.action, null_action], dim=1)
+        next_action = torch.cat([batch.next_action, null_action], dim=1)
+        position_reward = getattr(batch, f"response_{self.metric}")
+        position_reward = torch.cat([position_reward, torch.zeros((n, 1), device=dev)], dim=1)
+        reward_mask = batch.response_click
+        null_mask = (reward_mask.sum(dim=1) == 0).view(n, 1)
+        reward_mask = torch.cat([reward_mask.to(torch.bool), null_mask], dim=1)
+        return rlt.SlateQInput.from_dict({
+            "state_features": batch.state,
+            "next_state_features": batch.next_state,
+            "candidate_features": batch.doc,
+            "next_candidate_features": batch.next_doc,
+            "item_mask": item_mask,
+            "next_item_mask": next_item_mask,
+            "item_probability": batch.augmentation_value,
+            "next_item_probability": batch.next_augmentation_value,
+            "action": action,
+            "next_action": next_action,
+            "position_reward": position_reward,
+            "reward_mask": reward_mask,
+            "time_diff": None,
+            "not_terminal": ~batch.terminal,
+        })
+
+
 REPLAY_BUFFER_MAKER_MAP = {
     rlt.DiscreteDqnInput: DiscreteDqnInputMaker,
     rlt.PolicyNetworkInput: PolicyNetworkInputMaker,
     rlt.MemoryNetworkInput: MemoryNetworkInputMaker,
+    rlt.SlateQInput: SlateQInputMaker,
 }
 
 

@@ -4,24 +4,25 @@ discrete/discrete_dqn.py:63-116, discrete/discrete_qrdqn.py:73-121,
 discrete/discrete_c51dqn.py:43-88, parametric/parametric_dqn.py:45-81,
 actor_critic/sac.py:80-113, actor_critic/td3.py:70-102, discrete/discrete_crr.py:104-179,
 policy_gradient/reinforce.py, policy_gradient/ppo.py, model_based/world_model.py,
-model_based/cross_entropy_method.py): build the networks from the net
+model_based/cross_entropy_method.py, ranking/slate_q.py): build the networks from the net
 builders, copy the target, hand everything to the trainer; `create_policy` gives the online
 act-time policy.  Serving modules, data modules and reporters are out of scope (SURVEY.md
 section 2 rows 8, 12, 15, 16)."""
 from dataclasses import dataclass, field
-from typing import Union, Dict, List, Optional
+from typing import Union, Dict, List, Optional, Tuple
 
 from ..core import types as rlt
 from ..core.parameters import (CEMTrainerParameters, EvaluationParameters,
                                MDNRNNTrainerParameters, NormalizationData, NormalizationKey,
-                               RLParameters, Seq2RewardTrainerParameters)
+                               RLParameters, Seq2RewardTrainerParameters,
+                               SlateQTrainerParameters)
 from ..net_builder import (ActorFullyConnected, Categorical, DiscreteActorFullyConnected,
                            Dueling, DuelingQuantile, FullyConnected, GaussianFullyConnected, ParametricFullyConnected,
                            Quantile, Seq2RewardNetBuilder, ValueFullyConnected)
 from ..optimizer import Optimizer__Union
 from ..training import (C51Trainer, CEMTrainer, CRRWeightFn, DiscreteCRRTrainer, DQNTrainer,
                         MDNRNNTrainer, ParametricDQNTrainer, PPOTrainer, QRDQNTrainer, ReinforceTrainer,
-                        SACTrainer, Seq2RewardTrainer, TD3Trainer)
+                        SACTrainer, Seq2RewardTrainer, SlateQTrainer, TD3Trainer)
 
 
 def _device(use_gpu: bool):
@@ -556,3 +557,43 @@ class Seq2RewardModel:
         trainer = Seq2RewardTrainer(seq2reward_network=seq2reward_network,
                                     params=self.trainer_param)
         return trainer.to(dev)
+
+
+@dataclass
+class SlateQ:
+    """reagent/model_managers/ranking/slate_q.py and slate_q_base.py: a ParametricDQN
+    FullyConnected q network over (state, item) from the STATE and ITEM normalizations, its
+    target a copy, and SlateQTrainer with `trainer_param`.  slate_feature_id and slate_score_id
+    are kept for the configurations that name them; the preprocessing options, the reporter and
+    serving modules are out of scope."""
+    slate_size: int = -1
+    num_candidates: int = -1
+    slate_feature_id: int = 0
+    slate_score_id: Tuple[int, int] = (0, 0)
+    trainer_param: SlateQTrainerParameters = field(default_factory=SlateQTrainerParameters)
+    net_builder: ParametricFullyConnected = field(default_factory=ParametricFullyConnected)
+
+    def __post_init__(self):
+        assert self.slate_size > 0, f"Please set valid slate_size (currently {self.slate_size})"
+        assert self.num_candidates > 0, (
+            f"Please set valid num_candidates (currently {self.num_candidates})")
+        self.eval_parameters = self.trainer_param.evaluation
+
+    def build_trainer(self, normalization_data_map: Dict[str, NormalizationData], use_gpu: bool,
+                      reward_options=None) -> SlateQTrainer:
+        dev = _device(use_gpu)
+        q_network = self.net_builder.build_q_network(
+            normalization_data_map[NormalizationKey.STATE],
+            normalization_data_map[NormalizationKey.ITEM]).to(dev)
+        q_network_target = q_network.get_target_network()
+        return SlateQTrainer(q_network=q_network, q_network_target=q_network_target,
+                             slate_size=self.slate_size, **self.trainer_param.asdict()).to(dev)
+
+    def create_policy(self, trainer_module, serving: bool = False, normalization_data_map=None):
+        """slate_q_base.py:61-83: slate_q_scorer over every candidate, then the top slate_size."""
+        if serving:
+            raise NotImplementedError("serving modules are out of scope of reagent_b200")
+        from ..gym.policies import Policy, TopKSampler, slate_q_scorer
+
+        return Policy(scorer=slate_q_scorer(self.num_candidates, trainer_module.q_network),
+                      sampler=TopKSampler(k=self.slate_size))

@@ -19,4 +19,5 @@ from .seq2reward_trainer import (  # noqa: F401
     get_step_prediction,
     plan_short_sequence_q,
 )
+from .slate_q_trainer import NextSlateValueNormMethod, SlateQTrainer  # noqa: F401
 from .td3_trainer import TD3Trainer  # noqa: F401
