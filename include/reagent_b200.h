@@ -1207,6 +1207,81 @@ int rb200_seq2reward_plan(const rb200_seq2reward_plan_args_t* args, void* stream
 int rb200_seq2reward_compress_head(const rb200_seq2reward_compress_args_t* args, void* stream);
 
 /* ------------------------------------------------------------------------- */
+/* Seq2Slate transformer (reagent/models/seq2slate.py, rb200_seq2slate.cu): embedders, L    */
+/* post-norm encoder layers, then the decoder (AUTOREGRESSIVE: L - 1 TransformerDecoderLayers */
+/* and the head-averaged cross-attention weights of the last one; FRECHET_SORT: a masked      */
+/* softmax of encoder_scorer(memory)).  One CTA carries one slate through all of it; the      */
+/* decoder runs one position per step on cached self-attention keys / values, which is exact  */
+/* because position t depends only on positions <= t and on tgt_in_idx[0..t].               */
+/*   rb200_seq2slate_forward  decode FORCED (teacher forcing on tgt_in_idx / tgt_in_seq):    */
+/*                            probs [B, T, N+2], log_probs = log(clamp(probs, 1e-40)) and    */
+/*                            seq_log_prob [B] = log(clamp(prod_t probs[t, tgt_out_idx[t]],  */
+/*                            1e-40)); each output may be NULL (one must be given).           */
+/*   rb200_seq2slate_rank     decode GREEDY (first maximal index at every step) or SAMPLE     */
+/*                            (the first symbol whose running sum of probabilities exceeds    */
+/*                            noise[b, t] * their total, in candidate order): ranked_idx      */
+/*                            [B, T], probs (the ranked per-symbol probabilities, or NULL)    */
+/*                            and seq_prob [B] = clamp(prod, 1e-40).  FRECHET_SORT GREEDY is  */
+/*                            the argsort of the first step's probabilities (ties: lowest     */
+/*                            index first) with one-hot probs and seq_prob 1.                 */
+/* Indices count the padding and start symbols (candidate i is symbol i + 2); the decoder's   */
+/* first input in rank mode is the start symbol 1, whose features are zeros.                  */
+/* off[] holds the offsets in `params` of the reference's parameters() in order: per encoder  */
+/* layer 12 (in_proj w/b, out_proj w/b, linear1 w/b, linear2 w/b, norm1 w/b, norm2 w/b),     */
+/* encoder_scorer w/b, per decoder layer 18 (self_attn in/out, multihead_attn in/out, linear1, */
+/* linear2, norm1..3, each w/b), pos_embed w/b, state_embedder w/b, candidate_embedder w/b.    */
+/* Layouts (dense fp32 unless noted): state [B, S], src_seq [B, N, C], tgt_in_idx /           */
+/* tgt_out_idx / ranked_idx int64 [B, T], tgt_in_seq [B, T, C], noise [B, T].                 */
+/* Limits: 1 <= S, C <= 256, 2 <= dim_model <= 128 divisible by num_heads, 1 <=               */
+/* state_embed_dim < dim_model, dim_feedforward <= 512, 1 <= layers <= 4, 1 <= N <= 64 and    */
+/* 1 <= T <= N.  Each CTA loops over slates with a workspace slice of about 4 * (N(4d +       */
+/* max(3d, FFN)) + 2 L T d) bytes: in shared memory when that is at most 200 KiB (as many CTAs */
+/* as fit on the device), else in `workspace`, which then holds                               */
+/* rb200_seq2slate_workspace_bytes(args) for min(B, RB200_SEQ2SLATE_MAX_CTAS) CTAs (the size */
+/* is 0, and `workspace` may be NULL, on the shared-memory path).  Anything else is refused  */
+/* before any launch.                                                                         */
+/* ------------------------------------------------------------------------- */
+#define RB200_SEQ2SLATE_MAX_CANDIDATES 64
+#define RB200_SEQ2SLATE_MAX_DIM_MODEL 128
+#define RB200_SEQ2SLATE_MAX_FEEDFORWARD 512
+#define RB200_SEQ2SLATE_MAX_LAYERS 4
+#define RB200_SEQ2SLATE_MAX_INPUT 256
+#define RB200_SEQ2SLATE_MAX_PARAMS (30 * RB200_SEQ2SLATE_MAX_LAYERS + 8)
+#define RB200_SEQ2SLATE_MAX_CTAS 1056 /* 8 per SM of an H100 SXM */
+#define RB200_SEQ2SLATE_ARCH_AUTOREGRESSIVE 0
+#define RB200_SEQ2SLATE_ARCH_FRECHET_SORT 1
+#define RB200_SEQ2SLATE_DECODE_FORCED 0
+#define RB200_SEQ2SLATE_DECODE_GREEDY 1
+#define RB200_SEQ2SLATE_DECODE_SAMPLE 2
+typedef struct rb200_seq2slate_args {
+  int32_t batch, src_len, tgt_len, state_dim, candidate_dim, state_embed_dim;
+  int32_t dim_model, num_heads, dim_feedforward, layers, arch, decode;
+  const float* params;                           /* the arena */
+  int64_t n_params;
+  int64_t off[RB200_SEQ2SLATE_MAX_PARAMS];
+  const float* state;
+  const float* src_seq;
+  const int64_t* tgt_in_idx;                     /* FORCED */
+  const int64_t* tgt_out_idx;                    /* FORCED */
+  const float* tgt_in_seq;                       /* FORCED, AUTOREGRESSIVE */
+  const float* noise;                            /* SAMPLE: uniforms in [0, 1) */
+  float* probs;                                  /* [B, T, N + 2] or NULL */
+  float* log_probs;                              /* FORCED: [B, T, N + 2] or NULL */
+  float* seq_log_prob;                           /* FORCED: [B] or NULL */
+  int64_t* ranked_idx;                           /* rank */
+  float* seq_prob;                               /* rank: [B] */
+  float* workspace;
+  int64_t workspace_bytes;
+} rb200_seq2slate_args_t;
+/* 0 if the model shape is within the limits above, else RB200_E_INVALID (text via last_error) */
+int rb200_seq2slate_check_shape(int32_t state_dim, int32_t candidate_dim, int32_t state_embed_dim,
+                                int32_t dim_model, int32_t num_heads, int32_t dim_feedforward,
+                                int32_t layers, int32_t max_src_seq_len, int32_t max_tgt_seq_len);
+int64_t rb200_seq2slate_workspace_bytes(const rb200_seq2slate_args_t* args);
+int rb200_seq2slate_forward(const rb200_seq2slate_args_t* args, void* stream);
+int rb200_seq2slate_rank(const rb200_seq2slate_args_t* args, void* stream);
+
+/* ------------------------------------------------------------------------- */
 /* Counterfactual policy evaluation (rb200_ope.cu), reagent/evaluation/*.py.  Every input is */
 /* a dense row-major device array of the page's N rows; episodes are runs of equal mdp_id */
 /* in a page sorted by (mdp_id, sequence_number, row).  ep_off[E+1] are their row offsets. */

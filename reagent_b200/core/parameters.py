@@ -146,6 +146,16 @@ class SlateQTrainerParameters:
         return {f.name: getattr(self, f.name) for f in dataclasses.fields(self)}
 
 
+@dataclass(frozen=True)
+class TransformerParameters:
+    """reagent/core/parameters.py:183: the shape of a Seq2Slate transformer."""
+    num_heads: int = 1
+    dim_model: int = 64
+    dim_feedforward: int = 32
+    num_stacked_layers: int = 2
+    state_embed_dim: Optional[int] = None
+
+
 class NormalizationKey:
     STATE = "state"
     ACTION = "action"

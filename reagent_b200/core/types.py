@@ -359,3 +359,152 @@ class MemoryNetworkOutput(TensorDataClass):
     last_step_lstm_hidden: torch.Tensor
     last_step_lstm_cell: torch.Tensor
     all_steps_lstm_hidden: torch.Tensor
+
+
+PADDING_SYMBOL = 0
+DECODER_START_SYMBOL = 1
+
+
+def _gather_rows(data: torch.Tensor, index_2d: torch.Tensor) -> torch.Tensor:
+    """out[i, j] = data[i, index_2d[i, j]] (reagent/core/torch_utils.py:gather)."""
+    rows = torch.arange(data.shape[0], device=data.device).unsqueeze(1)
+    return data[rows, index_2d]
+
+
+@dataclass
+class PreprocessedRankingInput(TensorDataClass):
+    """A batch of slates (reference core/types.py:453).  Every index counts the padding
+    symbol 0 and the decoder start symbol 1, so candidate i is symbol i + 2."""
+    state: FeatureData
+    src_seq: FeatureData
+    src_src_mask: Optional[torch.Tensor] = None
+    tgt_in_seq: Optional[FeatureData] = None
+    tgt_out_seq: Optional[FeatureData] = None
+    tgt_tgt_mask: Optional[torch.Tensor] = None
+    slate_reward: Optional[torch.Tensor] = None
+    position_reward: Optional[torch.Tensor] = None
+    src_in_idx: Optional[torch.Tensor] = None
+    tgt_in_idx: Optional[torch.Tensor] = None
+    tgt_out_idx: Optional[torch.Tensor] = None
+    tgt_out_probs: Optional[torch.Tensor] = None
+    optim_tgt_in_idx: Optional[torch.Tensor] = None
+    optim_tgt_out_idx: Optional[torch.Tensor] = None
+    optim_tgt_in_seq: Optional[FeatureData] = None
+    optim_tgt_out_seq: Optional[FeatureData] = None
+    extras: Optional[ExtraData] = field(default_factory=ExtraData)
+
+    def batch_size(self) -> int:
+        return self.state.float_features.size()[0]
+
+    def __len__(self) -> int:
+        return self.batch_size()
+
+    @classmethod
+    def from_input(cls, state: torch.Tensor, candidates: torch.Tensor, device: torch.device,
+                   action: Optional[torch.Tensor] = None,
+                   optimal_action: Optional[torch.Tensor] = None,
+                   logged_propensities: Optional[torch.Tensor] = None,
+                   slate_reward: Optional[torch.Tensor] = None,
+                   position_reward: Optional[torch.Tensor] = None,
+                   extras: Optional[ExtraData] = None):
+        """Derive the decoder's indices and sequences from state [B, S], candidates [B, N, C]
+        and the 0-based slates `action` / `optimal_action` [B, T]: tgt_out_idx = action + 2,
+        tgt_in_idx = (1, tgt_out_idx[:, :-1]), and their candidate features (zeros for the start
+        symbol)."""
+        assert len(state.shape) == 2
+        assert len(candidates.shape) == 3
+        state = state.to(device)
+        candidates = candidates.to(device)
+        if action is not None:
+            assert len(action.shape) == 2
+            action = action.to(device)
+        if logged_propensities is not None:
+            assert len(logged_propensities.shape) == 2 and logged_propensities.shape[1] == 1
+            logged_propensities = logged_propensities.to(device)
+        batch_size, candidate_num, candidate_dim = candidates.shape
+        if slate_reward is not None:
+            assert len(slate_reward.shape) == 2 and slate_reward.shape[1] == 1
+            slate_reward = slate_reward.to(device)
+        if position_reward is not None:
+            assert position_reward.shape == action.shape
+            position_reward = position_reward.to(device)
+        src_in_idx = torch.arange(candidate_num, device=device).repeat(batch_size, 1) + 2
+        src_src_mask = torch.ones(batch_size, candidate_num, candidate_num,
+                                  device=device).type(torch.int8)
+
+        def process_tgt_seq(action):
+            if action is None:
+                return None, None, None, None, None
+            output_size = action.shape[1]
+            augmented = torch.cat(
+                (torch.zeros(batch_size, 2, candidate_dim, device=device), candidates), dim=1)
+            tgt_out_idx = action + 2
+            tgt_in_idx = torch.full((batch_size, output_size), DECODER_START_SYMBOL,
+                                    device=device)
+            tgt_in_idx[:, 1:] = tgt_out_idx[:, :-1]
+            tgt_out_seq = _gather_rows(augmented, tgt_out_idx)
+            tgt_in_seq = torch.zeros(batch_size, output_size, candidate_dim, device=device)
+            tgt_in_seq[:, 1:] = tgt_out_seq[:, :-1]
+            tgt_tgt_mask = ~torch.triu(
+                torch.ones(1, output_size, output_size, device=device, dtype=torch.bool),
+                diagonal=1)
+            return tgt_in_idx, tgt_out_idx, tgt_in_seq, tgt_out_seq, tgt_tgt_mask
+
+        tgt_in_idx, tgt_out_idx, tgt_in_seq, tgt_out_seq, tgt_tgt_mask = process_tgt_seq(action)
+        optim_in_idx, optim_out_idx, optim_in_seq, optim_out_seq, _ = process_tgt_seq(
+            optimal_action)
+        return cls.from_tensors(
+            state=state, src_seq=candidates, src_src_mask=src_src_mask, tgt_in_seq=tgt_in_seq,
+            tgt_out_seq=tgt_out_seq, tgt_tgt_mask=tgt_tgt_mask, slate_reward=slate_reward,
+            position_reward=position_reward, src_in_idx=src_in_idx, tgt_in_idx=tgt_in_idx,
+            tgt_out_idx=tgt_out_idx, tgt_out_probs=logged_propensities,
+            optim_tgt_in_idx=optim_in_idx, optim_tgt_out_idx=optim_out_idx,
+            optim_tgt_in_seq=optim_in_seq, optim_tgt_out_seq=optim_out_seq, extras=extras)
+
+    @classmethod
+    def from_tensors(cls, state: torch.Tensor, src_seq: torch.Tensor,
+                     src_src_mask: Optional[torch.Tensor] = None,
+                     tgt_in_seq: Optional[torch.Tensor] = None,
+                     tgt_out_seq: Optional[torch.Tensor] = None,
+                     tgt_tgt_mask: Optional[torch.Tensor] = None,
+                     slate_reward: Optional[torch.Tensor] = None,
+                     position_reward: Optional[torch.Tensor] = None,
+                     src_in_idx: Optional[torch.Tensor] = None,
+                     tgt_in_idx: Optional[torch.Tensor] = None,
+                     tgt_out_idx: Optional[torch.Tensor] = None,
+                     tgt_out_probs: Optional[torch.Tensor] = None,
+                     optim_tgt_in_idx: Optional[torch.Tensor] = None,
+                     optim_tgt_out_idx: Optional[torch.Tensor] = None,
+                     optim_tgt_in_seq: Optional[torch.Tensor] = None,
+                     optim_tgt_out_seq: Optional[torch.Tensor] = None,
+                     extras: Optional[ExtraData] = None, **kwargs):
+        """Wrap plain tensors; the sequences become FeatureData."""
+        for v in (state, src_seq):
+            assert isinstance(v, torch.Tensor)
+        for v in (src_src_mask, tgt_in_seq, tgt_out_seq, tgt_tgt_mask, slate_reward,
+                  position_reward, src_in_idx, tgt_in_idx, tgt_out_idx, tgt_out_probs,
+                  optim_tgt_in_idx, optim_tgt_out_idx, optim_tgt_in_seq, optim_tgt_out_seq):
+            assert v is None or isinstance(v, torch.Tensor)
+        assert extras is None or isinstance(extras, ExtraData)
+        fd = lambda t: None if t is None else FeatureData(float_features=t)  # noqa: E731
+        return cls(
+            state=FeatureData(float_features=state), src_seq=FeatureData(float_features=src_seq),
+            src_src_mask=src_src_mask, tgt_in_seq=fd(tgt_in_seq), tgt_out_seq=fd(tgt_out_seq),
+            tgt_tgt_mask=tgt_tgt_mask, slate_reward=slate_reward, position_reward=position_reward,
+            src_in_idx=src_in_idx, tgt_in_idx=tgt_in_idx, tgt_out_idx=tgt_out_idx,
+            tgt_out_probs=tgt_out_probs, optim_tgt_in_idx=optim_tgt_in_idx,
+            optim_tgt_out_idx=optim_tgt_out_idx, optim_tgt_in_seq=fd(optim_tgt_in_seq),
+            optim_tgt_out_seq=fd(optim_tgt_out_seq), extras=extras)
+
+
+@dataclass
+class RankingOutput(TensorDataClass):
+    # ranked symbols (candidate i is i + 2), [B, T]
+    ranked_tgt_out_idx: Optional[torch.Tensor] = None
+    # the probabilities of every symbol at each decoding step, [B, T, N + 2]
+    ranked_per_symbol_probs: Optional[torch.Tensor] = None
+    # the probability of each ranked sequence, [B, 1]
+    ranked_per_seq_probs: Optional[torch.Tensor] = None
+    # [B, 1] (PER_SEQ_LOG_PROB_MODE) or [B, T, N + 2] (PER_SYMBOL_LOG_PROB_DIST_MODE)
+    log_probs: Optional[torch.Tensor] = None
+    encoder_scores: Optional[torch.Tensor] = None

@@ -84,6 +84,7 @@ extern "C" int64_t rb200_abi_sizeof(const char* type_name) {
   RB200_SZ(rb200_seq2reward_args_t);
   RB200_SZ(rb200_seq2reward_plan_args_t);
   RB200_SZ(rb200_seq2reward_compress_args_t);
+  RB200_SZ(rb200_seq2slate_args_t);
 #undef RB200_SZ
   return -1;
 }

@@ -12,4 +12,9 @@ from .fully_connected_network import (  # noqa: F401
     FullyConnectedNetwork,
 )
 from .seq2reward_model import Seq2RewardNetwork  # noqa: F401
+from .seq2slate import (  # noqa: F401
+    Seq2SlateMode,
+    Seq2SlateOutputArch,
+    Seq2SlateTransformerNet,
+)
 from .world_model import MDNRNN, LstmArena, MemoryNetwork  # noqa: F401

@@ -4,10 +4,11 @@ dataclass -> arena-backed model.  Normalization data only sizes the input/output
 from dataclasses import dataclass, field
 from typing import List
 
-from ..core.parameters import NormalizationData
+from ..core.parameters import NormalizationData, TransformerParameters
 from ..models import (CategoricalDQN, DuelingQNetwork, FullyConnectedActor,
                       FullyConnectedCritic, FullyConnectedDQN, GaussianFullyConnectedActor)
 from ..models.fully_connected_network import FloatFeatureFullyConnected
+from ..models.seq2slate import Seq2SlateOutputArch
 from ..preprocessing.normalization import get_num_output_features
 
 
@@ -207,3 +208,24 @@ class Seq2RewardNetBuilder:
         return Seq2RewardNetwork(state_dim=_dim(state_normalization_data),
                                  action_dim=self.action_dim, num_hiddens=self.num_hiddens,
                                  num_hidden_layers=self.num_hidden_layers)
+
+
+@dataclass
+class SlateRankingTransformer:
+    """reagent/net_builder/slate_ranking/slate_ranking_transformer.py"""
+    output_arch: Seq2SlateOutputArch = Seq2SlateOutputArch.AUTOREGRESSIVE
+    temperature: float = 1.0
+    transformer: TransformerParameters = field(
+        default_factory=lambda: TransformerParameters(num_heads=2, dim_model=16,
+                                                      dim_feedforward=16, num_stacked_layers=2))
+
+    def build_slate_ranking_network(self, state_dim, candidate_dim, candidate_size, slate_size):
+        from ..models.seq2slate import Seq2SlateTransformerNet
+
+        return Seq2SlateTransformerNet(
+            state_dim=state_dim, candidate_dim=candidate_dim,
+            num_stacked_layers=self.transformer.num_stacked_layers,
+            num_heads=self.transformer.num_heads, dim_model=self.transformer.dim_model,
+            dim_feedforward=self.transformer.dim_feedforward, max_src_seq_len=candidate_size,
+            max_tgt_seq_len=slate_size, output_arch=self.output_arch,
+            temperature=self.temperature, state_embed_dim=self.transformer.state_embed_dim)
