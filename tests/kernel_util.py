@@ -1,5 +1,5 @@
-"""Constants and launch helpers of the kernel-level tests (the layer, Adam and loss-reduction
-kernels) that more than one test module uses."""
+"""Constants and launch helpers of the kernel-level tests (the layer, Adam, loss-reduction and
+actor-critic kernels) that more than one test module uses."""
 import ctypes as C
 
 import numpy as np
@@ -9,6 +9,58 @@ from reagent_b200 import _lib
 
 NAN = float("nan")
 NUM_SMS = 132
+E_SMEM = -3         # RB200_E_SMEM: no row tile fits in shared memory
+TOL = 1e-5          # the project's parity bar
+
+
+def _tol(length):
+    """Bound for a contraction of `length` terms run as one chain of MMAs into an fp32
+    accumulator.  The project's 1e-5 holds up to 256 terms; beyond that the accumulator's own
+    rounding (NVIDIA's tensor cores do not round the fp32 accumulation to nearest) adds up with
+    the number of k steps, so the bound grows linearly with the length.  Measured on an H100:
+    2.2e-5 for the forward at K = 1000, 3.3e-5 for one 4096-row weight-gradient slab."""
+    return TOL * max(1.0, length / 256)
+
+
+# pick_rows_cfg's four instances (threads, k-chunk) and the default choice
+CFGS = [None, (512, 32), (512, 16), (256, 32), (256, 16)]
+SMEM_FLOATS = 227 * 1024 // 4
+
+
+def _cfg_id(c):
+    return "default" if c is None else f"{c[0]}x{c[1]}"
+
+
+def _set_cfg(monkeypatch, cfg):
+    """Force the row-tile kernels onto one (threads, k-chunk) instance (None: their own
+    choice).  pick_rows_cfg reads RB200_FORCE_CFG at every launch."""
+    if cfg is None:
+        monkeypatch.delenv("RB200_FORCE_CFG", raising=False)
+    else:
+        monkeypatch.setenv("RB200_FORCE_CFG", f"{cfg[0]},{cfg[1]}")
+
+
+def _fits(cfg, batch, din, hmax, n_in, n_h, extra_per_row):
+    """Mirror of pick_rows_cfg (csrc/rb200_rows.cuh): does the forced (or any) tile fit?"""
+    return _pick(cfg, batch, din, hmax, n_in, n_h, extra_per_row) is not None
+
+
+def _pick(cfg, batch, din, hmax, n_in, n_h, extra_per_row):
+    """Mirror of pick_rows_cfg: the (threads, k-chunk) it launches, or None when none fits."""
+    r4 = lambda x: (x + 3) & ~3
+    ld_in, ld_h = r4(din) + 4, r4(hmax if hmax > 0 else 4) + 4
+    cands = [(512, 32), (512, 16), (256, 32), (256, 16)]
+    for nt, kc in cands:
+        R = (nt // 64) * 4
+        if cfg is not None:
+            if (nt, kc) != tuple(cfg):
+                continue
+        elif R == 32 and batch <= 16 * NUM_SMS:
+            continue
+        stage = max(256 * (kc + 4), kc * 264)
+        if 2 * stage + R * (n_in * ld_in + n_h * ld_h + extra_per_row) <= SMEM_FLOATS:
+            return (nt, kc)
+    return None
 
 
 def _padded(shape, offset=0, fill=NAN):

@@ -23,27 +23,12 @@ import torch
 from reagent_b200 import _lib
 from tests import golden_util as G
 from tests.builders import _record
-from tests.kernel_util import BETAS, EPS, GRAD_SCALE, LR, NAN, NUM_SMS, TAU, _padded, _seq_sum
+from tests.kernel_util import (BETAS, CFGS, E_SMEM, EPS, GRAD_SCALE, LR, NAN, NUM_SMS, TAU,
+                               TOL, _cfg_id, _fits, _padded, _seq_sum, _set_cfg, _tol)
 
 pytestmark = pytest.mark.gpu
 
-TOL = 1e-5          # the project's parity bar
-
-
-def _tol(length):
-    """Bound for a contraction of `length` terms run as one chain of MMAs into an fp32
-    accumulator.  The project's 1e-5 holds up to 256 terms; beyond that the accumulator's own
-    rounding (NVIDIA's tensor cores do not round the fp32 accumulation to nearest) adds up with
-    the number of k steps, so the bound grows linearly with the length.  Measured on an H100:
-    2.2e-5 for the forward at K = 1000, 3.3e-5 for one 4096-row weight-gradient slab."""
-    return TOL * max(1.0, length / 256)
-
-
-E_SMEM = -3
 ACTS = ["linear", "relu", "tanh", "leaky_relu", "sigmoid", "softplus"]
-# pick_rows_cfg's four instances (threads, k-chunk) and the default choice
-CFGS = [None, (512, 32), (512, 16), (256, 32), (256, 16)]
-SMEM_FLOATS = 227 * 1024 // 4
 
 
 def _lib_():
@@ -52,35 +37,6 @@ def _lib_():
 
 def _stream():
     return _lib.cur_stream()
-
-
-def _cfg_id(c):
-    return "default" if c is None else f"{c[0]}x{c[1]}"
-
-
-def _set_cfg(monkeypatch, cfg):
-    if cfg is None:
-        monkeypatch.delenv("RB200_FORCE_CFG", raising=False)
-    else:
-        monkeypatch.setenv("RB200_FORCE_CFG", f"{cfg[0]},{cfg[1]}")
-
-
-def _fits(cfg, batch, din, hmax, n_in, n_h, extra_per_row):
-    """Mirror of pick_rows_cfg (csrc/rb200_rows.cuh): does the forced (or any) tile fit?"""
-    r4 = lambda x: (x + 3) & ~3
-    ld_in, ld_h = r4(din) + 4, r4(hmax if hmax > 0 else 4) + 4
-    cands = [(512, 32), (512, 16), (256, 32), (256, 16)]
-    for nt, kc in cands:
-        R = (nt // 64) * 4
-        if cfg is not None:
-            if (nt, kc) != tuple(cfg):
-                continue
-        elif R == 32 and batch <= 16 * NUM_SMS:
-            continue
-        stage = max(256 * (kc + 4), kc * 264)
-        if 2 * stage + R * (n_in * ld_in + n_h * ld_h + extra_per_row) <= SMEM_FLOATS:
-            return True
-    return False
 
 
 # ------------------------------------------------------------------------------------------
