@@ -63,6 +63,46 @@ def _pick(cfg, batch, din, hmax, n_in, n_h, extra_per_row):
     return None
 
 
+def _r8(x):
+    return (x + 7) & ~7
+
+
+def _k2_image_bytes(N, K):
+    """image_bytes (csrc/rb200_dqn_tc_layout.cuh): one [K/4][rows][4] block per 128-row tile,
+    rows rounded up to 8 plus a 16-byte pad per k quad."""
+    return sum((_r8(K) // 4) * (_r8(min(N - 128 * t, 128)) * 16 + 16)
+               for t in range((N + 127) // 128))
+
+
+def _k2_tc_bytes(dims, double_q, do_backward):
+    """Mirror of rb200_dqn_tc_workspace_bytes (make_plan in csrc/rb200_dqn_tc.cu): the pack
+    size tc_images gives for `dims`, or 0 when the wgmma TD kernel does not take the shape and
+    K2 runs on the row-tile kernel.  `double_q` changes neither the images (the target's are
+    always packed) nor the shared memory (the q(s') buffer is always reserved)."""
+    del double_q
+    L = len(dims) - 1
+    if L < 1 or L > 8 or any(d > 4 * 128 or d > 32000 for d in dims[1:]):
+        return 0
+    if dims[0] > 32000 or dims[L] > 256:
+        return 0
+    fwd = sum(_k2_image_bytes(dims[l + 1], dims[l]) for l in range(L))
+    bwd = sum(_k2_image_bytes(dims[l], dims[l + 1]) for l in range(1, L)) if do_backward else 0
+    # shared memory: 3-stage ring of two 32-k chunk images of a full tile, two ping-pong
+    # activation operands and the last layer's dZ (k quads of 64 rows hi/lo + 16 B), the three
+    # q arrays [32][A + 1], action and mask rows, per-row scalars, the ring's mbarriers
+    ring, lbo_b, R = 3 * 2 * 8 * (128 * 16 + 16), 64 * 16 + 16, 32
+    A = dims[L]
+    maxd = [8, 8, A]
+    for i in range(L):
+        maxd[i & 1] = max(maxd[i & 1], dims[i])
+    a16 = lambda x: (x + 15) & ~15
+    o = ring + sum(_r8(m) // 4 * lbo_b for m in maxd)
+    o = a16(o + 3 * R * (A + 1) * 4)
+    o = a16(o + (2 * R * A + 4 * R + 8) * 4)
+    o = a16(o + 2 * 3 * 8)
+    return 2 * fwd + bwd + 4096 if o <= 232448 else 0
+
+
 def _padded(shape, offset=0, fill=NAN):
     """A CUDA fp32 tensor of `shape` starting `offset` floats into its allocation (offset 1:
     not 16-byte aligned, which sends the kernels down their scalar load / store paths)."""

@@ -314,7 +314,10 @@ def test_dueling_forward_heads_and_state_dict():
     assert torch.equal(qt(x), out)
 
 
-@pytest.mark.parametrize("S,sizes,A", [(128, [256, 128], 16), (10, [24, 12], 3), (36, [300, 130, 20], 9)])
+@pytest.mark.parametrize("S,sizes,A", [(128, [256, 128], 16), (10, [24, 12], 3), (36, [300, 130, 20], 9),
+                                     # the edges of the wgmma plan: K = 1 and 480, a one-row
+                                     # last tile, a fourth tile, A over 128
+                                     (1, [129], 7), (7, [400], 9), (480, [8], 4), (8, [8], 141)])
 def test_adam_writes_the_same_weight_images_as_the_pack_kernel(S, sizes, A):
     """The fused Adam kernel writes the hi/lo tensor-core images of the updated parameters;
     they must be bit-identical to what rb200_dqn_tc_pack builds from the same parameters."""
