@@ -52,8 +52,6 @@ inline size_t cem_smem(const CemDims& d) {
   return sizeof(float) * f + sizeof(double) * kCemR + sizeof(int) * (2 * kCemR + 4);
 }
 
-__device__ __forceinline__ float cem_sigmoid(float x) { return 1.f / (1.f + expf(-x)); }
-
 // sqrt(constrained_variance) of plan element c: min(((mean - lb) / 2)^2, ((ub - mean) / 2)^2,
 // var), every operation rounded as numpy rounds it
 __device__ __forceinline__ double cem_scale(const rb200_cem_args_t& a, int c, double mean,
@@ -225,9 +223,9 @@ __global__ void __launch_bounds__(kCemNT, 1) cem_rollout_kernel(const rb200_cem_
         for (int i = tid; i < R * H; i += NT) {
           const int r = i / H, jj = i - r * H;
           const float* g1 = scr + r * d.ld_s;
-          const float gi = cem_sigmoid(__fadd_rn(bhh[jj], g1[jj]));
+          const float gi = sigmoidf(__fadd_rn(bhh[jj], g1[jj]));
           const float gg = tanhf(__fadd_rn(bhh[2 * H + jj], g1[2 * H + jj]));
-          const float go = cem_sigmoid(__fadd_rn(bhh[3 * H + jj], g1[3 * H + jj]));
+          const float go = sigmoidf(__fadd_rn(bhh[3 * H + jj], g1[3 * H + jj]));
           const float cn = __fmul_rn(gi, gg);
           hout[r * d.ld_h + jj] = rows[r] >= 0 ? __fmul_rn(go, tanhf(cn)) : 0.f;
         }
@@ -281,7 +279,7 @@ __global__ void __launch_bounds__(kCemNT, 1) cem_rollout_kernel(const rb200_cem_
         if (lane == 0) {
           // reward * gamma ** j in fp32, accumulated in fp64; stop after a terminal draw
           acc[r] = __dadd_rn(acc[r], (double)__fmul_rn(y[d.NG - 2], a.discount[step]));
-          if (a.terminal_effective && !(nz[d.S + 1] < cem_sigmoid(y[d.NG - 1]))) alive[r] = 0;
+          if (a.terminal_effective && !(nz[d.S + 1] < sigmoidf(y[d.NG - 1]))) alive[r] = 0;
         }
       }
       if (!__syncthreads_or(tid < R && rows[tid] >= 0 && alive[tid])) break;

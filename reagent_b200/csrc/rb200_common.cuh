@@ -53,12 +53,14 @@ __host__ __device__ __forceinline__ int ceil_div(int a, int b) { return (a + b -
 // ----------------------------------------------------------------------------
 // activations (reagent/models/fully_connected_network.py:37-44)
 // ----------------------------------------------------------------------------
+__device__ __forceinline__ float sigmoidf(float x) { return 1.f / (1.f + expf(-x)); }
+
 __device__ __forceinline__ float act_fwd(float x, int act) {
   switch (act) {
     case RB200_ACT_RELU: return x > 0.f ? x : 0.f;
     case RB200_ACT_TANH: return tanhf(x);
     case RB200_ACT_LEAKY_RELU: return x > 0.f ? x : 0.01f * x;
-    case RB200_ACT_SIGMOID: return 1.f / (1.f + expf(-x));
+    case RB200_ACT_SIGMOID: return sigmoidf(x);
     case RB200_ACT_SOFTPLUS: return x > 20.f ? x : log1pf(expf(x));
     default: return x;
   }
@@ -98,6 +100,90 @@ __device__ __forceinline__ float warp_max(float v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
   return v;
+}
+
+// torch.argmax of a one-hot row of n values held by one warp (lanes take c = lane, lane + 32,
+// ...): the column of the first maximum, on every lane.  A row with no value above -inf (all
+// NaN, say) gives 0, as torch.argmax does for a row of NaNs.
+__device__ __forceinline__ int warp_first_argmax(const float* row, int n) {
+  const int lane = threadIdx.x & 31;
+  float lv = -INFINITY;
+  int li = n;
+  for (int c = lane; c < n; c += 32) {
+    const float v = row[c];
+    if (v > lv) { lv = v; li = c; }
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    const float ov = __shfl_xor_sync(0xffffffffu, lv, o);
+    const int oi = __shfl_xor_sync(0xffffffffu, li, o);
+    if (ov > lv || (ov == lv && oi < li)) { lv = ov; li = oi; }
+  }
+  if (li >= n) li = 0;
+  return li;
+}
+
+// Sum over the CTA of one fp64 value per thread, in a fixed order (butterfly within each warp,
+// then warps 0, 1, ... from 0.0); every thread gets the total.  The CTA has 32 * kWarps threads
+// and s_warp is shared memory with one slot per warp.
+template <int kWarps>
+__device__ __forceinline__ double block_sum_f64(double v, double (&s_warp)[kWarps]) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  __syncthreads();
+  if ((threadIdx.x & 31) == 0) s_warp[threadIdx.x >> 5] = v;
+  __syncthreads();
+  double t = 0.0;
+  for (int w = 0; w < kWarps; ++w) t += s_warp[w];
+  return t;
+}
+
+// ----------------------------------------------------------------------------
+// TF32 tensor-core products with 3xTF32 error compensation
+// ----------------------------------------------------------------------------
+// x = hi + lo with hi = x rounded to TF32;  a*b ~= a_lo*b_hi + a_hi*b_lo + a_hi*b_hi with fp32
+// accumulation in the MMA.  The dropped a_lo*b_lo term is ~2^-22 relative, which keeps the 1e-5
+// fp32 parity that plain TF32 (~1e-3) cannot hold.
+//
+// hi = x rounded to nearest (ties away) at 10 explicit mantissa bits, done with integer ops
+// (ptxas expands cvt.rna.tf32.f32 to 5 instructions; this is 2).  lo = x - hi is exact in fp32
+// and is handed to the MMA as is: the tensor core drops its low 13 bits, an error
+// <= 2^-11 |lo| <= 2^-22 |x|, the same order as the dropped lo*lo term, and unbiased because hi
+// is rounded to nearest.  3 instructions per element.
+__device__ __forceinline__ void split_tf32(float x, float& hi, float& lo) {
+  hi = __uint_as_float((__float_as_uint(x) + 0x1000u) & 0xffffe000u);
+  lo = x - hi;
+}
+// the same split as mma.sync operand registers
+__device__ __forceinline__ void split_tf32(float x, uint32_t& hi, uint32_t& lo) {
+  float h, l;
+  split_tf32(x, h, l);
+  hi = __float_as_uint(h);
+  lo = __float_as_uint(l);
+}
+__device__ __forceinline__ void split_tf32(const float4 v, float4& hi, float4& lo) {
+  split_tf32(v.x, hi.x, lo.x);
+  split_tf32(v.y, hi.y, lo.y);
+  split_tf32(v.z, hi.z, lo.z);
+  split_tf32(v.w, hi.w, lo.w);
+}
+
+// c += a . b on mma.sync.m16n8k8 (TF32 operands, fp32 accumulators)
+__device__ __forceinline__ void mma_tf32(float (&c)[4], const uint32_t (&a)[4],
+                                         const uint32_t (&b)[2]) {
+  asm volatile(
+      "mma.sync.aligned.m16n8k8.row.col.f32.tf32.tf32.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, "
+      "{%8,%9}, {%0,%1,%2,%3};\n"
+      : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b[0]), "r"(b[1]));
+}
+
+__device__ __forceinline__ void mma_3xtf32(float (&c)[4], const uint32_t (&ah)[4],
+                                           const uint32_t (&al)[4], const uint32_t (&bh)[2],
+                                           const uint32_t (&bl)[2]) {
+  mma_tf32(c, al, bh);
+  mma_tf32(c, ah, bl);
+  mma_tf32(c, ah, bh);
 }
 
 // First two passes of a softmax over one row held by one warp (lanes take c = lane, lane + 32,

@@ -113,21 +113,8 @@ crr_actor_head_kernel(const rb200_crr_actor_args_t a) {
   if (row < a.batch) {
     const size_t base = (size_t)row * A;
     const CrrLogits lg{a.actor_out + base, a.noise ? a.noise + base : nullptr};
-    // logged action: torch.argmax(action, dim=1), the first maximum
-    const float* act = a.action + base;
-    float lv = -INFINITY;
-    int li = A;
-    for (int c = lane; c < A; c += 32) {
-      const float v = act[c];
-      if (v > lv) { lv = v; li = c; }
-    }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-      const float ov = __shfl_xor_sync(0xffffffffu, lv, o);
-      const int oi = __shfl_xor_sync(0xffffffffu, li, o);
-      if (ov > lv || (ov == lv && oi < li)) { lv = ov; li = oi; }
-    }
-    if (li >= A) li = 0;  // a row of NaN actions: torch.argmax would also give an arbitrary index
+    // logged action: torch.argmax(action, dim=1)
+    const int li = warp_first_argmax(a.action + base, A);
     float mx, sum;
     warp_row_max_sumexp(lg, A, mx, sum);
     const float lsum = logf(sum);

@@ -285,7 +285,7 @@ dqn_td_tc_kernel(const Mlp q, const Mlp qt, const QDev p) {
       float* base = reinterpret_cast<float*>(smem_raw + p.buf_off[0]);
       const int r = idx / xnq, qd = idx - r * xnq;
       float4 h, l;
-      split4(v, h, l);
+      split_tf32(v, h, l);
       const int o = qd * (kQLboB / 4) + r * 4;
       *reinterpret_cast<float4*>(base + o) = h;
       *reinterpret_cast<float4*>(base + o + kQLoOff) = l;
@@ -382,10 +382,7 @@ dqn_td_tc_kernel(const Mlp q, const Mlp qt, const QDev p) {
           for (int kk = 0; kk < kQCK; ++kk)
 #pragma unroll
             for (int e = 0; e < 4; ++e) {
-              float h, lo_;
-              split1(v[kk][e], h, lo_);
-              fh[kk][e] = __float_as_uint(h);
-              fl[kk][e] = __float_as_uint(lo_);
+              split_tf32(v[kk][e], fh[kk][e], fl[kk][e]);
               wgmma_fence_operand(fh[kk][e]);
               wgmma_fence_operand(fl[kk][e]);
             }
@@ -488,7 +485,7 @@ dqn_td_tc_kernel(const Mlp q, const Mlp qt, const QDev p) {
 #pragma unroll
             for (int k = 0; k < 8; ++k) {
               float h, lo_;
-              split1(row0 + rowof(k) < B ? x[k] : 0.f, h, lo_);
+              split_tf32(row0 + rowof(k) < B ? x[k] : 0.f, h, lo_);
               ob[rowof(k) * 4] = h;
               ob[rowof(k) * 4 + kQLoOff] = lo_;
             }
@@ -576,7 +573,7 @@ dqn_td_tc_kernel(const Mlp q, const Mlp qt, const QDev p) {
         }
         if (a.do_backward) {
           float h, lo_;
-          split1(v, h, lo_);
+          split_tf32(v, h, lo_);
           float* o = zb + (c >> 2) * (kQLboB / 4) + (c & 3);
           o[0] = h;
           o[kQLoOff] = lo_;

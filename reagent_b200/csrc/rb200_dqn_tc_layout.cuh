@@ -84,12 +84,6 @@ inline TcImages tc_images(const rb200_mlp_t* q, int do_backward) {
   return im;
 }
 
-// hi = x rounded to nearest at 10 explicit mantissa bits (TF32), lo = x - hi (exact in fp32)
-__device__ __forceinline__ void tf32_split(float x, float& hi, float& lo) {
-  hi = __uint_as_float((__float_as_uint(x) + 0x1000u) & 0xffffe000u);
-  lo = x - hi;
-}
-
 // device view used by the Adam kernel to write the images of the parameters it updates
 struct TcPackView {
   int n_layers;

@@ -250,20 +250,8 @@ __global__ void __launch_bounds__(32 * kBcRowsPerBlock) bc_xent_head_kernel(cons
     const float* lab = a.labels + base;
     // z = scores + (-1e10) * (1 - mask), each operation rounded as torch does it
     const auto z = [x, m](int c) { return __fadd_rn(x[c], __fmul_rn(-1e10f, __fsub_rn(1.f, m[c]))); };
-    // label = first maximal entry of the one-hot row (torch.argmax over dim 1)
-    float lv = -INFINITY;
-    int li = A;
-    for (int c = lane; c < A; c += 32) {
-      const float v = lab[c];
-      if (v > lv) { lv = v; li = c; }
-    }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-      const float ov = __shfl_xor_sync(0xffffffffu, lv, o);
-      const int oi = __shfl_xor_sync(0xffffffffu, li, o);
-      if (ov > lv || (ov == lv && oi < li)) { lv = ov; li = oi; }
-    }
-    if (li >= A) li = 0;  // a row of NaN labels: torch.argmax would also give an arbitrary index
+    // label = torch.argmax(labels, dim=1)
+    const int li = warp_first_argmax(lab, A);
     // log_softmax: (z - max) - log(sum exp(z - max)); row loss -log_softmax[label]
     float mx, sum;
     warp_row_max_sumexp(z, A, mx, sum);

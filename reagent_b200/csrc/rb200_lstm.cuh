@@ -19,8 +19,6 @@ namespace rb200 {
 constexpr int kLstmNT = 256, kLstmTM = 4, kLstmKC = 32;
 constexpr int kLstmR = (kLstmNT / 64) * kLstmTM;  // 16 rows per CTA
 
-__device__ __forceinline__ float lstm_sigmoid(float x) { return 1.f / (1.f + expf(-x)); }
-
 // hs / cs [L, T+1, B, H]: slot s (0 = the initial state) of layer l, row b
 __device__ __forceinline__ size_t lstm_hc_idx(int T, int B, int H, int l, int s, int b) {
   return (((size_t)l * (T + 1) + s) * B + b) * H;
@@ -58,10 +56,10 @@ __device__ __forceinline__ void lstm_tile_step(const Args& a, int L, int H, int 
       const int r = i / H, j = i - r * H, b = row0 + r;
       const float* g1 = scr + r * ld_s;
       const float* g2 = g1 + ld_g;
-      const float gi = lstm_sigmoid(__fadd_rn(g2[j], g1[j]));
-      const float gf = lstm_sigmoid(__fadd_rn(g2[H + j], g1[H + j]));
+      const float gi = sigmoidf(__fadd_rn(g2[j], g1[j]));
+      const float gf = sigmoidf(__fadd_rn(g2[H + j], g1[H + j]));
       const float gg = tanhf(__fadd_rn(g2[2 * H + j], g1[2 * H + j]));
-      const float go = lstm_sigmoid(__fadd_rn(g2[3 * H + j], g1[3 * H + j]));
+      const float go = sigmoidf(__fadd_rn(g2[3 * H + j], g1[3 * H + j]));
       const float cn = __fadd_rn(__fmul_rn(gf, c[r * ld_h + j]), __fmul_rn(gi, gg));
       const float hn = __fmul_rn(go, tanhf(cn));
       c[r * ld_h + j] = b < B ? cn : 0.f;

@@ -329,7 +329,7 @@ __global__ void __launch_bounds__(kMdnNT, 1) mdnrnn_fwd_kernel(const rb200_mdnrn
       if (gl) dy[2 * GS + lane] = __fsub_rn(dz, __fmul_rn(expf(logpi), dzs));
       if (lane == 0) {
         dy[d.NG - 2] = __fmul_rn(__fdiv_rn(a.reward_weight, n_rows), __fmul_rn(2.f, __fsub_rn(rh, rt)));
-        dy[d.NG - 1] = __fmul_rn(__fdiv_rn(a.not_terminal_weight, n_rows), __fsub_rn(lstm_sigmoid(nt), yt));
+        dy[d.NG - 1] = __fmul_rn(__fdiv_rn(a.not_terminal_weight, n_rows), __fsub_rn(sigmoidf(nt), yt));
       }
     }
     __syncthreads();
@@ -431,18 +431,6 @@ __global__ void __launch_bounds__(kMdnNT, 1) mdnrnn_bwd_kernel(const rb200_mdnrn
 // per feature group; sums in fp64 over a fixed thread-strided order, so both are deterministic.
 // ---------------------------------------------------------------------------
 constexpr int kEvalNT = 256;
-
-// Sum over the CTA of one fp64 value per thread, in a fixed order; every thread gets the total.
-__device__ __forceinline__ double block_sum_f64(double v, double* s_warp) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  __syncthreads();
-  if ((threadIdx.x & 31) == 0) s_warp[threadIdx.x >> 5] = v;
-  __syncthreads();
-  double t = 0.0;
-  for (int w = 0; w < kEvalNT / 32; ++w) t += s_warp[w];
-  return t;
-}
 
 // compute_median_feature_value of group g over the rows of x = cat(action, state): a width-1
 // group gets its column mean; a wider (enum) group a one-hot at the first column whose count

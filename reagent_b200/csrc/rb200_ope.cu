@@ -146,19 +146,6 @@ ope_dr_rows_kernel(int n, int A, const float* prop, const float* mr, const float
   dr[b] = __fadd_rn(__fmul_rn(w, __fsub_rn(r[b], mrl[b])), d);
 }
 
-// fixed-order CTA sum of one double per thread (result in thread 0)
-__device__ __forceinline__ double block_sum_f64(double v, double* s_warp) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  __syncthreads();
-  if ((threadIdx.x & 31) == 0) s_warp[threadIdx.x >> 5] = v;
-  __syncthreads();
-  double t = 0.0;
-  if (threadIdx.x == 0)
-    for (int w = 0; w < (int)(blockDim.x >> 5); ++w) t += s_warp[w];
-  return t;
-}
-
 // one CTA per bootstrap sample: the mean of data[idx[s, :]] as an fp64 sum over fp64 (the caller
 // rounds it to float32 where the reference's sample is float32).  idx == NULL: index k of sample s is drawn
 // from Philox(seed, subsequence s * 256 + thread, offset) as a 64-bit value modulo n.

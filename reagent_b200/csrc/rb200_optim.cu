@@ -29,18 +29,6 @@ struct WgradParamsN {
 };
 using WgradParams = WgradParamsN<kMaxLayers>;
 
-__device__ __forceinline__ void wg_split(float x, uint32_t& hi, uint32_t& lo) {
-  hi = (__float_as_uint(x) + 0x1000u) & 0xffffe000u;
-  lo = __float_as_uint(x - __uint_as_float(hi));
-}
-__device__ __forceinline__ void wg_mma(float (&c)[4], const uint32_t (&a)[4], const uint32_t (&b)[2]) {
-  asm volatile(
-      "mma.sync.aligned.m16n8k8.row.col.f32.tf32.tf32.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, "
-      "{%8,%9}, {%0,%1,%2,%3};\n"
-      : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
-      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b[0]), "r"(b[1]));
-}
-
 template <int kJobs>
 __global__ void __launch_bounds__(kThreads) wgrad_kernel(const WgradParamsN<kJobs> p) {
   __shared__ __align__(16) float zs[2][kWgRows][kWgLd];
@@ -134,23 +122,19 @@ __global__ void __launch_bounds__(kThreads) wgrad_kernel(const WgradParamsN<kJob
 #pragma unroll
       for (int i = 0; i < 2; ++i) {
         const int n = wn + 16 * i + g;
-        wg_split(zs[buf][bb + t][n], ah[i][0], al[i][0]);
-        wg_split(zs[buf][bb + t][n + 8], ah[i][1], al[i][1]);
-        wg_split(zs[buf][bb + t + 4][n], ah[i][2], al[i][2]);
-        wg_split(zs[buf][bb + t + 4][n + 8], ah[i][3], al[i][3]);
+        split_tf32(zs[buf][bb + t][n], ah[i][0], al[i][0]);
+        split_tf32(zs[buf][bb + t][n + 8], ah[i][1], al[i][1]);
+        split_tf32(zs[buf][bb + t + 4][n], ah[i][2], al[i][2]);
+        split_tf32(zs[buf][bb + t + 4][n + 8], ah[i][3], al[i][3]);
       }
 #pragma unroll
       for (int j = 0; j < 2; ++j) {
         const int k = wk + 8 * j + g;
         uint32_t bh[2], bl[2];
-        wg_split(as[buf][bb + t][k], bh[0], bl[0]);
-        wg_split(as[buf][bb + t + 4][k], bh[1], bl[1]);
+        split_tf32(as[buf][bb + t][k], bh[0], bl[0]);
+        split_tf32(as[buf][bb + t + 4][k], bh[1], bl[1]);
 #pragma unroll
-        for (int i = 0; i < 2; ++i) {
-          wg_mma(acc[i][j], al[i], bh);
-          wg_mma(acc[i][j], ah[i], bl);
-          wg_mma(acc[i][j], ah[i], bh);
-        }
+        for (int i = 0; i < 2; ++i) mma_3xtf32(acc[i][j], ah[i], al[i], bh, bl);
       }
     }
     if (tk == 0 && tid < kWgTile) {

@@ -146,21 +146,8 @@ pg_head_kernel(const rb200_pg_head_args_t a) {
   if (row < a.rows) {  // whole warps: the block-level tail below needs every thread
     const size_t base = (size_t)row * A;
     const PgLogits lg{a.scores + base, a.mask ? a.mask + base : nullptr, a.temperature};
-    // logged action: Categorical.log_prob(action.argmax(1)), the first maximum
-    const float* act = a.action + base;
-    float lv = -INFINITY;
-    int li = A;
-    for (int c = lane; c < A; c += 32) {
-      const float v = act[c];
-      if (v > lv) { lv = v; li = c; }
-    }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-      const float ov = __shfl_xor_sync(0xffffffffu, lv, o);
-      const int oi = __shfl_xor_sync(0xffffffffu, li, o);
-      if (ov > lv || (ov == lv && oi < li)) { lv = ov; li = oi; }
-    }
-    if (li >= A) li = 0;  // a row of NaN actions: torch.argmax would also give an arbitrary index
+    // logged action: Categorical.log_prob(action.argmax(1))
+    const int li = warp_first_argmax(a.action + base, A);
     float mx, sum;
     warp_row_max_sumexp(lg, A, mx, sum);
     const float lse = __fadd_rn(mx, logf(sum));

@@ -122,10 +122,10 @@ __global__ void __launch_bounds__(kTcThreads, kTcCtasPerSm) tc_linear_fwd_kernel
       const int r = idx >> 3, q = idx & 7;
       const int off = q * kTcQuadStride + r * 4;  // [k quad][row][4], padded quad stride
       float4 h, l;
-      split4(ra[it], h, l);
+      split_tf32(ra[it], h, l);
       *reinterpret_cast<float4*>(a_hi + off) = h;
       *reinterpret_cast<float4*>(a_lo + off) = l;
-      split4(rb[it], h, l);
+      split_tf32(rb[it], h, l);
       *reinterpret_cast<float4*>(b_hi + off) = h;
       *reinterpret_cast<float4*>(b_lo + off) = l;
     }

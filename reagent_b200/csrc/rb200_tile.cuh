@@ -22,11 +22,8 @@ __host__ __device__ constexpr int wstage_floats() {
 }
 
 // ---------------------------------------------------------------------------
-// Tensor-core inner product: mma.sync.m16n8k8 TF32 with 3xTF32 error compensation.
-//   x = hi + lo (hi = rna_tf32(x), lo = rna_tf32(x - hi));  a*b ~= a_lo*b_hi + a_hi*b_lo + a_hi*b_hi
-// fp32 accumulation in the MMA; the dropped a_lo*b_lo term is ~2^-22 relative, which keeps the
-// 1e-5 parity bar of the north star (plain TF32 would be ~1e-3), with far fewer issue slots
-// than an FFMA loop.
+// Tensor-core inner product: mma.sync.m16n8k8 TF32 with 3xTF32 error compensation
+// (split_tf32 / mma_3xtf32, rb200_common.cuh), with far fewer issue slots than an FFMA loop.
 // Fragment <-> shared-memory mapping (g = lane/4, t = lane%4), all LDS.32 conflict-free:
 //   A (16x8, row-major tile of the activations, stride == 4 mod 32): a0 (g,t) a1 (g+8,t)
 //                                                                   a2 (g,t+4) a3 (g+8,t+4)
@@ -36,33 +33,6 @@ __host__ __device__ constexpr int wstage_floats() {
 // A warp owns ALL row tiles (R/16) and the 8-column tiles  warp, warp+NW, ...  of the chunk, so
 // narrow layers still spread over every warp.
 // ---------------------------------------------------------------------------
-__device__ __forceinline__ void split_tf32(float x, uint32_t& hi, uint32_t& lo) {
-  // hi = x rounded to nearest (ties away) at 10 explicit mantissa bits, done with integer ops
-  // (ptxas expands cvt.rna.tf32.f32 to 5 instructions; this is 2).  lo = x - hi is exact in
-  // fp32 and is handed to the MMA as is: the tensor core drops its low 13 bits, an error
-  // <= 2^-11 |lo| <= 2^-22 |x|, the same order as the dropped lo*lo term, and unbiased because
-  // hi is rounded to nearest.  3 instructions per element.
-  hi = (__float_as_uint(x) + 0x1000u) & 0xffffe000u;
-  lo = __float_as_uint(x - __uint_as_float(hi));
-}
-
-__device__ __forceinline__ void mma_tf32(float (&c)[4], const uint32_t (&a)[4],
-                                         const uint32_t (&b)[2]) {
-  asm volatile(
-      "mma.sync.aligned.m16n8k8.row.col.f32.tf32.tf32.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, "
-      "{%8,%9}, {%0,%1,%2,%3};\n"
-      : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
-      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b[0]), "r"(b[1]));
-}
-
-__device__ __forceinline__ void mma_3xtf32(float (&c)[4], const uint32_t (&ah)[4],
-                                           const uint32_t (&al)[4], const uint32_t (&bh)[2],
-                                           const uint32_t (&bl)[2]) {
-  mma_tf32(c, al, bh);
-  mma_tf32(c, ah, bl);
-  mma_tf32(c, ah, bh);
-}
-
 constexpr int kLWB = kNC + 8;  // bwd staging row stride (== 8 mod 32)
 
 // ---------------------------------------------------------------------------

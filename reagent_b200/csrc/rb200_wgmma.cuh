@@ -1,9 +1,7 @@
 // reagent_b200 -- wgmma / mbarrier / bulk-copy PTX helpers shared by the Hopper tensor-core
 // kernels (rb200_tc_gemm.cu, rb200_dqn_tc.cu).  sm_90a only.
 //
-// Every product is TF32 with 3xTF32 error compensation: x = hi + lo with hi = x rounded to
-// TF32 and lo = x - hi (exact in fp32); a.b ~ a_hi.b_hi + a_hi.b_lo + a_lo.b_hi carries ~22
-// mantissa bits, the 1e-5 fp32 parity plain TF32 (~1e-3) cannot hold.
+// Every product is TF32 with 3xTF32 error compensation (split_tf32, rb200_common.cuh).
 #pragma once
 #include "rb200_common.cuh"
 
@@ -59,18 +57,6 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
     if (ok) break;
     if (it > 400000LL) __trap();  // ~2 s (a failed try_wait blocks a few us): never spin forever on a protocol bug
   }
-}
-
-__device__ __forceinline__ void split4(const float4 v, float4& hi, float4& lo) {
-  uint32_t h;
-  h = (__float_as_uint(v.x) + 0x1000u) & 0xffffe000u; hi.x = __uint_as_float(h); lo.x = v.x - hi.x;
-  h = (__float_as_uint(v.y) + 0x1000u) & 0xffffe000u; hi.y = __uint_as_float(h); lo.y = v.y - hi.y;
-  h = (__float_as_uint(v.z) + 0x1000u) & 0xffffe000u; hi.z = __uint_as_float(h); lo.z = v.z - hi.z;
-  h = (__float_as_uint(v.w) + 0x1000u) & 0xffffe000u; hi.w = __uint_as_float(h); lo.w = v.w - hi.w;
-}
-__device__ __forceinline__ void split1(float x, float& hi, float& lo) {
-  hi = __uint_as_float((__float_as_uint(x) + 0x1000u) & 0xffffe000u);
-  lo = x - hi;
 }
 
 // ---- mbarrier transaction + 1-D bulk copy (TMA engine, no tensor map) ----

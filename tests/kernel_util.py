@@ -1,5 +1,5 @@
-"""Constants and launch helpers of the kernel-level tests (the layer, Adam, loss-reduction and
-actor-critic kernels) that more than one test module uses."""
+"""Constants and launch helpers of the kernel-level tests (the layer, Adam, loss-reduction,
+loss-head and actor-critic kernels) that more than one test module uses."""
 import ctypes as C
 
 import numpy as np
@@ -135,3 +135,17 @@ def _ws(n_partials, n_loss=1):
 def _set_ws(a, ws):
     a.loss_partials, a.loss, a.tile_counter = (ws["partials"].data_ptr(), ws["loss"].data_ptr(),
                                                ws["counter"].data_ptr())
+
+
+def _argmax_edge_rows(onehot):
+    """A copy of the one-hot rows `onehot` [B, A] whose first rows are the edges of
+    torch.argmax: a tie of columns A // 2 and A - 1, a tie across the whole row, and a row of
+    NaNs.  torch.argmax gives the first maximum, and 0 for the row of NaNs; the heads that read
+    a logged action or label must pick the same column."""
+    x = onehot.clone()
+    B, A = x.shape
+    tie = torch.zeros(A)
+    tie[[A // 2, A - 1]] = 1.0
+    for r, row in enumerate([tie, torch.ones(A), torch.full((A,), NAN)][:B]):
+        x[r] = row
+    return x

@@ -7,6 +7,7 @@ import torch
 
 from oracle import crr_oracle as CO
 from tests import golden_util as G
+from tests.kernel_util import _argmax_edge_rows
 
 pytestmark = pytest.mark.gpu
 TOL = 2e-5
@@ -125,9 +126,15 @@ def test_critic_head_matches_fp64(B, A, twin):
 @pytest.mark.parametrize("B,A", SHAPES)
 @pytest.mark.parametrize("entropy_coeff", [0.0, 0.4])
 def test_actor_head_matches_fp64(B, A, entropy_coeff):
+    """The first rows log tied and NaN actions; the reference takes torch.argmax of them."""
     d = _inputs(B, A, seed=2 * B + A, noise_scale=0.7 if A % 2 else None)
+    logged = _argmax_edge_rows(d["action"])
+    d["action"] = torch.nn.functional.one_hot(logged.argmax(1), A).float()
     kw = dict(beta=0.7, max_weight=3.0, entropy_coeff=entropy_coeff, clip_limit=2.0)
-    _, o = run_actor(d, **kw)
+    _, o = run_actor(dict(d, action=logged), **kw)
+    _, o_onehot = run_actor(d, **kw)
+    for k in o:
+        assert torch.equal(o[k], o_onehot[k]), k
     ref = CO.actor_head_fp64(d["actor_out"], d["noise"], d["q1"], d["action"], d["prob"], **kw)
     _close(o["w"], ref["weight"])
     _close(o["dz"], ref["dz"])

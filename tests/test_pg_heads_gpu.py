@@ -1,8 +1,9 @@
 """rb200_pg_head alone against the fp64 reference of oracle/pg_oracle.py, at A = 1, 33 and 1024
 (one column per lane, two, and 32), with masks, rows of several trajectories, the off-policy
 REINFORCE clip, PPO ratios on both sides of the clip and with the entropy bonus, the value
-baseline, and a PPO ratio exactly at both clip bounds, where torch.minimum ties and
-torch.clamp's closed interval pass the full gradient."""
+baseline, a PPO ratio exactly at both clip bounds, where torch.minimum ties and torch.clamp's
+closed interval pass the full gradient, and logged actions with tied maxima or NaNs, read as
+torch.argmax reads them."""
 import math
 
 import pytest
@@ -10,6 +11,7 @@ import torch
 
 from oracle import pg_oracle as PO
 from tests import golden_util as G
+from tests.kernel_util import _argmax_edge_rows
 
 pytestmark = pytest.mark.gpu
 
@@ -54,7 +56,8 @@ def _inputs(A, seed):
     R = sum(LENGTHS)
     scores = torch.randn(R, A, generator=g) * 2
     act = torch.randint(A, (R,), generator=g)
-    action = torch.nn.functional.one_hot(act, A).float()
+    action = _argmax_edge_rows(torch.nn.functional.one_hot(act, A).float())
+    act = action.argmax(1)  # the reference's logged action, which the head must pick too
     mask = (torch.rand(R, A, generator=g) > 0.3).float()
     mask[torch.arange(R), act] = 1.0
     returns = torch.randn(R, generator=g)
