@@ -1278,6 +1278,9 @@ int rb200_seq2slate_check_shape(int32_t state_dim, int32_t candidate_dim, int32_
                                 int32_t dim_model, int32_t num_heads, int32_t dim_feedforward,
                                 int32_t layers, int32_t max_src_seq_len, int32_t max_tgt_seq_len);
 int64_t rb200_seq2slate_workspace_bytes(const rb200_seq2slate_args_t* args);
+/* CTAs a launch of args runs, each looping over slates b, b + ctas, ... (on the shared-memory */
+/* path as many as fit on the current device at once), or a negative RB200_E_* code           */
+int rb200_seq2slate_ctas(const rb200_seq2slate_args_t* args);
 int rb200_seq2slate_forward(const rb200_seq2slate_args_t* args, void* stream);
 int rb200_seq2slate_rank(const rb200_seq2slate_args_t* args, void* stream);
 

@@ -1,6 +1,7 @@
 """float64 restatement of the Seq2Slate transformer (reagent/models/seq2slate.py) from a
 state_dict: the encoder, the teacher-forced decoder over the whole prefix (full recompute, as
-the reference does it) and the greedy rank that re-runs that decoder at every step.  It is
+the reference does it) and the greedy and sampled ranks that re-run that decoder at every
+step.  It is
 written from the math (post-norm layers, per-head softmax attention, the pytorch_decoder_mask
 masks), not from torch's transformer modules, and pinned against the reference's goldens by
 tests/test_seq2slate_cpu.py."""
@@ -146,3 +147,53 @@ def greedy_rank(sd, cfg, state, src_seq, T):
     idx = tin[:, 1:]
     seq = torch.gather(probs, 2, idx.unsqueeze(2)).squeeze(2).prod(1, keepdim=True)
     return idx, probs, seq.clamp(min=1e-40)
+
+
+def inverse_cdf(p, u):
+    """The sample rule on one step's probabilities p [B, M] and uniforms u [B]: the first j of
+    nonzero probability with cumsum(p)[j] > u * sum(p), else the last j of nonzero probability
+    (reached only when u * sum(p) is the total itself).  Returns (j [B], distance [B] of
+    u * sum(p) to the nearest cumsum boundary between two live symbols, inf if there is none):
+    a rounding smaller than that distance cannot change the choice."""
+    p = p.to(F64)
+    c = p.cumsum(1)
+    x = u.to(F64) * c[:, -1]  # the total summed in the same order as the running sum
+    live = p > 0
+    M = p.shape[1]
+    hit = live & (c > x.unsqueeze(1))
+    last = M - 1 - live.flip(1).to(torch.int8).argmax(1)
+    j = torch.where(hit.any(1), hit.to(torch.int8).argmax(1), last)
+    # the boundary after the last live symbol only separates it from the fallback, which
+    # picks it too
+    inner = live.clone()
+    inner[torch.arange(p.shape[0]), last] = False
+    dist = torch.where(inner, (c - x.unsqueeze(1)).abs(), torch.full_like(c, math.inf))
+    return j, dist.amin(1)
+
+
+def top2_gap(probs):
+    """[...]: the largest minus the second largest of probs [..., M] (the greedy choice's
+    distance to a tie)."""
+    top = probs.to(F64).topk(2, dim=-1).values
+    return top[..., 0] - top[..., 1]
+
+
+def sample_rank(sd, cfg, state, src_seq, T, noise):
+    """(ranked idx [B, T], per-symbol probs [B, T, N + 2], per-seq prob [B, 1] clamped at
+    1e-40, boundary distance [B, T]) of the sampled decode with uniforms noise [B, T] under the
+    rule of inverse_cdf, re-running the decoder over the whole prefix at every step."""
+    mem = encode(sd, cfg, state, src_seq)
+    B, N, C = src_seq.shape
+    feats = torch.cat((torch.zeros(B, 2, C, dtype=F64), src_seq.to(F64)), dim=1)
+    rows = torch.arange(B).unsqueeze(1)
+    tin = torch.full((B, 1), 1, dtype=torch.long)
+    probs = torch.zeros(B, T, N + 2, dtype=F64)
+    dist = torch.zeros(B, T, dtype=F64)
+    for t in range(T):
+        p = decode(sd, cfg, mem, state, tin, feats[rows, tin])[:, -1]
+        probs[:, t] = p
+        j, dist[:, t] = inverse_cdf(p, noise[:, t])
+        tin = torch.cat((tin, j.unsqueeze(1)), dim=1)
+    idx = tin[:, 1:]
+    seq = torch.gather(probs, 2, idx.unsqueeze(2)).squeeze(2).prod(1, keepdim=True)
+    return idx, probs, seq.clamp(min=1e-40), dist

@@ -507,26 +507,45 @@ extern "C" int64_t rb200_seq2slate_workspace_bytes(const rb200_seq2slate_args_t*
   return (int64_t)ctas * (int64_t)s2s_slice_bytes(a);
 }
 
+// CTAs of a launch: min(B, RB200_SEQ2SLATE_MAX_CTAS), and on the shared-memory path no more than
+// fit on the device at once.  CTA c carries slates c, c + ctas, c + 2 ctas, ...
+static int s2s_ctas(const rb200_seq2slate_args_t* a, int* ctas) {
+  const size_t slice = s2s_slice_bytes(a);
+  *ctas = a->batch < kS2sMaxCtas ? a->batch : kS2sMaxCtas;
+  if (slice > kS2sSmemMax) return 0;
+  if (cudaError_t e = opt_in_smem<seq2slate_kernel>(slice))
+    return check_cuda(e, "seq2slate_kernel smem opt-in");
+  int per_sm = 0, dev = 0, sms = 0;
+  if (cudaError_t e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, seq2slate_kernel,
+                                                                     kS2sThreads, slice))
+    return check_cuda(e, "seq2slate_kernel occupancy");
+  if (cudaError_t e = cudaGetDevice(&dev)) return check_cuda(e, "cudaGetDevice");
+  if (cudaError_t e = cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev))
+    return check_cuda(e, "cudaDeviceGetAttribute");
+  const long long fit = (long long)(per_sm > 0 ? per_sm : 1) * sms;
+  if (fit < *ctas) *ctas = (int)fit;
+  return 0;
+}
+
 static int s2s_launch(const rb200_seq2slate_args_t* a, void* stream) {
   const size_t slice = s2s_slice_bytes(a);
   const bool smem = slice <= kS2sSmemMax;
-  int ctas = a->batch < kS2sMaxCtas ? a->batch : kS2sMaxCtas;
-  if (smem) {
-    // as many slates in flight as fit on the device at once; each CTA loops over the rest
-    if (cudaError_t e = opt_in_smem<seq2slate_kernel>(slice))
-      return check_cuda(e, "seq2slate_kernel smem opt-in");
-    int per_sm = 0, dev = 0, sms = 0;
-    if (cudaError_t e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, seq2slate_kernel,
-                                                                       kS2sThreads, slice))
-      return check_cuda(e, "seq2slate_kernel occupancy");
-    if (cudaError_t e = cudaGetDevice(&dev)) return check_cuda(e, "cudaGetDevice");
-    if (cudaError_t e = cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev))
-      return check_cuda(e, "cudaDeviceGetAttribute");
-    const long long fit = (long long)(per_sm > 0 ? per_sm : 1) * sms;
-    if (fit < ctas) ctas = (int)fit;
-  }
+  int ctas = 0;
+  if (int rc = s2s_ctas(a, &ctas)) return rc;
   seq2slate_kernel<<<ctas, kS2sThreads, smem ? slice : 0, (cudaStream_t)stream>>>(*a, smem);
   return check_cuda(cudaGetLastError(), "seq2slate_kernel launch");
+}
+
+extern "C" int rb200_seq2slate_ctas(const rb200_seq2slate_args_t* a) {
+  const char* who = "rb200_seq2slate_ctas";
+  if (!a) { set_last_error("%s: args is null", who); return RB200_E_INVALID; }
+  if (int rc = s2s_check(a->state_dim, a->candidate_dim, a->state_embed_dim, a->dim_model,
+                         a->num_heads, a->dim_feedforward, a->layers, a->src_len, a->tgt_len, who))
+    return rc;
+  if (a->batch < 1) { set_last_error("%s: batch %d < 1", who, a->batch); return RB200_E_INVALID; }
+  int ctas = 0;
+  if (int rc = s2s_ctas(a, &ctas)) return rc;
+  return ctas;
 }
 
 extern "C" int rb200_seq2slate_forward(const rb200_seq2slate_args_t* a, void* stream) {
