@@ -856,6 +856,13 @@ int rb200_valid_index_build(const uint8_t* valid, int64_t capacity, int32_t* cou
 /*       distributional heads, which have no scalar TD error):                             */
 /*       p_i = ((double)|row_loss_i| / divisor + eps) ** alpha, divisor > 0 and finite      */
 /*       (N*N for the QR-DQN head's loss_partials, 1 for C51's).                           */
+/*   rb200_per_priority_exchange  the data-parallel write-back's first half: this rank's   */
+/*       n_local priorities (the two formulas above, the same fp64 arithmetic) gathered    */
+/*       into the whole B_global-long vector on every rank (rb200_per_exchange_args_t).    */
+/*   rb200_per_priority_apply  its second half: SumTree.set(idx_i, val_i) in order, as     */
+/*       rb200_sumtree_set_device but with the PER rule: a value that is not finite       */
+/*       applies none of them and sets status 3.  Every rank applies the same vector, so   */
+/*       every rank reaches the same tree, max_recorded and status.                        */
 /* status words are sticky error flags the host wrapper turns into the reference's        */
 /* exceptions: 1 = "Max sample attempts", 2 = negative priority, 3 = non-finite PER       */
 /* priority (a non-finite TD error or row loss).                                          */
@@ -912,6 +919,39 @@ int rb200_per_priority_update_rows(double* tree, int32_t depth, const int64_t* i
                                    const float* row_loss, int32_t n, double divisor, double alpha,
                                    double eps, double* p_out, double* max_recorded,
                                    int32_t* status, void* stream);
+
+/* Priority exchange of a data-parallel prioritized update over NVLink peer memory, the
+ * pattern of rb200_adam_args_t.dp_*.  Rank `rank` of `world` holds rows [row0, row0 + n_local)
+ * of the B_global-long update.  One launch (1) computes their priorities from row_loss
+ * (p = (|row_loss| / divisor + eps) ** alpha) or, with row_loss NULL, from td_target and
+ * q_selected (p = (|q_selected - td_target| + eps) ** alpha), bit-identical to
+ * rb200_per_priority_update[_rows]; (2) stores them at [row0, row0 + n_local) of parity
+ * (epoch & 1) of every rank's receive buffer; (3) issues one system-scope fence and raises
+ * its flag at every peer with the new epoch; (4) waits for the world - 1 peer flags
+ * (acquire loads, 4 s bound: a lost peer fails the step, never hangs) and (5) copies the
+ * gathered vector to out [B_global].
+ *   recv[r]  of rank r: double   [2][B_global]  (parity of the epoch)
+ *   flags[r] of rank r: uint32_t [2][world]     (parity, source rank), zero-initialised once
+ * recv / flags are DEVICE arrays of world peer-mapped pointers; epoch is this rank's [1]
+ * device counter, zero-initialised once and advanced by every call.  Two parities suffice:
+ * a rank cannot start exchange e + 1 before every peer has started exchange e.  With
+ * world == 1 recv, flags and epoch may be NULL and the priorities go straight to out. */
+typedef struct rb200_per_exchange_args {
+  const float* td_target;     /* [n_local] */
+  const float* q_selected;    /* [n_local] */
+  const float* row_loss;      /* [n_local] or NULL */
+  double divisor;             /* > 0 and finite when row_loss is given */
+  double alpha, eps;
+  int32_t n_local, row0, B_global;
+  int32_t world, rank;        /* world <= 256 */
+  double* const* recv;
+  uint32_t* const* flags;
+  uint32_t* epoch;
+  double* out;                /* [B_global] */
+} rb200_per_exchange_args_t;
+int rb200_per_priority_exchange(const rb200_per_exchange_args_t* args, void* stream);
+int rb200_per_priority_apply(double* tree, int32_t depth, const int64_t* idx, const double* val,
+                             int32_t n, double* max_recorded, int32_t* status, void* stream);
 
 /* ------------------------------------------------------------------------- */
 /* MDN-RNN (reagent/models/mdn_rnn.py, reagent/training/world_model/mdnrnn_trainer.py):  */

@@ -76,6 +76,7 @@ extern "C" int64_t rb200_abi_sizeof(const char* type_name) {
   RB200_SZ(rb200_pg_head_args_t);
   RB200_SZ(rb200_add_args_t);
   RB200_SZ(rb200_per_draw_args_t);
+  RB200_SZ(rb200_per_exchange_args_t);
   RB200_SZ(rb200_mdnrnn_args_t);
   RB200_SZ(rb200_mdnrnn_eval_args_t);
   RB200_SZ(rb200_mdnrnn_fill_args_t);

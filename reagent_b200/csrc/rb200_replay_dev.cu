@@ -247,6 +247,7 @@ struct SetSrc {
   double alpha, eps;
   double* p_out;             // [n] or NULL: the values, written by the leaf kernel
   int n;
+  bool per;                  // val path with PER semantics: a non-finite value applies none
 };
 
 __device__ __forceinline__ double set_value(const SetSrc& s, int i) {
@@ -267,7 +268,7 @@ __device__ int sets_applied(const SetSrc& s, int* code) {
   for (int i = threadIdx.x; i < s.n; i += blockDim.x) {
     const double v = set_value(s, i);
     if (v < 0.0 && i < neg) neg = i;
-    if (!s.val && !isfinite(v)) bad = true;
+    if ((!s.val || s.per) && !isfinite(v)) bad = true;
   }
   if (neg < s.n) atomicMin(&s_neg, neg);
   if (bad) s_bad = 1;
@@ -425,6 +426,68 @@ static int sumtree_update(double* tree, int depth, const SetSrc& s, double* max_
     sumtree_leaves_kernel<<<1, kSetThreads, kSetSmem, st>>>(tree, depth, s, c0, max_recorded, status);
   }
   return check_cuda(cudaGetLastError(), "sumtree update launch");
+}
+
+// ---------------------------------------------------------------------------
+// Data-parallel priority exchange (rb200_per_exchange_args_t): one CTA computes this rank's
+// priorities with set_value, pushes them into every rank's receive buffer, then flags / waits
+// as adam_soft_kernel does and copies the gathered vector out.  A few KB per update: the
+// single CTA's latency is well under the tree update that follows it.
+// ---------------------------------------------------------------------------
+constexpr int kExchangeThreads = 1024;
+
+struct ExchangeDev {
+  rb200_per_exchange_args_t a;
+};
+
+__global__ void __launch_bounds__(kExchangeThreads) per_priority_exchange_kernel(const ExchangeDev d) {
+  const rb200_per_exchange_args_t& a = d.a;
+  SetSrc s = {};
+  s.td_target = a.td_target;
+  s.q_selected = a.q_selected;
+  s.row_loss = a.row_loss;
+  s.divisor = a.divisor;
+  s.alpha = a.alpha;
+  s.eps = a.eps;
+  const int W = a.world, tid = threadIdx.x;
+  if (W == 1) {
+    for (int i = tid; i < a.n_local; i += kExchangeThreads) a.out[a.row0 + i] = set_value(s, i);
+    return;
+  }
+  const uint32_t t = *a.epoch + 1u;
+  const size_t par = t & 1u;
+  const size_t slot = par * (size_t)a.B_global + a.row0;
+  for (int i = tid; i < a.n_local; i += kExchangeThreads) {
+    const double p = set_value(s, i);
+    for (int r = 0; r < W; ++r) a.recv[r][slot + i] = p;  // own copy included
+  }
+  __syncthreads();
+  if (tid == 0) {
+    // one system-scope fence orders every push of the CTA (made visible to this thread by the
+    // barrier) before the flags, which are then relaxed stores posted back to back
+    __threadfence_system();
+    for (int r = 0; r < W; ++r) {
+      if (r == a.rank) continue;
+      uint32_t* f = a.flags[r] + par * W + a.rank;
+      asm volatile("st.relaxed.sys.global.u32 [%0], %1;\n" ::"l"(f), "r"(t) : "memory");
+    }
+  }
+  if (tid < W && tid != a.rank) {
+    const uint32_t* w = a.flags[a.rank] + par * W + tid;
+    unsigned long long t0 = 0, now = 0;
+    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t0));
+    for (;;) {
+      uint32_t v;
+      asm volatile("ld.acquire.sys.global.u32 %0, [%1];\n" : "=r"(v) : "l"(w) : "memory");
+      if (v == t) break;
+      asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(now));
+      if (now - t0 > 4000000000ull) __trap();  // 4 s: a lost peer fails the step, never hangs
+    }
+  }
+  __syncthreads();
+  const double* mine = a.recv[a.rank] + par * (size_t)a.B_global;
+  for (int i = tid; i < a.B_global; i += kExchangeThreads) a.out[i] = __ldcg(mine + i);
+  if (tid == 0) *a.epoch = t;
 }
 
 // ---------------------------------------------------------------------------
@@ -592,6 +655,47 @@ extern "C" int rb200_per_priority_update_rows(double* tree, int32_t depth, const
   s.alpha = alpha;
   s.eps = eps;
   s.p_out = p_out;
+  s.n = n;
+  return sumtree_update(tree, depth, s, max_recorded, status, (cudaStream_t)stream);
+}
+
+extern "C" int rb200_per_priority_exchange(const rb200_per_exchange_args_t* a, void* stream) {
+  if (!a) { set_last_error("rb200_per_priority_exchange: null argument"); return RB200_E_INVALID; }
+  const char* null_arg = !a->out ? "out"
+                         : a->row_loss ? nullptr
+                         : !a->td_target ? "td_target" : !a->q_selected ? "q_selected" : nullptr;
+  if (!null_arg && a->world > 1)
+    null_arg = !a->recv ? "recv" : !a->flags ? "flags" : !a->epoch ? "epoch" : nullptr;
+  if (null_arg) { set_last_error("rb200_per_priority_exchange: %s is null", null_arg); return RB200_E_INVALID; }
+  if (a->world < 1 || a->world > 256 || a->rank < 0 || a->rank >= a->world) {
+    set_last_error("rb200_per_priority_exchange: bad world %d / rank %d", a->world, a->rank);
+    return RB200_E_INVALID;
+  }
+  if (a->n_local <= 0 || a->row0 < 0 || a->B_global <= 0 || (int64_t)a->row0 + a->n_local > a->B_global) {
+    set_last_error("rb200_per_priority_exchange: rows [%d, %d + %d) outside B_global %d", a->row0,
+                   a->row0, a->n_local, a->B_global);
+    return RB200_E_INVALID;
+  }
+  if (a->row_loss && (!(a->divisor > 0.0) || !isfinite(a->divisor))) {
+    set_last_error("rb200_per_priority_exchange: divisor must be positive and finite, got %g", a->divisor);
+    return RB200_E_INVALID;
+  }
+  ExchangeDev d;
+  d.a = *a;
+  per_priority_exchange_kernel<<<1, kExchangeThreads, 0, (cudaStream_t)stream>>>(d);
+  return check_cuda(cudaGetLastError(), "per_priority_exchange_kernel launch");
+}
+
+extern "C" int rb200_per_priority_apply(double* tree, int32_t depth, const int64_t* idx,
+                                        const double* val, int32_t n, double* max_recorded,
+                                        int32_t* status, void* stream) {
+  const char* null_arg = !tree ? "tree" : !idx ? "idx" : !val ? "val" : !status ? "status" : nullptr;
+  if (null_arg) { set_last_error("rb200_per_priority_apply: %s is null", null_arg); return RB200_E_INVALID; }
+  if (depth < 0 || depth > 31 || n <= 0) { set_last_error("rb200_per_priority_apply: bad depth %d / n %d", depth, n); return RB200_E_INVALID; }
+  SetSrc s = {};
+  s.idx = (const long long*)idx;
+  s.val = val;
+  s.per = true;
   s.n = n;
   return sumtree_update(tree, depth, s, max_recorded, status, (cudaStream_t)stream);
 }

@@ -16,6 +16,7 @@ the whole step in one CUDA graph).  `sync_to_host()` brings the host mirrors (an
 `random` state) back, after which the buffer's ordinary host-side API continues the same
 streams bit for bit.
 """
+import itertools
 import math
 import random
 from dataclasses import dataclass
@@ -27,6 +28,7 @@ import torch
 from .. import _lib
 
 MAX_ADD = 1024  # transitions per rb200_replay_add_device launch
+_EXCHANGE_KEYS = itertools.count()  # peer-memory priority slices, in the order of first use
 
 
 @dataclass(frozen=True)
@@ -51,6 +53,18 @@ class PrioritizedUpdate:
             raise ValueError(f"beta_updates must be positive, got {self.beta_updates}")
 
 
+@dataclass(frozen=True)
+class PriorityShard:
+    """This rank's place in a data-parallel prioritized update: its rows are
+    [row0, row0 + n) of the `batch_global` drawn ones, and `group` is the process group whose
+    ranks hold the others (None: one rank).  The priorities of all rows are gathered on every
+    rank -- over NVLink peer memory when `enable_p2p(group)` ran, else by NCCL all-gather -- and
+    every rank applies the same vector to its replicated tree."""
+    row0: int
+    batch_global: int
+    group: object = None
+
+
 class DeviceReplay:
     def __init__(self, rb, stage_rows: int = 1, stage_slots: int = 1):
         if rb._stack_size != 1:
@@ -71,6 +85,7 @@ class DeviceReplay:
                                              dtype=torch.float64, device=dev)
             self.upload_host_rng()
         self._bounds = {}
+        self._exchange_key = None
         self._keys = [e.name for e in rb.get_add_args_signature()
                       if e.name not in ("terminal", "reward", "priority")]
         self._alloc_stage(stage_rows, stage_slots)
@@ -200,9 +215,16 @@ class DeviceReplay:
 
     def write_back_priorities(self, indices: torch.Tensor, td_target: torch.Tensor,
                               q_selected: torch.Tensor, per: PrioritizedUpdate,
-                              p_out: torch.Tensor):
+                              p_out: torch.Tensor, shard: Optional[PriorityShard] = None):
         """set_priority(indices, (|q_selected - td_target| + eps) ** alpha), in batch order; the
-        priorities also go to `p_out` (fp64).  A non-finite one applies none (status 3)."""
+        priorities also go to `p_out` (fp64).  A non-finite one applies none (status 3).
+        With `shard`, td_target / q_selected are this rank's rows of the global update, and
+        `indices` and `p_out` have all `shard.batch_global` of them (p_out: the gathered
+        priorities, the same on every rank)."""
+        if shard is not None:
+            a = _lib.PerExchangeArgsT()
+            a.td_target, a.q_selected = td_target.data_ptr(), q_selected.data_ptr()
+            return self._sharded_write_back(a, indices, td_target.numel(), per, p_out, shard)
         rc = _lib.lib().rb200_per_priority_update(
             self.tree.data_ptr(), self.rb.sum_tree.depth, indices.data_ptr(), td_target.data_ptr(),
             q_selected.data_ptr(), indices.numel(), float(per.alpha), float(per.eps),
@@ -212,17 +234,65 @@ class DeviceReplay:
         return p_out
 
     def write_back_row_priorities(self, indices: torch.Tensor, row_loss: torch.Tensor,
-                                  divisor: float, per: PrioritizedUpdate, p_out: torch.Tensor):
+                                  divisor: float, per: PrioritizedUpdate, p_out: torch.Tensor,
+                                  shard: Optional[PriorityShard] = None):
         """set_priority(indices, (|row_loss| / divisor + eps) ** alpha), in batch order, for the
         distributional heads, whose priority is the row's own loss (fp32 `row_loss`, fp64
         arithmetic); the priorities also go to `p_out` (fp64).  A non-finite one applies none
-        (status 3)."""
+        (status 3).  `shard`: as write_back_priorities."""
+        if shard is not None:
+            a = _lib.PerExchangeArgsT()
+            a.row_loss, a.divisor = row_loss.data_ptr(), float(divisor)
+            return self._sharded_write_back(a, indices, row_loss.numel(), per, p_out, shard)
         rc = _lib.lib().rb200_per_priority_update_rows(
             self.tree.data_ptr(), self.rb.sum_tree.depth, indices.data_ptr(), row_loss.data_ptr(),
             indices.numel(), float(divisor), float(per.alpha), float(per.eps), p_out.data_ptr(),
             self.max_priority.data_ptr(), self.status.data_ptr(), _lib.cur_stream())
         _lib.check(rc, "rb200_per_priority_update_rows")
         return p_out
+
+    def _sharded_write_back(self, a, indices, n_local: int, per: PrioritizedUpdate,
+                            p_out: torch.Tensor, shard: PriorityShard):
+        """Gather every rank's priorities into p_out (the exchange args `a` carry this rank's
+        sources), then apply them all in global batch order."""
+        from ..training.data_parallel import p2p_for
+
+        lib = _lib.lib()
+        a.alpha, a.eps = float(per.alpha), float(per.eps)
+        a.n_local, a.row0, a.B_global = n_local, shard.row0, shard.batch_global
+        a.world, a.rank = 1, 0
+        ex = None if shard.group is None else p2p_for(shard.group)
+        if shard.group is None or ex is not None:
+            if ex is not None:
+                if self._exchange_key is None:  # first sharded write-back: same order on all ranks
+                    self._exchange_key = ("per", next(_EXCHANGE_KEYS))
+                recv, flags, epoch = ex.priority_slice(self._exchange_key, shard.batch_global)
+                a.world, a.rank = ex.world, ex.rank
+                a.recv, a.flags, a.epoch = recv.data_ptr(), flags.data_ptr(), epoch.data_ptr()
+            a.out = p_out.data_ptr()
+            _lib.check(lib.rb200_per_priority_exchange(a, _lib.cur_stream()),
+                       "rb200_per_priority_exchange")
+        else:
+            import torch.distributed as dist
+
+            local = self._local_priorities(n_local)
+            a.row0, a.B_global, a.out = 0, n_local, local.data_ptr()
+            _lib.check(lib.rb200_per_priority_exchange(a, _lib.cur_stream()),
+                       "rb200_per_priority_exchange")
+            dist.all_gather_into_tensor(p_out, local, group=shard.group)
+        rc = lib.rb200_per_priority_apply(
+            self.tree.data_ptr(), self.rb.sum_tree.depth, indices.data_ptr(), p_out.data_ptr(),
+            indices.numel(), self.max_priority.data_ptr(), self.status.data_ptr(),
+            _lib.cur_stream())
+        _lib.check(rc, "rb200_per_priority_apply")
+        return p_out
+
+    def _local_priorities(self, n: int) -> torch.Tensor:
+        """This rank's fp64 priorities before an NCCL all-gather (one fixed buffer: graph-safe)."""
+        buf = getattr(self, "_local_prio", None)
+        if buf is None or buf.numel() != n:
+            buf = self._local_prio = torch.empty(n, dtype=torch.float64, device=self.dev)
+        return buf
 
     # ---- index selection ---------------------------------------------------------------
     def upload_host_rng(self):

@@ -20,12 +20,19 @@ class ActorCriticBase(RLTrainerMixin, ReAgentLightningModule):
         # noise_hook(name, shape, device) -> tensor lets tests inject the reference's
         # torch.randn_like draws; default: torch.randn on the device
         self.noise_hook = None
+        # (row0, B_global) while a data-parallel step trains rows [row0, row0 + B) of a global
+        # batch: the noise is then drawn for the whole batch and the shard takes its rows
+        self.noise_rows = None
         self._kernel_events = None
 
     def _noise(self, name, B, A, pins):
         """Device pointer of a [B, A] standard normal draw (kept alive in `pins`)."""
         if self.noise_hook is not None:
             return pins(self.noise_hook(name, (B, A), pins.device))
+        rows = getattr(self, "noise_rows", None)
+        if rows is not None:
+            row0, batch_global = rows
+            return pins(torch.randn(batch_global, A, device=pins.device)[row0:row0 + B])
         return pins(torch.randn(B, A, device=pins.device))
 
     def _workspace(self, B, device):

@@ -74,17 +74,9 @@ class P2PExchange:
         self._slices = {}
         dist.barrier(group=group)  # every pool is allocated, zeroed and mapped before any push
 
-    def slice_for(self, key, n: int):
-        """(recv pointer table, flag pointer table, stride, max_blocks) for the optimizer `key`
-        (call in the same order on every rank)."""
-        import torch
-
-        if key in self._slices:
-            return self._slices[key]
-        W = self.world
-        stride = (int(n) + 31) // 32 * 32
-        recv_bytes = 2 * W * stride * 4
-        flag_bytes = 2 * W * self.MAX_BLOCKS * 4
+    def _carve(self, recv_bytes: int, flag_bytes: int):
+        """(recv pointer table, flag pointer table) of the next free range of every rank's pool;
+        identical on all ranks as long as they carve in the same order."""
         off = (self._off + 255) // 256 * 256
         if off + recv_bytes + flag_bytes > self.pool_bytes:
             raise RuntimeError("P2PExchange pool exhausted: raise pool_bytes")
@@ -93,7 +85,30 @@ class P2PExchange:
         recv = torch.tensor([b + off for b in self.peer_base], dtype=torch.int64, device=dev)
         flags = torch.tensor([b + off + recv_bytes for b in self.peer_base], dtype=torch.int64,
                              device=dev)
+        return recv, flags
+
+    def slice_for(self, key, n: int):
+        """(recv pointer table, flag pointer table, stride, max_blocks) for the optimizer `key`
+        (call in the same order on every rank)."""
+        if key in self._slices:
+            return self._slices[key]
+        W = self.world
+        stride = (int(n) + 31) // 32 * 32
+        recv, flags = self._carve(2 * W * stride * 4, 2 * W * self.MAX_BLOCKS * 4)
         s = (recv, flags, stride, self.MAX_BLOCKS)
+        self._slices[key] = s
+        return s
+
+    def priority_slice(self, key, batch_global: int):
+        """(recv pointer table, flag pointer table, epoch counter) of `rb200_per_priority_exchange`
+        for the prioritized update `key` of `batch_global` rows: a fp64 [2][batch_global]
+        receive buffer and uint32 [2][world] flags per rank, next to the optimizer slices (call
+        in the same order on every rank).  The epoch is this rank's own device counter."""
+        if key in self._slices:
+            return self._slices[key]
+        recv, flags = self._carve(2 * int(batch_global) * 8, 2 * self.world * 4)
+        epoch = torch.zeros(1, dtype=torch.int32, device=recv.device)
+        s = (recv, flags, epoch)
         self._slices[key] = s
         return s
 

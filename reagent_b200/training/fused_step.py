@@ -22,14 +22,15 @@ on sample_discrete_dqn_batch under the same two limits; its exploration noise is
 torch.randn inside the graph, and a step returns its q1 loss.
 
 `FusedPolicyStep` is the device-resident online step for SACTrainer and TD3Trainer (continuous
-actions), with the same staging, draw, status words and optional prioritized replay.
+actions), with the same staging, draw, status words, optional prioritized replay and data
+parallel (`shard` + `process_group`).
 """
 from typing import Optional
 
 import numpy as np
 import torch
 
-from ..replay_memory.device_replay import DeviceReplay, PrioritizedUpdate
+from ..replay_memory.device_replay import DeviceReplay, PrioritizedUpdate, PriorityShard
 from ..replay_memory.prioritized_replay_buffer import PrioritizedReplayBuffer
 from .c51_trainer import C51Trainer
 from .discrete_crr_trainer import DiscreteCRRTrainer
@@ -51,6 +52,28 @@ _PRIORITY_SOURCES = {
     SACTrainer: (DeviceReplay.write_back_row_priorities, lambda t, ws: (ws["td_error"], 1.0)),
     TD3Trainer: (DeviceReplay.write_back_row_priorities, lambda t, ws: (ws["td_error"], 1.0)),
 }
+
+
+def _priority_shard(batch_size, shard, process_group) -> PriorityShard:
+    """The PriorityShard of a prioritized step's `shard = (rank, world)` on `process_group`;
+    world > 1 needs the group, and the group must have `world` ranks with this one `rank`."""
+    from .data_parallel import shard_rows
+
+    rank, world = (0, 1) if shard is None else (int(shard[0]), int(shard[1]))
+    if process_group is None:
+        if world > 1:
+            raise ValueError("per with shard needs process_group: every rank's priorities are "
+                             "gathered over it")
+    else:
+        import torch.distributed as dist
+
+        if world != dist.get_world_size(process_group) or rank != dist.get_rank(process_group):
+            raise ValueError(f"per with shard={tuple(shard) if shard else None} needs the "
+                             f"process group's (rank, world), "
+                             f"({dist.get_rank(process_group)}, "
+                             f"{dist.get_world_size(process_group)})")
+    row0, _ = shard_rows(batch_size, rank, world)
+    return PriorityShard(row0, batch_size, process_group)
 
 
 def _query_keyword(rb) -> str:
@@ -86,7 +109,14 @@ class FusedDqnStep:
         them.  The priority is computed from the TD error for DQN, and from the row's own
         distributional loss for QR-DQN (mean over the N^2 quantile pairs) and C51 (cross
         entropy).  Online, a transition staged without `priority` enters with the largest
-        priority recorded so far."""
+        priority recorded so far.
+
+        `per` with `shard` (and, for world > 1, `process_group` of that world): the tree is
+        replicated, every rank draws the same global indices and computes the importance
+        weights of all of them, and trains on its rows.  The priorities of all rows are then
+        gathered on every rank (DeviceReplay.write_back_priorities with a PriorityShard) and
+        applied in global batch order, so every rank's tree stays bit-identical;
+        `self.priorities` holds the gathered global vector."""
         if isinstance(trainer, ParametricDQNTrainer):
             if per is not None:
                 raise NotImplementedError("per does not cover ParametricDQNTrainer: its loss head "
@@ -115,9 +145,6 @@ class FusedDqnStep:
             if prefetch:
                 raise ValueError("per needs prefetch=False: a prefetched draw would run before "
                                  "the previous update's priority write-back")
-            if shard is not None or process_group is not None:
-                raise NotImplementedError("per is single-GPU: data-parallel write-back would need "
-                                          "every rank's TD errors")
             if type(trainer) not in self._per_trainers:
                 raise NotImplementedError("per covers DQNTrainer, QRDQNTrainer and C51Trainer; "
                                           "got " + type(trainer).__name__)
@@ -127,6 +154,12 @@ class FusedDqnStep:
         if online and rng != "device":
             raise ValueError("online=True needs rng='device' (device-resident replay)")
         self.rng, self.online = rng, bool(online)
+        self.prioritized = isinstance(replay_buffer, PrioritizedReplayBuffer)
+        if rng == "device" and not self.prioritized:
+            raise NotImplementedError("rng='device' covers the prioritized buffer")
+        self._shard = None
+        if per is not None and (shard is not None or process_group is not None):
+            self._shard = _priority_shard(batch_size, shard, process_group)
         self.trainer = trainer
         self.rb = replay_buffer
         self.B_global = batch_size
@@ -138,7 +171,6 @@ class FusedDqnStep:
             batch_size = hi - self.row0
         self.B = batch_size
         self.pg = process_group
-        self.prioritized = isinstance(replay_buffer, PrioritizedReplayBuffer)
         self._query_kw = _query_keyword(replay_buffer)
         self.dev = replay_buffer._dev()
         self.slots = []
@@ -152,8 +184,6 @@ class FusedDqnStep:
         replay_buffer._flush()
         self.dr = None
         if rng == "device":
-            if not self.prioritized:
-                raise NotImplementedError("rng='device' covers the prioritized buffer")
             # every slot's graph adds from its own staging block
             self.dr = getattr(replay_buffer, "_device_resident", None) or DeviceReplay(
                 replay_buffer, stage_rows=1, stage_slots=max(2, slots))
@@ -166,8 +196,10 @@ class FusedDqnStep:
             self.h2d_bytes = self.dr.h2d_bytes_per_add if self.online else 0
             self.d2h_bytes = 4 * self._loss_width + 8
             if per is not None:
-                self.weights = torch.empty(self.B, dtype=torch.float32, device=self.dev)
-                self.priorities = torch.empty(self.B, dtype=torch.float64, device=self.dev)
+                # the weights of all drawn rows: a shard's rows then get exactly the weights a
+                # single-GPU update gives them (p_min is over the whole draw)
+                self.weights = torch.empty(self.B_global, dtype=torch.float32, device=self.dev)
+                self.priorities = torch.empty(self.B_global, dtype=torch.float64, device=self.dev)
         # warm-up outside capture (lazy allocations, cudaFuncSetAttribute, optimizer state)
         self._one_update(None)
         torch.cuda.synchronize()
@@ -246,10 +278,11 @@ class FusedDqnStep:
         opt = self.trainer.optimizer_of(getattr(self.trainer, self._beta_net).arena)
         opt._ensure_state()
         self.dr.importance_weights(idx, opt.step_t, self.per, self.weights)
-        loss = self._train_batch(batch, importance_weights=self.weights)
+        loss = self._train_batch(batch,
+                                 importance_weights=self.weights[self.row0:self.row0 + self.B])
         write_back, inputs = _PRIORITY_SOURCES[type(self.trainer)]
         write_back(self.dr, idx, *inputs(self.trainer, self.trainer._ws), self.per,
-                   self.priorities)
+                   self.priorities, shard=self._shard)
         return loss
 
     def _prefetch_update(self, i, rnd_dev, overrides=None):
@@ -416,7 +449,11 @@ class FusedPolicyStep(FusedDqnStep):
     TD3 trains its actor on every `delayed_policy_update`-th batch only, a decision taken in
     Python; one graph is captured per phase (and staging slot) and `step()` picks it from its
     own update counter.  The constructor runs one eager warm-up update, which is batch 0.
-    `step()` returns the pinned host tensor that will hold [q1 loss, q2 loss] of the update."""
+    `step()` returns the pinned host tensor that will hold [q1 loss, q2 loss] of the update.
+
+    `shard=(rank, world)`, `process_group`: as FusedDqnStep's; each rank also draws the global
+    batch's noise and uses its own rows, so that a data-parallel run equals a single-GPU run
+    from the same seeds.  The losses are this rank's shard means."""
 
     _loss_width = 2
     _per_trainers = (SACTrainer, TD3Trainer)  # the exact types it covers, with or without per
@@ -430,9 +467,6 @@ class FusedPolicyStep(FusedDqnStep):
         if type(trainer) not in self._per_trainers:
             raise NotImplementedError("FusedPolicyStep covers SACTrainer and TD3Trainer; got "
                                       + type(trainer).__name__)
-        if shard is not None or process_group is not None:
-            raise NotImplementedError("FusedPolicyStep is single-GPU: a data-parallel priority "
-                                      "write-back would need every rank's TD errors")
         if rng != "device":
             raise ValueError("FusedPolicyStep needs rng='device' (device-resident replay)")
         if prefetch:
@@ -451,12 +485,12 @@ class FusedPolicyStep(FusedDqnStep):
         n0 = trainer.all_batches_processed
         # its warm-up (which also puts the action bounds on the device) is update 0
         super().__init__(trainer, replay_buffer, batch_size, slots=slots, rng="device",
-                         online=online, per=per)
+                         online=online, per=per, shard=shard, process_group=process_group)
         trainer.all_batches_processed = n0 + 1  # a capture runs the Python body, not an update
 
     def _gather(self, indices):
         return self.rb.sample_policy_network_batch(self.B, self.action_low, self.action_high,
-                                                   indices=indices)
+                                                   indices=indices[self.row0:self.row0 + self.B])
 
     def _one_update(self, rnd_dev):
         """One eager update (draw + train) of the next batch_idx, on the current stream: the
@@ -467,8 +501,14 @@ class FusedPolicyStep(FusedDqnStep):
         return loss
 
     def _train_batch(self, batch, **weights):
-        """Returns the critic losses; importance weights weight the critics only."""
-        return self.trainer.train_batch(batch, self._batch_idx, **weights)[0]
+        """Returns the critic losses; importance weights weight the critics only.  A shard
+        draws the global batch's noise and takes its own rows, as a single-GPU update would."""
+        t = self.trainer
+        t.noise_rows = (self.row0, self.B_global) if self.B != self.B_global else None
+        try:
+            return t.train_batch(batch, self._batch_idx, process_group=self.pg, **weights)[0]
+        finally:
+            t.noise_rows = None
 
     def _capture(self, i=0):
         graphs, hosts = [], []
